@@ -10,20 +10,17 @@
 #include <cuda_fp16.h>
 
 #include "fvs_common.h"
+#include "mem_device.cuh"
 
 namespace fvs {
 namespace alt {
 
-constexpr int SLICE = 1024;
+using mem::SLICE;
+using mem::butterfly_sum;
 constexpr float NEG = -100.0f;
 
 __device__ __forceinline__ float h2f(__half v) { return __half2float(v); }
 __device__ __forceinline__ float rh(float v) { return __half2float(__float2half_rn(v)); }
-__device__ __forceinline__ float butterfly_sum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = __fadd_rn(v, __shfl_xor_sync(0xffffffffu, v, o));
-  return v;
-}
 __device__ __forceinline__ bool better_max(float va, int ia, float vb, int ib) {  // NaN is maximal, then value, then first index
   const bool na = va != va, nb = vb != vb;
   if (na || nb) return (na && !nb) || (na && nb && ia < ib);

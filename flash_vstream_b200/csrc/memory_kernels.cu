@@ -4,8 +4,12 @@
 // "Reference-exact" means: every place where the reference's f16 PyTorch path rounds to binary16 we round too
 // (element-wise sub/mul, reduction results, sqrt, division), reductions accumulate in fp32, argmin takes the first
 // minimal index and lets NaN win. The ONE thing PyTorch leaves unspecified is the order of fp32 accumulation
-// inside a reduction; we fix a canonical order (documented at `slice_sqdiff` below) and oracle/fvs_oracle.py
+// inside a reduction; we fix a canonical order (documented at `slice_sqdiff` in mem_device.cuh) and oracle/fvs_oracle.py
 // mirrors it operation for operation, so kernel and oracle agree bit-for-bit.
+//
+// The k-means, abstract-memory, argsort and retrieval kernels here are the op-by-op form of the streaming step: each is a
+// launch shape around one per-unit function of mem_device.cuh, the same functions the fused consolidate_kernel
+// (stream_kernels.cu) calls, so the two paths compute the same bits.
 //
 // Reference anchors: compress_spatial_features vstream_arch.py:193-212; weighted_kmeans_feature
 // compress_functions.py:130-169; attention / get_weight vstream_arch.py:174-183,47-52; key retrieval
@@ -194,17 +198,8 @@ __global__ void __launch_bounds__(256) km_assign_kernel(KMBuffers B, int T, int 
   const int t = blockIdx.x * 8 + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
   if (t >= T) return;
-  float best = INFINITY;
-  int besti = 0x7fffffff;
-  for (int k = lane; k < K; k += 32) {
-    const float* p = B.part + (size_t(t) * K + k) * S;
-    float tot = 0.f;
-    for (int s = 0; s < S; ++s) tot = tot + p[s];
-    const float d = round_h(sqrtf(round_h(tot)));
-    if (besti == 0x7fffffff || argmin_better(d, k, best, besti)) { best = d; besti = k; }
-  }
-  warp_argmin(best, besti);
-  if (lane == 0) B.labels[t] = besti;
+  const int label = km_row_label(B.part + size_t(t) * K * S, K, S, lane);
+  if (lane == 0) B.labels[t] = label;
 }
 
 // one warp per (cluster j, slice s): weighted mean of the members (sequential in t), empty-cluster refill, and the
@@ -219,88 +214,9 @@ __global__ void __launch_bounds__(256) km_update_kernel(KMBuffers B, const uint1
   if (unit >= K * S) return;
   const int j = unit / S, s = unit % S;
   const int cur = B.st->cur;
-  const uint16_t* Cold = B.C[cur] + size_t(j) * PD + s * SLICE;
-  uint16_t* Cnew = B.C[cur ^ 1] + size_t(j) * PD + s * SLICE;
-
-  // weights_sum[j] (f16) and, for empty clusters, the rank among empty clusters (refills are consumed in j order).
-  // Every warp recomputes the per-cluster sums it needs from the labels: T is small (<= a few thousand).
-  float wsum_j = 0.f;
-  int empties_before = 0;
-  {
-    // lane-parallel over clusters 0..j to count empties (sum order inside a cluster: sequential in t)
-    for (int c = lane; c <= j; c += 32) {
-      float ws = 0.f;
-      for (int t = 0; t < T; ++t)
-        if (B.labels[t] == c) ws = ws + (w ? h2f(w[t]) : 1.0f);
-      const float wsh = round_h(ws);
-      if (c == j) wsum_j = wsh;
-      else if (!(wsh > 0.f)) empties_before++;
-    }
-    wsum_j = butterfly_sum(wsum_j);  // exactly one lane holds a non-zero value (or all zero)
-    empties_before = __reduce_add_sync(0xffffffffu, empties_before);
-  }
-  const bool nonempty = wsum_j > 0.f;
-
-  float acc[4][8];
-#pragma unroll
-  for (int i = 0; i < 4; ++i)
-#pragma unroll
-    for (int e = 0; e < 8; ++e) acc[i][e] = 0.f;
-  uint32_t outw[4][4];
-  if (nonempty) {
-    for (int t = 0; t < T; ++t) {
-      if (B.labels[t] != j) continue;
-      const __half wt = w ? __ushort_as_half(w[t]) : __float2half_rn(1.0f);
-      const __half2 wt2 = __half2half2(wt);
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const uint4 xv = *reinterpret_cast<const uint4*>(X + size_t(t) * PD + s * SLICE + i * 256 + lane * 8);
-        const uint32_t xw[4] = {xv.x, xv.y, xv.z, xv.w};
-#pragma unroll
-        for (int p = 0; p < 4; ++p) {
-          const __half2 pr = __hmul2(wt2, *reinterpret_cast<const __half2*>(&xw[p]));  // f16(w * x)
-          acc[i][2 * p] = acc[i][2 * p] + __low2float(pr);
-          acc[i][2 * p + 1] = acc[i][2 * p + 1] + __high2float(pr);
-        }
-      }
-    }
-#pragma unroll
-    for (int i = 0; i < 4; ++i)
-#pragma unroll
-      for (int p = 0; p < 4; ++p) {
-        // f16(f16(weighted_sum) / f16(weights_sum))
-        const float a = round_h(acc[i][2 * p]) / wsum_j, b = round_h(acc[i][2 * p + 1]) / wsum_j;
-        __half2 h = __floats2half2_rn(a, b);
-        outw[i][p] = *reinterpret_cast<uint32_t*>(&h);
-      }
-  } else {
-    const int src = refill_idx[B.st->refill_pos + empties_before];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const uint4 xv = *reinterpret_cast<const uint4*>(X + size_t(src) * PD + s * SLICE + i * 256 + lane * 8);
-      outw[i][0] = xv.x; outw[i][1] = xv.y; outw[i][2] = xv.z; outw[i][3] = xv.w;
-    }
-  }
-  // convergence partial: sum of float(f16(c_old - c_new))^2 in canonical slice order (squares NOT rounded: torch.norm)
-  float nacc = 0.f;
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const uint4 ov = *reinterpret_cast<const uint4*>(Cold + i * 256 + lane * 8);
-    const uint32_t ow[4] = {ov.x, ov.y, ov.z, ov.w};
-#pragma unroll
-    for (int p = 0; p < 4; ++p) {
-      const __half2 d = __hsub2(*reinterpret_cast<const __half2*>(&ow[p]), *reinterpret_cast<const __half2*>(&outw[i][p]));
-      const float dl = __low2float(d), dh = __high2float(d);
-      nacc = nacc + __fmul_rn(dl, dl);
-      nacc = nacc + __fmul_rn(dh, dh);
-    }
-    *reinterpret_cast<uint4*>(Cnew + i * 256 + lane * 8) = make_uint4(outw[i][0], outw[i][1], outw[i][2], outw[i][3]);
-  }
-  nacc = butterfly_sum(nacc);
-  if (lane == 0) {
-    B.normpart[j * S + s] = nacc;
-    if (s == 0) B.wsum[j] = f2h(wsum_j);
-  }
+  km_cluster_slice_update(X, w, B.labels, refill_idx + B.st->refill_pos, T, PD, S, j, s,
+                          B.C[cur] + size_t(j) * PD + s * SLICE, B.C[cur ^ 1] + size_t(j) * PD + s * SLICE, B.normpart,
+                          B.wsum, lane);
 }
 
 // single block: diff = f16(sum_k f16(sqrt(sum_s normpart))) ; break test; bookkeeping
@@ -311,9 +227,7 @@ __global__ void km_converge_kernel(KMBuffers B, int K, int PD, int iter, int max
   float diff = 0.f;
   int n_empty = 0;
   for (int k = 0; k < K; ++k) {
-    float tot = 0.f;
-    for (int s = 0; s < S; ++s) tot = tot + B.normpart[k * S + s];
-    diff = diff + round_h(sqrtf(tot));
+    diff = diff + centroid_shift(B.normpart, k, S);
     if (!(h2f(B.wsum[k]) > 0.f)) n_empty++;
   }
   const float diff_h = round_h(diff);
@@ -344,8 +258,8 @@ __global__ void km_finish_kernel(KMBuffers B, uint16_t* __restrict__ C_out, uint
 }
 
 // ------------------------------------------------------------------------------------------------ abstract memory
-// Rounding points follow the f16 PyTorch expression tree of vstream_arch.py:174-183 / :47-52.  Three small kernels
-// (projections: one block per row; softmax: one block; apply: grid over T1 x D) instead of one serial block.
+// Three small kernels (projections: one block per row; softmax: one block; apply: grid over T1 x D) instead of one serial
+// block; the arithmetic is abs_proj_dot / abs_softmax_row / abs_apply_elem of mem_device.cuh.
 struct AbsScratch {
   float* q;      // [T1, H]  (f16-rounded values)
   float* k;      // [T2, H]
@@ -365,11 +279,8 @@ __global__ void __launch_bounds__(256) abs_proj_kernel(const uint16_t* __restric
   float* out = isq ? S.q + size_t(r) * H : S.k + size_t(r - T1) * H;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
   for (int h = warp; h < H; h += nwarps) {
-    const uint16_t* wrow = W + size_t(h) * D;
-    float acc = 0.f;
-    for (int d = lane; d < D; d += 32) acc = fmaf(h2f(x[d]), h2f(wrow[d]), acc);
-    acc = butterfly_sum(acc);
-    if (lane == 0) out[h] = round_h(acc + h2f(b[h]));  // one rounding after the bias (addmm epilogue)
+    const float v = abs_proj_dot(x, W + size_t(h) * D, b + h, D, lane);
+    if (lane == 0) out[h] = v;
   }
 }
 
@@ -377,31 +288,8 @@ __global__ void __launch_bounds__(256) abs_softmax_kernel(AbsScratch S, int T1, 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
   const float sqrtH = sqrtf(float(H));
   for (int i = warp; i < T1; i += nwarps) {  // one warp per memory row
-    float mx = -INFINITY;
-    for (int j = lane; j < T2; j += 32) {
-      float acc = 0.f;
-      for (int h = 0; h < H; ++h) acc = fmaf(S.q[i * H + h], S.k[j * H + h], acc);
-      const float sc = round_h(round_h(acc) / sqrtH);  // f16(f16(q k^T) / sqrt(H))
-      S.wgt[i * T2 + j] = sc;
-      mx = fmaxf(mx, sc);
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-    float sum = 0.f;
-    for (int j = lane; j < T2; j += 32) {
-      const float e = expf(S.wgt[i * T2 + j] - mx);
-      S.wgt[i * T2 + j] = e;
-      sum += e;
-    }
-    sum = butterfly_sum(sum);
-    float dsum = 0.f;
-    for (int j = lane; j < T2; j += 32) {
-      const float wv = round_h(round_h(S.wgt[i * T2 + j] / sum) * ratio);  // f16(f16(softmax) * ratio)
-      S.wgt[i * T2 + j] = wv;
-      dsum += wv;
-    }
-    dsum = butterfly_sum(dsum);
-    if (lane == 0) S.decay[i] = round_h(dsum);
+    const float decay = abs_softmax_row(S.q, S.k, i, S.wgt + i * T2, T2, H, sqrtH, ratio, lane);
+    if (lane == 0) S.decay[i] = decay;
   }
 }
 
@@ -411,10 +299,7 @@ __global__ void __launch_bounds__(256) abs_apply_kernel(const uint16_t* __restri
   const int i = blockIdx.y;
   const int d = blockIdx.x * blockDim.x + threadIdx.x;
   if (d >= D) return;
-  float acc = 0.f;
-  for (int j = 0; j < T2; ++j) acc = fmaf(S.wgt[i * T2 + j], h2f(F[size_t(j) * D + d]), acc);
-  const float keep = round_h(h2f(M[size_t(i) * D + d]) * round_h(1.0f - S.decay[i]));
-  Mout[size_t(i) * D + d] = f2h(keep + round_h(acc));
+  Mout[size_t(i) * D + d] = abs_apply_elem(S.wgt + i * T2, F, T2, D, d, M[size_t(i) * D + d], S.decay[i]);
 }
 
 // ------------------------------------------------------------------------------------------------ argsort / retrieval
@@ -426,64 +311,25 @@ __global__ void argsort_desc_kernel(const void* __restrict__ w, int K, long long
           : dt == FVS_BF16 ? __uint_as_float(uint32_t(static_cast<const uint16_t*>(w)[i]) << 16)
                            : h2f(static_cast<const uint16_t*>(w)[i]);
   __syncthreads();
-  for (int i = threadIdx.x; i < K; i += blockDim.x) {
-    const float vi = sv[i];
-    const bool ni = vi != vi;
-    int rank = 0;
-    for (int j = 0; j < K; ++j) {
-      const float vj = sv[j];
-      const bool nj = vj != vj;
-      bool before;  // does j come before i in descending stable order?
-      if (ni || nj) before = (nj && !ni) || (nj && ni && j < i);
-      else before = vj > vi || (vj == vi && j < i);
-      rank += before ? 1 : 0;
-    }
-    order[rank] = i;
-  }
+  for (int i = threadIdx.x; i < K; i += blockDim.x) order[stable_desc_rank(i, K, [&](int j) { return sv[j]; })] = i;
 }
 
-// one warp per (l, k): d = f16(sqrt(f16(sum_p f16(sum_d f16(f16(a-b)^2))))).  Per-patch sum over D (D % 256 == 0) is ONE
-// warp pass: lane l owns elements i*256 + l*8 + e, sequential in (i, e), then the butterfly (oracle: _lane_sum).
+// one warp per (l, k): key_distance of working-set row l and key candidate order[k]
 __global__ void __launch_bounds__(256) key_dist_kernel(const uint16_t* __restrict__ lm, const long long* __restrict__ order,
                                                        float* __restrict__ dist, int L, int P, int D, int key_len) {
   const int unit = blockIdx.x * 8 + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
   if (unit >= L * key_len) return;
   const int l = unit / key_len, k = unit % key_len;
-  const uint16_t* a = lm + size_t(l) * P * D;
-  const uint16_t* b = lm + size_t(order[k]) * P * D;
-  float tot = 0.f;
-  for (int p = 0; p < P; ++p) {
-    float acc = 0.f;
-    for (int i = 0; i < D / 256; ++i) {
-      const uint4 av = *reinterpret_cast<const uint4*>(a + size_t(p) * D + i * 256 + lane * 8);
-      const uint4 bv = *reinterpret_cast<const uint4*>(b + size_t(p) * D + i * 256 + lane * 8);
-      const uint32_t aw[4] = {av.x, av.y, av.z, av.w};
-      const uint32_t bw[4] = {bv.x, bv.y, bv.z, bv.w};
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        const __half2 d = __hsub2(*reinterpret_cast<const __half2*>(&aw[q]), *reinterpret_cast<const __half2*>(&bw[q]));
-        const __half2 s = __hmul2(d, d);
-        acc = acc + __low2float(s);
-        acc = acc + __high2float(s);
-      }
-    }
-    tot = tot + round_h(butterfly_sum(acc));
-  }
-  if (lane == 0) dist[unit] = round_h(sqrtf(round_h(tot)));
+  const float d = key_distance(lm + size_t(l) * P * D, lm + size_t(order[k]) * P * D, P, D, lane);
+  if (lane == 0) dist[unit] = d;
 }
 
 __global__ void key_argmin_kernel(const float* __restrict__ dist, long long* __restrict__ idx_out, int L, int key_len) {
   const int k = blockIdx.x;
   const int lane = threadIdx.x;  // one warp
-  float best = INFINITY;
-  int besti = 0x7fffffff;
-  for (int l = lane; l < L; l += 32) {
-    const float d = dist[l * key_len + k];
-    if (besti == 0x7fffffff || argmin_better(d, l, best, besti)) { best = d; besti = l; }
-  }
-  warp_argmin(best, besti);
-  if (lane == 0) idx_out[k] = besti;
+  const int best = warp_argmin_of(L, [&](int l) { return dist[l * key_len + k]; }, lane);
+  if (lane == 0) idx_out[k] = best;
 }
 
 __global__ void gather_rows_kernel(const uint4* __restrict__ src, const long long* __restrict__ idx, uint4* __restrict__ out,

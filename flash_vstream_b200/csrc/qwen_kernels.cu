@@ -6,21 +6,19 @@
 // HBM/ALU-bound integer and fp32/16-bit element work (the contractions have <= 64 rows on one side: ~0.5 flop/byte, so
 // they run as split-K sweeps on the CUDA cores, not as tensor-core GEMMs).  Arithmetic follows the reference's PyTorch
 // expression trees: one rounding per op in the op's dtype, fp32 accumulation inside reductions in the canonical slice order
-// of memory_kernels.cu (fp32 products are rounded before they are added — no FMA — and 16-bit x 16-bit products are exact,
+// of mem_device.cuh (fp32 products are rounded before they are added — no FMA — and 16-bit x 16-bit products are exact,
 // so oracle/qwen_oracle.py reproduces every bit with numpy).
 #include "fvs_common.h"
 #include "fvs_ptx.cuh"
+#include "mem_device.cuh"
 
 namespace fvs {
 namespace qwen {
 
-constexpr int SLICE = 1024;
-
-__device__ __forceinline__ float butterfly_sum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = __fadd_rn(v, __shfl_xor_sync(0xffffffffu, v, o));
-  return v;
-}
+using mem::SLICE;
+using mem::argmin_better;
+using mem::butterfly_sum;
+using mem::warp_argmin;
 
 // element -> fp32 (exact widening); dt: FVS_F16 / FVS_BF16 / FVS_F32
 __device__ __forceinline__ float ld_f32(const void* base, size_t i, int dt) {
@@ -33,19 +31,6 @@ __device__ __forceinline__ float round_to(float v, int dt) {
   if (dt == FVS_BF16) return __bfloat162float(__float2bfloat16_rn(v));
   if (dt == FVS_F16) return __half2float(__float2half_rn(v));
   return v;
-}
-__device__ __forceinline__ bool argmin_better(float va, int ia, float vb, int ib) {  // NaN wins, then value, then index
-  const bool na = va != va, nb = vb != vb;
-  if (na || nb) return (na && !nb) || (na && nb && ia < ib);
-  return va < vb || (va == vb && ia < ib);
-}
-__device__ __forceinline__ void warp_argmin(float& v, int& i) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    const float ov = __shfl_xor_sync(0xffffffffu, v, o);
-    const int oi = __shfl_xor_sync(0xffffffffu, i, o);
-    if (argmin_better(ov, oi, v, i)) { v = ov; i = oi; }
-  }
 }
 
 // ------------------------------------------------------------------------------------------------ temporal_pool

@@ -15,8 +15,10 @@
 //      argsort of the cluster weights, key-frame distances + argmin, the abstract-memory update (a dedicated block that
 //      overlaps the Lloyd phases), and the write-back of [Turing | long | key | current] into the prefix buffer, which is
 //      laid out in the reader's order (vstream_arch.py:483) so the LLM's visual prefix is a VIEW of the bank.
-// The arithmetic is the reference-exact f16 arithmetic of memory_kernels.cu (same device functions, same canonical
-// summation order), so the bank is bit-identical to the unfused kernels and to oracle/fvs_oracle.py.
+// Every unit of work (a row's slice partials and label, a (cluster, slice) update, a convergence term, an argsort rank, a
+// key distance, an abstract-memory dot product / softmax row / output element) is a device function of mem_device.cuh that
+// the op-by-op kernels of memory_kernels.cu call too; this kernel adds only the launch shape, barriers and bookkeeping.  So
+// the bank is bit-identical to the op-by-op path and to oracle/fvs_oracle.py.
 //
 // Readers in other processes / on other GPUs (the LLM rank) map the prefix buffer through CUDA IPC and take a consistent
 // snapshot with fvs_bank_snapshot: the kernel brackets its write-back with a sequence counter (odd while writing).
@@ -42,7 +44,6 @@ constexpr int kMaxS = 32;    // 1024-element slices per long-memory row
 struct StepArgs {
   // ---- shapes (all host-known: the data-dependent part of a step is only WHICH rows win)
   int D, PDl, PDa, S;          // channel dim; elements of a long row (b*b*D) / a frame row (a*a*D); PDl / 1024
-  int has_memory;              // 0: first call of the stream (state <- the clip itself, vstream_arch.py:669-672)
   int T, K, do_kmeans;         // k-means over T = old long rows + new frames, K = long_len; do_kmeans = T > K > 0
   int kl;                      // key frames retrieved this step = min(key_len, #sorted weights)
   int n_tur_in, tur_len, abs_chunks, H;   // Turing working rows, memory rows, number of <= tur_len-row chunks folded in
@@ -65,7 +66,6 @@ struct StepArgs {
   const uint16_t *Wq, *bq, *Wk, *bk;
   // ---- workspace
   uint16_t* C[2];              // [K, PDl] centroid ping-pong
-  float* part;                 // [T, K, S]
   float* normpart;             // [K, S]
   uint16_t* wsum;              // [K]
   float* dist;                 // [T, kl]
@@ -100,8 +100,7 @@ __device__ __forceinline__ void group_sync(unsigned int* ctr, unsigned int n, un
 // ---------------------------------------------------------------------------------------------------- abstract memory
 // attention_feature (compress_functions.py:263-277) on a small group of blocks, concurrently with the Lloyd loop: per chunk
 // of <= tur_len new rows, projections (one warp per (row, h) dot product) | softmax * ratio and row decay (one warp per
-// memory row) | M' = M (1 - decay) + W F.  Arithmetic and rounding points = abs_proj / abs_softmax / abs_apply of
-// memory_kernels.cu.  Result: Mbuf[(chunks-1)&1].
+// memory row) | M' = M (1 - decay) + W F.  Result: Mbuf[(chunks-1)&1].
 __device__ void abstract_group(const StepArgs& A, int gb, int ng) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int T1 = A.tur_len, D = A.D, H = A.H;
@@ -116,49 +115,18 @@ __device__ void abstract_group(const StepArgs& A, int gb, int ng) {
       const int r = u / H, h = u % H;
       const bool isq = r < T1;
       const uint16_t* x = isq ? M + size_t(r) * D : F + size_t(r - T1) * D;
-      const uint16_t* wrow = (isq ? A.Wq : A.Wk) + size_t(h) * D;
-      float acc = 0.f;
-      for (int d = lane; d < D; d += 32) acc = fmaf(h2f(x[d]), h2f(wrow[d]), acc);
-      acc = butterfly_sum(acc);
-      if (lane == 0) (isq ? A.absq + r * H : A.absk + (r - T1) * H)[h] = round_h(acc + h2f((isq ? A.bq : A.bk)[h]));
+      const float v = abs_proj_dot(x, (isq ? A.Wq : A.Wk) + size_t(h) * D, (isq ? A.bq : A.bk) + h, D, lane);
+      if (lane == 0) (isq ? A.absq + r * H : A.absk + (r - T1) * H)[h] = v;
     }
     group_sync(A.abs_ctr, ng, target);
     for (int i = gb * kWarps + warp; i < T1; i += ng * kWarps) {   // softmax * ratio, row decay
-      float* wrow = A.abswgt + size_t(i) * T1;
-      float mx = -INFINITY;
-      for (int j = lane; j < T2; j += 32) {
-        float acc = 0.f;
-        for (int h = 0; h < H; ++h) acc = fmaf(A.absq[i * H + h], A.absk[j * H + h], acc);
-        const float sc = round_h(round_h(acc) / A.sqrtH);
-        wrow[j] = sc;
-        mx = fmaxf(mx, sc);
-      }
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-      float sum = 0.f;
-      for (int j = lane; j < T2; j += 32) {
-        const float e = expf(wrow[j] - mx);
-        wrow[j] = e;
-        sum += e;
-      }
-      sum = butterfly_sum(sum);
-      float dsum = 0.f;
-      for (int j = lane; j < T2; j += 32) {
-        const float wv = round_h(round_h(wrow[j] / sum) * A.ratio);
-        wrow[j] = wv;
-        dsum += wv;
-      }
-      dsum = butterfly_sum(dsum);
-      if (lane == 0) A.absdecay[i] = round_h(dsum);
+      const float decay = abs_softmax_row(A.absq, A.absk, i, A.abswgt + size_t(i) * T1, T2, H, A.sqrtH, A.ratio, lane);
+      if (lane == 0) A.absdecay[i] = decay;
     }
     group_sync(A.abs_ctr, ng, target);
-    for (int o = gb * kThreads + threadIdx.x; o < T1 * D; o += ng * kThreads) {   // M' = f16( f16(M * f16(1 - decay)) + f16(W @ F) )
+    for (int o = gb * kThreads + threadIdx.x; o < T1 * D; o += ng * kThreads) {   // M' = M (1 - decay) + W F
       const int i = o / D, d = o % D;
-      const float* wrow = A.abswgt + size_t(i) * T1;
-      float acc = 0.f;
-      for (int j = 0; j < T2; ++j) acc = fmaf(wrow[j], h2f(F[size_t(j) * D + d]), acc);
-      const float keep = round_h(h2f(M[size_t(i) * D + d]) * round_h(1.0f - A.absdecay[i]));
-      Mout[o] = f2h(keep + round_h(acc));
+      Mout[o] = abs_apply_elem(A.abswgt + size_t(i) * T1, F, T2, D, d, M[size_t(i) * D + d], A.absdecay[i]);
     }
     if (c + 1 < A.abs_chunks) group_sync(A.abs_ctr, ng, target);
     M = Mout;
@@ -211,108 +179,25 @@ __global__ void __launch_bounds__(kThreads, 1) consolidate_kernel(const StepArgs
         }
         __syncthreads();
         if (warp == 0) {
-          float best = INFINITY;
-          int besti = 0x7fffffff;
-          for (int k = lane; k < K; k += 32) {
-            float tot = 0.f;
-            for (int sl = 0; sl < S; ++sl) tot = tot + s_part[k * S + sl];
-            const float d = round_h(sqrtf(round_h(tot)));
-            if (besti == 0x7fffffff || argmin_better(d, k, best, besti)) { best = d; besti = k; }
-          }
-          warp_argmin(best, besti);
-          if (lane == 0) A.labels_out[t] = besti;
+          const int label = km_row_label(s_part, K, S, lane);
+          if (lane == 0) A.labels_out[t] = label;
         }
         __syncthreads();
       }
       group_sync(A.km_ctr, nwork, km_target);
-      {
-        for (int t = threadIdx.x; t < T; t += kThreads) s_labels[t] = A.labels_out[t];
-        __syncthreads();
-        // phase C: one warp per (cluster j, slice s): mean of the members (unit weights), empty-cluster refill, ||dc||^2 partial
-        for (int unit = wb * kWarps + warp; unit < K * S; unit += nwork * kWarps) {
-          const int j = unit / S, s = unit % S;
-          const uint16_t* Cold = (have_c ? A.C[cur] + size_t(j) * PD : A.LW + size_t(A.init_idx[j]) * PD) + s * SLICE;
-          uint16_t* Cnew = A.C[nxt] + size_t(j) * PD + s * SLICE;
-          float wsum_j = 0.f;
-          int empties_before = 0;
-          for (int c = lane; c <= j; c += 32) {
-            float ws = 0.f;
-            for (int t = 0; t < T; ++t)
-              if (s_labels[t] == c) ws = ws + 1.0f;
-            const float wsh = round_h(ws);
-            if (c == j) wsum_j = wsh;
-            else if (!(wsh > 0.f)) empties_before++;
-          }
-          wsum_j = butterfly_sum(wsum_j);
-          empties_before = __reduce_add_sync(0xffffffffu, empties_before);
-          const bool nonempty = wsum_j > 0.f;
-          float acc[4][8];
-#pragma unroll
-          for (int i = 0; i < 4; ++i)
-#pragma unroll
-            for (int e = 0; e < 8; ++e) acc[i][e] = 0.f;
-          uint32_t outw[4][4];
-          if (nonempty) {
-            const __half2 wt2 = __half2half2(__float2half_rn(1.0f));
-            for (int t = 0; t < T; ++t) {
-              if (s_labels[t] != j) continue;
-#pragma unroll
-              for (int i = 0; i < 4; ++i) {
-                const uint4 xv = *reinterpret_cast<const uint4*>(A.LW + size_t(t) * PD + s * SLICE + i * 256 + lane * 8);
-                const uint32_t xw[4] = {xv.x, xv.y, xv.z, xv.w};
-#pragma unroll
-                for (int p = 0; p < 4; ++p) {
-                  const __half2 pr = __hmul2(wt2, *reinterpret_cast<const __half2*>(&xw[p]));  // f16(w * x)
-                  acc[i][2 * p] = acc[i][2 * p] + __low2float(pr);
-                  acc[i][2 * p + 1] = acc[i][2 * p + 1] + __high2float(pr);
-                }
-              }
-            }
-#pragma unroll
-            for (int i = 0; i < 4; ++i)
-#pragma unroll
-              for (int p = 0; p < 4; ++p) {
-                const float a = round_h(acc[i][2 * p]) / wsum_j, b = round_h(acc[i][2 * p + 1]) / wsum_j;
-                __half2 h = __floats2half2_rn(a, b);
-                outw[i][p] = *reinterpret_cast<uint32_t*>(&h);
-              }
-          } else {
-            const int src = A.refill_idx[refill_pos + empties_before];
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              const uint4 xv = *reinterpret_cast<const uint4*>(A.LW + size_t(src) * PD + s * SLICE + i * 256 + lane * 8);
-              outw[i][0] = xv.x; outw[i][1] = xv.y; outw[i][2] = xv.z; outw[i][3] = xv.w;
-            }
-          }
-          float nacc = 0.f;
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const uint4 ov = *reinterpret_cast<const uint4*>(Cold + i * 256 + lane * 8);
-            const uint32_t ow[4] = {ov.x, ov.y, ov.z, ov.w};
-#pragma unroll
-            for (int p = 0; p < 4; ++p) {
-              const __half2 d = __hsub2(*reinterpret_cast<const __half2*>(&ow[p]), *reinterpret_cast<const __half2*>(&outw[i][p]));
-              const float dl = __low2float(d), dh = __high2float(d);
-              nacc = nacc + __fmul_rn(dl, dl);
-              nacc = nacc + __fmul_rn(dh, dh);
-            }
-            *reinterpret_cast<uint4*>(Cnew + i * 256 + lane * 8) = make_uint4(outw[i][0], outw[i][1], outw[i][2], outw[i][3]);
-          }
-          nacc = butterfly_sum(nacc);
-          if (lane == 0) {
-            A.normpart[j * S + s] = nacc;
-            if (s == 0) A.wsum[j] = f2h(wsum_j);
-          }
-        }
+      for (int t = threadIdx.x; t < T; t += kThreads) s_labels[t] = A.labels_out[t];
+      __syncthreads();
+      // phase C: one warp per (cluster j, slice s): mean of the members (unit weights), empty-cluster refill, ||dc||^2 partial
+      for (int unit = wb * kWarps + warp; unit < K * S; unit += nwork * kWarps) {
+        const int j = unit / S, s = unit % S;
+        const uint16_t* Cold = (have_c ? A.C[cur] + size_t(j) * PD : A.LW + size_t(A.init_idx[j]) * PD) + s * SLICE;
+        km_cluster_slice_update(A.LW, nullptr, s_labels, A.refill_idx + refill_pos, T, PD, S, j, s, Cold,
+                                A.C[nxt] + size_t(j) * PD + s * SLICE, A.normpart, A.wsum, lane);
       }
       group_sync(A.km_ctr, nwork, km_target);
       // phase D (every block for itself, identical result): diff = f16(sum_k f16(sqrt(sum_s normpart))) < f16(tol) ?
       if (warp == 0) {
-        for (int k = lane; k < K; k += 32) {
-          float tot = 0.f;
-          for (int s = 0; s < S; ++s) tot = tot + A.normpart[k * S + s];
-          s_v[k] = round_h(sqrtf(tot));
-        }
+        for (int k = lane; k < K; k += 32) s_v[k] = centroid_shift(A.normpart, k, S);
         __syncwarp();
         if (lane == 0) {
           float diff = 0.f;
@@ -350,51 +235,17 @@ __global__ void __launch_bounds__(kThreads, 1) consolidate_kernel(const StepArgs
   if (kl > 0 && !abs_block) {
     // stable descending argsort of the cluster weights (pass-through: all ones -> identity)
     if (A.do_kmeans) {
-      for (int i = threadIdx.x; i < K; i += kThreads) {
-        const float vi = h2f(A.wsum[i]);
-        const bool ni = vi != vi;
-        int rank = 0;
-        for (int j = 0; j < K; ++j) {
-          const float vj = h2f(A.wsum[j]);
-          const bool nj = vj != vj;
-          bool before;
-          if (ni || nj) before = (nj && !ni) || (nj && ni && j < i);
-          else before = vj > vi || (vj == vi && j < i);
-          rank += before ? 1 : 0;
-        }
-        s_order[rank] = i;
-      }
+      for (int i = threadIdx.x; i < K; i += kThreads)
+        s_order[stable_desc_rank(i, K, [&](int j) { return h2f(A.wsum[j]); })] = i;
     } else {
       for (int i = threadIdx.x; i < kl; i += kThreads) s_order[i] = i;
     }
     __syncthreads();
-    // d[l,k] = f16(sqrt(f16(sum_p f16(sum_d f16(f16(a-b)^2))))), one warp per (l, k); rows of the PRE-clustering working set
-    const int P = PD / D;
-    {
-      for (int unit = wb * kWarps + warp; unit < T * kl; unit += nwork * kWarps) {
-        const int l = unit / kl, k = unit % kl;
-        const uint16_t* a = A.LW + size_t(l) * PD;
-        const uint16_t* b = A.LW + size_t(s_order[k]) * PD;
-        float tot = 0.f;
-        for (int p = 0; p < P; ++p) {
-          float acc = 0.f;
-          for (int i = 0; i < D / 256; ++i) {
-            const uint4 av = *reinterpret_cast<const uint4*>(a + size_t(p) * D + i * 256 + lane * 8);
-            const uint4 bv = *reinterpret_cast<const uint4*>(b + size_t(p) * D + i * 256 + lane * 8);
-            const uint32_t aw[4] = {av.x, av.y, av.z, av.w};
-            const uint32_t bw[4] = {bv.x, bv.y, bv.z, bv.w};
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              const __half2 d = __hsub2(*reinterpret_cast<const __half2*>(&aw[q]), *reinterpret_cast<const __half2*>(&bw[q]));
-              const __half2 sq = __hmul2(d, d);
-              acc = acc + __low2float(sq);
-              acc = acc + __high2float(sq);
-            }
-          }
-          tot = tot + round_h(butterfly_sum(acc));
-        }
-        if (lane == 0) A.dist[unit] = round_h(sqrtf(round_h(tot)));
-      }
+    // key distances, one warp per (l, k); rows of the PRE-clustering working set
+    for (int unit = wb * kWarps + warp; unit < T * kl; unit += nwork * kWarps) {
+      const int l = unit / kl, k = unit % kl;
+      const float d = key_distance(A.LW + size_t(l) * PD, A.LW + size_t(s_order[k]) * PD, PD / D, D, lane);
+      if (lane == 0) A.dist[unit] = d;
     }
   }
   if (blockIdx.x == 0 && threadIdx.x == 0) {
@@ -406,13 +257,7 @@ __global__ void __launch_bounds__(kThreads, 1) consolidate_kernel(const StepArgs
   cur = A.info_out[4];
   if (kl > 0) {
     if (warp < kl) {   // first-index / NaN-wins argmin over the working-set rows (every block for itself)
-      float best = INFINITY;
-      int besti = 0x7fffffff;
-      for (int l = lane; l < T; l += 32) {
-        const float d = A.dist[l * kl + warp];
-        if (besti == 0x7fffffff || argmin_better(d, l, best, besti)) { best = d; besti = l; }
-      }
-      warp_argmin(best, besti);
+      const int besti = warp_argmin_of(T, [&](int l) { return A.dist[l * kl + warp]; }, lane);
       if (lane == 0) {
         s_idx[warp] = besti;
         if (blockIdx.x == 0) A.key_idx_out[warp] = besti;
@@ -499,7 +344,7 @@ __global__ void snapshot_kernel(const uint4* __restrict__ prefix, const unsigned
 inline size_t al(size_t v) { return (v + 255) & ~size_t(255); }
 
 struct Carve {
-  uint16_t* C[2]; float* part; float* normpart; uint16_t* wsum; float* dist; uint16_t* Mbuf[2];
+  uint16_t* C[2]; float* normpart; uint16_t* wsum; float* dist; uint16_t* Mbuf[2];
   float *absq, *absk, *abswgt, *absdecay;
   int* labels; int* info; long long* key_idx; unsigned int* done_ctr;   // done_ctr[0..2] = {finished blocks, k-means group, abstract group}
   size_t total;
@@ -518,7 +363,6 @@ Carve carve(const fvs_star_config& c, int chunk_cap, void* base) {
   const size_t K = c.long_len > 0 ? c.long_len : 1;
   w.C[0] = (uint16_t*)take(K * PDl * 2);
   w.C[1] = (uint16_t*)take(K * PDl * 2);
-  w.part = (float*)take(Tmax * K * S * 4);
   w.normpart = (float*)take(K * S * 4);
   w.wsum = (uint16_t*)take(K * 2);
   w.dist = (float*)take(Tmax * kMaxKey * 4);
@@ -633,7 +477,6 @@ int fvs_stream_step(const fvs_star_config* cfg, fvs_bank* bank, const fvs_ntm_we
   // ---- 2. the update
   StepArgs A = {};
   A.D = D; A.PDl = int(PDl); A.PDa = int(PDa); A.S = int(PDl / SLICE);
-  A.has_memory = has_memory ? 1 : 0;
   A.T = n_long_old + t;
   A.K = cfg->long_len;
   A.do_kmeans = (has_memory && A.K > 0 && A.T > A.K) ? 1 : 0;
@@ -669,7 +512,7 @@ int fvs_stream_step(const fvs_star_config* cfg, fvs_bank* bank, const fvs_ntm_we
   A.refill_idx = refill_idx;
   FVS_REQUIRE(!A.do_kmeans || (init_idx && refill_idx), "fvs_stream_step: k-means draws (init_idx, refill_idx) missing");
   if (ntm) { A.Wq = (const uint16_t*)ntm->q_w; A.bq = (const uint16_t*)ntm->q_b; A.Wk = (const uint16_t*)ntm->k_w; A.bk = (const uint16_t*)ntm->k_b; }
-  A.C[0] = w.C[0]; A.C[1] = w.C[1]; A.part = w.part; A.normpart = w.normpart; A.wsum = w.wsum; A.dist = w.dist;
+  A.C[0] = w.C[0]; A.C[1] = w.C[1]; A.normpart = w.normpart; A.wsum = w.wsum; A.dist = w.dist;
   A.Mbuf[0] = w.Mbuf[0]; A.Mbuf[1] = w.Mbuf[1]; A.labels_out = w.labels; A.info_out = w.info; A.key_idx_out = w.key_idx;
   A.done_ctr = w.done_ctr;
   A.km_ctr = w.done_ctr + 1;

@@ -38,7 +38,7 @@ SLICE = 1024
 
 
 # ----------------------------------------------------------------------------------------------------------------
-# canonical fp32 reductions (mirrored by csrc/memory_kernels.cu: slice_sqdiff / butterfly_sum)
+# canonical fp32 reductions (mirrored by csrc/mem_device.cuh: slice_sqdiff / butterfly_sum)
 # ----------------------------------------------------------------------------------------------------------------
 def _slice_sum(terms: np.ndarray) -> np.ndarray:
     """terms [..., n*1024] fp32 -> [..., n] fp32.  Within a 1024-slice lane l owns elements i*256 + l*8 + e
