@@ -5,6 +5,7 @@ ViT-L/14 frame encoding + Flash-Memory consolidation, behind the reference's own
     flash_vstream_b200.vstream_arch         <->  flash_vstream.model.vstream_arch (hot-path half)
     flash_vstream_b200.clip_encoder         <->  flash_vstream.model.multimodal_encoder.clip_encoder
     flash_vstream_b200.ops                  tensor-level wrappers over the C ABI (include/fvs_b200.h)
+    flash_vstream_b200.StreamPool           many streams on one GPU, stepped together (multistream.py)
     flash_vstream_b200.install()            rebinds the reference's modules to these implementations
 
 All arithmetic happens in libfvs_b200.so (hand-written CUDA for sm_90a).  There is no CPU fallback: importing the
@@ -22,3 +23,10 @@ def install():
 
 def native_library_path():
     return str(_lib.lib_path())
+
+
+def __getattr__(name):      # StreamPool imports torch: loaded on first use, so that importing the package stays cheap
+    if name == "StreamPool":
+        from .multistream import StreamPool
+        return StreamPool
+    raise AttributeError(f"module {__name__!r} has no attribute {name!r}")

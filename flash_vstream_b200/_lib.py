@@ -54,6 +54,11 @@ class Bank(C.Structure):         # fvs_bank
                 ("n_tur", C.c_int32), ("n_cur", C.c_int32), ("n_frames", C.c_int64), ("step", C.c_uint64)]
 
 
+class StreamJob(C.Structure):    # fvs_stream_job
+    _fields_ = [("bank", C.POINTER(Bank)), ("ntm", C.POINTER(NtmWeights)), ("frames", C.c_int), ("init_idx", C.c_void_p),
+                ("refill_idx", C.c_void_p), ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t)]
+
+
 KLARGE_EUCLIDEAN, KLARGE_COSINE = 0, 1
 INPUT_PIXELS, INPUT_FEATURES = 0, 1
 
@@ -85,6 +90,8 @@ SIGNATURES = {
     "fvs_bank_prefix": (_i, [C.POINTER(StarConfig), C.POINTER(Bank), C.POINTER(_vp), _i64p]),
     "fvs_stream_step": (_i, [C.POINTER(StarConfig), C.POINTER(Bank), C.POINTER(NtmWeights), _vp, _vp, _i, _i, _vp, _vp,
                              _vp, _sz, _vp, _sz, _vp]),
+    "fvs_stream_step_multi": (_i, [C.POINTER(StarConfig), C.POINTER(StreamJob), _i, _vp, _vp, _i, _vp, _sz, _i, _vp]),
+    "fvs_stream_plan": (_i, [C.POINTER(StarConfig), C.POINTER(StreamJob), _i, _i, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
     "fvs_stream_step_info": (_i, [C.POINTER(StarConfig), C.POINTER(Bank), _vp, C.POINTER(_vp), C.POINTER(_vp), C.POINTER(_vp),
                                   C.POINTER(_vp)]),
     "fvs_bank_snapshot": (_i, [_vp, _vp, _vp, C.c_int64, _i, _i, _i, _vp, _vp]),

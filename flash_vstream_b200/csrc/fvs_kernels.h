@@ -27,8 +27,26 @@ int im2col_launch(const void* pixels, void* patches, int B, int S, int P, int Kp
 int drop_cls_launch(const void* x, const void* delta, void* out, int B, int tokens, int D, int dtype, cudaStream_t stream,
                     bool keep_cls = false);
 
-// memory_kernels.cu
-int pool3_residual_launch(const float* x, const void* delta, void* out_a, void* out_b, void* out_c, int T, int g, int a,
-                          int b, int D, cudaStream_t stream);
+// memory_kernels.cu: the three pooled STAR levels (pool3_kernel) of consecutive frames into per-destination outputs.
+// Destination i takes the next dst[i].frames frames of the concatenation: its frame f goes to rows a + f*a*a*D,
+// b + f*b*b*D and c + f*D (b / c may be null).  pool3_launch pools frames [f0, f0 + n) of the concatenation from `in`
+// (whose frame 0 is frame f0): the ViT encoder's fp32 residual stream [.., g*g+1, D] (residual) or f16 features
+// [.., g*g, D].  One launch per kPoolDst destinations the range touches.
+struct Pool3Dst {
+  void *a, *b, *c;
+  int frames;
+};
+constexpr int kPoolDst = 32;
+struct Pool3Table {   // kernel-parameter form of up to kPoolDst destinations; first[j] = first frame of the launch for j
+  int n;
+  int first[kPoolDst + 1];
+  uint16_t *a[kPoolDst], *b[kPoolDst], *c[kPoolDst];
+};
+int pool3_launch(const void* in, bool residual, const Pool3Dst* dst, int n_dst, int f0, int n, int g, int a, int b, int D,
+                 cudaStream_t stream);
+
+// vit_engine.cu: fvs_vit_encode_pool3 with the pooled levels going to n_dst destinations (frames of dst[0], then dst[1], ...)
+int vit_encode_pool3(fvs_vit_t h, const void* pixels, const Pool3Dst* dst, int n_dst, int a, int b, void* workspace,
+                     size_t workspace_bytes, cudaStream_t stream);
 
 }  // namespace fvs

@@ -15,6 +15,7 @@
 // compress_functions.py:130-169; attention / get_weight vstream_arch.py:174-183,47-52; key retrieval
 // vstream_arch.py:261-268, 681-688.
 #include "fvs_common.h"
+#include "fvs_kernels.h"
 #include "fvs_ptx.cuh"
 #include "mem_device.cuh"
 
@@ -63,12 +64,19 @@ __global__ void pool_kernel(const uint16_t* __restrict__ feat, uint16_t* __restr
 // shape) instead of the finished feature map: token (1 + p) of frame t contributes f16(x + delta) — exactly the value
 // drop_cls_kernel would have written to hidden_states[-2][:, 1:] (clip_encoder.py:35,50-51) — so the [T,576,D] feature
 // map is never materialised on the streaming path (SURVEY.md §8d: 4.17 -> 2.99 MB/frame).
+// Frame t of the launch belongs to destination j = the last with dst.first[j] <= t; its rows go to that destination's own
+// outputs (one stream's frame buffer / long / Turing working-set rows), so one launch pools the clips of many streams.
 template <int kMaxCells, bool kResidual>
 __global__ void __launch_bounds__(512) pool3_kernel(const void* __restrict__ feat_, const uint16_t* __restrict__ delta,
-                                                    uint16_t* __restrict__ out_a, uint16_t* __restrict__ out_b,
-                                                    uint16_t* __restrict__ out_c, int g, int a, int b, int D) {
+                                                    const __grid_constant__ Pool3Table dst, int g, int a, int b, int D) {
   __shared__ __half lvl_a[kMaxCells][64];
   const int t = blockIdx.x, slab = blockIdx.y;
+  int j = 0;
+  while (j + 1 < dst.n && t >= dst.first[j + 1]) ++j;
+  const int tl = t - dst.first[j];
+  uint16_t* __restrict__ out_a = dst.a[j];
+  uint16_t* __restrict__ out_b = dst.b[j];
+  uint16_t* __restrict__ out_c = dst.c[j];
   const int ka = g / a;
   const int ncell = a * a;
   const int v = threadIdx.x & 7;  // 8 vectors of 8 channels = 64 channels
@@ -119,7 +127,7 @@ __global__ void __launch_bounds__(512) pool3_kernel(const void* __restrict__ fea
       lvl_a[cell][v * 8 + 2 * p] = __low2half(h);
       lvl_a[cell][v * 8 + 2 * p + 1] = __high2half(h);
     }
-    *reinterpret_cast<uint4*>(out_a + (size_t(t) * ncell + cell) * D + slab * 64 + v * 8) = make_uint4(o[0], o[1], o[2], o[3]);
+    *reinterpret_cast<uint4*>(out_a + (size_t(tl) * ncell + cell) * D + slab * 64 + v * 8) = make_uint4(o[0], o[1], o[2], o[3]);
   }
   __syncthreads();
   const int ch = threadIdx.x & 63;
@@ -131,13 +139,13 @@ __global__ void __launch_bounds__(512) pool3_kernel(const void* __restrict__ fea
       float acc = 0.f;
       for (int ky = 0; ky < kb; ++ky)
         for (int kx = 0; kx < kb; ++kx) acc += __half2float(lvl_a[(oy * kb + ky) * a + ox * kb + kx][ch]);
-      out_b[(size_t(t) * b * b + cell) * D + slab * 64 + ch] = f2h(acc / divb);
+      out_b[(size_t(tl) * b * b + cell) * D + slab * 64 + ch] = f2h(acc / divb);
     }
   }
   if (out_c && threadIdx.x < 64) {
     float acc = 0.f;
     for (int cell = 0; cell < ncell; ++cell) acc += __half2float(lvl_a[cell][ch]);
-    out_c[size_t(t) * D + slab * 64 + ch] = f2h(acc / float(ncell));
+    out_c[size_t(tl) * D + slab * 64 + ch] = f2h(acc / float(ncell));
   }
 }
 
@@ -346,16 +354,46 @@ inline size_t al(size_t v) { return (v + 255) & ~size_t(255); }
 }  // namespace fvs
 
 namespace fvs {
-// encoder tail of the streaming path (vit_engine.cu): pool the three STAR levels straight from the fp32 residual stream
-int pool3_residual_launch(const float* x, const void* delta, void* out_a, void* out_b, void* out_c, int T, int g, int a,
-                          int b, int D, cudaStream_t stream) {
+int pool3_launch(const void* in, bool residual, const Pool3Dst* dst, int n_dst, int f0, int n, int g, int a, int b, int D,
+                 cudaStream_t stream) {
   using namespace mem;
-  if (!(x && out_a)) return set_error(FVS_EINVAL, "pool3_residual: null pointer");
-  if (!(T > 0 && g % a == 0 && (out_b == nullptr || (b > 0 && a % b == 0)) && D % 64 == 0 && a * a <= 64))
-    return set_error(FVS_EINVAL, "pool3_residual: bad pooling sizes g=%d a=%d b=%d D=%d", g, a, b, D);
-  pool3_kernel<64, true><<<dim3(T, D / 64), 512, 0, stream>>>(x, (const uint16_t*)delta, (uint16_t*)out_a,
-                                                              (uint16_t*)out_b, (uint16_t*)out_c, g, a, b, D);
-  FVS_CHECK_LAUNCH("pool3_kernel<residual>");
+  if (!(in && dst && n_dst > 0 && f0 >= 0 && n > 0)) return set_error(FVS_EINVAL, "pool3: null pointer or empty range");
+  if (!(g % a == 0 && D % 64 == 0 && a * a <= 64)) return set_error(FVS_EINVAL, "pool3: bad pooling sizes g=%d a=%d b=%d D=%d", g, a, b, D);
+  long long total = 0;
+  for (int i = 0; i < n_dst; ++i) {
+    if (!(dst[i].a && dst[i].frames > 0 && (dst[i].b == nullptr || (b > 0 && a % b == 0))))
+      return set_error(FVS_EINVAL, "pool3: destination %d: null output, no frames or bad b=%d", i, b);
+    total += dst[i].frames;
+  }
+  if (f0 + (long long)n > total) return set_error(FVS_EINVAL, "pool3: frames [%d, %d) beyond the %lld destination frames", f0, f0 + n, total);
+  const size_t ca = size_t(a) * a * D, cb = size_t(b) * b * D;
+  const size_t in_frame = residual ? size_t(g * g + 1) * D * 4 : size_t(g) * g * D * 2;   // bytes of one input frame
+  int i = 0, base = 0;                           // destination i starts at frame `base` of the concatenation
+  while (base + dst[i].frames <= f0) base += dst[i++].frames;
+  for (int done = 0; done < n;) {               // one launch per kPoolDst destinations (one launch when the range spans fewer)
+    Pool3Table tab = {};
+    int lf = 0;
+    while (tab.n < kPoolDst && done + lf < n) {
+      const int skip = f0 + done + lf - base;    // frames of destination i written by an earlier range
+      const int take = dst[i].frames - skip < n - done - lf ? dst[i].frames - skip : n - done - lf;
+      auto at = [&](void* p, size_t row) { return p ? static_cast<uint16_t*>(p) + size_t(skip) * row : nullptr; };
+      tab.first[tab.n] = lf;
+      tab.a[tab.n] = at(dst[i].a, ca); tab.b[tab.n] = at(dst[i].b, cb); tab.c[tab.n] = at(dst[i].c, size_t(D));
+      ++tab.n;
+      lf += take;
+      if (skip + take == dst[i].frames) base += dst[i++].frames;
+    }
+    tab.first[tab.n] = lf;
+    const void* src = static_cast<const uint8_t*>(in) + size_t(done) * in_frame;
+    if (residual) {
+      pool3_kernel<64, true><<<dim3(lf, D / 64), 512, 0, stream>>>(src, nullptr, tab, g, a, b, D);
+      FVS_CHECK_LAUNCH("pool3_kernel<residual>");
+    } else {
+      pool3_kernel<64, false><<<dim3(lf, D / 64), 512, 0, stream>>>(src, nullptr, tab, g, a, b, D);
+      FVS_CHECK_LAUNCH("pool3_kernel");
+    }
+    done += lf;
+  }
   return FVS_OK;
 }
 }  // namespace fvs
@@ -384,10 +422,8 @@ int fvs_spatial_pool3(const void* feat, void* out_a, void* out_b, void* out_c, i
   FVS_REQUIRE(dtype == FVS_F16, "fvs_spatial_pool3: only f16 is implemented");
   FVS_REQUIRE(T > 0 && g % a == 0 && (out_b == nullptr || (b > 0 && a % b == 0)), "fvs_spatial_pool3: bad pooling sizes g=%d a=%d b=%d", g, a, b);
   FVS_REQUIRE(D % 64 == 0 && a * a <= 64, "fvs_spatial_pool3: D %% 64 and a*a <= 64 required");
-  pool3_kernel<64, false><<<dim3(T, D / 64), 512, 0, (cudaStream_t)stream>>>(feat, nullptr, (uint16_t*)out_a,
-                                                                             (uint16_t*)out_b, (uint16_t*)out_c, g, a, b, D);
-  FVS_CHECK_LAUNCH("pool3_kernel");
-  return FVS_OK;
+  const Pool3Dst dst = {out_a, out_b, out_c, T};
+  return pool3_launch(feat, false, &dst, 1, 0, T, g, a, b, D, (cudaStream_t)stream);
 }
 
 size_t fvs_kmeans_workspace_bytes(int T, int K, int PD) {

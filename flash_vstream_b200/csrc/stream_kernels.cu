@@ -10,7 +10,7 @@
 //   1. the three pooled STAR levels, written straight into the bank's arrays — by the encoder's tail
 //      (fvs_vit_encode_pool3: pooled from the fp32 residual stream, the [t,576,D] feature map is never stored) or by
 //      pool3_kernel when the caller brings finished ViT features;
-//   2. ONE cooperative kernel (consolidate_kernel) that walks the whole update with grid-wide barriers and a DEVICE-SIDE
+//   2. ONE cooperative kernel (consolidate_kernel) that walks the whole update with block-group barriers and a DEVICE-SIDE
 //      early exit: Lloyd iterations (distance partials | assign + weighted mean + refill + convergence partial), stable
 //      argsort of the cluster weights, key-frame distances + argmin, the abstract-memory update (a dedicated block that
 //      overlaps the Lloyd phases), and the write-back of [Turing | long | key | current] into the prefix buffer, which is
@@ -20,9 +20,15 @@
 // the op-by-op kernels of memory_kernels.cu call too; this kernel adds only the launch shape, barriers and bookkeeping.  So
 // the bank is bit-identical to the op-by-op path and to oracle/fvs_oracle.py.
 //
+// fvs_stream_step_multi steps many banks the same way: one pooling pass for all their clips, then as few cooperative launches
+// of consolidate_kernel as fit on the device, each job on its own range of blocks with its own barriers.
+//
 // Readers in other processes / on other GPUs (the LLM rank) map the prefix buffer through CUDA IPC and take a consistent
 // snapshot with fvs_bank_snapshot: the kernel brackets its write-back with a sequence counter (odd while writing).
 #include <cooperative_groups.h>
+
+#include <cstdio>
+#include <vector>
 
 #include "fvs_common.h"
 #include "fvs_kernels.h"
@@ -71,8 +77,8 @@ struct StepArgs {
   float* dist;                 // [T, kl]
   uint16_t* Mbuf[2];           // [tur_len, D] abstract-memory ping-pong
   float *absq, *absk, *abswgt, *absdecay;   // [tur_len, H] x 2, [tur_len, tur_len], [tur_len] scratch of the abstract group
-  int n_abs_blocks;            // blocks [gridDim.x - n_abs_blocks, gridDim.x) form the abstract-memory group
-  unsigned int *km_ctr, *abs_ctr;   // arrival counters of the two block groups' barriers (zero at launch)
+  int n_abs_blocks;            // the job's last n_abs_blocks blocks form the abstract-memory group
+  unsigned int *km_ctr, *abs_ctr, *job_ctr;   // arrival counters of the two block groups' and the whole job's barriers (zero at launch)
   int* labels_out;             // [T]
   int* info_out;               // {exit_step, refills, converged, kmeans_ran}
   long long* key_idx_out;      // [kl]
@@ -134,8 +140,23 @@ __device__ void abstract_group(const StepArgs& A, int gb, int ng) {
 }
 
 // ---------------------------------------------------------------------------------------------------- the step kernel
-__global__ void __launch_bounds__(kThreads, 1) consolidate_kernel(const StepArgs A) {
-  cg::grid_group grid = cg::this_grid();
+// One cooperative launch (a "wave") advances up to kJobs banks.  Job j owns the contiguous blocks [first[j], first[j+1]):
+// its Lloyd-loop blocks, then its abstract-memory blocks.  Every barrier of a job counts that job's blocks only, so no
+// stream waits for another, and every phase is a stride loop over independent units of mem_device.cuh, so a bank's bits do
+// not depend on how many blocks its job gets.  fvs_stream_step is the one-job wave (kJobs = 1).
+template <int kJobs>
+struct Wave {
+  int n;
+  int first[kJobs + 1];
+  StepArgs job[kJobs];
+};
+
+template <int kJobs>
+__global__ void __launch_bounds__(kThreads, 1) consolidate_kernel(const __grid_constant__ Wave<kJobs> W) {
+  int j = 0;
+  if constexpr (kJobs > 1)
+    while (j + 1 < W.n && int(blockIdx.x) >= W.first[j + 1]) ++j;
+  const StepArgs& A = W.job[j];
   __shared__ int s_labels[kMaxT];
   __shared__ float s_part[kMaxK * kMaxS];   // distance partials of ONE row against every centroid slice
   __shared__ float s_v[kMaxK];
@@ -144,19 +165,19 @@ __global__ void __launch_bounds__(kThreads, 1) consolidate_kernel(const StepArgs
   __shared__ int s_flag[4];
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int G = gridDim.x;
+  const int G = W.first[j + 1] - W.first[j];          // this job's blocks
+  const int wb = int(blockIdx.x) - W.first[j];         // block index within the job
   const int nwork = G - A.n_abs_blocks;               // blocks [0, nwork): Lloyd loop + key distances; the rest: abstract memory
-  const bool abs_block = int(blockIdx.x) >= nwork;
-  const int wb = blockIdx.x;
-  unsigned int km_target = 0;
+  const bool abs_block = wb >= nwork;
+  unsigned int km_target = 0, job_target = 0;
   const int D = A.D, PD = A.PDl, S = A.S, T = A.T, K = A.K;
 
   // readers see an odd sequence number from before the first barrier until the write-back has completed
-  if (blockIdx.x == 0 && threadIdx.x == 0) {
+  if (wb == 0 && threadIdx.x == 0) {
     atomicAdd_system(&A.header[0], 1ull);
     __threadfence_system();
   }
-  if (abs_block) abstract_group(A, int(blockIdx.x) - nwork, A.n_abs_blocks);
+  if (abs_block) abstract_group(A, wb - nwork, A.n_abs_blocks);
 
   // ------------------------------------------------------------------ Lloyd loop (compress_functions.py:135-156)
   int have_c = 0, cur = 0, refill_pos = 0, exit_step = 0, converged = 0;
@@ -222,11 +243,11 @@ __global__ void __launch_bounds__(kThreads, 1) consolidate_kernel(const StepArgs
     if (!have_c) {
       // broke at the very first iteration: the result is the initial draw X[init_idx]; materialise it so that the
       // write-back below never permutes the working set in place
-      for (size_t i = size_t(blockIdx.x) * kThreads + threadIdx.x; i < size_t(K) * (PD / 8); i += size_t(nwork) * kThreads) {
+      for (size_t i = size_t(wb) * kThreads + threadIdx.x; i < size_t(K) * (PD / 8); i += size_t(nwork) * kThreads) {
         const int k = int(i / (PD / 8)), v = int(i % (PD / 8));
         reinterpret_cast<uint4*>(A.C[0])[i] = reinterpret_cast<const uint4*>(A.LW + size_t(A.init_idx[k]) * PD)[v];
       }
-      cur = 0;     // (the grid-wide barrier below orders these writes before the write-back reads them)
+      cur = 0;     // (the job-wide barrier below orders these writes before the write-back reads them)
     }
   }
 
@@ -248,19 +269,19 @@ __global__ void __launch_bounds__(kThreads, 1) consolidate_kernel(const StepArgs
       if (lane == 0) A.dist[unit] = d;
     }
   }
-  if (blockIdx.x == 0 && threadIdx.x == 0) {
+  if (wb == 0 && threadIdx.x == 0) {
     A.info_out[0] = exit_step; A.info_out[1] = refill_pos; A.info_out[2] = converged; A.info_out[3] = A.do_kmeans;
     A.info_out[4] = cur;       // which centroid buffer holds the result (the abstract group's blocks need it for the write-back)
   }
-  // the ONE grid-wide barrier: Lloyd loop, key distances and the abstract memory are all complete behind it
-  grid.sync();
+  // the ONE job-wide barrier: Lloyd loop, key distances and the abstract memory are all complete behind it
+  group_sync(A.job_ctr, G, job_target);
   cur = A.info_out[4];
   if (kl > 0) {
     if (warp < kl) {   // first-index / NaN-wins argmin over the working-set rows (every block for itself)
       const int besti = warp_argmin_of(T, [&](int l) { return A.dist[l * kl + warp]; }, lane);
       if (lane == 0) {
         s_idx[warp] = besti;
-        if (blockIdx.x == 0) A.key_idx_out[warp] = besti;
+        if (wb == 0) A.key_idx_out[warp] = besti;
       }
     }
     __syncthreads();
@@ -279,7 +300,7 @@ __global__ void __launch_bounds__(kThreads, 1) consolidate_kernel(const StepArgs
     const uint4* long_src = reinterpret_cast<const uint4*>(A.do_kmeans ? A.C[cur] : A.LW);
     const uint4* fr = reinterpret_cast<const uint4*>(A.frames);
     uint4* pre = reinterpret_cast<uint4*>(A.prefix);
-    for (size_t i = size_t(blockIdx.x) * kThreads + threadIdx.x; i < n5; i += size_t(G) * kThreads) {
+    for (size_t i = size_t(wb) * kThreads + threadIdx.x; i < n5; i += size_t(G) * kThreads) {
       if (i < n1) {
         pre[i] = tur_src[i];
       } else if (i < n2) {
@@ -295,7 +316,7 @@ __global__ void __launch_bounds__(kThreads, 1) consolidate_kernel(const StepArgs
       }
     }
   }
-  // the last block to finish publishes the counters and makes the sequence number even again
+  // the job's last block to finish publishes its counters and makes the sequence number even again
   __syncthreads();
   if (threadIdx.x == 0) {
     __threadfence_system();
@@ -306,6 +327,7 @@ __global__ void __launch_bounds__(kThreads, 1) consolidate_kernel(const StepArgs
       *A.done_ctr = 0u;
       *A.km_ctr = 0u;
       *A.abs_ctr = 0u;
+      *A.job_ctr = 0u;
       __threadfence_system();
       atomicAdd_system(&A.header[0], 1ull);
     }
@@ -346,7 +368,7 @@ inline size_t al(size_t v) { return (v + 255) & ~size_t(255); }
 struct Carve {
   uint16_t* C[2]; float* normpart; uint16_t* wsum; float* dist; uint16_t* Mbuf[2];
   float *absq, *absk, *abswgt, *absdecay;
-  int* labels; int* info; long long* key_idx; unsigned int* done_ctr;   // done_ctr[0..2] = {finished blocks, k-means group, abstract group}
+  int* labels; int* info; long long* key_idx; unsigned int* done_ctr;   // done_ctr[0..3] = {finished blocks, k-means group, abstract group, job}
   size_t total;
 };
 Carve carve(const fvs_star_config& c, int chunk_cap, void* base) {
@@ -393,6 +415,261 @@ int check_config(const fvs_star_config* c, const char* who) {
               "%s: memory lengths out of range (long %d <= %d, Turing %d <= 64)", who, c->long_len, kMaxK, c->tur_len);
   FVS_REQUIRE(c->key_len >= 0 && c->key_len <= kMaxKey, "%s: key_len %d > %d", who, c->key_len, kMaxKey);
   FVS_REQUIRE(c->ntm_dim > 0 && c->ntm_dim <= 64, "%s: ntm_dim %d out of range", who, c->ntm_dim);
+  return FVS_OK;
+}
+
+constexpr int kWaveJobs = 32;   // jobs per cooperative launch (the per-job kernel arguments travel as kernel parameters)
+
+// One job of a step, validated: its kernel arguments, its pooling destination and the blocks it wants.
+struct JobPrep {
+  StepArgs A;
+  Carve w;
+  Pool3Dst dst;
+  int units;   // blocks of its widest Lloyd / key-distance phase
+};
+
+// Every check of one job; fills the kernel arguments without touching the bank or the device.
+int prepare_job(const fvs_star_config* cfg, const fvs_stream_job& job, const char* who, JobPrep& P) {
+  const fvs_bank* bank = job.bank;
+  FVS_REQUIRE(bank && job.workspace, "%s: null argument", who);
+  FVS_REQUIRE(bank->prefix && bank->long_work && bank->tur_work && bank->frames && bank->header, "%s: bank buffers missing", who);
+  const int t = job.frames;
+  FVS_REQUIRE(t > 0 && t <= bank->chunk_cap, "%s: %d frames per call, bank was sized for <= %d", who, t, bank->chunk_cap);
+  FVS_REQUIRE(bank->n_frames + t <= bank->frames_cap, "%s: frame buffer full (%lld + %d > %lld): grow it first", who,
+              (long long)bank->n_frames, t, (long long)bank->frames_cap);
+  const Carve w = carve(*cfg, bank->chunk_cap, job.workspace);
+  FVS_REQUIRE(job.workspace_bytes >= w.total, "%s: workspace too small (%zu < %zu)", who, job.workspace_bytes, w.total);
+  const int D = cfg->D, a = cfg->cur_size, b = cfg->long_size;
+  const size_t PDa = size_t(a) * a * D, PDl = size_t(b) * b * D;
+  const bool has_memory = bank->step > 0;
+  const int n_long_old = has_memory ? bank->n_long : 0, n_tur_old = has_memory ? bank->n_tur : 0;
+  int64_t lrows, trows, prows;
+  fvs_bank_rows(cfg, bank->chunk_cap, &lrows, &trows, &prows);
+  FVS_REQUIRE(n_long_old + t <= lrows && n_tur_old + t <= trows, "%s: working set overflow", who);
+
+  // pooled levels of this clip -> frame buffer / long working set / Turing working set
+  P.dst.a = static_cast<uint16_t*>(bank->frames) + size_t(bank->n_frames) * PDa;
+  P.dst.b = static_cast<uint16_t*>(bank->long_work) + size_t(n_long_old) * PDl;
+  P.dst.c = static_cast<uint16_t*>(bank->tur_work) + size_t(n_tur_old) * D;
+  P.dst.frames = t;
+
+  StepArgs& A = P.A;
+  A = {};
+  A.D = D; A.PDl = int(PDl); A.PDa = int(PDa); A.S = int(PDl / SLICE);
+  A.T = n_long_old + t;
+  A.K = cfg->long_len;
+  A.do_kmeans = (has_memory && A.K > 0 && A.T > A.K) ? 1 : 0;
+  FVS_REQUIRE(A.T <= kMaxT, "%s: working set of %d rows > %d", who, A.T, kMaxT);
+  FVS_REQUIRE(A.S <= kMaxS, "%s: long rows of %d slices > %d", who, A.S, kMaxS);
+  const int n_sorted = A.do_kmeans ? A.K : A.T;
+  A.kl = (has_memory && cfg->long_len > 0) ? (cfg->key_len < n_sorted ? cfg->key_len : n_sorted) : 0;
+  A.n_tur_in = n_tur_old + t;
+  A.tur_len = cfg->tur_len;
+  A.abs_chunks = 0;
+  if (has_memory && cfg->tur_len > 0 && A.n_tur_in > cfg->tur_len)
+    A.abs_chunks = (A.n_tur_in - cfg->tur_len + cfg->tur_len - 1) / cfg->tur_len;
+  FVS_REQUIRE(A.abs_chunks == 0 || job.ntm, "%s: abstract-memory weights missing", who);
+  A.H = cfg->ntm_dim;
+  A.ratio = cfg->ratio;
+  A.sqrtH = sqrtf(float(cfg->ntm_dim));
+  A.cur_start = cfg->cur_len < t ? cfg->cur_len : t;
+  A.n_frames_after = bank->n_frames + t;
+  // lengths of 0 switch a memory off (offline guard vstream_arch.py:253,271; the reference's streaming branch has no such
+  // guard and would raise — this is the natural extension, used for the 256-token bank of SURVEY.md §8d(2))
+  A.n_tur_new = cfg->tur_len == 0 ? 0 : (A.abs_chunks > 0 ? cfg->tur_len : A.n_tur_in);
+  A.n_long_new = cfg->long_len == 0 ? 0 : (A.do_kmeans ? A.K : A.T);
+  A.n_cur_new = A.kl + A.cur_start;
+  A.max_iter = 10;                                                   // compress_functions.py:133
+  A.tol_h = __half_as_ushort(__float2half_rn(1e-4f));                // tol compared in the tensor dtype
+  A.LW = static_cast<uint16_t*>(bank->long_work);
+  A.TW = static_cast<uint16_t*>(bank->tur_work);
+  A.frames = static_cast<const uint16_t*>(bank->frames);
+  A.prefix = static_cast<uint16_t*>(bank->prefix);
+  A.header = static_cast<unsigned long long*>(bank->header);
+  A.step = bank->step + 1;
+  A.init_idx = job.init_idx;
+  A.refill_idx = job.refill_idx;
+  FVS_REQUIRE(!A.do_kmeans || (job.init_idx && job.refill_idx), "%s: k-means draws (init_idx, refill_idx) missing", who);
+  const fvs_ntm_weights* ntm = job.ntm;
+  if (ntm) { A.Wq = (const uint16_t*)ntm->q_w; A.bq = (const uint16_t*)ntm->q_b; A.Wk = (const uint16_t*)ntm->k_w; A.bk = (const uint16_t*)ntm->k_b; }
+  A.C[0] = w.C[0]; A.C[1] = w.C[1]; A.normpart = w.normpart; A.wsum = w.wsum; A.dist = w.dist;
+  A.Mbuf[0] = w.Mbuf[0]; A.Mbuf[1] = w.Mbuf[1]; A.labels_out = w.labels; A.info_out = w.info; A.key_idx_out = w.key_idx;
+  A.done_ctr = w.done_ctr;
+  A.km_ctr = w.done_ctr + 1;
+  A.abs_ctr = w.done_ctr + 2;
+  A.job_ctr = w.done_ctr + 3;
+  A.absq = w.absq; A.absk = w.absk; A.abswgt = w.abswgt; A.absdecay = w.absdecay;
+  const int64_t need_rows = int64_t(A.n_tur_new) + int64_t(A.n_long_new) * b * b + int64_t(A.n_cur_new) * a * a;
+  FVS_REQUIRE(need_rows <= prows, "%s: prefix of %lld rows exceeds the buffer (%lld)", who, (long long)need_rows, (long long)prows);
+
+  // blocks for the widest phase (the abstract-memory group comes on top)
+  int units = 8;
+  if (A.do_kmeans) {
+    units = A.T;                                            // phase A: one block per row
+    const int uc = (A.K * A.S + kWarps - 1) / kWarps;        // phase C: one warp per (cluster, slice)
+    if (uc > units) units = uc;
+  }
+  const int ue = (A.T * A.kl + kWarps - 1) / kWarps;
+  if (ue > units) units = ue;
+  P.units = units;
+  P.w = w;
+  return FVS_OK;
+}
+
+int min_blocks(const JobPrep& P) { return 1 + (P.A.abs_chunks > 0 ? 1 : 0); }
+
+// Launch plan for `budget` co-resident blocks per launch.  A job wants blocks for its widest phase plus an abstract-memory
+// group (16 blocks, 1 on small budgets) when its Turing memory folds a chunk — alone in a launch, exactly the grid of a
+// single-stream step.  Jobs are packed in order into as few waves as the budget allows (at least the minimum of every job,
+// at most kWaveJobs jobs); in a wave whose wants exceed the budget every job gets its minimum plus a share of the spare
+// blocks in proportion to what it wants beyond it (cumulative rounding: the shares add up to exactly the spare blocks).
+// Returns the number of waves, or an error when a job's minimum exceeds the budget.
+int plan_waves(const JobPrep* P, int n, int budget, const char* api, int* km_out, int* abs_out, int* wave_out) {
+  std::vector<int> km_want(n), abs_want(n);
+  for (int i = 0; i < n; ++i) {
+    FVS_REQUIRE(min_blocks(P[i]) <= budget, "%s: job %d needs at least %d blocks per launch, the budget is %d", api, i,
+                min_blocks(P[i]), budget);
+    abs_want[i] = P[i].A.abs_chunks > 0 ? (budget >= 64 ? 16 : 1) : 0;
+    const int room = budget - abs_want[i];
+    km_want[i] = P[i].units < room ? P[i].units : room;
+    if (km_want[i] < 1) km_want[i] = 1;
+  }
+  int waves = 0;
+  for (int s = 0; s < n; ++waves) {
+    int e = s, need = 0;
+    long long want = 0;
+    while (e < n && e - s < kWaveJobs && need + min_blocks(P[e]) <= budget) {
+      need += min_blocks(P[e]);
+      want += km_want[e] + abs_want[e];
+      ++e;
+    }
+    const long long spare = budget - need, excess = want - need;
+    long long cum = 0, given = 0;
+    auto share = [&](int extra) {
+      if (want <= budget) return extra;
+      cum += extra;
+      const long long upto = spare * cum / excess;
+      const long long g = upto - given;
+      given = upto;
+      return int(g);
+    };
+    for (int i = s; i < e; ++i) {
+      const int abs_min = P[i].A.abs_chunks > 0 ? 1 : 0;
+      km_out[i] = 1 + share(km_want[i] - 1);
+      abs_out[i] = abs_min + share(abs_want[i] - abs_min);
+      wave_out[i] = waves;
+    }
+    s = e;
+  }
+  return waves;
+}
+
+// Co-resident blocks of one cooperative launch: one per SM at most (the block groups spin on barriers).
+int device_budget(int* out) {
+  static int cap = 0;
+  if (cap == 0) {
+    int p1 = 0, pn = 0;
+    FVS_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&p1, consolidate_kernel<1>, kThreads, 0));
+    FVS_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&pn, consolidate_kernel<kWaveJobs>, kThreads, 0));
+    const int per_sm = p1 < pn ? p1 : pn;
+    const int co = (per_sm > 0 ? per_sm : 1) * device_sm_count();
+    cap = device_sm_count() < co ? device_sm_count() : co;
+  }
+  *out = cap;
+  return FVS_OK;
+}
+
+// Validate every job (no CUDA call, nothing touched), then plan for `budget` blocks (0: query the device).
+int prepare_all(const fvs_star_config* cfg, const fvs_stream_job* jobs, int n, const char* api, bool multi,
+                std::vector<JobPrep>& P) {
+  int r = check_config(cfg, api);
+  if (r) return r;
+  FVS_REQUIRE(jobs && n > 0, "%s: no jobs", api);
+  P.resize(n);
+  for (int i = 0; i < n; ++i) {
+    char who[64];
+    if (multi) snprintf(who, sizeof who, "%s: job %d", api, i);
+    else snprintf(who, sizeof who, "%s", api);
+    if ((r = prepare_job(cfg, jobs[i], who, P[i]))) return r;
+    for (int k = 0; k < i; ++k) {
+      FVS_REQUIRE(jobs[k].bank != jobs[i].bank && jobs[k].bank->header != jobs[i].bank->header,
+                  "%s: jobs %d and %d step the same bank", api, k, i);
+      FVS_REQUIRE(jobs[k].workspace != jobs[i].workspace, "%s: jobs %d and %d share a workspace", api, k, i);
+    }
+  }
+  return FVS_OK;
+}
+
+template <int kJobs>
+int launch_wave(const JobPrep* P, int n, const int* km, const int* ab, cudaStream_t stream) {
+  Wave<kJobs> W;
+  W.n = n;
+  W.first[0] = 0;
+  for (int i = 0; i < n; ++i) {
+    W.job[i] = P[i].A;
+    W.job[i].n_abs_blocks = ab[i];
+    W.first[i + 1] = W.first[i] + km[i] + ab[i];
+  }
+  void* args[] = {&W};
+  FVS_CUDA_OK(cudaLaunchCooperativeKernel((const void*)consolidate_kernel<kJobs>, dim3(W.first[n]), dim3(kThreads), args, 0,
+                                          stream));
+  FVS_CHECK_LAUNCH("consolidate_kernel");
+  return FVS_OK;
+}
+
+// fvs_stream_step / fvs_stream_step_multi: validate everything, then pool every clip (one encoder pass / one pool3 launch
+// for all jobs), then the consolidation waves; the host counters move only once every launch is enqueued.
+int step_jobs(const fvs_star_config* cfg, fvs_stream_job* jobs, int n, fvs_vit_t vit, const void* input, int input_kind,
+              void* vit_workspace, size_t vit_workspace_bytes, int max_blocks, cudaStream_t stream, bool multi) {
+  const char* api = multi ? "fvs_stream_step_multi" : "fvs_stream_step";
+  FVS_REQUIRE(input, "%s: null argument", api);
+  FVS_REQUIRE(input_kind == FVS_INPUT_PIXELS || input_kind == FVS_INPUT_FEATURES, "%s: bad input_kind %d", api, input_kind);
+  FVS_REQUIRE(input_kind != FVS_INPUT_PIXELS || (vit && vit_workspace), "%s: pixels need a ViT handle and its workspace", api);
+  FVS_REQUIRE(max_blocks >= 0, "%s: max_blocks %d < 0", api, max_blocks);
+  std::vector<JobPrep> P;
+  int r = prepare_all(cfg, jobs, n, api, multi, P);
+  if (r) return r;
+  for (int i = 0; i < n; ++i)
+    FVS_REQUIRE(max_blocks == 0 || min_blocks(P[i]) <= max_blocks, "%s: job %d needs at least %d blocks per launch, max_blocks is %d",
+                api, i, min_blocks(P[i]), max_blocks);
+  int budget = 0;
+  if ((r = device_budget(&budget))) return r;
+  if (max_blocks > 0 && max_blocks < budget) budget = max_blocks;
+  std::vector<int> km(n), ab(n), wave(n);
+  const int waves = plan_waves(P.data(), n, budget, api, km.data(), ab.data(), wave.data());
+  if (waves < 0) return waves;
+
+  // ---- 1. pooled levels of every clip, straight into each bank
+  std::vector<Pool3Dst> dst(n);
+  int total = 0;
+  for (int i = 0; i < n; ++i) dst[i] = P[i].dst, total += P[i].dst.frames;
+  if (input_kind == FVS_INPUT_PIXELS) {
+    if ((r = vit_encode_pool3(vit, input, dst.data(), n, cfg->cur_size, cfg->long_size, vit_workspace, vit_workspace_bytes, stream)))
+      return r;
+  } else {
+    if ((r = pool3_launch(input, false, dst.data(), n, 0, total, cfg->grid, cfg->cur_size, cfg->long_size, cfg->D, stream))) return r;
+  }
+
+  // ---- 2. the updates, one cooperative launch per wave
+  for (int i = 0; i < n; ++i)
+    if (jobs[i].bank->step == 0) FVS_CUDA_OK(cudaMemsetAsync(P[i].w.done_ctr, 0, 16, stream));
+  for (int s = 0; s < n;) {
+    int e = s;
+    while (e < n && wave[e] == wave[s]) ++e;
+    r = e - s == 1 ? launch_wave<1>(&P[s], 1, &km[s], &ab[s], stream)
+                   : launch_wave<kWaveJobs>(&P[s], e - s, &km[s], &ab[s], stream);
+    if (r) return r;
+    s = e;
+  }
+
+  for (int i = 0; i < n; ++i) {
+    fvs_bank* bank = jobs[i].bank;
+    bank->n_frames += jobs[i].frames;
+    bank->n_long = P[i].A.n_long_new;
+    bank->n_tur = P[i].A.n_tur_new;
+    bank->n_cur = P[i].A.n_cur_new;
+    bank->step += 1;
+  }
   return FVS_OK;
 }
 
@@ -443,116 +720,32 @@ int fvs_bank_prefix(const fvs_star_config* cfg, const fvs_bank* bank, void** pre
 int fvs_stream_step(const fvs_star_config* cfg, fvs_bank* bank, const fvs_ntm_weights* ntm, fvs_vit_t vit,
                     const void* input, int input_kind, int frames, const int32_t* init_idx, const int32_t* refill_idx,
                     void* vit_workspace, size_t vit_workspace_bytes, void* workspace, size_t workspace_bytes,
-                    fvs_stream_t stream_) {
-  int r = check_config(cfg, "fvs_stream_step");
+                    fvs_stream_t stream) {
+  fvs_stream_job job = {bank, ntm, frames, init_idx, refill_idx, workspace, workspace_bytes};
+  return step_jobs(cfg, &job, 1, vit, input, input_kind, vit_workspace, vit_workspace_bytes, 0, (cudaStream_t)stream, false);
+}
+
+int fvs_stream_step_multi(const fvs_star_config* cfg, fvs_stream_job* jobs, int n_jobs, fvs_vit_t vit, const void* input,
+                          int input_kind, void* vit_workspace, size_t vit_workspace_bytes, int max_blocks, fvs_stream_t stream) {
+  return step_jobs(cfg, jobs, n_jobs, vit, input, input_kind, vit_workspace, vit_workspace_bytes, max_blocks,
+                   (cudaStream_t)stream, true);
+}
+
+int fvs_stream_plan(const fvs_star_config* cfg, const fvs_stream_job* jobs, int n_jobs, int budget, int32_t* blocks_out,
+                    int32_t* wave_out) {
+  FVS_REQUIRE(budget > 0 && blocks_out && wave_out, "fvs_stream_plan: budget must be > 0 and outputs non-null");
+  std::vector<JobPrep> P;
+  int r = prepare_all(cfg, jobs, n_jobs, "fvs_stream_plan", true, P);
   if (r) return r;
-  FVS_REQUIRE(bank && input && workspace, "fvs_stream_step: null argument");
-  FVS_REQUIRE(bank->prefix && bank->long_work && bank->tur_work && bank->frames && bank->header, "fvs_stream_step: bank buffers missing");
-  FVS_REQUIRE(frames > 0 && frames <= bank->chunk_cap, "fvs_stream_step: %d frames per call, bank was sized for <= %d", frames, bank->chunk_cap);
-  FVS_REQUIRE(input_kind == FVS_INPUT_PIXELS || input_kind == FVS_INPUT_FEATURES, "fvs_stream_step: bad input_kind %d", input_kind);
-  FVS_REQUIRE(input_kind != FVS_INPUT_PIXELS || (vit && vit_workspace), "fvs_stream_step: pixels need a ViT handle and its workspace");
-  FVS_REQUIRE(bank->n_frames + frames <= bank->frames_cap, "fvs_stream_step: frame buffer full (%lld + %d > %lld): grow it first",
-              (long long)bank->n_frames, frames, (long long)bank->frames_cap);
-  const Carve w = carve(*cfg, bank->chunk_cap, workspace);
-  FVS_REQUIRE(workspace_bytes >= w.total, "fvs_stream_step: workspace too small (%zu < %zu)", workspace_bytes, w.total);
-  cudaStream_t stream = (cudaStream_t)stream_;
-  const int D = cfg->D, a = cfg->cur_size, b = cfg->long_size, t = frames;
-  const size_t PDa = size_t(a) * a * D, PDl = size_t(b) * b * D;
-  const bool has_memory = bank->step > 0;
-  const int n_long_old = has_memory ? bank->n_long : 0, n_tur_old = has_memory ? bank->n_tur : 0;
-  int64_t lrows, trows, prows;
-  fvs_bank_rows(cfg, bank->chunk_cap, &lrows, &trows, &prows);
-  FVS_REQUIRE(n_long_old + t <= lrows && n_tur_old + t <= trows, "fvs_stream_step: working set overflow");
-
-  // ---- 1. pooled levels of this clip -> frame buffer / long working set / Turing working set
-  uint16_t* out_a = static_cast<uint16_t*>(bank->frames) + size_t(bank->n_frames) * PDa;
-  uint16_t* out_b = static_cast<uint16_t*>(bank->long_work) + size_t(n_long_old) * PDl;
-  uint16_t* out_c = static_cast<uint16_t*>(bank->tur_work) + size_t(n_tur_old) * D;
-  if (input_kind == FVS_INPUT_PIXELS) {
-    if ((r = fvs_vit_encode_pool3(vit, input, out_a, out_b, out_c, t, a, b, vit_workspace, vit_workspace_bytes, stream_))) return r;
-  } else {
-    if ((r = fvs_spatial_pool3(input, out_a, out_b, out_c, t, cfg->grid, a, b, D, FVS_F16, stream_))) return r;
+  std::vector<int> km(n_jobs), ab(n_jobs), wave(n_jobs);
+  const int waves = plan_waves(P.data(), n_jobs, budget, "fvs_stream_plan", km.data(), ab.data(), wave.data());
+  if (waves < 0) return waves;
+  for (int i = 0; i < n_jobs; ++i) {
+    blocks_out[2 * i] = km[i];
+    blocks_out[2 * i + 1] = ab[i];
+    wave_out[i] = wave[i];
   }
-
-  // ---- 2. the update
-  StepArgs A = {};
-  A.D = D; A.PDl = int(PDl); A.PDa = int(PDa); A.S = int(PDl / SLICE);
-  A.T = n_long_old + t;
-  A.K = cfg->long_len;
-  A.do_kmeans = (has_memory && A.K > 0 && A.T > A.K) ? 1 : 0;
-  FVS_REQUIRE(A.T <= kMaxT, "fvs_stream_step: working set of %d rows > %d", A.T, kMaxT);
-  FVS_REQUIRE(A.S <= kMaxS, "fvs_stream_step: long rows of %d slices > %d", A.S, kMaxS);
-  const int n_sorted = A.do_kmeans ? A.K : A.T;
-  A.kl = (has_memory && cfg->long_len > 0) ? (cfg->key_len < n_sorted ? cfg->key_len : n_sorted) : 0;
-  A.n_tur_in = n_tur_old + t;
-  A.tur_len = cfg->tur_len;
-  A.abs_chunks = 0;
-  if (has_memory && cfg->tur_len > 0 && A.n_tur_in > cfg->tur_len)
-    A.abs_chunks = (A.n_tur_in - cfg->tur_len + cfg->tur_len - 1) / cfg->tur_len;
-  FVS_REQUIRE(A.abs_chunks == 0 || ntm, "fvs_stream_step: abstract-memory weights missing");
-  A.H = cfg->ntm_dim;
-  A.ratio = cfg->ratio;
-  A.sqrtH = sqrtf(float(cfg->ntm_dim));
-  A.cur_start = cfg->cur_len < t ? cfg->cur_len : t;
-  A.n_frames_after = bank->n_frames + t;
-  // lengths of 0 switch a memory off (offline guard vstream_arch.py:253,271; the reference's streaming branch has no such
-  // guard and would raise — this is the natural extension, used for the 256-token bank of SURVEY.md §8d(2))
-  A.n_tur_new = cfg->tur_len == 0 ? 0 : (A.abs_chunks > 0 ? cfg->tur_len : A.n_tur_in);
-  A.n_long_new = cfg->long_len == 0 ? 0 : (A.do_kmeans ? A.K : A.T);
-  A.n_cur_new = A.kl + A.cur_start;
-  A.max_iter = 10;                                                   // compress_functions.py:133
-  A.tol_h = __half_as_ushort(__float2half_rn(1e-4f));                // tol compared in the tensor dtype
-  A.LW = static_cast<uint16_t*>(bank->long_work);
-  A.TW = static_cast<uint16_t*>(bank->tur_work);
-  A.frames = static_cast<const uint16_t*>(bank->frames);
-  A.prefix = static_cast<uint16_t*>(bank->prefix);
-  A.header = static_cast<unsigned long long*>(bank->header);
-  A.step = bank->step + 1;
-  A.init_idx = init_idx;
-  A.refill_idx = refill_idx;
-  FVS_REQUIRE(!A.do_kmeans || (init_idx && refill_idx), "fvs_stream_step: k-means draws (init_idx, refill_idx) missing");
-  if (ntm) { A.Wq = (const uint16_t*)ntm->q_w; A.bq = (const uint16_t*)ntm->q_b; A.Wk = (const uint16_t*)ntm->k_w; A.bk = (const uint16_t*)ntm->k_b; }
-  A.C[0] = w.C[0]; A.C[1] = w.C[1]; A.normpart = w.normpart; A.wsum = w.wsum; A.dist = w.dist;
-  A.Mbuf[0] = w.Mbuf[0]; A.Mbuf[1] = w.Mbuf[1]; A.labels_out = w.labels; A.info_out = w.info; A.key_idx_out = w.key_idx;
-  A.done_ctr = w.done_ctr;
-  A.km_ctr = w.done_ctr + 1;
-  A.abs_ctr = w.done_ctr + 2;
-  A.absq = w.absq; A.absk = w.absk; A.abswgt = w.abswgt; A.absdecay = w.absdecay;
-  const int64_t need_rows = int64_t(A.n_tur_new) + int64_t(A.n_long_new) * b * b + int64_t(A.n_cur_new) * a * a;
-  FVS_REQUIRE(need_rows <= prows, "fvs_stream_step: prefix of %lld rows exceeds the buffer (%lld)", (long long)need_rows, (long long)prows);
-
-  // grid: enough blocks for the widest phase, one more for the abstract memory; all co-resident (cooperative launch)
-  int units = 8;
-  if (A.do_kmeans) {
-    units = A.T;                                            // phase A: one block per row
-    const int uc = (A.K * A.S + kWarps - 1) / kWarps;        // phase C: one warp per (cluster, slice)
-    if (uc > units) units = uc;
-  }
-  const int ue = (A.T * A.kl + kWarps - 1) / kWarps;
-  if (ue > units) units = ue;
-  static int max_blocks = 0;
-  if (max_blocks == 0) {
-    int per_sm = 0;
-    FVS_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, consolidate_kernel, kThreads, 0));
-    max_blocks = (per_sm > 0 ? per_sm : 1) * device_sm_count();
-  }
-  // one block per SM at most (the groups spin on barriers); a handful of blocks for the abstract memory, the rest for the Lloyd loop
-  const int cap = device_sm_count() < max_blocks ? device_sm_count() : max_blocks;
-  A.n_abs_blocks = A.abs_chunks > 0 ? (cap >= 64 ? 16 : 1) : 0;
-  if (units > cap - A.n_abs_blocks) units = cap - A.n_abs_blocks;
-  if (units < 1) units = 1;
-  const int G = units + A.n_abs_blocks;
-  if (bank->step == 0) FVS_CUDA_OK(cudaMemsetAsync(w.done_ctr, 0, 16, stream));
-  void* args[] = {&A};
-  FVS_CUDA_OK(cudaLaunchCooperativeKernel((const void*)consolidate_kernel, dim3(G), dim3(kThreads), args, 0, stream));
-  FVS_CHECK_LAUNCH("consolidate_kernel");
-
-  bank->n_frames += t;
-  bank->n_long = A.n_long_new;
-  bank->n_tur = A.n_tur_new;
-  bank->n_cur = A.n_cur_new;
-  bank->step += 1;
-  return FVS_OK;
+  return waves;
 }
 
 int fvs_stream_step_info(const fvs_star_config* cfg, const fvs_bank* bank, void* workspace, int32_t** labels, int32_t** info,

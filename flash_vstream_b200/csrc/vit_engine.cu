@@ -303,8 +303,8 @@ size_t fvs_vit_workspace_bytes(fvs_vit_t h, int max_frames) {
 // tail selector of encode_impl
 struct VitTail {
   void* out = nullptr;                                   // full feature map [frames, tokens(-1), hidden] ...
-  void *pool_a = nullptr, *pool_b = nullptr, *pool_c = nullptr;   // ... or the three pooled STAR levels
-  int a = 0, b = 0;
+  const fvs::Pool3Dst* pool = nullptr;                   // ... or the three pooled STAR levels of every frame
+  int n_pool = 0, a = 0, b = 0;
 };
 
 static int encode_impl(fvs_vit_t h, const void* pixels, const VitTail& tail, int frames, void* workspace,
@@ -334,16 +334,35 @@ static int encode_impl(fvs_vit_t h, const void* pixels, const VitTail& tail, int
                                nf, T, H, c.dtype, stream, c.keep_cls != 0)))
         return r;
     } else {
-      const size_t D = size_t(H);
-      auto adv = [&](void* p, int cells) { return p ? static_cast<uint16_t*>(p) + size_t(f0) * cells * D : nullptr; };
-      if ((r = pool3_residual_launch(reinterpret_cast<const float*>(ws.x), nullptr,
-                                     adv(tail.pool_a, tail.a * tail.a), adv(tail.pool_b, tail.b * tail.b), adv(tail.pool_c, 1),
-                                     nf, h->grid, tail.a, tail.b, H, stream)))
-        return r;
+      if ((r = pool3_launch(ws.x, true, tail.pool, tail.n_pool, f0, nf, h->grid, tail.a, tail.b, H, stream))) return r;
     }
   }
   return FVS_OK;
 }
+
+}  // extern "C"
+
+namespace fvs {
+int vit_encode_pool3(fvs_vit_t h, const void* pixels, const Pool3Dst* dst, int n_dst, int a, int b, void* workspace,
+                     size_t workspace_bytes, cudaStream_t stream) {
+  FVS_REQUIRE(h && pixels && dst && n_dst > 0 && workspace, "fvs_vit_encode_pool3: null argument");
+  FVS_REQUIRE(h->cfg.dtype == FVS_F16 && !h->cfg.keep_cls,
+              "fvs_vit_encode_pool3: needs an f16 tower with select_feature 'patch' (the reference casts to float16 before pooling, vstream_arch.py:649)");
+  int frames = 0;
+  for (int i = 0; i < n_dst; ++i) {
+    FVS_REQUIRE(dst[i].a && dst[i].frames > 0, "fvs_vit_encode_pool3: destination %d has no output or no frames", i);
+    FVS_REQUIRE(a > 0 && h->grid % a == 0 && a * a <= 64 && (dst[i].b == nullptr || (b > 0 && a % b == 0)),
+                "fvs_vit_encode_pool3: bad pooling sizes grid=%d a=%d b=%d", h->grid, a, b);
+    frames += dst[i].frames;
+  }
+  VitTail tail;
+  tail.pool = dst; tail.n_pool = n_dst;
+  tail.a = a; tail.b = b;
+  return encode_impl(h, pixels, tail, frames, workspace, workspace_bytes, stream, "fvs_vit_encode_pool3");
+}
+}  // namespace fvs
+
+extern "C" {
 
 int fvs_vit_encode(fvs_vit_t h, const void* pixels, void* out, int frames, void* workspace, size_t workspace_bytes,
                    fvs_stream_t stream_) {
@@ -358,16 +377,9 @@ int fvs_vit_encode(fvs_vit_t h, const void* pixels, void* out, int frames, void*
 int fvs_vit_encode_pool3(fvs_vit_t h, const void* pixels, void* out_a, void* out_b, void* out_c, int frames, int a, int b,
                          void* workspace, size_t workspace_bytes, fvs_stream_t stream_) {
   using namespace fvs;
-  FVS_REQUIRE(h && pixels && out_a && workspace, "fvs_vit_encode_pool3: null argument");
-  FVS_REQUIRE(frames > 0, "fvs_vit_encode_pool3: frames must be > 0");
-  FVS_REQUIRE(h->cfg.dtype == FVS_F16 && !h->cfg.keep_cls,
-              "fvs_vit_encode_pool3: needs an f16 tower with select_feature 'patch' (the reference casts to float16 before pooling, vstream_arch.py:649)");
-  FVS_REQUIRE(a > 0 && h->grid % a == 0 && a * a <= 64 && (out_b == nullptr || (b > 0 && a % b == 0)),
-              "fvs_vit_encode_pool3: bad pooling sizes grid=%d a=%d b=%d", h->grid, a, b);
-  VitTail tail;
-  tail.pool_a = out_a; tail.pool_b = out_b; tail.pool_c = out_c;
-  tail.a = a; tail.b = b;
-  return encode_impl(h, pixels, tail, frames, workspace, workspace_bytes, static_cast<cudaStream_t>(stream_), "fvs_vit_encode_pool3");
+  FVS_REQUIRE(out_a && frames > 0, "fvs_vit_encode_pool3: null output or frames <= 0");
+  const Pool3Dst dst = {out_a, out_b, out_c, frames};
+  return vit_encode_pool3(h, pixels, &dst, 1, a, b, workspace, workspace_bytes, static_cast<cudaStream_t>(stream_));
 }
 
 }  // extern "C"

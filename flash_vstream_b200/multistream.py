@@ -1,0 +1,193 @@
+"""Many video streams on one GPU: a pool of persistent banks stepped together (fvs_stream_step_multi, include/fvs_b200.h).
+
+One `StreamPool.step` encodes the clips of every listed stream in the ViT's micro-batches (weights read once per
+micro-batch instead of once per stream) and consolidates all their banks in as few cooperative launches as fit on the
+device.  Each stream's result is bit-identical to running it alone through the single-stream path
+(`FlashVStreamB200.embed_video_streaming` / `consolidate_streaming`) with the same draws.
+
+RNG contract.  In the reference every stream's memory manager is its own spawned process, so every stream has its own
+generators.  Here every stream owns a torch CPU + CUDA generator state and a `random.Random`, all seeded from
+`open(seed)`: its k-means draws (torch.randperm on the device, pre-drawn random.randint refill candidates) come from its
+own generators and its refill count is settled lazily against its own `random.Random`, exactly as
+compress_functions.sync_rng does for the global one.  So a stream draws what the single-stream path draws after
+`torch.manual_seed(seed); random.seed(seed)`, and the global torch / random state is never touched.
+"""
+from __future__ import annotations
+
+import os
+import random
+from typing import Optional
+
+import torch
+
+from . import ops
+from .compress_functions import MAX_ITER, _note_consumed
+
+REFERENCE_GRID = 24   # ViT-L/14 at 336 px: the patch grid of finished features when the model has no tower of its own
+
+
+class _StreamRng:
+    """one stream's generators: torch CPU + CUDA states swapped in around its draws, and its own random.Random"""
+
+    def __init__(self, seed: int, device: torch.device):
+        self.device = device
+        g = torch.Generator()
+        g.manual_seed(seed)
+        gc = torch.Generator(device=device)
+        gc.manual_seed(seed)
+        self.cpu, self.cuda = g.get_state(), gc.get_state()
+        self.py = random.Random(seed)
+        self.unsettled = []       # [T, pinned info | None, event | None] per draw, as in compress_functions
+
+    def settle(self):
+        while self.unsettled:
+            T, info_h, ev = self.unsettled.pop(0)
+            if info_h is None:
+                continue
+            ev.synchronize()
+            for _ in range(int(info_h[1])):
+                self.py.randint(0, T - 1)
+
+    def save(self):
+        return self.cpu, self.cuda, self.py.getstate(), list(self.unsettled)
+
+    def restore(self, st):
+        self.cpu, self.cuda, pys, self.unsettled = st
+        self.py.setstate(pys)
+
+    def draw(self, T: int, K: int):
+        """(init_idx, refill_idx, token): compress_functions._draw on this stream's generators"""
+        self.settle()
+        cpu0, cuda0 = torch.get_rng_state(), torch.cuda.get_rng_state(self.device)
+        try:
+            torch.set_rng_state(self.cpu)
+            torch.cuda.set_rng_state(self.cuda, self.device)
+            init_idx = torch.randperm(T, device=self.device)[:K].to(torch.int32)       # compress_functions.py:134
+            self.cpu, self.cuda = torch.get_rng_state(), torch.cuda.get_rng_state(self.device)
+        finally:
+            torch.set_rng_state(cpu0)
+            torch.cuda.set_rng_state(cuda0, self.device)
+        rng = random.Random()
+        rng.setstate(self.py.getstate())
+        refill = [rng.randint(0, T - 1) for _ in range(MAX_ITER * K)]                 # compress_functions.py:152
+        refill_idx = torch.tensor(refill, dtype=torch.int32).pin_memory().to(self.device, non_blocking=True)
+        token = [T, None, None]
+        self.unsettled.append(token)
+        return init_idx, refill_idx, token
+
+
+class _Stream:
+    def __init__(self, bank: ops.StreamBank, rng: _StreamRng):
+        self.bank, self.rng = bank, rng
+
+
+class StreamPool:
+    """A pool of streams sharing one model's tower, abstract-memory weights and STAR config.
+
+    `open(seed)` -> sid; `step({sid: clip, ...})` advances the listed streams in one batched step (clips: pixels
+    [t,3,S,S] or [1,t,3,S,S] for a model with a ViT engine, or finished features [t, grid*grid, D] f16; t <= chunk_cap);
+    `prefix(sid)` / `state(sid)` are views of the stream's bank; `bank(sid)` is the ops.StreamBank itself (hand it to
+    serve.export_bank / MemoryReader).  `close(sid)` resets the bank and keeps it for the next `open`.  Configs the
+    fused streaming step does not cover raise NotImplementedError: stream them through the model's single-stream path."""
+
+    def __init__(self, model, *, chunk_cap: int = 1, max_streams: Optional[int] = None):
+        host = model.get_model()
+        ntm = host.attention_model
+        D = ntm.q_proj.weight.shape[1]
+        tower = host.get_vision_tower()
+        engine = getattr(tower, "engine", None) if tower is not None else None
+        if engine is not None and (engine.dtype != torch.float16 or engine.keep_cls):
+            engine = None          # the pooled encoder tail needs an f16 tower with select_feature 'patch'
+        self.vit = engine
+        grid = engine.grid if engine is not None else REFERENCE_GRID
+        s = model._star_cfg()
+        knob = model._fused_reject(s, grid, D, torch.float16)
+        if knob is not None:
+            raise NotImplementedError(f"StreamPool: {knob} is outside what the batched streaming step covers; stream this "
+                                      f"config through the model's single-stream path")
+        self.cfg = model._fused_cfg(s, grid, D, torch.float16)
+        self.ntm = (ntm.q_proj.weight, ntm.q_proj.bias, ntm.k_proj.weight, ntm.k_proj.bias)
+        self.device = ntm.q_proj.weight.device
+        if self.device.type != "cuda":
+            raise ops.L.FvsError("StreamPool needs the model on a CUDA device (no CPU fallback)")
+        self.chunk_cap = int(chunk_cap)
+        self.max_streams = max_streams
+        self._streams: dict[int, _Stream] = {}
+        self._free: list[ops.StreamBank] = []
+        self._next = 0
+
+    # ---- streams -------------------------------------------------------------------------------------------------------
+    def open(self, seed: Optional[int] = None) -> int:
+        if self.max_streams is not None and len(self._streams) >= self.max_streams:
+            raise RuntimeError(f"StreamPool is full ({self.max_streams} streams)")
+        bank = self._free.pop() if self._free else ops.StreamBank(self.cfg, self.ntm, chunk_cap=self.chunk_cap, device=self.device)
+        bank.reset()
+        if seed is None:
+            seed = int.from_bytes(os.urandom(8), "little") >> 1
+        sid = self._next
+        self._next += 1
+        self._streams[sid] = _Stream(bank, _StreamRng(int(seed), self.device))
+        return sid
+
+    def close(self, sid: int):
+        st = self._streams.pop(sid)
+        st.bank.reset()
+        self._free.append(st.bank)
+
+    def __len__(self):
+        return len(self._streams)
+
+    def bank(self, sid: int) -> ops.StreamBank:
+        return self._streams[sid].bank
+
+    def prefix(self, sid: int) -> torch.Tensor:
+        """[Turing | long | key | current] of the stream: a view of its bank (vstream_arch.py:483)"""
+        return self._streams[sid].bank.prefix()
+
+    def state(self, sid: int):
+        """(cur, long, Turing, frame buffer) views, as StreamBank.state()"""
+        return self._streams[sid].bank.state()
+
+    # ---- one batched step ----------------------------------------------------------------------------------------------
+    def step(self, clips: dict, draws: Optional[dict] = None, *, max_blocks: int = 0):
+        """One step of every stream in `clips` ({sid: clip}); the others do not move.  draws={sid: (init_idx, refill_idx)}
+        bypasses a stream's generators.  If any stream's step is refused, no stream moves and no generator advances."""
+        draws = draws or {}
+        sids = list(clips)
+        streams = [self._streams[sid] for sid in sids]
+        inputs = []
+        for sid in sids:
+            x = clips[sid]
+            if x.ndim == 5:
+                assert x.shape[0] == 1, "one clip per stream"
+                x = x[0]
+            inputs.append(x)
+        pixels = {x.ndim == 4 and x.shape[1] == 3 for x in inputs}
+        if len(pixels) != 1:
+            raise ValueError("one step takes either pixels or features for every stream")
+        vit = None
+        if pixels.pop():
+            if self.vit is None:
+                raise NotImplementedError("pixels need the model's ViT engine (an f16 tower with select_feature 'patch')")
+            vit = self.vit
+        for st, x in zip(streams, inputs):
+            if x.shape[0] > st.bank.chunk_cap:
+                raise ValueError(f"clip of {x.shape[0]} frames > chunk_cap {st.bank.chunk_cap}")
+        saved = [st.rng.save() for st in streams]
+        dr, tokens = [], []
+        try:
+            for sid, st, x in zip(sids, streams, inputs):
+                t, token = x.shape[0], None
+                d = draws.get(sid)
+                if d is None and st.bank.needs_draws(t):
+                    *d, token = st.rng.draw(st.bank.working_rows(t), st.bank.cfg.long_len)
+                dr.append(d)
+                tokens.append(token)
+            ops.stream_step_many([st.bank for st in streams], inputs, vit=vit, draws=dr, max_blocks=max_blocks)
+        except BaseException:
+            for st, sv in zip(streams, saved):
+                st.rng.restore(sv)
+            raise
+        for st, token in zip(streams, tokens):
+            if token is not None:      # learn (asynchronously) how many refill candidates the device consumed
+                _note_consumed(token, st.bank.info()[1])

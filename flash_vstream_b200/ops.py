@@ -438,6 +438,65 @@ class StreamBank:
         return lab, info, key, wsum
 
 
+def stream_step_many(banks, inputs, *, vit: Optional[VitEncoder] = None, draws=None, max_blocks: int = 0):
+    """One step for many streams (fvs_stream_step_multi): banks[i] takes clip inputs[i] — pixels [t_i,3,S,S] (with `vit`)
+    or finished ViT features [t_i, grid*grid, D] f16.  Bit-identical to banks[0].step(inputs[0], ...), then banks[1]...,
+    with the same draws.  draws: None or a list with (init_idx, refill_idx) | None per bank.  max_blocks caps the blocks
+    of one consolidation launch (0 = the device's co-residency limit).  If any bank's step is refused, no bank moves."""
+    banks, inputs = list(banks), list(inputs)
+    if not banks or len(banks) != len(inputs):
+        raise ValueError(f"{len(banks)} banks for {len(inputs)} clips")
+    draws = list(draws) if draws is not None else [None] * len(banks)
+    if len(draws) != len(banks):
+        raise ValueError(f"{len(draws)} draws for {len(banks)} banks")
+    if len({id(b) for b in banks}) != len(banks):
+        raise ValueError("a bank appears twice in one step")
+    _chk_cuda(*inputs)
+    b0 = banks[0]
+    for b in banks:
+        if any(getattr(b.cfg, n) != getattr(b0.cfg, n) for n, _ in b0.cfg._fields_):
+            raise ValueError("every bank of one step must have the same STAR config")
+        if b.device != b0.device:
+            raise ValueError("every bank of one step must live on the same device")
+    jobs = (L.StreamJob * len(banks))()
+    for i, (bank, inp, dr) in enumerate(zip(banks, inputs, draws)):      # host validation first: nothing moves on a refusal
+        t = inp.shape[0]
+        if t > bank.chunk_cap:
+            raise ValueError(f"clip of {t} frames > chunk_cap {bank.chunk_cap}")
+        init_idx, refill_idx = dr if dr is not None else (None, None)
+        if bank.needs_draws(t):
+            if init_idx is None or refill_idx is None:
+                raise ValueError("this step runs the weighted k-means: pass draws=(init_idx, refill_idx)")
+            assert init_idx.dtype == torch.int32 and refill_idx.dtype == torch.int32
+            assert init_idx.numel() >= bank.cfg.long_len and refill_idx.numel() >= 10 * bank.cfg.long_len
+        jobs[i].frames = t
+        jobs[i].init_idx, jobs[i].refill_idx = L.ptr(init_idx), L.ptr(refill_idx)
+    if vit is not None:
+        inputs = [x.to(vit.dtype) if x.dtype != vit.dtype else x for x in inputs]
+        for x in inputs:
+            assert tuple(x.shape[1:]) == (3, vit.image, vit.image), x.shape
+    else:
+        for x in inputs:
+            assert x.dtype == torch.float16 and x.shape[1] == b0.cfg.grid ** 2 and x.shape[2] == b0.D, x.shape
+    inp = _c(torch.cat(inputs, dim=0)) if len(inputs) > 1 else _c(inputs[0])
+    for i, bank in enumerate(banks):
+        t = inputs[i].shape[0]
+        bank._reserve_frames(t)
+        jobs[i].bank = C.pointer(bank.bank)
+        jobs[i].ntm = C.pointer(bank.ntm) if bank.ntm is not None else None
+        jobs[i].workspace, jobs[i].workspace_bytes = L.ptr(bank.ws), bank.ws.numel()
+    if vit is not None:
+        vit.reserve(min(inp.shape[0], max(vit.max_batch, 1)))
+        kind, vh, vws, vwsn = L.INPUT_PIXELS, vit._h, L.ptr(vit._ws), vit._ws.numel()
+    else:
+        kind, vh, vws, vwsn = L.INPUT_FEATURES, None, None, 0
+    last_T = [bank.working_rows(inputs[i].shape[0]) for i, bank in enumerate(banks)]
+    L.check(b0.lib.fvs_stream_step_multi(C.byref(b0.cfg), jobs, len(banks), vh, L.ptr(inp), kind, vws, vwsn, int(max_blocks),
+                                         L.cur_stream()), "fvs_stream_step_multi")
+    for bank, T in zip(banks, last_T):
+        bank._last_T = T
+
+
 def bank_snapshot(prefix_buf: torch.Tensor, header: torch.Tensor, cur_size: int, long_size: int, out: Optional[torch.Tensor] = None,
                   status: Optional[torch.Tensor] = None):
     """Consistent copy of a bank prefix that another process / GPU may be updating (seqlock, see fvs_bank_snapshot).

@@ -224,19 +224,34 @@ class VStreamMetaForCausalLM:
             self.video_embedding_memory[:] = []
 
     # ---- fused path: fvs_stream_step on a persistent bank ----------------------------------------------------------
+    def _fused_reject(self, s, grid, D, dtype):
+        """None when this STAR config can run as fvs_stream_step, else the knob that keeps it on the op-by-op path"""
+        if not self.fvs_fused_stream:
+            return "fvs_fused_stream"
+        if self.fvs_tie_order != "stable" or "_order" in self.__dict__:   # a replayed / custom tie order: op-by-op only
+            return "fvs_tie_order"
+        if s.sample_type != 'weighted_kmeans':
+            return "video_sample_type"
+        a, b = s.compress_size, s.long_size
+        ntm = self.get_model().attention_model
+        checks = (("compress_type", 'mean' in (getattr(self.config, "compress_type", None) or '')),
+                  ("compress_Turing_memory_size", s.tur_size == 1),
+                  ("dtype", dtype == torch.float16),
+                  ("compress_size", a > 0 and grid % a == 0 and grid != a and a * a <= 64),
+                  ("compress_long_memory_size", b > 0 and a % b == 0 and a != b),
+                  ("hidden size", D % 256 == 0 and (b * b * D) % 1024 == 0),
+                  ("video_long_memory_length", 0 <= s.long_len <= 64),
+                  ("video_Turing_memory_length", 0 < s.tur_len <= 64),
+                  ("video_current_memory_length", s.cur_len >= 0),
+                  ("attention_model", ntm.q_proj.weight.shape[0] <= 64 and ntm.q_proj.weight.shape[1] == D))
+        return next((knob for knob, ok in checks if not ok), None)
+
     def _fused_cfg(self, s, grid, D, dtype):
         """dict for ops.StreamBank when this STAR config can run as fvs_stream_step, else None (op-by-op path)"""
-        if not self.fvs_fused_stream or self.fvs_tie_order != "stable" or s.sample_type != 'weighted_kmeans' \
-                or "_order" in self.__dict__:     # a replayed / custom tie order only exists on the op-by-op path
+        if self._fused_reject(s, grid, D, dtype) is not None:
             return None
         a, b = s.compress_size, s.long_size
         ntm = self.get_model().attention_model
-        ok = ('mean' in (getattr(self.config, "compress_type", None) or '') and s.tur_size == 1 and dtype == torch.float16
-              and a > 0 and b > 0 and grid % a == 0 and grid != a and a % b == 0 and a != b and a * a <= 64 and D % 256 == 0
-              and (b * b * D) % 1024 == 0 and 0 <= s.long_len <= 64 and 0 < s.tur_len <= 64 and s.cur_len >= 0
-              and ntm.q_proj.weight.shape[0] <= 64 and ntm.q_proj.weight.shape[1] == D)
-        if not ok:
-            return None
         return dict(D=D, grid=grid, cur_size=a, long_size=b, long_len=s.long_len, tur_len=s.tur_len, cur_len=s.cur_len,
                     key_len=KEY_LENGTH, ntm_dim=ntm.q_proj.weight.shape[0], ratio=s.ratio)
 

@@ -261,6 +261,35 @@ int fvs_stream_step(const fvs_star_config* cfg_h, fvs_bank* bank_h, const fvs_nt
                     const void* input, int input_kind, int frames, const int32_t* init_idx, const int32_t* refill_idx,
                     void* vit_workspace, size_t vit_workspace_bytes, void* workspace, size_t workspace_bytes,
                     fvs_stream_t stream);
+/* Many streams in one call.  Job i steps bank i with a clip of `frames` frames; the clips lie back to back in `input`
+ * (job 0's frames, then job 1's, ...; pixels or features as for fvs_stream_step, one input_kind for all).  The call is
+ * bit-identical to calling fvs_stream_step for job 0, then job 1, ... with the same draws: every bank array, prefix,
+ * header and fvs_stream_step_info diagnostic — whatever point of its stream each bank is at (first step, warm-up,
+ * steady state) and whatever the clip lengths.  The ViT is invariant to batch composition, so all clips are encoded
+ * together in the engine's micro-batches, and each frame's pooled levels go straight into its own bank.  The
+ * consolidation runs as few cooperative launches ("waves") as the co-residency limit allows: each job owns a contiguous
+ * range of blocks and its own barriers, and its bits do not depend on how many blocks it gets.
+ * Every job is validated before anything is enqueued (a bank or workspace in two jobs, frames > chunk_cap, a full frame
+ * buffer, draws missing where the k-means runs, a workspace too small, ...): on FVS_EINVAL nothing was launched and no
+ * bank counter or header changed.  Jobs may share one fvs_ntm_weights.  max_blocks caps the blocks of one launch
+ * (0 = the device's co-residency limit); per-job tables travel as kernel parameters (no allocation, no host sync). */
+typedef struct fvs_stream_job {
+  fvs_bank* bank;                     /* host struct; its counters advance only when the call succeeds */
+  const fvs_ntm_weights* ntm;
+  int frames;                         /* 1 <= frames <= bank->chunk_cap */
+  const int32_t* init_idx;            /* device draws, as for fvs_stream_step */
+  const int32_t* refill_idx;
+  void* workspace;                    /* this bank's own fvs_stream_workspace_bytes(cfg, bank->chunk_cap) bytes */
+  size_t workspace_bytes;
+} fvs_stream_job;
+int fvs_stream_step_multi(const fvs_star_config* cfg_h, fvs_stream_job* jobs_h, int n_jobs, fvs_vit_t vit, const void* input,
+                          int input_kind, void* vit_workspace, size_t vit_workspace_bytes, int max_blocks,
+                          fvs_stream_t stream);
+/* The launch plan fvs_stream_step_multi uses for a budget of `budget` blocks per launch (pure host arithmetic, validates
+ * like the step, no CUDA call): job i gets blocks_h[2i] Lloyd-loop blocks and blocks_h[2i+1] abstract-memory blocks in
+ * launch waves_h[i].  Returns the number of launches (>= 1) or a negative error code. */
+int fvs_stream_plan(const fvs_star_config* cfg_h, const fvs_stream_job* jobs_h, int n_jobs, int budget, int32_t* blocks_h,
+                    int32_t* waves_h);
 /* device pointers (inside `workspace`) to the last step's diagnostics: labels int32 [T], info int32 [4] = {exit step,
  * refills consumed, converged, k-means ran}, key_idx int64 [key_len], wsum f16 [long_len] */
 int fvs_stream_step_info(const fvs_star_config* cfg_h, const fvs_bank* bank_h, void* workspace, int32_t** labels_out_h,
