@@ -1,73 +1,34 @@
 """Drop-in mirror of flash_vstream.model.compress_functions (reference file, cited per function) running on the
 sm_90a kernels.  Same names, argument meaning, return tuples and pass-through rules as the reference.
 
-RNG contract.  The reference's weighted k-means consumes two RNG streams: torch.randperm(T, device=X.device) for
-the initial centroids (compress_functions.py:134) and Python's random.randint for empty-cluster refills (:152).
-`weighted_kmeans_feature` below draws from the SAME generators in the same way, so a caller that seeds torch and
-random sees the same draws as with the reference on the same device; the draws can also be passed explicitly
-(init_idx= / refill_idx=) which is what the parity tests do.
+RNG: every default draw comes from `draws.GLOBAL`, the global generators the reference draws from (contract in
+draws.py); explicit draws (init_idx= / refill_idx= / coins=) bypass it, which is what the parity tests do.
 """
 from __future__ import annotations
 
-import random
 from typing import Optional
 
 import torch
 
 from . import ops
+from .draws import GLOBAL, DrawSource
 
 MAX_ITER = 10      # compress_functions.py:133 (max_iter=10)
 TOL = 1e-4         # compress_functions.py:133 (tol=1e-4)
-
-# Python's `random` and the refills.  The reference calls random.randint once per EMPTY cluster (:152) — a data-dependent
-# number of draws that is only known after the Lloyd loop has run on the device.  We pre-draw MAX_ITER*K candidates from a
-# PRIVATE clone of the global generator (so the global state is not touched at call time) and, once the consumed count is
-# known, advance the global generator by exactly that many draws — never rewind it.  In the common case (no empty cluster)
-# the global state is therefore never modified; a user's random.seed() between two calls is never undone.  The count is
-# read back asynchronously (4 ints, pinned) and settled at the next draw or by sync_rng().
-_unsettled = []    # [T, pinned info tensor | None, event | None]
 
 
 def sync_rng():
     """Bring Python's `random` to the state the reference would have left: advance it by the refill draws the device
     consumed in the calls made so far.  Blocks on their (tiny) read-backs."""
-    while _unsettled:
-        T, info_h, ev = _unsettled.pop(0)
-        if info_h is None:
-            continue
-        ev.synchronize()
-        for _ in range(int(info_h[1])):
-            random.randint(0, T - 1)
+    GLOBAL.settle()
 
 
-def _draw(T: int, K: int, device):
-    sync_rng()                               # the clone below must start where the reference's generator would be
-    init_idx = torch.randperm(T, device=device)[:K].to(torch.int32)          # compress_functions.py:134
-    rng = random.Random()
-    rng.setstate(random.getstate())
-    refill = [rng.randint(0, T - 1) for _ in range(MAX_ITER * K)]            # compress_functions.py:152 (candidates)
-    refill_idx = torch.tensor(refill, dtype=torch.int32).pin_memory().to(device, non_blocking=True)
-    token = [T, None, None]
-    _unsettled.append(token)
-    return init_idx, refill_idx, token
-
-
-def _note_consumed(token, info: torch.Tensor):
-    """`info` = the kernel's device int32[4] (info[1] = refills consumed): start its read-back, settle later"""
-    info_h = torch.empty(4, dtype=torch.int32).pin_memory()
-    info_h.copy_(info[:4], non_blocking=True)
-    ev = torch.cuda.Event()
-    ev.record()
-    token[1], token[2] = info_h, ev
-
-
-def draw_kmeans(T: int, K: int, device, bank=None):
-    """(init_idx, refill_idx) for a k-means over T rows drawn like the reference draws them (torch.randperm on the tensor's
-    device, random.randint candidates); with `bank` (ops.StreamBank) the consumed count is read from its next step."""
-    init_idx, refill_idx, token = _draw(T, K, device)
-    if bank is not None:
-        bank._rng_token = token
-    return init_idx, refill_idx
+def kmeans_draws(source: DrawSource, T: int, K: int, device):
+    """(init_idx, refill_idx, Refills) for a weighted k-means over T rows, drawn from `source` as the reference draws them:
+    torch.randperm on the rows' device (compress_functions.py:134) and random.randint refill candidates (:152)"""
+    init_idx = source.randperm(T, device)[:K].to(torch.int32)
+    refill_idx, refills = source.refill_candidates(T, MAX_ITER * K, device)
+    return init_idx, refill_idx, refills
 
 
 def weighted_kmeans_device(img_feature: torch.Tensor, video_max_frames: int, weights: Optional[torch.Tensor] = None,
@@ -83,13 +44,13 @@ def weighted_kmeans_device(img_feature: torch.Tensor, video_max_frames: int, wei
     if T <= T0:
         w = weights if weights is not None else torch.ones(T, dtype=img_feature.dtype, device=img_feature.device)
         return img_feature, w, None, None
-    token = None
+    refills = None
     if init_idx is None or refill_idx is None:
-        init_idx, refill_idx, token = _draw(T, T0, img_feature.device)
+        init_idx, refill_idx, refills = kmeans_draws(GLOBAL, T, T0, img_feature.device)
     X = img_feature.reshape(T, P * D)
     C, wsum, labels, info = ops.weighted_kmeans(X, weights_in, init_idx, refill_idx, T0, MAX_ITER, TOL)
-    if token is not None:
-        _note_consumed(token, info)
+    if refills is not None:
+        refills.consumed_from(info)
     return C.view(T0, P, D), wsum, labels, info
 
 
@@ -127,8 +88,7 @@ def _coins(n, coins, device):
     """the random.randint(0, 1) flips of the drop variants (compress_functions.py:38, :194): exactly one per incoming frame,
     so drawing them ahead consumes Python's `random` stream exactly like the reference"""
     if coins is None:
-        sync_rng()
-        coins = [random.randint(0, 1) for _ in range(n)]
+        coins = GLOBAL.randints(0, 1, n)
     return torch.as_tensor(list(coins), dtype=torch.int32).to(device)
 
 
@@ -214,22 +174,17 @@ def kmeans_feature(img_feature, video_max_frames, img_similarity=None, *, init_i
     if T <= T0:
         return img_feature, img_similarity, [[[i] for i in range(T)]]
     dev = img_feature.device
-    drew = False
     if init_idx is None:
-        init_idx = torch.randperm(T)[:T0]
+        init_idx = GLOBAL.randperm(T, "cpu")[:T0]
     if refill_idx is None:
-        sync_rng()
-        rng = random.Random()
-        rng.setstate(random.getstate())                                  # candidates from a private clone (see sync_rng)
-        refill_idx = [rng.randint(0, T - 1) for _ in range(MAX_ITER * T0)]
-        drew = True
-    refill = [int(v) for v in refill_idx]
-    refill = refill + [0] * (MAX_ITER * T0 - len(refill))
+        refill_dev, _ = GLOBAL.refill_candidates(T, MAX_ITER * T0, dev)
+    else:
+        refill = [int(v) for v in refill_idx]
+        refill_dev = torch.tensor(refill + [0] * (MAX_ITER * T0 - len(refill)), dtype=torch.int32).to(dev)
     C, labels, info = ops.alt_kmeans(img_feature.reshape(T, P * D), torch.as_tensor(init_idx).to(device=dev, dtype=torch.int32),
-                                     torch.tensor(refill, dtype=torch.int32).to(dev), T0, MAX_ITER, TOL)
+                                     refill_dev, T0, MAX_ITER, TOL)
     lab = labels.cpu().tolist()
-    if drew:
-        for _ in range(int(info[1])):                                    # what the reference would have drawn (:107)
-            random.randint(0, T - 1)
+    if refill_idx is None:
+        GLOBAL.consume(T, int(info[1]))                                  # what the reference would have drawn (:107)
     step_indices = [[j for j in range(T) if lab[j] == i] for i in range(T0)]
     return C.view(T0, P, D), img_similarity, [step_indices]

@@ -5,79 +5,25 @@ micro-batch instead of once per stream) and consolidates all their banks in as f
 device.  Each stream's result is bit-identical to running it alone through the single-stream path
 (`FlashVStreamB200.embed_video_streaming` / `consolidate_streaming`) with the same draws.
 
-RNG contract.  In the reference every stream's memory manager is its own spawned process, so every stream has its own
-generators.  Here every stream owns a torch CPU + CUDA generator state and a `random.Random`, all seeded from
-`open(seed)`: its k-means draws (torch.randperm on the device, pre-drawn random.randint refill candidates) come from its
-own generators and its refill count is settled lazily against its own `random.Random`, exactly as
-compress_functions.sync_rng does for the global one.  So a stream draws what the single-stream path draws after
-`torch.manual_seed(seed); random.seed(seed)`, and the global torch / random state is never touched.
+RNG: each stream owns a `draws.DrawSource` seeded by `open(seed)` (contract in draws.py), so a stream draws what the
+single-stream path draws after `torch.manual_seed(seed); random.seed(seed)` and never touches the global generators.
 """
 from __future__ import annotations
 
 import os
-import random
 from typing import Optional
 
 import torch
 
 from . import ops
-from .compress_functions import MAX_ITER, _note_consumed
+from .compress_functions import kmeans_draws
+from .draws import DrawSource
 
 REFERENCE_GRID = 24   # ViT-L/14 at 336 px: the patch grid of finished features when the model has no tower of its own
 
 
-class _StreamRng:
-    """one stream's generators: torch CPU + CUDA states swapped in around its draws, and its own random.Random"""
-
-    def __init__(self, seed: int, device: torch.device):
-        self.device = device
-        g = torch.Generator()
-        g.manual_seed(seed)
-        gc = torch.Generator(device=device)
-        gc.manual_seed(seed)
-        self.cpu, self.cuda = g.get_state(), gc.get_state()
-        self.py = random.Random(seed)
-        self.unsettled = []       # [T, pinned info | None, event | None] per draw, as in compress_functions
-
-    def settle(self):
-        while self.unsettled:
-            T, info_h, ev = self.unsettled.pop(0)
-            if info_h is None:
-                continue
-            ev.synchronize()
-            for _ in range(int(info_h[1])):
-                self.py.randint(0, T - 1)
-
-    def save(self):
-        return self.cpu, self.cuda, self.py.getstate(), list(self.unsettled)
-
-    def restore(self, st):
-        self.cpu, self.cuda, pys, self.unsettled = st
-        self.py.setstate(pys)
-
-    def draw(self, T: int, K: int):
-        """(init_idx, refill_idx, token): compress_functions._draw on this stream's generators"""
-        self.settle()
-        cpu0, cuda0 = torch.get_rng_state(), torch.cuda.get_rng_state(self.device)
-        try:
-            torch.set_rng_state(self.cpu)
-            torch.cuda.set_rng_state(self.cuda, self.device)
-            init_idx = torch.randperm(T, device=self.device)[:K].to(torch.int32)       # compress_functions.py:134
-            self.cpu, self.cuda = torch.get_rng_state(), torch.cuda.get_rng_state(self.device)
-        finally:
-            torch.set_rng_state(cpu0)
-            torch.cuda.set_rng_state(cuda0, self.device)
-        rng = random.Random()
-        rng.setstate(self.py.getstate())
-        refill = [rng.randint(0, T - 1) for _ in range(MAX_ITER * K)]                 # compress_functions.py:152
-        refill_idx = torch.tensor(refill, dtype=torch.int32).pin_memory().to(self.device, non_blocking=True)
-        token = [T, None, None]
-        self.unsettled.append(token)
-        return init_idx, refill_idx, token
-
-
 class _Stream:
-    def __init__(self, bank: ops.StreamBank, rng: _StreamRng):
+    def __init__(self, bank: ops.StreamBank, rng: DrawSource):
         self.bank, self.rng = bank, rng
 
 
@@ -126,7 +72,7 @@ class StreamPool:
             seed = int.from_bytes(os.urandom(8), "little") >> 1
         sid = self._next
         self._next += 1
-        self._streams[sid] = _Stream(bank, _StreamRng(int(seed), self.device))
+        self._streams[sid] = _Stream(bank, DrawSource(int(seed), self.device))
         return sid
 
     def close(self, sid: int):
@@ -170,24 +116,21 @@ class StreamPool:
             if self.vit is None:
                 raise NotImplementedError("pixels need the model's ViT engine (an f16 tower with select_feature 'patch')")
             vit = self.vit
-        for st, x in zip(streams, inputs):
-            if x.shape[0] > st.bank.chunk_cap:
-                raise ValueError(f"clip of {x.shape[0]} frames > chunk_cap {st.bank.chunk_cap}")
-        saved = [st.rng.save() for st in streams]
-        dr, tokens = [], []
+        snaps = [st.rng.snapshot() for st in streams]
+        dr, refills = [], []
         try:
             for sid, st, x in zip(sids, streams, inputs):
-                t, token = x.shape[0], None
+                t, r = x.shape[0], None
                 d = draws.get(sid)
                 if d is None and st.bank.needs_draws(t):
-                    *d, token = st.rng.draw(st.bank.working_rows(t), st.bank.cfg.long_len)
+                    *d, r = kmeans_draws(st.rng, st.bank.working_rows(t), st.bank.cfg.long_len, self.device)
                 dr.append(d)
-                tokens.append(token)
+                refills.append(r)
             ops.stream_step_many([st.bank for st in streams], inputs, vit=vit, draws=dr, max_blocks=max_blocks)
         except BaseException:
-            for st, sv in zip(streams, saved):
-                st.rng.restore(sv)
+            for st, snap in zip(streams, snaps):
+                st.rng.rewind(snap)
             raise
-        for st, token in zip(streams, tokens):
-            if token is not None:      # learn (asynchronously) how many refill candidates the device consumed
-                _note_consumed(token, st.bank.info()[1])
+        for st, r in zip(streams, refills):
+            if r is not None:          # learn (asynchronously) how many refill candidates the device consumed
+                r.consumed_from(st.bank.info()[1])

@@ -396,32 +396,8 @@ class StreamBank:
     # ---- one clip -----------------------------------------------------------------------------------------------------
     def step(self, inp: torch.Tensor, *, vit: Optional["VitEncoder"] = None, draws=None):
         """inp: pixels [t,3,S,S] (with `vit`) or finished ViT features [t, grid*grid, D] f16.  draws = (init_idx int32 [K],
-        refill_idx int32 [10*K]) device tensors, needed when needs_draws(t)."""
-        _chk_cuda(inp)
-        inp = _c(inp)
-        t = inp.shape[0]
-        if t > self.chunk_cap:
-            raise ValueError(f"clip of {t} frames > chunk_cap {self.chunk_cap}")
-        self._reserve_frames(t)
-        init_idx, refill_idx = draws if draws is not None else (None, None)
-        if self.needs_draws(t):
-            if init_idx is None or refill_idx is None:
-                raise ValueError("this step runs the weighted k-means: pass draws=(init_idx, refill_idx)")
-            assert init_idx.dtype == torch.int32 and refill_idx.dtype == torch.int32
-            assert init_idx.numel() >= self.cfg.long_len and refill_idx.numel() >= 10 * self.cfg.long_len
-        if vit is not None:
-            if inp.dtype != vit.dtype:
-                inp = inp.to(vit.dtype)
-            assert tuple(inp.shape[1:]) == (3, vit.image, vit.image), inp.shape
-            vit.reserve(min(t, max(vit.max_batch, 1)))
-            kind, vh, vws, vwsn = L.INPUT_PIXELS, vit._h, L.ptr(vit._ws), vit._ws.numel()
-        else:
-            assert inp.dtype == torch.float16 and inp.shape[1] == self.cfg.grid ** 2 and inp.shape[2] == self.D, inp.shape
-            kind, vh, vws, vwsn = L.INPUT_FEATURES, None, None, 0
-        self._last_T = self.working_rows(t)
-        L.check(self.lib.fvs_stream_step(C.byref(self.cfg), C.byref(self.bank), C.byref(self.ntm) if self.ntm is not None else None,
-                                         vh, L.ptr(inp), kind, t, L.ptr(init_idx), L.ptr(refill_idx), vws, vwsn, L.ptr(self.ws),
-                                         self.ws.numel(), L.cur_stream()), "fvs_stream_step")
+        refill_idx int32 [10*K]) device tensors, needed when needs_draws(t).  The one-bank case of stream_step_many."""
+        stream_step_many([self], [inp], vit=vit, draws=[draws])
 
     def info(self):
         """device views of the last step's diagnostics: labels int32 [T], info int32 [4], key_idx int64 [<=key_len],

@@ -1,28 +1,22 @@
 """Drop-in mirror of Flash-VStream-Qwen/models/compress_functions.py for the path the Qwen Flash Memory takes by default
 (`flash_memory_temporal_method='kmeans_ordered'`): weighted_kmeans_ordered_feature (:181-298), on the sm_90a kernels.
 
-RNG contract.  The reference consumes torch.randperm(n_unique, device=X.device) for the initial centroids (:211) and
-Python's random.randint once per empty cluster (:258).  The function below draws from the same generators in the same way
-(randint draws are made ahead for every possible refill, then Python's `random` state is rewound and advanced by the count
-the device actually consumed), or replays explicit draws (init_idx= / refill_idx= / order=), which is what the parity tests
-do with the draws recorded from the reference.
+RNG: default draws come from `draws.GLOBAL`, the global generators the reference draws from (contract in draws.py);
+explicit draws (init_idx= / refill_idx= / order=) bypass it, which is what the parity tests do with the draws recorded
+from the reference.
 """
 from __future__ import annotations
 
-import random
 from typing import Optional
 
 import numpy as np
 import torch
 
 from . import ops as Q
+from ..draws import GLOBAL, to_device
 
 MAX_ITER = 10   # compress_functions.py:203 (max_iter=10)
 TOL = 1e-4      # compress_functions.py:203 (tol=1e-4)
-
-
-def _to_dev_i32(values, device):
-    return torch.tensor(list(values), dtype=torch.int32).pin_memory().to(device, non_blocking=True)
 
 
 def weighted_kmeans_ordered_feature(img_feature: torch.Tensor, video_max_frames: int, weights: Optional[torch.Tensor] = None,
@@ -53,23 +47,20 @@ def weighted_kmeans_ordered_feature(img_feature: torch.Tensor, video_max_frames:
         lab = labels.cpu().tolist()
     else:
         K = T0
-        state = None
         if init_idx is None:
-            init_idx = torch.randperm(U, device=dev)[:K]                # :218
+            init_idx = GLOBAL.randperm(U, dev)[:K]                      # :218
         init_idx = torch.as_tensor(init_idx).to(device=dev, dtype=torch.int32)
         if refill_idx is None:
-            state = random.getstate()
-            refill_idx = [random.randint(0, T - 1) for _ in range(MAX_ITER * K)]   # :258, drawn ahead
-        refill = list(int(v) for v in refill_idx)
-        refill = refill + [0] * (MAX_ITER * K - len(refill))
-        C, wsum, labels, info = Q.kmeans_ordered(X, w32, uniq_idx, init_idx, _to_dev_i32(refill, dev), K, MAX_ITER, TOL)
+            refill_dev, _ = GLOBAL.refill_candidates(T, MAX_ITER * K, dev)    # :258, drawn ahead
+        else:
+            refill = list(int(v) for v in refill_idx)
+            refill_dev = to_device(refill + [0] * (MAX_ITER * K - len(refill)), np.int32, dev)
+        C, wsum, labels, info = Q.kmeans_ordered(X, w32, uniq_idx, init_idx, refill_dev, K, MAX_ITER, TOL)
         lab = labels.cpu().tolist()                                     # the member lists need the labels on the host
         info_h = info.cpu().tolist()
         exit_step = info_h[0]
-        if state is not None:                                           # leave `random` where the reference would
-            random.setstate(state)
-            for _ in range(info_h[1]):
-                random.randint(0, T - 1)
+        if refill_idx is None:                                          # leave `random` where the reference would
+            GLOBAL.consume(T, info_h[1])
     step_indices = [[] for _ in range(K)]
     for j, l in enumerate(lab):                                         # :274-277
         step_indices[l].append(j)

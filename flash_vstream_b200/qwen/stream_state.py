@@ -13,7 +13,7 @@ enqueue pass with ONE 32-byte read-back at its end:
     been enqueued; the step is published once that copy has landed and says the enqueued work was the right work;
   * the right work is the common case: the reference draws `torch.randperm(n_unique)` for the initial centroids, so the
     step assumes all T rows are distinct (n_unique == T), draws randperm(T) and runs the non-degenerate branch; should the
-    read-back show duplicates, the CUDA generator is rewound and the clip is redone through the synchronous path
+    read-back show duplicates, the torch generators are rewound and the clip is redone through the synchronous path
     (weighted_kmeans_ordered_feature), which handles every branch of the reference;
   * timestamps (mean member index), their ordering and the sorted gather run on the device (fvs_qwen_kmeans_finalize); the
     member lists the reference returns are materialised lazily — nothing in the streaming step reads them;
@@ -26,7 +26,6 @@ list on top of this object.
 """
 from __future__ import annotations
 
-import random
 from typing import Optional
 
 import numpy as np
@@ -34,6 +33,7 @@ import torch
 
 from . import compress_functions as CF
 from .. import ops as O
+from ..draws import GLOBAL, to_device
 
 _KMEANS_METHODS = ("kmeans_ordered", "fast_kmeans_ordered")
 
@@ -59,17 +59,6 @@ class RowBank:
 
     def rows(self) -> torch.Tensor:
         return self.buf[: self.n]
-
-
-def _dev_i32(values, device) -> torch.Tensor:
-    """host integers -> device int32 through pinned memory (a pageable H2D copy would serialise the stream)"""
-    a = np.ascontiguousarray(np.asarray(values, dtype=np.int32))
-    return torch.from_numpy(a).pin_memory().to(device, non_blocking=True)
-
-
-def _dev_i64(values, device) -> torch.Tensor:
-    a = np.ascontiguousarray(np.asarray(values, dtype=np.int64))
-    return torch.from_numpy(a).pin_memory().to(device, non_blocking=True)
 
 
 class QwenStreamState:
@@ -129,23 +118,21 @@ class QwenStreamState:
         if not fast:
             self._compress_sync(cand, cand_w, T, d, start_idx, t)
         else:
-            rng_state = None
+            snap = None
             init = d.get("init_idx")
             if init is None:
-                rng_state = torch.cuda.get_rng_state(dev)
-                init_dev = torch.randperm(T, device=dev)[:T0].to(torch.int32)       # randperm(n_unique), assuming n_unique == T
+                snap = GLOBAL.snapshot(dev)
+                init_dev = GLOBAL.randperm(T, dev)[:T0].to(torch.int32)          # randperm(n_unique), assuming n_unique == T
             else:
-                init_dev = _dev_i32(np.asarray(init)[:T0], dev)
+                init_dev = to_device(np.asarray(init)[:T0], np.int32, dev)
             refill = d.get("refill_idx")
-            clone = None
-            if refill is None:                                                       # candidates from a private copy of `random`
-                clone = random.Random()
-                clone.setstate(random.getstate())
-                refill = [clone.randint(0, T - 1) for _ in range(CF.MAX_ITER * T0)]
-            refill = list(int(v) for v in refill)
-            refill_dev = _dev_i32(refill + [0] * (CF.MAX_ITER * T0 - len(refill)), dev)
+            if refill is None:
+                refill_dev, _ = GLOBAL.refill_candidates(T, CF.MAX_ITER * T0, dev)
+            else:
+                refill = list(int(v) for v in refill)
+                refill_dev = to_device(refill + [0] * (CF.MAX_ITER * T0 - len(refill)), np.int32, dev)
             order = d.get("ts_order")
-            order_dev = None if order is None else _dev_i64(order, dev)
+            order_dev = None if order is None else to_device(order, np.int64, dev)
             km = CF.ordered_kmeans_enqueue(cand, T0, cand_w, init_dev, refill_dev, order_dev)
             tem_x, tem_w, tem_ts = km["feat"].view(T0 * P, D), km["weights"], km["timestamps"]
             self._enqueue_rest(tem_x, tem_w, tem_ts, T0, km["members"], d)
@@ -157,17 +144,16 @@ class QwenStreamState:
             done.record()
             done.synchronize()
             n_unique, _, consumed, _, _, empty = (int(v) for v in self._readback[:6])
-            valid = n_unique >= T0 and (rng_state is None or n_unique == T)
+            valid = n_unique >= T0 and (snap is None or n_unique == T)
             if valid:
                 if empty:
                     raise ZeroDivisionError("division by zero")          # sum(indices) / len(indices), compress_functions.py:279
-                if clone is not None:
-                    for _ in range(consumed):                              # leave `random` where the reference would
-                        random.randint(0, T - 1)
+                if refill is None:
+                    GLOBAL.consume(T, consumed)                            # leave `random` where the reference would
                 self.fast_steps += 1
             else:                                                          # duplicates among the rows: the general path
-                if rng_state is not None:
-                    torch.cuda.set_rng_state(rng_state, dev)
+                if snap is not None:
+                    GLOBAL.rewind(snap)
                 self.redone_steps += 1
                 self._compress_sync(cand, cand_w, T, d, start_idx, t)
         return bank, small_bank

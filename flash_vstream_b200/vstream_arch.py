@@ -19,8 +19,9 @@ import torch
 import torch.nn as nn
 
 from . import ops
-from .compress_functions import (attention_feature, drop_feature, k_drop_feature, k_merge_feature, kmeans_feature,
-                                 merge_feature, weighted_kmeans_device, weighted_kmeans_feature)
+from .compress_functions import (attention_feature, drop_feature, k_drop_feature, k_merge_feature, kmeans_draws,
+                                 kmeans_feature, merge_feature, weighted_kmeans_device, weighted_kmeans_feature)
+from .draws import GLOBAL
 
 KEY_LENGTH = 3  # hard-coded in the reference (vstream_arch.py:263, :683)
 
@@ -275,14 +276,12 @@ class VStreamMetaForCausalLM:
         elif bank.steps == 0:
             return False            # the state in `video_embedding_memory` was not produced by this bank
         t = inp.shape[0]
+        refills = None
         if draws is None and bank.needs_draws(t):
-            from .compress_functions import draw_kmeans
-            draws = draw_kmeans(bank.working_rows(t), bank.cfg.long_len, bank.device, bank)
+            *draws, refills = kmeans_draws(GLOBAL, bank.working_rows(t), bank.cfg.long_len, bank.device)
         bank.step(inp, vit=vit, draws=draws)
-        token = bank.__dict__.pop("_rng_token", None)
-        if token is not None:       # we drew the candidates ourselves: learn (asynchronously) how many the device consumed
-            from .compress_functions import _note_consumed
-            _note_consumed(token, bank.info()[1])
+        if refills is not None:     # we drew the candidates ourselves: learn (asynchronously) how many the device consumed
+            refills.consumed_from(bank.info()[1])
         self._publish(list(bank.state()))
         return True
 

@@ -1,5 +1,6 @@
 """Timing script (not a pytest file): many single-frame streams on one GPU, batched (StreamPool.step, one
-fvs_stream_step_multi per round) against the same streams stepped one after the other (fvs_stream_step per stream).
+fvs_stream_step_multi per round) against the same streams stepped one after the other (StreamBank.step per stream: a
+one-bank call, so one consolidation launch per stream).
 
 ViT-L/14 at 336 px (random weights, 23 layers run, f16) and the default 681-token STAR config; every step takes one frame
 from device-resident pixels, with pre-drawn k-means draws as bench.py uses, so the timed region has no host RNG work.

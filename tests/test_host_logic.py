@@ -226,34 +226,6 @@ def test_prefix_allgather_gloo_world2():
     assert res == [(0, True), (1, True)]
 
 
-def test_rng_contract_never_rewinds_python_random():
-    """ADVICE r1: the refill candidates come from a private clone of `random`; the global generator is only ever ADVANCED
-    by the number of draws the device consumed (0 in the common case), never rewound over what the user did in between"""
-    import random
-    from flash_vstream_b200 import compress_functions as cf
-
-    class Ev:
-        def synchronize(self):
-            pass
-
-    cf._unsettled.clear()
-    random.seed(5)
-    cf._unsettled.append([26, torch.tensor([1, 0, 1, 0], dtype=torch.int32), Ev()])      # nothing consumed
-    random.seed(7)                                                                        # the user reseeds in between
-    cf.sync_rng()
-    probe = random.random()
-    random.seed(7)
-    assert probe == random.random(), "global RNG state was touched although no refill was consumed"
-    cf._unsettled.append([26, torch.tensor([1, 2, 1, 0], dtype=torch.int32), Ev()])      # two refills consumed
-    random.seed(11)
-    cf.sync_rng()
-    probe = random.random()
-    random.seed(11)
-    random.randint(0, 25), random.randint(0, 25)
-    assert probe == random.random(), "the global RNG must be advanced by exactly the consumed draws"
-    assert not cf._unsettled
-
-
 def test_inference_only_guard_and_metric_meter():
     from types import SimpleNamespace
     from flash_vstream_b200 import multimodal_projector as mp

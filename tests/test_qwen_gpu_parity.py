@@ -121,6 +121,38 @@ def test_kmeans_ordered_pass_through_and_rng(qwen):
     assert res[0][2] == random.random()
 
 
+def test_kmeans_ordered_draws_after_pending_llava_refills(qwen):
+    """Python's `random` is one generator for both model families: the refills a LLaVA k-means consumed, still pending
+    (weighted_kmeans_device reads the count back asynchronously), are applied before a Qwen k-means draws its candidates,
+    so the Qwen draws are the ones the reference's single `random` would give"""
+    pkg, _ = qwen
+    import random
+    from flash_vstream_b200 import compress_functions as LCF
+    name = "ko_zero_weight_f32"                                       # zero weights: clusters get refilled
+    c = QI.KMEANS_CASES[name]
+    x, w = QI.kmeans_input(c)
+    init = _load("qwen_kmeans.npz")[name + "_init"]
+    LCF.sync_rng()
+    random.seed(17)
+    rows = torch.ones(10, 4, 256, dtype=torch.float16, device="cuda")   # identical rows: every cluster but one empties
+    *_, info = LCF.weighted_kmeans_device(rows, 4)                     # no sync_rng(): its refill count stays pending
+    got = pkg.weighted_kmeans_ordered_feature(x.cuda(), c["K"], w.cuda(), init_idx=init)
+    consumed = int(info[1])
+    assert consumed > 0
+
+    def with_refills_after(skip):
+        random.seed(17)
+        for _ in range(skip):
+            random.randint(0, rows.shape[0] - 1)
+        refill = [random.randint(0, c["T"] - 1) for _ in range(10 * c["K"])]
+        return pkg.weighted_kmeans_ordered_feature(x.cuda(), c["K"], w.cuda(), init_idx=init, refill_idx=refill)
+    want, unsettled = with_refills_after(consumed), with_refills_after(0)
+    assert got[3] != unsettled[3], "the input must be one on which the LLaVA refills change the Qwen result"
+    assert got[3] == want[3]
+    for a, b in zip(got[:3], want[:3]):
+        same_bits(a, b)
+
+
 def test_kmeans_ordered_full_size_properties(qwen):
     """BASELINE-size CSM update: 61 half-resolution frames of 144 tokens x 1280 -> 60 centroids (PD = 184320)."""
     pkg, _ = qwen
