@@ -33,6 +33,7 @@
 #include "fvs_common.h"
 #include "fvs_kernels.h"
 #include "mem_device.cuh"
+#include "seqlock.cuh"
 
 namespace cg = cooperative_groups;
 
@@ -173,10 +174,7 @@ __global__ void __launch_bounds__(kThreads, 1) consolidate_kernel(const __grid_c
   const int D = A.D, PD = A.PDl, S = A.S, T = A.T, K = A.K;
 
   // readers see an odd sequence number from before the first barrier until the write-back has completed
-  if (wb == 0 && threadIdx.x == 0) {
-    atomicAdd_system(&A.header[0], 1ull);
-    __threadfence_system();
-  }
+  if (wb == 0 && threadIdx.x == 0) seqlock::write_begin(&A.header[0]);
   if (abs_block) abstract_group(A, wb - nwork, A.n_abs_blocks);
 
   // ------------------------------------------------------------------ Lloyd loop (compress_functions.py:135-156)
@@ -328,8 +326,7 @@ __global__ void __launch_bounds__(kThreads, 1) consolidate_kernel(const __grid_c
       *A.km_ctr = 0u;
       *A.abs_ctr = 0u;
       *A.job_ctr = 0u;
-      __threadfence_system();
-      atomicAdd_system(&A.header[0], 1ull);
+      seqlock::write_end(&A.header[0]);
     }
   }
 }
@@ -343,9 +340,8 @@ __global__ void snapshot_kernel(const uint4* __restrict__ prefix, const unsigned
   cg::grid_group grid = cg::this_grid();
   __shared__ unsigned long long s_hdr[6];
   if (threadIdx.x == 0) {
+    s_hdr[0] = seqlock::read_open(header);
     const volatile unsigned long long* h = header;
-    s_hdr[0] = h[0];
-    __threadfence_system();
     for (int i = 1; i < 6; ++i) s_hdr[i] = h[i];
   }
   __syncthreads();
@@ -356,9 +352,8 @@ __global__ void snapshot_kernel(const uint4* __restrict__ prefix, const unsigned
   __threadfence_system();
   grid.sync();
   if (blockIdx.x == 0 && threadIdx.x == 0) {
-    const volatile unsigned long long* h = header;
     status[0] = s_hdr[0];
-    status[1] = h[0];
+    status[1] = seqlock::read_close(header);
     for (int i = 1; i < 6; ++i) status[1 + i] = s_hdr[i];
   }
 }

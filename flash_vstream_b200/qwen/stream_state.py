@@ -80,6 +80,7 @@ class QwenStreamState:
         self.tem_members = None
         self._readback = None                 # pinned int32 [8]: n_unique, info[4], flags
         self.fast_steps = self.redone_steps = 0
+        self.steps = 0                        # clips whose step completed (a clip that raises is not counted)
 
     # ------------------------------------------------------------------------------------------------ one clip
     def step(self, x_new: torch.Tensor, small_new: torch.Tensor, t: int, grid, small_grid, start_idx: int,
@@ -156,6 +157,7 @@ class QwenStreamState:
                     GLOBAL.rewind(snap)
                 self.redone_steps += 1
                 self._compress_sync(cand, cand_w, T, d, start_idx, t)
+        self.steps += 1
         return bank, small_bank
 
     # ------------------------------------------------------------------------------------------------ pieces

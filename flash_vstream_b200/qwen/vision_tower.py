@@ -24,16 +24,23 @@ class QwenVisionBlocksB200:
         dev = torch.device(device)
         if dev.type != "cuda":
             raise L.FvsError("QwenVisionBlocksB200 needs a CUDA device (no CPU fallback)")
+        if dev.index is None:
+            dev = torch.device("cuda", torch.cuda.current_device())
         self.dtype, self.device, self.depth, self.heads = dtype, dev, depth, heads
+        self._ctor = dict(depth=depth, heads=heads, ln_eps=ln_eps, dtype=dtype, use_graphs=use_graphs,
+                          graph_max_rows=graph_max_rows)
         # CUDA-graph replay of the whole encode for small clips (a few hundred launches of 5-40 us kernels each): one graph
         # per grid signature, static input / output buffers, bit-identical to the eager launches
         self.use_graphs, self.graph_max_rows, self._graphs = use_graphs, graph_max_rows, {}
-        self._keep = []
-        k = lambda t: (self._keep.append(t.detach().to(device=dev, dtype=dtype).contiguous()), self._keep[-1])[1]
+        self._sd = {}                                         # the prepared device weights, under the state-dict keys
+
+        def k(key, t):
+            self._sd[key] = t.detach().to(device=dev, dtype=dtype).contiguous()
+            return self._sd[key]
         pw = state_dict["patch_embed.proj.weight"]
         self.embed = pw.shape[0]
         self.patch_dim = pw[0].numel()
-        self.patch_w = k(pw.reshape(self.embed, -1))
+        self.patch_w = k("patch_embed.proj.weight", pw.reshape(self.embed, -1))
         self.mlp = state_dict["blocks.0.mlp.fc1.weight"].shape[0] if depth else 4 * self.embed
         arr = (L.VitLayerWeights * max(depth, 1))()
         names = dict(ln1_w="norm1.weight", ln1_b="norm1.bias", qkv_w="attn.qkv.weight", qkv_b="attn.qkv.bias",
@@ -41,7 +48,7 @@ class QwenVisionBlocksB200:
                      fc1_w="mlp.fc1.weight", fc1_b="mlp.fc1.bias", fc2_w="mlp.fc2.weight", fc2_b="mlp.fc2.bias")
         for i in range(depth):
             for field, key in names.items():
-                setattr(arr[i], field, k(state_dict[f"blocks.{i}.{key}"]).data_ptr())
+                setattr(arr[i], field, k(f"blocks.{i}.{key}", state_dict[f"blocks.{i}.{key}"]).data_ptr())
         head_dim = self.embed // heads
         dim = head_dim // 2                                   # VisionRotaryEmbedding(head_dim // 2)
         inv_freq = 1.0 / (10000.0 ** (torch.arange(0, dim, 2, dtype=torch.float) / dim))
@@ -53,6 +60,24 @@ class QwenVisionBlocksB200:
                                                  L.cur_stream()), "fvs_qwen_vit_create")
             torch.cuda.current_stream().synchronize()          # the permuted weight copies are complete; originals of
         self._ws: Optional[torch.Tensor] = None               # qkv / proj are no longer referenced by the handle
+
+    # The reference's CLI pickles the whole model into its memory-manager process (cli_server_2gpu.py:301-304).  A ctypes
+    # handle cannot travel; the prepared weights can (torch.multiprocessing shares CUDA tensors by IPC handle, plain pickle
+    # copies them), and the handle is rebuilt from them on the other side.
+    def __getstate__(self):
+        return {"ctor": self._ctor, "weights": self._sd, "device": str(self.device)}
+
+    def __setstate__(self, st):
+        self.__init__(st["weights"], device=st["device"], **st["ctor"])
+
+    def to(self, device) -> "QwenVisionBlocksB200":
+        """the same blocks on `device`: self when already there, else a new handle over copies of the weights"""
+        dev = torch.device(device)
+        if dev.type == "cuda" and dev.index is None:
+            dev = torch.device("cuda", torch.cuda.current_device())
+        if dev == self.device:
+            return self
+        return QwenVisionBlocksB200(self._sd, device=dev, **self._ctor)
 
     @classmethod
     def from_module(cls, visual, **kw):

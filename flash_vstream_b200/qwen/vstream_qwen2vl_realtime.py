@@ -17,12 +17,13 @@ Differences from the reference (behaviour-preserving):
 from __future__ import annotations
 
 import time
-from threading import Lock
 from typing import Callable, Optional
 
 import torch
 import torch.nn as nn
 
+from .. import _lib as L
+from ..vstream_arch import _is_manager_proxy
 from . import vstream_qwen2vl_model as _offline
 from .compress_functions import weighted_kmeans_ordered_feature
 from .patch_merger import PatchMerger
@@ -70,6 +71,18 @@ class VisualB200(nn.Module):
         self.flash_memory, self.merger, self.encode_patches = flash_memory, merger, encode_patches
         self._dtype, self._device = dtype, torch.device(device)
 
+    def _apply(self, fn, recurse=True):
+        """.cuda() / .to(device) of this module or of its host also move the injected tower (QwenVisionBlocksB200.to), so
+        `torch.cuda.set_device(1); model.cuda()` in the reference's memory-manager process puts the whole vision side on
+        cuda:1 (cli_server_2gpu.py:198-199)."""
+        super()._apply(fn, recurse)
+        dev = fn(torch.empty(0, device=self._device)).device
+        if dev != self._device:
+            self._device = dev
+            if hasattr(self.encode_patches, "to"):
+                self.encode_patches = self.encode_patches.to(dev)
+        return self
+
     def get_dtype(self):
         return self._dtype
 
@@ -106,8 +119,21 @@ class RealtimeStreamingMixin:
     def init_streaming(self):
         self.use_video_streaming_mode = True
         self.video_embedding_memory = []
-        self.video_embedding_mem_lock = Lock()
+        from torch.multiprocessing import Lock      # what the reference hangs there (vstream_qwen2vl_realtime.py:43,529):
+        self.video_embedding_mem_lock = Lock()      # shared with a spawned memory-manager process when the model is passed to it
         self.stream_state = None
+
+    def __getstate__(self):
+        """The reference's CLI pickles the whole model into its memory-manager process (cli_server_2gpu.py:301-304).  The
+        streaming state is not transferred, so a host with a stream in progress refuses; a publication stays with the
+        process that exported it."""
+        state = self.__dict__.get("stream_state")
+        if state is not None and state.n_frames > 0:
+            raise L.FvsError("a Qwen2-VL host with a stream in progress cannot be pickled: init_streaming() first, or hand "
+                             "the reader its tensors (flash_vstream_b200.qwen.serve.export_qwen_memory)")
+        d = dict(super().__getstate__())
+        d.pop("_qwen_publication", None)
+        return d
 
     def get_video_embedding_memory_cuda_list(self):
         with self.video_embedding_mem_lock:
@@ -132,15 +158,31 @@ class RealtimeStreamingMixin:
         else:
             hs, ws = h, w
             x_new = small_new = feats
+        pub = self.__dict__.get("_qwen_publication")              # set by qwen.serve.export_qwen_memory (opt-in)
         if self.stream_state is None or not self.video_embedding_memory:
             self.stream_state = QwenStreamState(self.visual.flash_memory, self.visual.merger)
+            if pub is not None:
+                pub.new_stream()
         time_3 = time.perf_counter()
         self.stream_state.step(x_new, small_new, t, (h, w), (hs, ws), start_idx, draws=draws)
         time_6 = time.perf_counter()
-        with self.video_embedding_mem_lock:
-            self.video_embedding_memory[:] = self.stream_state.as_list()
+        if pub is not None:
+            pub.publish(self.stream_state)                         # the clip is final: one launch, under the seqlock
+        self._publish(self.stream_state.as_list())
         time_7 = time.perf_counter()
         return [time_0, time_1, time_2, time_3, time_6, time_6, time_6, time_7]
+
+    def _publish(self, new_list):
+        """`self.video_embedding_memory[:] = [...]` under the lock (:620-624).  The reference's CLI hangs a Manager().list()
+        there and reads it from another process (cli_server_2gpu.py:301, :632-640): a Manager server cannot forward CUDA IPC
+        handles, so the items travel as host copies, the reference's own cost.  The two feature banks (items 7 and 9) are
+        read by nobody on the LLM side (prepare_realtime_inference unpacks and drops them) nor by this writer (the stream
+        state owns them), so empty stand-ins travel instead of the whole O(n) banks; the thw items stay exact."""
+        mem = self.video_embedding_memory
+        if _is_manager_proxy(mem):
+            new_list = [v[:0].cpu() if i in (7, 9) else v.cpu() if torch.is_tensor(v) else v for i, v in enumerate(new_list)]
+        with self.video_embedding_mem_lock:
+            mem[:] = new_list
 
     def prepare_realtime_inference(self, position_ids, visual_position_ids):
         """:632-640"""

@@ -433,6 +433,32 @@ int fvs_qwen_klarge_retrieve(const void* tem_x, const int64_t* klarge_idx, const
 int fvs_qwen_am_rope(const int64_t* spa_positions, int spa_t, int spa_h, int spa_w, const int64_t* tem_positions, int tem_t,
                      int tem_h, int tem_w, int64_t visual_start_id, int64_t* out, fvs_stream_t stream);
 
+/* ---- publication of the Qwen2-VL streaming memory for readers in other processes / on other GPUs ----------------------
+ * One device allocation (so one CUDA IPC handle) of fvs_qwen_pub_layout(...) bytes:
+ *   header        8 x uint64 {seq, epoch, clips, n_frames, n_tem, n_spa, rows, grid}: seq is odd while a publish is writing
+ *                 and only ever grows; grid packs (h, w, hs, ws) as 16-bit fields, h in the low bits;
+ *   tem_timestamp fp32 [tem_len] at layout[1];
+ *   spa_positions int64 [spa_len] at layout[2];
+ *   video_embeds  16-bit [rows_cap, dim] at layout[3]: DAM rows (n_spa * h * w / 4) then CSM rows (n_tem * hs * ws / 4).
+ * rows_cap = spa_len * h * w / 4 + tem_len * hs * ws / 4 (the memory at its fullest for this grid). */
+/* layout_out int64[5] = {rows_cap, tem_timestamp offset, spa_positions offset, video_embeds offset, total bytes} */
+int fvs_qwen_pub_layout(int tem_len, int spa_len, int h, int w, int hs, int ws, int dim, int64_t* layout_out);
+/* One launch on `stream`: seq odd, copy the clip's n_tem timestamps, n_spa positions and `rows` embedding rows into the
+ * publication, a grid-wide barrier, the counters, seq even.  rows must equal n_spa * h * w / 4 + n_tem * hs * ws / 4. */
+int fvs_qwen_publish(void* pub, size_t pub_bytes, int tem_len, int spa_len, int64_t rows_cap, int dim,
+                     const void* video_embeds, int64_t rows, const float* tem_timestamp, int n_tem,
+                     const int64_t* spa_positions, int n_spa, int h, int w, int hs, int ws, uint64_t epoch, uint64_t clips,
+                     int64_t n_frames, fvs_stream_t stream);
+/* Consistent copy of a (possibly IPC-mapped or peer) publication into the caller's buffers on the current device:
+ * embeds_out [out_rows >= rows_cap, dim], ts_out fp32 [ts_cap >= tem_len], pos_out int64 [pos_cap >= spa_len].
+ * status (device uint64[9]) = {seq before, seq after, epoch, clips, n_frames, n_tem, n_spa, rows, grid}; the copy is valid
+ * iff status[0] == status[1] and even.  Counts read from a torn header are clamped to the capacities, so nothing outside
+ * the publication or the outputs is touched.  A publication on another device needs peer access: it is enabled once per
+ * device pair; a pair that cannot peer is refused (FVS_EINVAL). */
+int fvs_qwen_snapshot(const void* pub, size_t pub_bytes, int tem_len, int spa_len, int64_t rows_cap, int dim,
+                      void* embeds_out, int64_t out_rows, float* ts_out, int64_t ts_cap, int64_t* pos_out, int64_t pos_cap,
+                      uint64_t* status, fvs_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
