@@ -112,6 +112,9 @@ FVS_DEVICE void fence_proxy_async_smem() { asm volatile("fence.proxy.async.share
 FVS_DEVICE void named_bar_sync(uint32_t id, uint32_t nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
+FVS_DEVICE void named_bar_arrive(uint32_t id, uint32_t nthreads) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
 
 // ---------------------------------------------------------------- TMA
 FVS_DEVICE void tma_prefetch_desc(const CUtensorMap* m) {
@@ -199,6 +202,14 @@ FVS_DEVICE void wgmma_pin(float (&d)[N]) {
 template <int N, bool kBF16, int kTB>
 struct Wgmma;
 template <int kTB> struct Wgmma<16, false, kTB> {
+  // D[64x16] (+)= A[smem] * B[smem]
+  static FVS_DEVICE void ss(float (&d)[8], uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, %11;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "l"(a), "l"(b), "r"(acc), "n"(kTB));
+  }
   // D[64x16] (+)= A[registers: 4 x 32 bit per thread] * B[smem]
   static FVS_DEVICE void rs(float (&d)[8], const uint32_t (&a)[4], uint64_t b, uint32_t acc) {
     asm volatile(
@@ -291,6 +302,14 @@ template <int kTB> struct Wgmma<256, false, kTB> {
 };
 
 template <int kTB> struct Wgmma<16, true, kTB> {
+  // D[64x16] (+)= A[smem] * B[smem]
+  static FVS_DEVICE void ss(float (&d)[8], uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, %11;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "l"(a), "l"(b), "r"(acc), "n"(kTB));
+  }
   // D[64x16] (+)= A[registers: 4 x 32 bit per thread] * B[smem]
   static FVS_DEVICE void rs(float (&d)[8], const uint32_t (&a)[4], uint64_t b, uint32_t acc) {
     asm volatile(
