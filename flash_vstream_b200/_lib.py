@@ -59,6 +59,12 @@ class StreamJob(C.Structure):    # fvs_stream_job
                 ("refill_idx", C.c_void_p), ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t)]
 
 
+class ResampleAxis(C.Structure):  # fvs_resample_axis
+    _fields_ = [(n, C.c_int) for n in ("in_size", "out_size", "first", "count", "taps", "span_first", "span_count")] + \
+               [("bounds", C.c_void_p), ("coeffs", C.c_void_p)]
+
+
+PRE_CLIP, PRE_QWEN = 0, 1
 KLARGE_EUCLIDEAN, KLARGE_COSINE = 0, 1
 INPUT_PIXELS, INPUT_FEATURES = 0, 1
 
@@ -127,6 +133,11 @@ SIGNATURES = {
     "fvs_qwen_publish": (_i, [_vp, _sz, _i, _i, C.c_int64, _i, _vp, C.c_int64, _vp, _i, _vp, _i, _i, _i, _i, _i, C.c_uint64,
                               C.c_uint64, C.c_int64, _vp]),
     "fvs_qwen_snapshot": (_i, [_vp, _sz, _i, _i, C.c_int64, _i, _vp, C.c_int64, _vp, C.c_int64, _vp, C.c_int64, _vp, _vp]),
+    # frame pre-processing (uint8 RGB frames -> tower pixels)
+    "fvs_resample_plan": (_i, [_i, _i, _i, _i, C.POINTER(ResampleAxis), C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
+    "fvs_preprocess_workspace_bytes": (_sz, [C.POINTER(ResampleAxis), C.POINTER(ResampleAxis), _i]),
+    "fvs_preprocess": (_i, [_vp, _i, _i, _i, _i, C.POINTER(ResampleAxis), C.POINTER(ResampleAxis), _vp, _i, _i, _vp, _vp, _sz,
+                            _vp]),
 }
 
 _lib = None

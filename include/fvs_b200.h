@@ -459,6 +459,45 @@ int fvs_qwen_snapshot(const void* pub, size_t pub_bytes, int tem_len, int spa_le
                       void* embeds_out, int64_t out_rows, float* ts_out, int64_t ts_cap, int64_t* pos_out, int64_t pos_cap,
                       uint64_t* status, fvs_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------------------------------
+ * Frame pre-processing: decoded uint8 RGB frames [T, H, W, 3] -> the pixels the vision towers take, bit-identical to
+ * the reference's CPU processors: LLaVA's CLIPImageProcessor.preprocess(clip)['pixel_values'].half()
+ * (Flash-VStream-LLaVA/flash_vstream/serve/cli_video_stream.py:186) and Qwen2-VL's
+ * FlashVStreamQwen2VLImageProcessor._preprocess (Flash-VStream-Qwen/models/vstream_qwen2vl_processor.py:38-157, called
+ * from cli_server_2gpu.py:214-219).  The resize is Pillow's fixed-point BICUBIC resample (transformers'
+ * image_transforms.resize); rescale + normalize come in as a float32 [3, 256] table, one value per channel and byte.
+ * ------------------------------------------------------------------------------------------------------------------ */
+typedef struct fvs_resample_axis {
+  int in_size, out_size;        /* source length -> resized length */
+  int first, count;             /* the window of the resized axis that is produced: [first, first + count) */
+  int taps;                     /* coefficients per output: 2 * ceil(2 * max(in_size / out_size, 1)) + 1 */
+  int span_first, span_count;   /* the source indices the window reads */
+  const int32_t* bounds;        /* device int32 [count, 2] = {first source index, taps used}, 8-byte aligned */
+  const int32_t* coeffs;        /* device int32 [count, taps], 22 fractional bits */
+} fvs_resample_axis;
+enum { FVS_PRE_CLIP = 0, FVS_PRE_QWEN = 1 };
+
+/* Host: PIL's per-axis plan (precompute_coeffs + normalize_coeffs_8bpc, in double, in PIL's order, no FMA contraction)
+ * for the window [first, first + count) of in_size -> out_size.  Fills every field of *axis_h but bounds / coeffs, which
+ * are left as they were (the caller points them at its device copies).  bounds_h [count, 2] and coeffs_h [count, taps]
+ * are filled when given (both or neither): call once without them to learn `taps`. */
+int fvs_resample_plan(int in_size, int out_size, int first, int count, fvs_resample_axis* axis_h, int32_t* bounds_h,
+                      int32_t* coeffs_h);
+/* uint8 workspace fvs_preprocess needs for `frames` frames: frames * 3 * y.span_count * x.count (0 on bad arguments) */
+size_t fvs_preprocess_workspace_bytes(const fvs_resample_axis* x_h, const fvs_resample_axis* y_h, int frames);
+/* Two launches on `stream`, no allocation, no synchronisation.  frames: device uint8 [T, H, W, C = 3]; x_h / y_h: host
+ * structs of fvs_resample_plan with device tables; table: device float32 [3, 256].
+ *   FVS_PRE_CLIP: out f16 [T, 3, y.count, x.count] (the resize with the center crop folded into the windows);
+ *   FVS_PRE_QWEN: out fp32 pixel_values_videos [max(T, 2) / 2 * gh * gw, 1176] with gh = y.out_size / 14,
+ *                 gw = x.out_size / 14 — the patchify of vstream_qwen2vl_processor.py:141-155; a one-frame clip fills both
+ *                 temporal slots (:136-137).  The windows must be whole, T 1 or even, and both sizes multiples of 28 * pool.
+ * FVS_EINVAL, with nothing launched, on null pointers, C != 3, an empty input, a plan that does not match the frames or
+ * fvs_resample_plan, a window outside the resized image, a workspace below fvs_preprocess_workspace_bytes, or a Qwen2-VL
+ * call breaking the rules above. */
+int fvs_preprocess(const uint8_t* frames, int T, int H, int W, int C, const fvs_resample_axis* x_h,
+                   const fvs_resample_axis* y_h, const float* table, int layout, int pool, void* out, void* workspace,
+                   size_t workspace_bytes, fvs_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
