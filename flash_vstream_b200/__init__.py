@@ -8,6 +8,7 @@ ViT-L/14 frame encoding + Flash-Memory consolidation, behind the reference's own
     flash_vstream_b200.StreamPool           many streams on one GPU, stepped together (multistream.py)
     flash_vstream_b200.CLIPFramePreprocessor, .Qwen2VLFramePreprocessor
                                             decoded uint8 frames -> tower pixels on the GPU (preprocess.py)
+    flash_vstream_b200.StreamCheckpoint     a live stream's state on the host / on disk: suspend, resume, move (checkpoint.py)
     flash_vstream_b200.install()            rebinds the reference's modules to these implementations
 
 All arithmetic happens in libfvs_b200.so (hand-written CUDA for sm_90a).  There is no CPU fallback: importing the
@@ -34,4 +35,7 @@ def __getattr__(name):      # StreamPool imports torch: loaded on first use, so 
     if name in ("CLIPFramePreprocessor", "Qwen2VLFramePreprocessor"):
         from . import preprocess
         return getattr(preprocess, name)
+    if name == "StreamCheckpoint":
+        from .checkpoint import StreamCheckpoint
+        return StreamCheckpoint
     raise AttributeError(f"module {__name__!r} has no attribute {name!r}")

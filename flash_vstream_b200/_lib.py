@@ -93,7 +93,9 @@ SIGNATURES = {
     "fvs_stream_workspace_bytes": (_sz, [C.POINTER(StarConfig), _i]),
     "fvs_bank_rows": (_i, [C.POINTER(StarConfig), _i, _i64p, _i64p, _i64p]),
     "fvs_bank_reset": (_i, [C.POINTER(Bank), _vp]),
-    "fvs_bank_prefix": (_i, [C.POINTER(StarConfig), C.POINTER(Bank), C.POINTER(_vp), _i64p]),
+    "fvs_bank_restore": (_i, [C.POINTER(StarConfig), C.POINTER(Bank), C.c_int32, C.c_int32, C.c_int32, C.c_int64, C.c_uint64,
+                              _vp, _vp, _vp, _vp, _vp]),
+    "fvs_bank_prefix": (_i,[C.POINTER(StarConfig), C.POINTER(Bank), C.POINTER(_vp), _i64p]),
     "fvs_stream_step": (_i, [C.POINTER(StarConfig), C.POINTER(Bank), C.POINTER(NtmWeights), _vp, _vp, _i, _i, _vp, _vp,
                              _vp, _sz, _vp, _sz, _vp]),
     "fvs_stream_step_multi": (_i, [C.POINTER(StarConfig), C.POINTER(StreamJob), _i, _vp, _vp, _i, _vp, _sz, _i, _vp]),

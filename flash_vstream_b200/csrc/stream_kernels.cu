@@ -358,6 +358,28 @@ __global__ void snapshot_kernel(const uint4* __restrict__ prefix, const unsigned
   }
 }
 
+// ---------------------------------------------------------------------------------------------------- restore
+// prefix <- src and header words 1-5 <- the restored counters, under the writer side of the seqlock: a reader that has the
+// bank mapped (a bank of a closed stream that StreamPool hands to a new one may still be) sees the old prefix or the
+// restored one, never a mix.  src is a device pointer or a pinned host pointer (read over PCIe through UVA).
+__global__ void __launch_bounds__(256) restore_kernel(const uint4* __restrict__ src, uint4* __restrict__ prefix,
+                                                      unsigned long long* __restrict__ header, size_t n_vecs,
+                                                      unsigned long long n_tur, unsigned long long n_long,
+                                                      unsigned long long n_cur, unsigned long long n_frames,
+                                                      unsigned long long step) {
+  cg::grid_group grid = cg::this_grid();
+  if (blockIdx.x == 0 && threadIdx.x == 0) seqlock::write_begin(&header[0]);
+  grid.sync();
+  for (size_t i = size_t(blockIdx.x) * blockDim.x + threadIdx.x; i < n_vecs; i += size_t(gridDim.x) * blockDim.x)
+    prefix[i] = src[i];
+  __threadfence_system();
+  grid.sync();
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    header[1] = n_tur; header[2] = n_long; header[3] = n_cur; header[4] = n_frames; header[5] = step;
+    seqlock::write_end(&header[0]);
+  }
+}
+
 inline size_t al(size_t v) { return (v + 255) & ~size_t(255); }
 
 struct Carve {
@@ -701,6 +723,84 @@ int fvs_bank_reset(fvs_bank* bank, fvs_stream_t stream) {
   bank->n_long = bank->n_tur = bank->n_cur = 0;
   bank->step = 0;
   FVS_CUDA_OK(cudaMemsetAsync(bank->header, 0, 64, (cudaStream_t)stream));
+  return FVS_OK;
+}
+
+int fvs_bank_restore(const fvs_star_config* cfg, fvs_bank* bank, int32_t n_tur, int32_t n_long, int32_t n_cur,
+                     int64_t n_frames, uint64_t step, const void* prefix_src, const void* long_src, const void* tur_src,
+                     const void* frames_src, fvs_stream_t stream) {
+  const char* api = "fvs_bank_restore";
+  int r = check_config(cfg, api);
+  if (r) return r;
+  FVS_REQUIRE(bank, "%s: null bank", api);
+  FVS_REQUIRE(bank->prefix && bank->long_work && bank->tur_work && bank->frames && bank->header, "%s: bank buffers missing", api);
+  FVS_REQUIRE(bank->chunk_cap > 0, "%s: chunk_cap must be > 0", api);
+  int64_t lrows, trows, prows;
+  if ((r = fvs_bank_rows(cfg, bank->chunk_cap, &lrows, &trows, &prows))) return r;
+  // a first clip longer than a memory leaves that many rows (the k-means / abstract update only start at the second step),
+  // so the working sets hold up to max(length, chunk_cap) rows between steps — lrows / trows less one clip
+  const int64_t lcap = lrows - bank->chunk_cap, tcap = trows - bank->chunk_cap;
+  FVS_REQUIRE(n_long >= 0 && n_long <= lcap, "%s: n_long %d > %lld (long_len %d, chunk_cap %d)", api, n_long, (long long)lcap,
+              cfg->long_len, bank->chunk_cap);
+  FVS_REQUIRE(n_tur >= 0 && n_tur <= tcap, "%s: n_tur %d > %lld (tur_len %d, chunk_cap %d)", api, n_tur, (long long)tcap,
+              cfg->tur_len, bank->chunk_cap);
+  FVS_REQUIRE(n_cur >= 0 && n_cur <= cfg->key_len + cfg->cur_len, "%s: n_cur %d > key_len + cur_len (%d)", api, n_cur,
+              cfg->key_len + cfg->cur_len);
+  const int a2 = cfg->cur_size * cfg->cur_size, b2 = cfg->long_size * cfg->long_size;
+  const int64_t rows = int64_t(n_tur) + int64_t(n_long) * b2 + int64_t(n_cur) * a2;
+  FVS_REQUIRE(rows <= prows, "%s: prefix of %lld rows exceeds the buffer (%lld)", api, (long long)rows, (long long)prows);
+  FVS_REQUIRE(n_frames >= 0 && n_frames <= bank->frames_cap, "%s: %lld frames > frames_cap %lld: grow the frame buffer first",
+              api, (long long)n_frames, (long long)bank->frames_cap);
+  FVS_REQUIRE((step == 0) == (n_frames == 0), "%s: step %llu with %lld frames (step is 0 exactly when no frame was seen)", api,
+              (unsigned long long)step, (long long)n_frames);
+  FVS_REQUIRE(step > 0 || (n_tur == 0 && n_long == 0 && n_cur == 0), "%s: a state at step 0 holds no memory rows", api);
+  FVS_REQUIRE(rows == 0 || prefix_src, "%s: prefix_src is null", api);
+  FVS_REQUIRE(n_long == 0 || long_src, "%s: long_src is null", api);
+  FVS_REQUIRE(n_tur == 0 || tur_src, "%s: tur_src is null", api);
+  FVS_REQUIRE(n_frames == 0 || frames_src, "%s: frames_src is null", api);
+
+  // every source must be readable by the bank's device: its own memory or pinned host memory (a pageable pointer would
+  // fault in the kernel, another device's memory needs peer mappings the caller did not ask for)
+  cudaPointerAttributes at;
+  FVS_CUDA_OK(cudaPointerGetAttributes(&at, bank->header));
+  const int dev = at.device;
+  const void* srcs[4] = {rows ? prefix_src : nullptr, n_long ? long_src : nullptr, n_tur ? tur_src : nullptr,
+                         n_frames ? frames_src : nullptr};
+  const char* names[4] = {"prefix_src", "long_src", "tur_src", "frames_src"};
+  for (int i = 0; i < 4; ++i) {
+    if (!srcs[i]) continue;
+    FVS_CUDA_OK(cudaPointerGetAttributes(&at, srcs[i]));
+    FVS_REQUIRE(at.type == cudaMemoryTypeHost || ((at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged) &&
+                                                 at.device == dev),
+                "%s: %s is neither pinned host memory nor memory of the bank's device %d", api, names[i], dev);
+  }
+
+  cudaStream_t s = (cudaStream_t)stream;
+  const size_t D = size_t(cfg->D);
+  if (n_long) FVS_CUDA_OK(cudaMemcpyAsync(bank->long_work, long_src, size_t(n_long) * b2 * D * 2, cudaMemcpyDefault, s));
+  if (n_tur) FVS_CUDA_OK(cudaMemcpyAsync(bank->tur_work, tur_src, size_t(n_tur) * D * 2, cudaMemcpyDefault, s));
+  if (n_frames) FVS_CUDA_OK(cudaMemcpyAsync(bank->frames, frames_src, size_t(n_frames) * a2 * D * 2, cudaMemcpyDefault, s));
+
+  static int per_sm = 0;
+  if (per_sm == 0) FVS_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, restore_kernel, 256, 0));
+  const uint4* src = static_cast<const uint4*>(prefix_src);
+  uint4* pre = static_cast<uint4*>(bank->prefix);
+  unsigned long long* hdr = static_cast<unsigned long long*>(bank->header);
+  size_t n_vecs = size_t(rows) * (D / 8);
+  unsigned long long w[5] = {(unsigned long long)n_tur, (unsigned long long)n_long, (unsigned long long)n_cur,
+                             (unsigned long long)n_frames, (unsigned long long)step};
+  const size_t want = (n_vecs + 255) / 256;
+  const size_t cap = size_t(per_sm > 0 ? per_sm : 1) * device_sm_count();
+  const unsigned blocks = unsigned(want < 1 ? 1 : (want < cap ? want : cap));
+  void* args[] = {&src, &pre, &hdr, &n_vecs, &w[0], &w[1], &w[2], &w[3], &w[4]};
+  FVS_CUDA_OK(cudaLaunchCooperativeKernel((const void*)restore_kernel, dim3(blocks), dim3(256), args, 0, s));
+  FVS_CHECK_LAUNCH("restore_kernel");
+
+  bank->n_tur = n_tur;
+  bank->n_long = n_long;
+  bank->n_cur = n_cur;
+  bank->n_frames = n_frames;
+  bank->step = step;
   return FVS_OK;
 }
 

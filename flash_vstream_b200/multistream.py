@@ -63,17 +63,45 @@ class StreamPool:
         self._next = 0
 
     # ---- streams -------------------------------------------------------------------------------------------------------
-    def open(self, seed: Optional[int] = None) -> int:
+    def open(self, seed: Optional[int] = None, *, checkpoint=None) -> int:
+        """A new stream -> its sid.  With `checkpoint` (a StreamCheckpoint of `checkpoint(sid)`, from this pool or another,
+        on any device), the stream continues where the checkpoint left it: its bank and its draw source's generators.  A
+        checkpoint without a draw source (from the single-stream model, whose draws come from the global generators) needs
+        `seed=` for the generators the stream draws from from here on."""
         if self.max_streams is not None and len(self._streams) >= self.max_streams:
             raise RuntimeError(f"StreamPool is full ({self.max_streams} streams)")
+        if checkpoint is not None and checkpoint.rng is None and seed is None:
+            raise ValueError("StreamPool.open: this checkpoint carries no draw source (single-stream model): pass seed=")
         bank = self._free.pop() if self._free else ops.StreamBank(self.cfg, self.ntm, chunk_cap=self.chunk_cap, device=self.device)
-        bank.reset()
-        if seed is None:
+        if checkpoint is None:
+            bank.reset()
+        else:
+            try:
+                bank.restore(checkpoint)
+            except BaseException:
+                self._free.append(bank)
+                raise
+        if seed is None and checkpoint is None:
             seed = int.from_bytes(os.urandom(8), "little") >> 1
+        rng = DrawSource(int(seed) if seed is not None else 0, self.device)
+        if checkpoint is not None and checkpoint.rng is not None:
+            r = checkpoint.rng
+            rng.cpu = r["cpu"].clone()
+            rng.cuda = r["cuda"].clone() if rng.cuda is not None and r["cuda"] is not None else rng.cuda
+            rng.py.setstate(r["py"])
         sid = self._next
         self._next += 1
-        self._streams[sid] = _Stream(bank, DrawSource(int(seed), self.device))
+        self._streams[sid] = _Stream(bank, rng)
         return sid
+
+    def checkpoint(self, sid: int):
+        """The stream's state as a StreamCheckpoint in pinned host memory: its bank and its draw source (settled first:
+        this blocks on the source's pending refill read-backs, so no consumed count is lost or applied twice).  Suspend =
+        checkpoint(sid) then close(sid); resume = open(checkpoint=...)."""
+        from . import checkpoint as CK
+        st = self._streams[sid]
+        st.rng.settle()
+        return st.bank.checkpoint(rng=CK.rng_state(st.rng))
 
     def close(self, sid: int):
         st = self._streams.pop(sid)

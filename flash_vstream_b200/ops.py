@@ -375,6 +375,41 @@ class StreamBank:
             self.bank.frames = new.data_ptr()
             self.bank.frames_cap = new.shape[0]
 
+    # ---- checkpoint / restore (DESIGN.md §3.12) ------------------------------------------------------------------------
+    def checkpoint(self, rng: Optional[dict] = None):
+        """The stream's state as a checkpoint.StreamCheckpoint in pinned host memory: prefix, long / Turing working sets,
+        frame buffer and counters.  Call it from the writer, between steps: on the current stream those arrays are a
+        consistent state.  Returns once the copies have landed."""
+        from . import checkpoint as CK
+        b = self.bank
+        counters = dict(n_tur=b.n_tur, n_long=b.n_long, n_cur=b.n_cur, n_frames=b.n_frames, step=b.step)
+        with torch.cuda.device(self.device):
+            ck = CK.llava(CK.star_config(self.cfg), counters, self.prefix(), self.long_work[:b.n_long],
+                          self.tur_work[:b.n_tur], self.frames[:b.n_frames], rng=rng)
+            torch.cuda.current_stream().synchronize()
+        return ck
+
+    def restore(self, ckpt):
+        """Continue the stream of `ckpt` in this bank (any device, any chunk_cap whose capacities hold it): same STAR
+        config or ValueError; the frame buffer grows as needed.  One fvs_bank_restore: the working sets and frames by copy
+        engine, the prefix and header under the seqlock, so readers that have this bank mapped never see a mix."""
+        from . import checkpoint as CK
+        CK.check_star(ckpt, self.cfg, "StreamBank.restore")
+        n = ckpt.counters
+        srcs = [ckpt.tensor(k) for k in ("prefix", "long", "tur", "frames")]
+        for t in srcs:
+            if t.numel() and not (t.is_cuda and t.device == self.device) and not (not t.is_cuda and t.is_pinned()):
+                raise ValueError("StreamBank.restore: checkpoint tensors must be pinned host memory or on the bank's device")
+        with torch.cuda.device(self.device):
+            if n["n_frames"] > self.frames.shape[0]:
+                self._reserve_frames(n["n_frames"] - self.bank.n_frames)
+            L.check(self.lib.fvs_bank_restore(C.byref(self.cfg), C.byref(self.bank), n["n_tur"], n["n_long"], n["n_cur"],
+                                              n["n_frames"], n["step"], *[t.data_ptr() if t.numel() else None for t in srcs],
+                                              L.cur_stream()), "fvs_bank_restore")
+            self.ws.zero_()       # the step's arrival counters start at zero (a fresh bank's workspace is uninitialised)
+            torch.cuda.current_stream().synchronize()    # the sources may be freed as soon as this returns
+        self._last_T = 0
+
     def __getstate__(self):     # see VitEncoder.__getstate__; the stream state itself is not transferred (a fresh bank)
         if self.steps > 0:
             raise L.FvsError("a StreamBank with a stream in progress cannot be pickled: reset_video_stream() first, or hand the "

@@ -205,6 +205,82 @@ class QwenStreamState:
             cand.reshape(T * P, D), self._thw(T, small=True), flash.temporal_length, cand_w, ts_in, draws=d)
         self._enqueue_rest(tem_x, tem_w, tem_ts, int(tem_thw[0]), members, d)
 
+    # ------------------------------------------------------------------------------------------------ checkpoint / restore
+    # What a step reads: the three banks, the CSM (tem_x, weights; n_tem), n_frames and the grids; what as_list() and a
+    # publication read besides: timestamps, spa_positions, spa_x and video_embeds.  spa_x is bank_x[spa_positions], so it
+    # is rebuilt by a bit-exact gather; the member lists are read by no step (only by spatial_enhance of the step that
+    # made them), so a restored state has none, like a reset one.
+    def _config(self, dim, dtype):
+        return {"flash": dict(self.flash.config), "grid": None if self.grid is None else list(self.grid),
+                "small_grid": None if self.small_grid is None else list(self.small_grid), "dtype": dtype, "dim": dim,
+                "merger_dim": None if self.merger is None else int(self.merger.dim)}
+
+    def checkpoint(self):
+        """The state as a checkpoint.StreamCheckpoint in pinned host memory (filled rows only; returns once the copies
+        have landed).  Call it between steps, from the writer."""
+        from .. import checkpoint as CK
+        n = self.n_frames
+        counters = {"n_frames": n, "steps": self.steps, "n_tem": self.n_tem,
+                    "n_spa": 0 if self.spa_positions is None else int(self.spa_positions.numel()),
+                    "fast_steps": self.fast_steps, "redone_steps": self.redone_steps,
+                    "merged": int(self.bank_merged.n > 0),
+                    "tem_weights_dtype": None if self.tem_weights is None else CK.dtype_name(self.tem_weights.dtype),
+                    "tem_timestamp_dtype": "float32" if n == 0 else CK.dtype_name(self.tem_timestamp.dtype)}
+        if n == 0:
+            return CK.qwen(self._config(0, "float16"), counters, {})
+        x = self.bank_x.rows()
+        tensors = {"bank_x": x, "bank_small": self.bank_small.rows(), "tem_x": self.tem_x,
+                   "tem_timestamp": self.tem_timestamp, "spa_positions": self.spa_positions}
+        if self.tem_weights is not None:          # temporal_method 'sample' keeps no weights
+            tensors["tem_weights"] = self.tem_weights
+        if self.bank_merged.n:
+            tensors["bank_merged"] = self.bank_merged.rows()
+        if self.merger is not None:
+            tensors["video_embeds"] = self.video_embeds
+        with torch.cuda.device(x.device):
+            ck = CK.qwen(self._config(int(x.shape[-1]), CK.dtype_name(x.dtype)), counters, tensors)
+            torch.cuda.current_stream().synchronize()
+        return ck
+
+    @classmethod
+    def restore(cls, ckpt, flash, merger, device) -> "QwenStreamState":
+        """A state on `device` that continues `ckpt` bit for bit; `flash` / `merger` must have the configuration the
+        checkpoint was taken with (ValueError naming the field otherwise)."""
+        from .. import checkpoint as CK
+        if ckpt.family != CK.QWEN:
+            raise ValueError(f"QwenStreamState.restore: a {ckpt.family!r} checkpoint is not a Qwen2-VL stream's")
+        c, n = ckpt.config, ckpt.counters
+        if c["flash"] != dict(flash.config):
+            bad = next(k for k in set(c["flash"]) | set(flash.config) if c["flash"].get(k) != flash.config.get(k))
+            raise ValueError(f"QwenStreamState.restore: config.flash.{bad} of the checkpoint ({c['flash'].get(bad)}) "
+                             f"differs from the FlashMemory's ({flash.config.get(bad)})")
+        md = None if merger is None else int(merger.dim)
+        if n["n_frames"] and c["merger_dim"] != md:
+            raise ValueError(f"QwenStreamState.restore: config.merger_dim of the checkpoint ({c['merger_dim']}) differs "
+                             f"from the merger's ({md})")
+        st = cls(flash, merger)
+        if n["n_frames"] == 0:
+            return st
+        dev = torch.device(device)
+        with torch.cuda.device(dev):
+            get = lambda k: ckpt.tensor(k).to(dev, non_blocking=True)
+            st.bank_x.append(get("bank_x"))
+            st.bank_small.append(get("bank_small"))
+            if n["merged"]:
+                st.bank_merged.append(get("bank_merged"))
+            st.n_frames, st.steps = n["n_frames"], n["steps"]
+            st.fast_steps, st.redone_steps = n["fast_steps"], n["redone_steps"]
+            st.grid, st.small_grid = tuple(c["grid"]), tuple(c["small_grid"])
+            st.tem_x, st.tem_timestamp = get("tem_x"), get("tem_timestamp")
+            st.tem_weights = get("tem_weights") if "tem_weights" in ckpt.tensors else None
+            st.n_tem = n["n_tem"]
+            st.spa_positions = get("spa_positions")
+            bank = st.bank_x.rows()
+            st.spa_x = O.gather_rows(bank, st.spa_positions) if n["n_spa"] else bank[0:0]
+            st.video_embeds = get("video_embeds") if "video_embeds" in ckpt.tensors else None
+            torch.cuda.current_stream().synchronize()     # the pinned sources may be freed as soon as this returns
+        return st
+
     # ------------------------------------------------------------------------------------------------ the reference's list
     def as_list(self):
         """the 13 items of `video_embedding_memory` (:620-624); the thw entries are host tensors, everything else lives in HBM"""

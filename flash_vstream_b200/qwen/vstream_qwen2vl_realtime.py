@@ -172,6 +172,41 @@ class RealtimeStreamingMixin:
         time_7 = time.perf_counter()
         return [time_0, time_1, time_2, time_3, time_6, time_6, time_6, time_7]
 
+    # ---- suspend / resume (DESIGN.md §3.12) ---------------------------------------------------------------------------
+    def save_video_stream(self):
+        """The stream in progress as a checkpoint.StreamCheckpoint (pinned host memory) that load_video_stream continues
+        bit for bit, here, in another process or on another GPU.  Draws come from the global generators (draws.GLOBAL):
+        settled first, neither stored nor set — a resumed stream continues from the resuming process's generators."""
+        from ..draws import GLOBAL
+        state = self.__dict__.get("stream_state")
+        if state is None or state.n_frames == 0 or not self.video_embedding_memory:
+            raise ValueError("save_video_stream: no stream in progress")
+        GLOBAL.settle()
+        return state.checkpoint()
+
+    def load_video_stream(self, ckpt):
+        """Continue the stream of `ckpt` in this host: `stream_state` is restored on the vision side's device and the
+        13-item list republished.  An exported host (qwen.serve.export_qwen_memory) must have the checkpoint's grid; its
+        readers see the resumed memory under a new epoch."""
+        from .. import checkpoint as CK
+        if ckpt.family != CK.QWEN:
+            raise ValueError(f"load_video_stream: a {ckpt.family!r} checkpoint is not a Qwen2-VL stream's")
+        pub = self.__dict__.get("_qwen_publication")
+        if pub is not None and ckpt.counters["n_frames"] and \
+                (tuple(ckpt.config["grid"]), tuple(ckpt.config["small_grid"])) != (pub.grid, pub.small_grid):
+            raise ValueError(f"load_video_stream: config.grid {ckpt.config['grid']} / {ckpt.config['small_grid']} is not "
+                             f"the exported grid {pub.grid} / {pub.small_grid}")
+        state = QwenStreamState.restore(ckpt, self.visual.flash_memory, self.visual.merger, self.visual.get_device())
+        if state.n_frames == 0:
+            self.stream_state = None
+            self._publish([])
+            return
+        self.stream_state = state
+        if pub is not None:
+            pub.new_stream()
+            pub.publish(state)
+        self._publish(state.as_list())
+
     def _publish(self, new_list):
         """`self.video_embedding_memory[:] = [...]` under the lock (:620-624).  The reference's CLI hangs a Manager().list()
         there and reads it from another process (cli_server_2gpu.py:301, :632-640): a Manager server cannot forward CUDA IPC

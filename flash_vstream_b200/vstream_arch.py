@@ -8,6 +8,11 @@ Differences by design (DESIGN.md "state residency"): all per-stream state stays 
 `.cpu()` / Manager-list round trips (vstream_arch.py:650,672-676,693-695) are gone; `video_embedding_memory` is still
 written as `[cur, long, Turing, buffer]` under the lock, but holds CUDA tensors (the unmodified reader at
 vstream_arch.py:480-485 calls `.to(device)` on them, a no-op).
+
+A stream on the fused path can be suspended and resumed (`save_video_stream` / `load_video_stream`, DESIGN.md §3.12), in
+another process or on another GPU.  Its k-means draws come from the global generators (draws.GLOBAL), which a checkpoint
+neither stores nor sets: a resumed stream continues from the resuming process's global generators, as the reference's would
+after a restart.
 """
 from __future__ import annotations
 
@@ -373,6 +378,56 @@ class VStreamMetaForCausalLM:
             tur_c, _ = attention_feature(Turing_memory, s.tur_len, self.attention, update_ratio=s.ratio)
         self._publish([cur_memory, long_c, tur_c, buf])
         return []
+
+    # ---- suspend / resume (DESIGN.md §3.12) -------------------------------------------------------------------------
+    def _fused_knob(self):
+        """the knob that keeps this model's stream off the fused path"""
+        tower = self.get_model().get_vision_tower()
+        engine = getattr(tower, "engine", None) if tower is not None else None
+        D = self.get_model().attention_model.q_proj.weight.shape[1]
+        return self._fused_reject(self._star_cfg(), engine.grid if engine is not None else 24, D, torch.float16) \
+            or "fvs_chunk_cap"      # fused config, but a clip longer than the bank was streamed op by op
+
+    def save_video_stream(self):
+        """The stream in progress as a checkpoint.StreamCheckpoint (pinned host memory) that `load_video_stream` continues
+        bit for bit, here or in another process or on another GPU.  Fused path only (the op-by-op path raises
+        NotImplementedError naming the knob).  The draws of this model come from the global generators (draws.GLOBAL):
+        they are settled first but neither stored nor set, so a resumed stream continues from the resuming process's global
+        generators — as the reference's would after a restart."""
+        bank = self.__dict__.get("_fvs_bank")
+        mem = self.video_embedding_memory
+        if mem is None or len(mem) == 0:
+            raise ValueError("save_video_stream: no stream in progress")
+        # the op-by-op path keeps its own frame buffer (_fvs_buf); on the fused path the bank is the stream (a Manager list
+        # holds host copies of its state)
+        fused = bank is not None and bank.steps > 0 and "_fvs_buf" not in self.__dict__ and \
+            (_is_manager_proxy(mem) or mem[0].data_ptr() == bank.state()[0].data_ptr())
+        if not fused:
+            raise NotImplementedError(f"save_video_stream: this stream runs op by op ({self._fused_knob()}); "
+                                      f"checkpoints cover the fused streaming step")
+        GLOBAL.settle()
+        return bank.checkpoint()
+
+    def load_video_stream(self, ckpt):
+        """Continue the stream of `ckpt` (from save_video_stream or StreamPool.checkpoint) in this model: the bank is
+        restored and `video_embedding_memory` republished, so the unmodified reader and a Manager-list reader see the
+        resumed memory.  A StreamPool checkpoint's own generators are not used: this model draws from the global ones."""
+        from . import checkpoint as CK
+        if ckpt.family != CK.LLAVA:
+            raise ValueError(f"load_video_stream: a {ckpt.family!r} checkpoint is not a LLaVA stream's")
+        c = ckpt.config
+        cfg = self._fused_cfg(self._star_cfg(), int(c["grid"]), int(c["D"]), torch.float16)
+        if cfg is None:
+            raise NotImplementedError(f"load_video_stream: this model streams op by op "
+                                      f"({self._fused_reject(self._star_cfg(), int(c['grid']), int(c['D']), torch.float16)}); "
+                                      f"checkpoints cover the fused streaming step")
+        CK.check_star(ckpt, cfg, "load_video_stream")       # before the current stream is dropped
+        device = self.get_model().attention_model.q_proj.weight.device
+        self.reset_video_stream()
+        bank = self._get_bank(cfg, 1, device)
+        bank.restore(ckpt)
+        if bank.steps > 0:
+            self._publish(list(bank.state()))
 
     def cat_proj(self, all_features):
         """vstream_arch.py:279-284: concatenate the per-video prefixes, project them together, split back"""

@@ -250,6 +250,25 @@ size_t fvs_stream_workspace_bytes(const fvs_star_config* cfg_h, int chunk_cap);
 int fvs_bank_rows(const fvs_star_config* cfg_h, int chunk_cap, int64_t* long_work_rows_h, int64_t* tur_work_rows_h,
                   int64_t* prefix_rows_h);
 int fvs_bank_reset(fvs_bank* bank_h, fvs_stream_t stream);
+/* Restore a stream's state into `bank` (same STAR config; any chunk_cap whose capacities hold it), e.g. a checkpoint taken
+ * on another device or in another process.  Sources are device pointers on the bank's device or pinned host pointers (UVA);
+ * counts are the saved bank's host counters:
+ *   prefix_src [rows, D] packed [Turing | long | key + current] with rows = n_tur + n_long*long_size^2 + n_cur*cur_size^2;
+ *   long_src [n_long, long_size^2*D]; tur_src [n_tur, D]; frames_src [n_frames, cur_size^2*D].
+ * Saving needs no entry point: between two steps, on the writer's stream, prefix[:rows], long_work[:n_long],
+ * tur_work[:n_tur] and frames[:n_frames] are a consistent state.
+ * The working sets and the frame buffer are copied with cudaMemcpyAsync; the prefix and header words 1-5 by one cooperative
+ * kernel under the writer side of the seqlock (seq odd, copy, fence + grid barrier, counters, seq even), so a reader that
+ * has the bank mapped sees the old prefix or the restored one, never a mix, and seq keeps growing.
+ * Limits: n_long <= max(long_len, chunk_cap), n_tur <= max(tur_len, chunk_cap) (a first clip longer than a memory leaves
+ * that many rows), n_cur <= key_len + cur_len, the prefix rows within fvs_bank_rows' capacity, n_frames <= frames_cap,
+ * step == 0 exactly when n_frames == 0 (and then no memory rows), sources non-null where their count is non-zero.
+ * Validated before anything is enqueued; on FVS_EINVAL nothing was launched and no counter or header changed.
+ * The next fvs_stream_step needs the bank's workspace arrival counters at zero: a workspace that completed a step, or
+ * a zeroed one. */
+int fvs_bank_restore(const fvs_star_config* cfg_h, fvs_bank* bank_h, int32_t n_tur, int32_t n_long, int32_t n_cur,
+                     int64_t n_frames, uint64_t step, const void* prefix_src, const void* long_src, const void* tur_src,
+                     const void* frames_src, fvs_stream_t stream);
 /* prefix pointer (= bank->prefix) and its current row count; pure host arithmetic */
 int fvs_bank_prefix(const fvs_star_config* cfg_h, const fvs_bank* bank_h, void** prefix_out_h, int64_t* rows_out_h);
 /* One clip of `frames` frames into the bank: pooling (encoder tail or pool3) + ONE cooperative kernel doing the weighted
