@@ -130,6 +130,10 @@ SIGNATURES = {
     "fvs_qwen_klarge_workspace_bytes": (_sz, [_i, _i, _i]),
     "fvs_qwen_klarge_retrieve": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _sz, _vp]),
     "fvs_qwen_am_rope": (_i, [_vp, _i, _i, _i, _vp, _i, _i, _i, C.c_int64, _vp, _vp]),
+    # two-tier feature bank of the Qwen2-VL streaming state
+    "fvs_qwen_dam_gather": (_i, [_vp, _i, C.c_int64, _vp, _vp, C.c_int64, _vp, _i, _vp, _i, _vp, _vp, C.c_int64, C.c_int64,
+                                 _i, _vp, _vp, _vp, _vp]),
+    "fvs_host_device_ptr": (_i, [_vp, C.POINTER(_vp)]),
     # publication of the Qwen2-VL streaming memory (seqlock)
     "fvs_qwen_pub_layout": (_i, [_i, _i, _i, _i, _i, _i, _i, _i64p]),
     "fvs_qwen_publish": (_i, [_vp, _sz, _i, _i, C.c_int64, _i, _vp, C.c_int64, _vp, _i, _vp, _i, _i, _i, _i, _i, C.c_uint64,

@@ -201,11 +201,12 @@ def llava(config: dict, counters: dict, prefix, long, tur, frames, rng: Optional
     return StreamCheckpoint(LLAVA, cfg, cnt, tensors, rng=rng)
 
 
-def qwen(config: dict, counters: dict, tensors: dict, pin: Optional[bool] = None) -> StreamCheckpoint:
+def qwen(config: dict, counters: dict, tensors: dict, pin: Optional[bool] = None,
+         owned: Optional[dict] = None) -> StreamCheckpoint:
     """A "qwen2vl-flash" checkpoint; `tensors` as listed in the module docstring (device views are copied asynchronously
-    on the current stream)."""
+    on the current stream).  `owned`: host tensors made for this checkpoint alone, taken without another copy."""
     pin = _pin_default() if pin is None else pin
-    return StreamCheckpoint(QWEN, config, counters, {k: _host(v, pin) for k, v in tensors.items()})
+    return StreamCheckpoint(QWEN, config, counters, {**{k: _host(v, pin) for k, v in tensors.items()}, **(owned or {})})
 
 
 def star_config(cfg) -> dict:

@@ -1,6 +1,7 @@
 """Tensor-level wrappers over the fvs_qwen_* entry points of include/fvs_b200.h (no CPU path; torch = memory + streams)."""
 from __future__ import annotations
 
+import ctypes as C
 from typing import Optional
 
 import torch
@@ -120,6 +121,40 @@ def klarge_retrieve(tem_x: torch.Tensor, klarge_idx: torch.Tensor, bank: torch.T
                                          code, L.ptr(idx), L.ptr(dist), L.ptr(ws), ws.numel(), L.cur_stream()),
             "fvs_qwen_klarge_retrieve")
     return (idx, dist) if want_dist else idx
+
+
+def host_device_ptr(t: torch.Tensor) -> int:
+    """the mapped device address of a pinned host tensor (what a kernel dereferences for a zero-copy read)"""
+    assert not t.is_cuda
+    out = C.c_void_p()
+    L.check(L.load().fvs_host_device_ptr(t.data_ptr(), C.byref(out)), "fvs_host_device_ptr")
+    return out.value
+
+
+def dam_gather(picks: torch.Tensor, n_frames: int, dev_x: Optional[torch.Tensor], dev_merged: Optional[torch.Tensor],
+               n_dev: int, chunks: Optional[torch.Tensor], chunk_frames: int, x_frame_elems: int, merged_frame_elems: int,
+               prev=None, spa_x_out: Optional[torch.Tensor] = None, merged_out: Optional[torch.Tensor] = None,
+               host_fetches: Optional[torch.Tensor] = None):
+    """fvs_qwen_dam_gather: spa_x_out[i] = x[picks[i]], merged_out[i] = merged[picks[i]] over the two-tier bank.
+    dev_x / dev_merged: the device tier (frames [0, n_dev)); chunks: device int64 table of the host chunks' mapped
+    pointers; prev = (picks [m], x [m, ...], merged [m, ...] or None) of the previous step's DAM, or None; host_fetches:
+    device int64 [1] counter.  The outputs are the caller's fresh tensors of the bank's dtype."""
+    _chk_cuda(picks, dev_x, dev_merged, chunks, spa_x_out, merged_out, host_fetches)
+    assert picks.dtype == torch.int64 and (chunks is None or chunks.dtype == torch.int64)
+    out = spa_x_out if spa_x_out is not None else merged_out
+    for t in (spa_x_out, merged_out):
+        assert t is None or (t.is_contiguous() and t.dtype == out.dtype)
+    m, px, pm = 0, None, None
+    if prev is not None and prev[0] is not None and prev[0].numel():
+        pp, px, pm = prev
+        _chk_cuda(pp, px, pm)
+        m = pp.numel()
+    L.check(L.load().fvs_qwen_dam_gather(
+        L.ptr(_c(picks)), picks.numel(), int(n_frames), L.ptr(dev_x), L.ptr(dev_merged), int(n_dev), L.ptr(chunks),
+        int(chunk_frames), L.ptr(None if m == 0 else _c(pp)), m, L.ptr(px), L.ptr(pm), int(x_frame_elems),
+        int(merged_frame_elems), L.dtype_code(out.dtype), L.ptr(spa_x_out), L.ptr(merged_out), L.ptr(host_fetches),
+        L.cur_stream()), "fvs_qwen_dam_gather")
+    return spa_x_out, merged_out
 
 
 def am_rope(spa_positions: torch.Tensor, spa_grid, tem_positions: torch.Tensor, tem_grid, visual_start_id: int,

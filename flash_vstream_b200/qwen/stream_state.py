@@ -26,16 +26,48 @@ list on top of this object.
 """
 from __future__ import annotations
 
+import numbers
 from typing import Optional
 
 import numpy as np
 import torch
 
 from . import compress_functions as CF
-from .. import ops as O
+from . import ops as Q
 from ..draws import GLOBAL, to_device
 
 _KMEANS_METHODS = ("kmeans_ordered", "fast_kmeans_ordered")
+CHUNK_BYTES = 1 << 28     # pinned host memory per chunk of spilled frames (the host allocator rounds up to a power of two)
+
+
+def check_device_frames(v, who: str = "device_frames") -> Optional[int]:
+    """None (every frame of the full-resolution and merged banks stays in HBM) or an integer >= 0; ValueError otherwise"""
+    if v is None:
+        return None
+    if isinstance(v, bool) or not isinstance(v, numbers.Integral) or v < 0:
+        raise ValueError(f"{who} must be an integer >= 0 or None, got {v!r}")
+    return int(v)
+
+
+def chunk_frames(frame_bytes: int, chunk_bytes: int = CHUNK_BYTES) -> int:
+    """frames per host chunk: as many whole frames (x row + merged row) as fit in chunk_bytes, at least one"""
+    return max(1, chunk_bytes // frame_bytes)
+
+
+def placement(n0: int, t: int, device_frames: Optional[int], per_chunk: int):
+    """Where frames [n0, n0 + t) of the two-tier bank go, as (chunk, dst, src, count) spans: chunk -1 is the device tier
+    (dst = frame index), chunk c >= 0 the c-th host chunk (dst = frame within the chunk); src = frame within the clip.
+    Frames below device_frames stay in HBM; frame f >= device_frames is frame f - device_frames of the host tier."""
+    cap = n0 + t if device_frames is None else device_frames
+    k = max(0, min(t, cap - n0))
+    spans = [(-1, n0, 0, k)] if k else []
+    s = k
+    while s < t:
+        c, off = divmod(n0 + s - cap, per_chunk)
+        cnt = min(t - s, per_chunk - off)
+        spans.append((c, off, s, cnt))
+        s += cnt
+    return spans
 
 
 class RowBank:
@@ -62,14 +94,26 @@ class RowBank:
 
 
 class QwenStreamState:
-    """flash: the streaming FlashMemory (temporal_length / spatial_length in frames, methods); merger: PatchMerger."""
+    """flash: the streaming FlashMemory (temporal_length / spatial_length in frames, methods); merger: PatchMerger.
+    device_frames: how many frames of the full-resolution and merged banks stay in HBM (None: all of them).  Later frames
+    are copied to pinned host chunks as they arrive and never move again; a step reads only its retrieved frames from
+    them (fvs_qwen_dam_gather).  The half-resolution bank, which the retrieval sweeps whole, always stays in HBM."""
 
-    def __init__(self, flash, merger):
+    CHUNK_BYTES = CHUNK_BYTES
+
+    def __init__(self, flash, merger, device_frames=None):
         self.flash, self.merger = flash, merger
+        self.device_frames = check_device_frames(device_frames)
         self.reset()
 
     def reset(self):
         self.bank_x, self.bank_small, self.bank_merged = RowBank(), RowBank(), RowBank()
+        self.host_chunks = []                 # pinned chunks of frames >= device_frames: [F x rows | F merged rows]
+        self._chunk_table = None              # device int64: the chunks' mapped device pointers
+        self.n_host = 0                       # frames in the host chunks
+        self._layout = None                   # (dtype, x row shape, merged row shape or None) of a bank frame
+        self._prev_dam = None                 # (spa_positions, spa_x, DAM rows of video_embeds) before the current step
+        self.host_fetches = None              # device int64 [1]: retrieved frames read from the host chunks so far
         self.n_frames = 0
         self.grid = None                      # (h, w) of a full-resolution frame; the half-resolution grid is (hs, ws)
         self.small_grid = None
@@ -96,10 +140,11 @@ class QwenStreamState:
         assert self.grid == (h, w) and self.small_grid == (hs, ws), "Tensors are not equal"   # merge_thw of the reference (:551-555)
         T0, S0 = flash.temporal_length, flash.spatial_length
         # ---- banks (and, once per frame, the merged rows of the frame)
-        bank = self.bank_x.append(x_new.view(t, h * w, D))
+        self._prev_dam = self._dam()
         small_bank = self.bank_small.append(small_new.view(t, hs * ws, D))
-        if S0 > 0 and self.merger is not None:
-            self.bank_merged.append(self.merger(x_new).view(t, h * w // 4, -1))
+        merged = self.merger(x_new).view(t, h * w // 4, -1) if S0 > 0 and self.merger is not None else None
+        self._append_frames(x_new.view(t, h * w, D), merged, dev)
+        bank = self.bank_x.rows() if self.bank_x.n else None
         self.n_frames += t
         # ---- CSM input: carried centroids followed by the clip's half-resolution frames
         T = self.n_tem + t
@@ -157,6 +202,7 @@ class QwenStreamState:
                     GLOBAL.rewind(snap)
                 self.redone_steps += 1
                 self._compress_sync(cand, cand_w, T, d, start_idx, t)
+        self._prev_dam = None                 # the old DAM is the readers' now, not ours to keep alive
         self.steps += 1
         return bank, small_bank
 
@@ -172,28 +218,111 @@ class QwenStreamState:
         h, w = self.grid
         D = tem_x.shape[-1]
         n = self.n_frames
-        bank, small_bank = self.bank_x.rows(), self.bank_small.rows()
+        small_bank = self.bank_small.rows()
+        dt, dev = small_bank.dtype, small_bank.device
         self.tem_x, self.tem_weights, self.tem_timestamp, self.n_tem, self.tem_members = tem_x, tem_w, tem_ts, n_tem, members
         if flash.spatial_length > 0:
             tem_pos = torch.round(tem_ts.float()).to(torch.int64)
-            spa_x, spa_thw, picks = flash.spatial_enhance(
-                x=bank.view(n * h * w, D), small_x=small_bank.view(-1, D), thw=self._thw(n), tem_x=tem_x,
-                tem_thw=self._thw(n_tem, small=True), tem_weights=tem_w, tem_positions=tem_pos, tem_indices=members, draws=d)
-            n_spa = int(spa_thw[0])
+            picks = flash.spatial_picks(small_bank.view(-1, D), n, tem_x, self._thw(n_tem, small=True), tem_w, tem_pos,
+                                        draws=d)
+            n_spa = picks.numel()                                   # min(n, spatial_length): known on the host
         else:
-            spa_x, picks, n_spa = bank[0:0], torch.empty(0, dtype=torch.int64, device=bank.device), 0
+            picks, n_spa = torch.empty(0, dtype=torch.int64, device=dev), 0
+        whole = n_spa == n and self.n_host == 0           # memory still filling: the DAM is the whole bank, a view of it
+        spa_x = self.bank_x.rows() if whole else torch.empty(n_spa, h * w, D, dtype=dt, device=dev)
         self.spa_x, self.spa_positions = spa_x, picks
-        if self.merger is None:
-            self.video_embeds = None
-            return
         pm = h * w // 4                                               # merged tokens of a retrieved frame
-        rows_tem = tem_x.shape[0] // 4
-        out = torch.empty(n_spa * pm + rows_tem, self.merger.dim, dtype=tem_x.dtype, device=tem_x.device)
-        if n_spa:
-            O.gather_rows(self.bank_merged.rows(), picks, out=out[: n_spa * pm].view(n_spa, pm, -1))
-        if rows_tem:
+        out = None
+        if self.merger is not None:
+            out = torch.empty(n_spa * pm + tem_x.shape[0] // 4, self.merger.dim, dtype=tem_x.dtype, device=tem_x.device)
+        # one launch writes the retrieved frames and their merged rows (fresh tensors: readers may hold the old ones)
+        gather_x = n_spa > 0 and not whole
+        gather_m = n_spa > 0 and out is not None
+        if gather_x or gather_m:
+            self._gather(picks, spa_x if gather_x else None, out[: n_spa * pm].view(n_spa, pm, -1) if gather_m else None,
+                         self._prev_dam)
+        if out is not None and out.shape[0] > n_spa * pm:
             self.merger(tem_x, out=out[n_spa * pm:])
         self.video_embeds = out
+
+    # ------------------------------------------------------------------------------------------------ two-tier bank
+    def _dam(self):
+        """the current DAM as a previous-step source for fvs_qwen_dam_gather: (picks, spa_x, DAM rows of video_embeds)"""
+        if self.spa_positions is None or self.spa_positions.numel() == 0 or not self.spa_x.is_cuda:
+            return None
+        m = self.spa_positions.numel()
+        ve = self.video_embeds
+        return self.spa_positions, self.spa_x, None if ve is None else ve[: m * self.spa_x.shape[1] // 4]
+
+    def _per_chunk(self) -> int:
+        dt, xs, ms = self._layout
+        return chunk_frames((xs.numel() + (0 if ms is None else ms.numel())) * dt.itemsize, self.CHUNK_BYTES)
+
+    def _chunk(self, c: int, dev):
+        """views (x rows [F, ...], merged rows [F, ...] or None) of host chunk c, allocated (with its table entry) on first
+        use"""
+        dt, xs, ms = self._layout
+        F, fx, fm = self._per_chunk(), xs.numel(), 0 if ms is None else ms.numel()
+        while len(self.host_chunks) <= c:
+            k = len(self.host_chunks)
+            buf = torch.empty(F * (fx + fm), dtype=dt, pin_memory=True)
+            tab = self._chunk_table
+            if tab is None or tab.numel() <= k:
+                tab = torch.zeros(max(16, 2 * k), dtype=torch.int64, device=dev)
+                if k:
+                    tab[:k].copy_(self._chunk_table[:k])
+                self._chunk_table = tab
+            tab[k].fill_(Q.host_device_ptr(buf))                  # stream-ordered: no host wait
+            self.host_chunks.append(buf)
+        buf = self.host_chunks[c]
+        return buf[: F * fx].view(F, *xs), None if ms is None else buf[F * fx:].view(F, *ms)
+
+    def _append_frames(self, x3, m3, dev):
+        """frames x3 [t, h*w, D] (merged rows m3 [t, h*w/4, merger_dim] or None), on the device or the host, appended to
+        the two-tier bank; copies to the host chunks are asynchronous on the current stream, ordered before any later
+        gather that may read them"""
+        if self._layout is None:
+            self._layout = (x3.dtype, torch.Size(x3.shape[1:]), None if m3 is None else torch.Size(m3.shape[1:]))
+        n0 = self.bank_x.n + self.n_host
+        for c, dst, s, cnt in placement(n0, x3.shape[0], self.device_frames, self._per_chunk()):
+            if c < 0:
+                self.bank_x.append(x3[s: s + cnt].to(dev, non_blocking=True))
+                if m3 is not None:
+                    self.bank_merged.append(m3[s: s + cnt].to(dev, non_blocking=True))
+                continue
+            cx, cm = self._chunk(c, dev)
+            cx[dst: dst + cnt].copy_(x3[s: s + cnt], non_blocking=True)
+            if m3 is not None:
+                cm[dst: dst + cnt].copy_(m3[s: s + cnt], non_blocking=True)
+            self.n_host += cnt
+
+    def _gather(self, picks, spa_x, merged, prev):
+        dt, xs, ms = self._layout
+        if self.host_fetches is None:
+            self.host_fetches = torch.zeros(1, dtype=torch.int64, device=picks.device)
+        Q.dam_gather(picks, self.bank_x.n + self.n_host, self.bank_x.buf if self.bank_x.n else None,
+                     self.bank_merged.buf if self.bank_merged.n else None, self.bank_x.n, self._chunk_table,
+                     self._per_chunk(), xs.numel(), 0 if ms is None else ms.numel(), prev=prev, spa_x_out=spa_x,
+                     merged_out=merged, host_fetches=self.host_fetches)
+
+    def host_fetch_count(self) -> int:
+        """retrieved frames read from the host chunks since the stream started here (synchronises; tests and timing)"""
+        return 0 if self.host_fetches is None else int(self.host_fetches.item())
+
+    def _bank_on_host(self, merged: bool) -> torch.Tensor:
+        """the whole full-resolution (or merged) bank as one pinned host tensor: device rows D2H, chunk rows H2H"""
+        dt, xs, ms = self._layout
+        rb = self.bank_merged if merged else self.bank_x
+        out = torch.empty((self.n_frames,) + tuple(ms if merged else xs), dtype=dt, pin_memory=True)
+        if rb.n:
+            out[: rb.n].copy_(rb.rows(), non_blocking=True)
+        torch.cuda.current_stream().synchronize()                    # the spills of the last steps have landed
+        s, F = rb.n, self._per_chunk()
+        for c in range(len(self.host_chunks)):
+            cnt = min(F, rb.n + self.n_host - s)
+            out[s: s + cnt].copy_(self._chunk(c, None)[int(merged)][:cnt])
+            s += cnt
+        return out
 
     def _compress_sync(self, cand, cand_w, T, d, start_idx, t):
         """every other branch of temporal_compress (:149-183): pass-through while the memory is filling, temporal_length 0,
@@ -223,29 +352,36 @@ class QwenStreamState:
         counters = {"n_frames": n, "steps": self.steps, "n_tem": self.n_tem,
                     "n_spa": 0 if self.spa_positions is None else int(self.spa_positions.numel()),
                     "fast_steps": self.fast_steps, "redone_steps": self.redone_steps,
-                    "merged": int(self.bank_merged.n > 0),
+                    "merged": int(n > 0 and self._layout[2] is not None),
                     "tem_weights_dtype": None if self.tem_weights is None else CK.dtype_name(self.tem_weights.dtype),
                     "tem_timestamp_dtype": "float32" if n == 0 else CK.dtype_name(self.tem_timestamp.dtype)}
         if n == 0:
             return CK.qwen(self._config(0, "float16"), counters, {})
-        x = self.bank_x.rows()
-        tensors = {"bank_x": x, "bank_small": self.bank_small.rows(), "tem_x": self.tem_x,
-                   "tem_timestamp": self.tem_timestamp, "spa_positions": self.spa_positions}
+        small = self.bank_small.rows()
+        tensors = {"bank_small": small, "tem_x": self.tem_x, "tem_timestamp": self.tem_timestamp,
+                   "spa_positions": self.spa_positions}
         if self.tem_weights is not None:          # temporal_method 'sample' keeps no weights
             tensors["tem_weights"] = self.tem_weights
-        if self.bank_merged.n:
-            tensors["bank_merged"] = self.bank_merged.rows()
         if self.merger is not None:
             tensors["video_embeds"] = self.video_embeds
-        with torch.cuda.device(x.device):
-            ck = CK.qwen(self._config(int(x.shape[-1]), CK.dtype_name(x.dtype)), counters, tensors)
+        with torch.cuda.device(small.device):
+            owned = {}                            # spilled banks: assembled in pinned memory here, taken as they are
+            for name, merged in (("bank_x", False), ("bank_merged", True)):
+                if merged and not counters["merged"]:
+                    continue
+                if self.n_host:
+                    owned[name] = self._bank_on_host(merged)
+                else:
+                    tensors[name] = (self.bank_merged if merged else self.bank_x).rows()
+            ck = CK.qwen(self._config(int(small.shape[-1]), CK.dtype_name(small.dtype)), counters, tensors, owned=owned)
             torch.cuda.current_stream().synchronize()
         return ck
 
     @classmethod
-    def restore(cls, ckpt, flash, merger, device) -> "QwenStreamState":
+    def restore(cls, ckpt, flash, merger, device, device_frames=None) -> "QwenStreamState":
         """A state on `device` that continues `ckpt` bit for bit; `flash` / `merger` must have the configuration the
-        checkpoint was taken with (ValueError naming the field otherwise)."""
+        checkpoint was taken with (ValueError naming the field otherwise).  The banks' frames are placed by this state's
+        `device_frames`, whatever the cap of the state that took the checkpoint."""
         from .. import checkpoint as CK
         if ckpt.family != CK.QWEN:
             raise ValueError(f"QwenStreamState.restore: a {ckpt.family!r} checkpoint is not a Qwen2-VL stream's")
@@ -258,16 +394,14 @@ class QwenStreamState:
         if n["n_frames"] and c["merger_dim"] != md:
             raise ValueError(f"QwenStreamState.restore: config.merger_dim of the checkpoint ({c['merger_dim']}) differs "
                              f"from the merger's ({md})")
-        st = cls(flash, merger)
+        st = cls(flash, merger, device_frames)
         if n["n_frames"] == 0:
             return st
         dev = torch.device(device)
         with torch.cuda.device(dev):
             get = lambda k: ckpt.tensor(k).to(dev, non_blocking=True)
-            st.bank_x.append(get("bank_x"))
+            st._append_frames(ckpt.tensor("bank_x"), ckpt.tensor("bank_merged") if n["merged"] else None, dev)
             st.bank_small.append(get("bank_small"))
-            if n["merged"]:
-                st.bank_merged.append(get("bank_merged"))
             st.n_frames, st.steps = n["n_frames"], n["steps"]
             st.fast_steps, st.redone_steps = n["fast_steps"], n["redone_steps"]
             st.grid, st.small_grid = tuple(c["grid"]), tuple(c["small_grid"])
@@ -275,19 +409,24 @@ class QwenStreamState:
             st.tem_weights = get("tem_weights") if "tem_weights" in ckpt.tensors else None
             st.n_tem = n["n_tem"]
             st.spa_positions = get("spa_positions")
-            bank = st.bank_x.rows()
-            st.spa_x = O.gather_rows(bank, st.spa_positions) if n["n_spa"] else bank[0:0]
+            h, w = st.grid
+            st.spa_x = torch.empty(n["n_spa"], h * w, int(c["dim"]), dtype=st._layout[0], device=dev)
+            if n["n_spa"]:
+                st._gather(st.spa_positions, st.spa_x, None, None)
             st.video_embeds = get("video_embeds") if "video_embeds" in ckpt.tensors else None
             torch.cuda.current_stream().synchronize()     # the pinned sources may be freed as soon as this returns
         return st
 
     # ------------------------------------------------------------------------------------------------ the reference's list
     def as_list(self):
-        """the 13 items of `video_embedding_memory` (:620-624); the thw entries are host tensors, everything else lives in HBM"""
+        """the 13 items of `video_embedding_memory` (:620-624); the thw entries are host tensors, everything else lives in HBM.
+        Once frames have spilled to the host chunks, item 7 (the full-resolution bank, which no reader of the list uses) is
+        the zero-row stand-in x[:0]; its thw (item 8) stays exact."""
         n, h, w = self.n_frames, *self.grid
         n_spa = 0 if self.spa_positions is None else int(self.spa_positions.numel())
         ve = self.video_embeds
+        small = self.bank_small.rows().view(-1, self.tem_x.shape[-1])
+        x = self.bank_x.rows().view(n * h * w, -1) if self.n_host == 0 else small[:0]
         return [self.tem_x, self._thw(self.n_tem, small=True), self.tem_weights, self.tem_timestamp,
                 self.spa_x, self._thw(n_spa), self.spa_positions,
-                self.bank_x.rows().view(n * h * w, -1), self._thw(n), self.bank_small.rows().view(-1, self.tem_x.shape[-1]),
-                self._thw(n, small=True), ve, None if ve is None else ve.shape]
+                x, self._thw(n), small, self._thw(n, small=True), ve, None if ve is None else ve.shape]

@@ -151,24 +151,31 @@ class FlashMemory(nn.Module):
         t, h, w = _ints(thw)
         xdim = x.shape[-1]
         bank = x.reshape(t, h * w, xdim)
+        picks = self.spatial_picks(small_x, t, tem_x, tem_thw, tem_weights, tem_positions, draws=draws)
         if t <= self.spatial_length:    # the whole bank fits
-            return bank, _with_t(thw, t), torch.arange(t, device=x.device).long()
+            return bank, _with_t(thw, t), picks
+        return O.gather_rows(bank, picks), _with_t(thw, self.spatial_length), picks
+
+    def spatial_picks(self, small_x, t, tem_x, tem_thw, tem_weights, tem_positions, draws: Optional[dict] = None):
+        """The frame indices spatial_enhance retrieves from a bank of t frames (int64 [min(t, spatial_length)], on
+        small_x's device) without touching the full-resolution bank: a caller that keeps that bank elsewhere gathers
+        the frames itself (stream_state.QwenStreamState)."""
+        dev = small_x.device
+        if t <= self.spatial_length:
+            return torch.arange(t, device=dev).long()
         if self.spatial_method not in _SPATIAL_METHODS:
             raise ValueError(f"spatial_method should be one of {_SPATIAL_METHODS}")
         n = self.spatial_length
         if self.spatial_method == 'sample':
-            picks = torch.linspace(0, t - 1, n).round().long().to(x.device)
-        else:
-            order = (draws or {}).get("weight_order")        # torch.argsort(tem_weights, descending=True) of the reference
-            ranked = O.argsort_desc(tem_weights) if order is None else \
-                torch.as_tensor(order).to(device=x.device, dtype=torch.int64)
-            heaviest = ranked[:n]
-            if self.spatial_method == 'nearest':
-                picks = tem_positions[heaviest]               # index plumbing only
-            else:   # 'klarge_retrieve' (Euclidean distance) / 'klarge_retrieve_cos' (argmin of the cosine similarity, :208-215)
-                picks = self._klarge_retrieve(tem_x.reshape(_ints(tem_thw)[0], -1), heaviest, small_x.reshape(t, -1),
-                                              "cosine" if self.spatial_method == 'klarge_retrieve_cos' else "euclidean")
-        return O.gather_rows(bank, picks), _with_t(thw, n), picks
+            return torch.linspace(0, t - 1, n).round().long().to(dev)
+        order = (draws or {}).get("weight_order")            # torch.argsort(tem_weights, descending=True) of the reference
+        ranked = O.argsort_desc(tem_weights) if order is None else torch.as_tensor(order).to(device=dev, dtype=torch.int64)
+        heaviest = ranked[:n]
+        if self.spatial_method == 'nearest':
+            return tem_positions[heaviest]                    # index plumbing only
+        # 'klarge_retrieve' (Euclidean distance) / 'klarge_retrieve_cos' (argmin of the cosine similarity, :208-215)
+        return self._klarge_retrieve(tem_x.reshape(_ints(tem_thw)[0], -1), heaviest, small_x.reshape(t, -1),
+                                     "cosine" if self.spatial_method == 'klarge_retrieve_cos' else "euclidean")
 
     def _klarge_retrieve(self, centroids, klarge_indices, bank, metric="euclidean"):
         """efficient_euclidean_distance / cosine_similarity + argmin (:197-215, :231-238) in the 16-bit dtype of the

@@ -27,7 +27,7 @@ from ..vstream_arch import _is_manager_proxy
 from . import vstream_qwen2vl_model as _offline
 from .compress_functions import weighted_kmeans_ordered_feature
 from .patch_merger import PatchMerger
-from .stream_state import QwenStreamState
+from .stream_state import QwenStreamState, check_device_frames
 
 
 class FlashMemory(_offline.FlashMemory):
@@ -114,7 +114,22 @@ class VisualB200(nn.Module):
 class RealtimeStreamingMixin:
     """embed_new_video_clip / prepare_realtime_inference / get_video_embedding_memory_cuda_list of
     FlashVStreamQwen2VLModel (:531-640) over a device-resident QwenStreamState (stream_state.py).  The host provides
-    `self.visual` (VisualB200-like: flash_memory, merger, forward_simple_not_merge, get_dtype, get_device)."""
+    `self.visual` (VisualB200-like: flash_memory, merger, forward_simple_not_merge, get_dtype, get_device).
+
+    fvs_bank_device_frames: None (default: every bank frame in HBM) or an integer >= 0 — how many frames of the
+    full-resolution and merged feature banks stay in HBM; later frames go to pinned host memory and a step reads back only
+    the frames it retrieves (DESIGN.md §3.13).  Results are bit-identical either way.  It applies from the next stream
+    (and to load_video_stream); changing it in the middle of a stream raises ValueError."""
+
+    fvs_bank_device_frames = None
+
+    def _bank_device_frames(self):
+        cap = check_device_frames(self.fvs_bank_device_frames, "fvs_bank_device_frames")
+        st = self.__dict__.get("stream_state")
+        if st is not None and st.n_frames > 0 and self.video_embedding_memory and st.device_frames != cap:
+            raise ValueError(f"fvs_bank_device_frames changed from {st.device_frames} to {cap} in the middle of a stream: "
+                             f"it takes effect with the next stream (init_streaming())")
+        return cap
 
     def init_streaming(self):
         self.use_video_streaming_mode = True
@@ -146,6 +161,7 @@ class RealtimeStreamingMixin:
         with the read-back ("temporal_compress" .. "merger" of the reference's meter are one bucket here: time_3..time_6)."""
         time_0 = time.perf_counter()
         assert self.use_video_streaming_mode
+        cap = self._bank_device_frames()
         grid_host = video_grid_thw.cpu()          # the grid stays on the host: every shape below comes from it (a CUDA grid
         t, h, w = (int(v) for v in grid_host.reshape(-1, 3)[0].tolist())   # costs one sync here, a host grid none)
         pixel_values_videos = pixel_values_videos.type(self.visual.get_dtype()).to(self.visual.get_device(), non_blocking=True)
@@ -160,7 +176,7 @@ class RealtimeStreamingMixin:
             x_new = small_new = feats
         pub = self.__dict__.get("_qwen_publication")              # set by qwen.serve.export_qwen_memory (opt-in)
         if self.stream_state is None or not self.video_embedding_memory:
-            self.stream_state = QwenStreamState(self.visual.flash_memory, self.visual.merger)
+            self.stream_state = QwenStreamState(self.visual.flash_memory, self.visual.merger, device_frames=cap)
             if pub is not None:
                 pub.new_stream()
         time_3 = time.perf_counter()
@@ -196,7 +212,9 @@ class RealtimeStreamingMixin:
                 (tuple(ckpt.config["grid"]), tuple(ckpt.config["small_grid"])) != (pub.grid, pub.small_grid):
             raise ValueError(f"load_video_stream: config.grid {ckpt.config['grid']} / {ckpt.config['small_grid']} is not "
                              f"the exported grid {pub.grid} / {pub.small_grid}")
-        state = QwenStreamState.restore(ckpt, self.visual.flash_memory, self.visual.merger, self.visual.get_device())
+        cap = check_device_frames(self.fvs_bank_device_frames, "fvs_bank_device_frames")
+        state = QwenStreamState.restore(ckpt, self.visual.flash_memory, self.visual.merger, self.visual.get_device(),
+                                        device_frames=cap)
         if state.n_frames == 0:
             self.stream_state = None
             self._publish([])

@@ -452,6 +452,26 @@ int fvs_qwen_klarge_retrieve(const void* tem_x, const int64_t* klarge_idx, const
 int fvs_qwen_am_rope(const int64_t* spa_positions, int spa_t, int spa_h, int spa_w, const int64_t* tem_positions, int tem_t,
                      int tem_h, int tem_w, int64_t visual_start_id, int64_t* out, fvs_stream_t stream);
 
+/* ---- two-tier feature bank of the Qwen2-VL streaming state (DESIGN.md §3.13) --------------------------------------------
+ * Frames [0, n_dev) of the full-resolution bank (x, x_frame_elems 16-bit elements per frame) and of the PatchMerger bank
+ * (merged, merged_frame_elems per frame) are contiguous device rows dev_x / dev_merged.  Frames [n_dev, n_frames) live in
+ * pinned host chunks: chunk c holds frames n_dev + c*chunk_frames + [0, chunk_frames) as [chunk_frames x rows |
+ * chunk_frames merged rows]; host_chunks is a DEVICE table of the chunks' mapped device pointers (fvs_host_device_ptr).
+ *
+ * fvs_qwen_dam_gather: one launch writes, for every pick i (picks: device int64 [n], e.g. fvs_qwen_klarge_retrieve's
+ * output), spa_x_out[i] = x[picks[i]] and merged_out[i] = merged[picks[i]] (either output may be NULL; not both).  Each
+ * pick is read from the first source that has it: the device tier; the previous step's DAM (prev_picks [m], prev_x
+ * [m, x_frame_elems], prev_merged [m, merged_frame_elems] — HBM rows that already hold those frames); the host chunk, as
+ * zero-copy 16-byte loads.  *host_fetches (device, optional) grows by the number of picks read from the host.  A pick
+ * outside [0, n_frames) yields zero rows.  The outputs must not alias any source.  Row tensors 16-byte aligned, frame
+ * sizes multiples of 16 bytes, n <= 65535.  FVS_EINVAL with nothing launched on a bad argument. */
+int fvs_qwen_dam_gather(const int64_t* picks, int n, int64_t n_frames, const void* dev_x, const void* dev_merged,
+                        int64_t n_dev, const void* const* host_chunks, int chunk_frames, const int64_t* prev_picks, int m,
+                        const void* prev_x, const void* prev_merged, int64_t x_frame_elems, int64_t merged_frame_elems,
+                        int dtype, void* spa_x_out, void* merged_out, uint64_t* host_fetches, fvs_stream_t stream);
+/* *dev_out = the device address of pinned host memory `host` (cudaHostGetDevicePointer); FVS_EINVAL if it is not pinned */
+int fvs_host_device_ptr(const void* host, void** dev_out);
+
 /* ---- publication of the Qwen2-VL streaming memory for readers in other processes / on other GPUs ----------------------
  * One device allocation (so one CUDA IPC handle) of fvs_qwen_pub_layout(...) bytes:
  *   header        8 x uint64 {seq, epoch, clips, n_frames, n_tem, n_spa, rows, grid}: seq is odd while a publish is writing
