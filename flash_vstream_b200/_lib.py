@@ -51,7 +51,8 @@ class NtmWeights(C.Structure):   # fvs_ntm_weights
 class Bank(C.Structure):         # fvs_bank
     _fields_ = [("prefix", C.c_void_p), ("long_work", C.c_void_p), ("tur_work", C.c_void_p), ("frames", C.c_void_p),
                 ("header", C.c_void_p), ("frames_cap", C.c_int64), ("chunk_cap", C.c_int32), ("n_long", C.c_int32),
-                ("n_tur", C.c_int32), ("n_cur", C.c_int32), ("n_frames", C.c_int64), ("step", C.c_uint64)]
+                ("n_tur", C.c_int32), ("n_cur", C.c_int32), ("n_frames", C.c_int64), ("step", C.c_uint64),
+                ("frames_window", C.c_int64)]
 
 
 class StreamJob(C.Structure):    # fvs_stream_job

@@ -191,14 +191,16 @@ class StreamCheckpoint:
 
 # ---------------------------------------------------------------------------------------------------- builders
 def llava(config: dict, counters: dict, prefix, long, tur, frames, rng: Optional[dict] = None,
-          pin: Optional[bool] = None) -> StreamCheckpoint:
+          pin: Optional[bool] = None, owned: Optional[dict] = None) -> StreamCheckpoint:
     """A "llava-star" checkpoint from a bank's views (device or host; device sources are copied asynchronously on the
-    current stream — synchronise it before reading the tensors)."""
+    current stream — synchronise it before reading the tensors).  `owned`: host tensors made for this checkpoint alone,
+    taken without another copy (their views above are then None)."""
     pin = _pin_default() if pin is None else pin
     cfg = {k: config[k] for k in STAR_FIELDS}
     cnt = {k: int(counters[k]) for k in LLAVA_COUNTERS}
-    tensors = {"prefix": _host(prefix, pin), "long": _host(long, pin), "tur": _host(tur, pin), "frames": _host(frames, pin)}
-    return StreamCheckpoint(LLAVA, cfg, cnt, tensors, rng=rng)
+    views = {"prefix": prefix, "long": long, "tur": tur, "frames": frames}
+    tensors = {k: _host(v, pin) for k, v in views.items() if v is not None}
+    return StreamCheckpoint(LLAVA, cfg, cnt, {**tensors, **(owned or {})}, rng=rng)
 
 
 def qwen(config: dict, counters: dict, tensors: dict, pin: Optional[bool] = None,

@@ -84,7 +84,19 @@ struct StepArgs {
   int* info_out;               // {exit_step, refills, converged, kmeans_ran}
   long long* key_idx_out;      // [kl]
   unsigned int* done_ctr;
+  // ---- device window of the frame buffer (fvs_bank.frames_window; read by the tiered kernel only)
+  long long clip_first;        // global index of this clip's first frame
+  long long window;            // frames [0, window) stay in `frames`; 0: uncapped
 };
+
+// Row of `frames` that holds global frame g of the clip starting at frame clip_first, in a bank whose device window is
+// `window` frames (0: uncapped, the row is g).  Frames below the window are at their own index; the clip's frames at or
+// past it follow the window in order, in the chunk_cap-row slot — so a clip's rows are contiguous whether it lies below
+// the window, straddles it or lies past it.  The pooled tail writes through it (prepare_job) and the write-back reads the
+// current frames through it.
+__host__ __device__ __forceinline__ long long frame_row(long long g, long long clip_first, long long window) {
+  return (window == 0 || g < window) ? g : window + g - (clip_first > window ? clip_first : window);
+}
 
 // ---------------------------------------------------------------------------------------------------- group barrier
 // Barrier among a GROUP of co-resident blocks (the launch is cooperative, so spinning is safe): a monotonic arrival counter,
@@ -144,7 +156,8 @@ __device__ void abstract_group(const StepArgs& A, int gb, int ng) {
 // One cooperative launch (a "wave") advances up to kJobs banks.  Job j owns the contiguous blocks [first[j], first[j+1]):
 // its Lloyd-loop blocks, then its abstract-memory blocks.  Every barrier of a job counts that job's blocks only, so no
 // stream waits for another, and every phase is a stride loop over independent units of mem_device.cuh, so a bank's bits do
-// not depend on how many blocks its job gets.  fvs_stream_step is the one-job wave (kJobs = 1).
+// not depend on how many blocks its job gets.  fvs_stream_step is the one-job wave (kJobs = 1).  kTier: some job of the
+// wave has a device window (the current frames are read through frame_row); uncapped waves run the kTier = false code.
 template <int kJobs>
 struct Wave {
   int n;
@@ -152,7 +165,7 @@ struct Wave {
   StepArgs job[kJobs];
 };
 
-template <int kJobs>
+template <int kJobs, bool kTier>
 __global__ void __launch_bounds__(kThreads, 1) consolidate_kernel(const __grid_constant__ Wave<kJobs> W) {
   int j = 0;
   if constexpr (kJobs > 1)
@@ -305,7 +318,10 @@ __global__ void __launch_bounds__(kThreads, 1) consolidate_kernel(const __grid_c
         pre[i] = long_src[i - n1];
       } else if (i < n3) {
         const size_t r = (i - n2) / vA, c = (i - n2) % vA;
-        const long long row = r < size_t(kl) ? s_idx[r] : A.n_frames_after - A.cur_start + (long long)(r - kl);
+        long long row = r < size_t(kl) ? s_idx[r] : A.n_frames_after - A.cur_start + (long long)(r - kl);
+        if constexpr (kTier) {   // key rows are below the window (s_idx < T <= long_work_rows <= window): unmapped
+          if (r >= size_t(kl)) row = frame_row(row, A.clip_first, A.window);
+        }
         pre[i] = fr[size_t(row) * vA + c];
       } else if (i < n4) {
         reinterpret_cast<uint4*>(A.LW)[i - n3] = long_src[i - n3];
@@ -435,6 +451,17 @@ int check_config(const fvs_star_config* c, const char* who) {
   return FVS_OK;
 }
 
+// A bank's device window (fvs_bank.frames_window): 0, or at least the long working set's rows (every key frame index is
+// a row of it) with room for one clip's slot behind it.
+int check_window(const fvs_bank* bank, int64_t lrows, const char* who) {
+  const int64_t N = bank->frames_window;
+  FVS_REQUIRE(N == 0 || N >= lrows, "%s: frames_window %lld < %lld, the long working set's rows (max(long_len, chunk_cap) + "
+              "chunk_cap): key frames are read from below the window", who, (long long)N, (long long)lrows);
+  FVS_REQUIRE(N == 0 || N + bank->chunk_cap <= bank->frames_cap, "%s: frames_cap %lld < frames_window %lld + chunk_cap %d",
+              who, (long long)bank->frames_cap, (long long)N, bank->chunk_cap);
+  return FVS_OK;
+}
+
 constexpr int kWaveJobs = 32;   // jobs per cooperative launch (the per-job kernel arguments travel as kernel parameters)
 
 // One job of a step, validated: its kernel arguments, its pooling destination and the blocks it wants.
@@ -452,20 +479,24 @@ int prepare_job(const fvs_star_config* cfg, const fvs_stream_job& job, const cha
   FVS_REQUIRE(bank->prefix && bank->long_work && bank->tur_work && bank->frames && bank->header, "%s: bank buffers missing", who);
   const int t = job.frames;
   FVS_REQUIRE(t > 0 && t <= bank->chunk_cap, "%s: %d frames per call, bank was sized for <= %d", who, t, bank->chunk_cap);
-  FVS_REQUIRE(bank->n_frames + t <= bank->frames_cap, "%s: frame buffer full (%lld + %d > %lld): grow it first", who,
-              (long long)bank->n_frames, t, (long long)bank->frames_cap);
+  int64_t lrows, trows, prows;
+  fvs_bank_rows(cfg, bank->chunk_cap, &lrows, &trows, &prows);
+  int r = check_window(bank, lrows, who);
+  if (r) return r;
+  const int64_t row0 = frame_row(bank->n_frames, bank->n_frames, bank->frames_window);   // the clip's first row in `frames`
+  FVS_REQUIRE(row0 + t <= bank->frames_cap, "%s: frame buffer full (%lld + %d > %lld): grow it first", who,
+              (long long)row0, t, (long long)bank->frames_cap);
   const Carve w = carve(*cfg, bank->chunk_cap, job.workspace);
   FVS_REQUIRE(job.workspace_bytes >= w.total, "%s: workspace too small (%zu < %zu)", who, job.workspace_bytes, w.total);
   const int D = cfg->D, a = cfg->cur_size, b = cfg->long_size;
   const size_t PDa = size_t(a) * a * D, PDl = size_t(b) * b * D;
   const bool has_memory = bank->step > 0;
   const int n_long_old = has_memory ? bank->n_long : 0, n_tur_old = has_memory ? bank->n_tur : 0;
-  int64_t lrows, trows, prows;
-  fvs_bank_rows(cfg, bank->chunk_cap, &lrows, &trows, &prows);
   FVS_REQUIRE(n_long_old + t <= lrows && n_tur_old + t <= trows, "%s: working set overflow", who);
 
-  // pooled levels of this clip -> frame buffer / long working set / Turing working set
-  P.dst.a = static_cast<uint16_t*>(bank->frames) + size_t(bank->n_frames) * PDa;
+  // pooled levels of this clip -> frame buffer (its rows are contiguous there, see frame_row) / long working set / Turing
+  // working set
+  P.dst.a = static_cast<uint16_t*>(bank->frames) + size_t(row0) * PDa;
   P.dst.b = static_cast<uint16_t*>(bank->long_work) + size_t(n_long_old) * PDl;
   P.dst.c = static_cast<uint16_t*>(bank->tur_work) + size_t(n_tur_old) * D;
   P.dst.frames = t;
@@ -512,6 +543,8 @@ int prepare_job(const fvs_star_config* cfg, const fvs_stream_job& job, const cha
   A.C[0] = w.C[0]; A.C[1] = w.C[1]; A.normpart = w.normpart; A.wsum = w.wsum; A.dist = w.dist;
   A.Mbuf[0] = w.Mbuf[0]; A.Mbuf[1] = w.Mbuf[1]; A.labels_out = w.labels; A.info_out = w.info; A.key_idx_out = w.key_idx;
   A.done_ctr = w.done_ctr;
+  A.clip_first = bank->n_frames;
+  A.window = bank->frames_window;
   A.km_ctr = w.done_ctr + 1;
   A.abs_ctr = w.done_ctr + 2;
   A.job_ctr = w.done_ctr + 3;
@@ -585,10 +618,13 @@ int plan_waves(const JobPrep* P, int n, int budget, const char* api, int* km_out
 int device_budget(int* out) {
   static int cap = 0;
   if (cap == 0) {
-    int p1 = 0, pn = 0;
-    FVS_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&p1, consolidate_kernel<1>, kThreads, 0));
-    FVS_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&pn, consolidate_kernel<kWaveJobs>, kThreads, 0));
-    const int per_sm = p1 < pn ? p1 : pn;
+    int p[4] = {0, 0, 0, 0};
+    FVS_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&p[0], consolidate_kernel<1, false>, kThreads, 0));
+    FVS_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&p[1], consolidate_kernel<kWaveJobs, false>, kThreads, 0));
+    FVS_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&p[2], consolidate_kernel<1, true>, kThreads, 0));
+    FVS_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&p[3], consolidate_kernel<kWaveJobs, true>, kThreads, 0));
+    int per_sm = p[0];
+    for (int i = 1; i < 4; ++i) per_sm = p[i] < per_sm ? p[i] : per_sm;
     const int co = (per_sm > 0 ? per_sm : 1) * device_sm_count();
     cap = device_sm_count() < co ? device_sm_count() : co;
   }
@@ -622,14 +658,16 @@ int launch_wave(const JobPrep* P, int n, const int* km, const int* ab, cudaStrea
   Wave<kJobs> W;
   W.n = n;
   W.first[0] = 0;
+  bool tier = false;
   for (int i = 0; i < n; ++i) {
     W.job[i] = P[i].A;
     W.job[i].n_abs_blocks = ab[i];
     W.first[i + 1] = W.first[i] + km[i] + ab[i];
+    tier = tier || P[i].A.window > 0;
   }
   void* args[] = {&W};
-  FVS_CUDA_OK(cudaLaunchCooperativeKernel((const void*)consolidate_kernel<kJobs>, dim3(W.first[n]), dim3(kThreads), args, 0,
-                                          stream));
+  const void* fn = tier ? (const void*)consolidate_kernel<kJobs, true> : (const void*)consolidate_kernel<kJobs, false>;
+  FVS_CUDA_OK(cudaLaunchCooperativeKernel(fn, dim3(W.first[n]), dim3(kThreads), args, 0, stream));
   FVS_CHECK_LAUNCH("consolidate_kernel");
   return FVS_OK;
 }
@@ -749,8 +787,12 @@ int fvs_bank_restore(const fvs_star_config* cfg, fvs_bank* bank, int32_t n_tur, 
   const int a2 = cfg->cur_size * cfg->cur_size, b2 = cfg->long_size * cfg->long_size;
   const int64_t rows = int64_t(n_tur) + int64_t(n_long) * b2 + int64_t(n_cur) * a2;
   FVS_REQUIRE(rows <= prows, "%s: prefix of %lld rows exceeds the buffer (%lld)", api, (long long)rows, (long long)prows);
-  FVS_REQUIRE(n_frames >= 0 && n_frames <= bank->frames_cap, "%s: %lld frames > frames_cap %lld: grow the frame buffer first",
-              api, (long long)n_frames, (long long)bank->frames_cap);
+  if ((r = check_window(bank, lrows, api))) return r;
+  const int64_t window = bank->frames_window;
+  FVS_REQUIRE(n_frames >= 0 && (window > 0 || n_frames <= bank->frames_cap),
+              "%s: %lld frames > frames_cap %lld: grow the frame buffer first", api, (long long)n_frames,
+              (long long)bank->frames_cap);
+  const int64_t dev_frames = window > 0 && n_frames > window ? window : n_frames;   // the rest stays with the caller
   FVS_REQUIRE((step == 0) == (n_frames == 0), "%s: step %llu with %lld frames (step is 0 exactly when no frame was seen)", api,
               (unsigned long long)step, (long long)n_frames);
   FVS_REQUIRE(step > 0 || (n_tur == 0 && n_long == 0 && n_cur == 0), "%s: a state at step 0 holds no memory rows", api);
@@ -779,7 +821,7 @@ int fvs_bank_restore(const fvs_star_config* cfg, fvs_bank* bank, int32_t n_tur, 
   const size_t D = size_t(cfg->D);
   if (n_long) FVS_CUDA_OK(cudaMemcpyAsync(bank->long_work, long_src, size_t(n_long) * b2 * D * 2, cudaMemcpyDefault, s));
   if (n_tur) FVS_CUDA_OK(cudaMemcpyAsync(bank->tur_work, tur_src, size_t(n_tur) * D * 2, cudaMemcpyDefault, s));
-  if (n_frames) FVS_CUDA_OK(cudaMemcpyAsync(bank->frames, frames_src, size_t(n_frames) * a2 * D * 2, cudaMemcpyDefault, s));
+  if (dev_frames) FVS_CUDA_OK(cudaMemcpyAsync(bank->frames, frames_src, size_t(dev_frames) * a2 * D * 2, cudaMemcpyDefault, s));
 
   static int per_sm = 0;
   if (per_sm == 0) FVS_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, restore_kernel, 256, 0));

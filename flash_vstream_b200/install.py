@@ -33,6 +33,7 @@ def install():
         patched.append(f"VStreamMetaForCausalLM.{name}")
     Ref.fvs_tie_order = Mine.fvs_tie_order
     Ref.fvs_fused_stream, Ref.fvs_chunk_cap = Mine.fvs_fused_stream, Mine.fvs_chunk_cap
+    Ref.fvs_bank_device_frames = Mine.fvs_bank_device_frames
     from . import multimodal_projector as my_proj
     ref_proj = importlib.import_module("flash_vstream.model.multimodal_projector.builder")
     ref_proj.build_vision_projector = my_proj.build_vision_projector

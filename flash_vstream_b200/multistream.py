@@ -34,9 +34,12 @@ class StreamPool:
     [t,3,S,S] or [1,t,3,S,S] for a model with a ViT engine, or finished features [t, grid*grid, D] f16; t <= chunk_cap);
     `prefix(sid)` / `state(sid)` are views of the stream's bank; `bank(sid)` is the ops.StreamBank itself (hand it to
     serve.export_bank / MemoryReader).  `close(sid)` resets the bank and keeps it for the next `open`.  Configs the
-    fused streaming step does not cover raise NotImplementedError: stream them through the model's single-stream path."""
+    fused streaming step does not cover raise NotImplementedError: stream them through the model's single-stream path.
+    `device_frames` (ops.StreamBank): every bank of the pool keeps only that many frames of its frame buffer in HBM, the
+    later ones in pinned host memory, so a stream's HBM stays what it was when the bank was made."""
 
-    def __init__(self, model, *, chunk_cap: int = 1, max_streams: Optional[int] = None):
+    def __init__(self, model, *, chunk_cap: int = 1, max_streams: Optional[int] = None,
+                 device_frames: Optional[int] = None):
         host = model.get_model()
         ntm = host.attention_model
         D = ntm.q_proj.weight.shape[1]
@@ -57,6 +60,7 @@ class StreamPool:
         if self.device.type != "cuda":
             raise ops.L.FvsError("StreamPool needs the model on a CUDA device (no CPU fallback)")
         self.chunk_cap = int(chunk_cap)
+        self.device_frames = ops.device_window(self.cfg, self.chunk_cap, device_frames)
         self.max_streams = max_streams
         self._streams: dict[int, _Stream] = {}
         self._free: list[ops.StreamBank] = []
@@ -72,7 +76,8 @@ class StreamPool:
             raise RuntimeError(f"StreamPool is full ({self.max_streams} streams)")
         if checkpoint is not None and checkpoint.rng is None and seed is None:
             raise ValueError("StreamPool.open: this checkpoint carries no draw source (single-stream model): pass seed=")
-        bank = self._free.pop() if self._free else ops.StreamBank(self.cfg, self.ntm, chunk_cap=self.chunk_cap, device=self.device)
+        bank = self._free.pop() if self._free else ops.StreamBank(self.cfg, self.ntm, chunk_cap=self.chunk_cap, device=self.device,
+                                                                  device_frames=self.device_frames)
         if checkpoint is None:
             bank.reset()
         else:

@@ -9,6 +9,7 @@ from typing import Optional
 import torch
 
 from . import _lib as L
+from . import host_tier as HT
 
 
 def _chk_cuda(*ts):
@@ -305,6 +306,32 @@ def gather_rows(src: torch.Tensor, idx: torch.Tensor, out: Optional[torch.Tensor
 
 
 # --------------------------------------------------------------------------------------------- streaming step on a bank
+def star_config(cfg) -> "L.StarConfig":
+    """the L.StarConfig of a dict of the reference's STAR knobs (an L.StarConfig passes through)"""
+    if isinstance(cfg, L.StarConfig):
+        return cfg
+    return L.StarConfig(int(cfg["D"]), int(cfg["grid"]), int(cfg["cur_size"]), int(cfg["long_size"]), int(cfg["long_len"]),
+                        int(cfg["tur_len"]), int(cfg["cur_len"]), int(cfg.get("key_len", 3)), int(cfg["ntm_dim"]),
+                        float(cfg["ratio"]))
+
+
+def min_device_frames(cfg, chunk_cap: int) -> int:
+    """the smallest device_frames of a bank with this STAR config (dict or L.StarConfig) and chunk_cap: the long working
+    set's rows of fvs_bank_rows, max(long_len, chunk_cap) + chunk_cap — a key frame is frames[i] for such a row i"""
+    lw = C.c_int64()
+    L.check(L.load().fvs_bank_rows(C.byref(star_config(cfg)), int(chunk_cap), C.byref(lw), None, None), "fvs_bank_rows")
+    return lw.value
+
+
+def device_window(cfg, chunk_cap: int, device_frames, who: str = "device_frames") -> Optional[int]:
+    """device_frames validated for a bank of this config: None or an integer >= min_device_frames; ValueError otherwise"""
+    v = HT.check_device_frames(device_frames, who)
+    if v is not None and v < (m := min_device_frames(cfg, chunk_cap)):
+        raise ValueError(f"{who} {v} < {m}: a LLaVA bank keeps at least its long working set's rows (max(long_len, "
+                         f"chunk_cap) + chunk_cap) of frames in HBM, since every key frame is read from there")
+    return v
+
+
 class StreamBank:
     """One stream's persistent Flash memory on the GPU (fvs_bank + fvs_stream_step, include/fvs_b200.h): the state of
     embed_video_streaming (vstream_arch.py:611-697) — [cur, long, Turing, frame buffer] — lives in caller-owned device
@@ -312,33 +339,43 @@ class StreamBank:
     `self.prefix()` — a view, never a concatenation.  All shapes of a step are host-known, so nothing here synchronises.
 
     cfg: dict with the reference's knobs (D, grid, cur_size, long_size, long_len, tur_len, cur_len, key_len, ntm_dim,
-    ratio); ntm: (q_w, q_b, k_w, k_b) f16 CUDA tensors of NeuralTuringMachine.q_proj / k_proj."""
+    ratio); ntm: (q_w, q_b, k_w, k_b) f16 CUDA tensors of NeuralTuringMachine.q_proj / k_proj.
 
-    def __init__(self, cfg: dict, ntm, *, chunk_cap: int = 32, frames_cap: int = 256, device="cuda"):
+    device_frames: None (default: the whole frame buffer in HBM, grown as needed) or N >= min_device_frames(): frames
+    [0, N) stay in `frames`, which also holds a slot of chunk_cap rows for the clip's frames at or past N and never grows;
+    after each step those frames are copied (asynchronously, on the step's stream) to pinned host chunks.  A step reads
+    only key frames (below N) and the clip's own frames, so the bank's bits do not depend on the cap (DESIGN.md §3.14)."""
+
+    CHUNK_BYTES = 1 << 25     # pinned host memory per chunk: 256 frames (4 minutes at 1 fps) of the default 8x8x1024 level
+
+    def __init__(self, cfg: dict, ntm, *, chunk_cap: int = 32, frames_cap: int = 256, device="cuda",
+                 device_frames: Optional[int] = None):
         self.lib = L.load()
         self.device = torch.device(device)
         if self.device.type != "cuda":
             raise L.FvsError("StreamBank needs a CUDA device (no CPU fallback)")
-        self.cfg = L.StarConfig(int(cfg["D"]), int(cfg["grid"]), int(cfg["cur_size"]), int(cfg["long_size"]),
-                                int(cfg["long_len"]), int(cfg["tur_len"]), int(cfg["cur_len"]), int(cfg.get("key_len", 3)),
-                                int(cfg["ntm_dim"]), float(cfg["ratio"]))
+        self.cfg = star_config(cfg)
         self.D, self.pa, self.pb = self.cfg.D, self.cfg.cur_size ** 2, self.cfg.long_size ** 2
         self.chunk_cap = int(chunk_cap)
         lw, tw, pr = C.c_int64(), C.c_int64(), C.c_int64()
         L.check(self.lib.fvs_bank_rows(C.byref(self.cfg), self.chunk_cap, C.byref(lw), C.byref(tw), C.byref(pr)), "fvs_bank_rows")
+        self.device_frames = device_window(self.cfg, self.chunk_cap, device_frames)
         f16 = torch.float16
+        rows = max(int(frames_cap), 2 * self.chunk_cap) if self.device_frames is None else self.device_frames + self.chunk_cap
         with torch.cuda.device(self.device):
             self.prefix_buf = torch.zeros(pr.value, self.D, dtype=f16, device=self.device)
             self.long_work = torch.zeros(lw.value, self.pb, self.D, dtype=f16, device=self.device)
             self.tur_work = torch.zeros(tw.value, 1, self.D, dtype=f16, device=self.device)
-            self.frames = torch.empty(max(int(frames_cap), 2 * self.chunk_cap), self.pa, self.D, dtype=f16, device=self.device)
+            self.frames = torch.empty(rows, self.pa, self.D, dtype=f16, device=self.device)
             self.header = torch.zeros(8, dtype=torch.int64, device=self.device)
             self.ws = torch.empty(self.lib.fvs_stream_workspace_bytes(C.byref(self.cfg), self.chunk_cap), dtype=torch.uint8,
                                   device=self.device)
         self._ntm_keep = [t.detach().to(device=self.device, dtype=f16).contiguous() for t in ntm] if ntm is not None else None
         self.ntm = L.NtmWeights(*[t.data_ptr() for t in self._ntm_keep]) if ntm is not None else None
         self.bank = L.Bank(self.prefix_buf.data_ptr(), self.long_work.data_ptr(), self.tur_work.data_ptr(),
-                           self.frames.data_ptr(), self.header.data_ptr(), self.frames.shape[0], self.chunk_cap, 0, 0, 0, 0, 0)
+                           self.frames.data_ptr(), self.header.data_ptr(), self.frames.shape[0], self.chunk_cap, 0, 0, 0, 0, 0,
+                           self.device_frames or 0)
+        self.host_chunks: list = []      # pinned [per_chunk, a*a, D] chunks of frames >= device_frames
 
     # ---- state as the reference sees it (views of the bank) ---------------------------------------------------------
     @property
@@ -355,19 +392,68 @@ class StreamBank:
 
     def state(self):
         """(cur [n_cur, a*a, D], long [n_long, b*b, D], Turing [n_tur, 1, D], frame buffer [n, a*a, D]) — views in the order
-        of `video_embedding_memory` (vstream_arch.py:694)"""
+        of `video_embedding_memory` (vstream_arch.py:694).  Once frames have left HBM (device_frames), the frame buffer is
+        the zero-row stand-in frames[:0], as the Manager-list publication sends it; frame_buffer() builds the whole one."""
         b = self.bank
         o1 = b.n_tur
         o2 = o1 + b.n_long * self.pb
         tur = self.prefix_buf[:o1].view(b.n_tur, 1, self.D)
         lng = self.prefix_buf[o1:o2].view(b.n_long, self.pb, self.D)
         cur = self.prefix_buf[o2:o2 + b.n_cur * self.pa].view(b.n_cur, self.pa, self.D)
-        return cur, lng, tur, self.frames[:b.n_frames]
+        return cur, lng, tur, self.frames[:0] if self.n_host() else self.frames[:b.n_frames]
+
+    def n_host(self) -> int:
+        """frames of the stream kept in the host chunks (those at or past device_frames)"""
+        return 0 if self.device_frames is None else max(0, self.bank.n_frames - self.device_frames)
+
+    def frame_buffer(self) -> torch.Tensor:
+        """the whole frame buffer [n_frames, a*a, D] (img_feature_buffer): the device view frames[:n_frames] while every
+        frame is in HBM, else built in pinned host memory — device rows D2H, host chunks H2H (synchronises the current
+        stream, so the spills of the last steps have landed)"""
+        n, nh = self.bank.n_frames, self.n_host()
+        if nh == 0:
+            return self.frames[:n]
+        N, F = self.device_frames, self._per_chunk()
+        out = torch.empty(n, self.pa, self.D, dtype=self.frames.dtype, pin_memory=True)
+        with torch.cuda.device(self.device):
+            out[:N].copy_(self.frames[:N], non_blocking=True)
+            torch.cuda.current_stream().synchronize()
+        for c in range((nh + F - 1) // F):
+            cnt = min(F, nh - c * F)
+            out[N + c * F:N + c * F + cnt].copy_(self.host_chunks[c][:cnt])
+        return out
 
     def reset(self):
         L.check(self.lib.fvs_bank_reset(C.byref(self.bank), L.cur_stream()), "fvs_bank_reset")
+        self.host_chunks = []
+
+    # ---- host tier (device_frames) -------------------------------------------------------------------------------------
+    def _per_chunk(self) -> int:
+        return HT.chunk_frames(self.pa * self.D * self.frames.element_size(), self.CHUNK_BYTES)
+
+    def _chunk(self, c: int) -> torch.Tensor:
+        """pinned host chunk c [per_chunk, a*a, D], allocated on first use"""
+        while len(self.host_chunks) <= c:
+            self.host_chunks.append(torch.empty(self._per_chunk(), self.pa, self.D, dtype=self.frames.dtype, pin_memory=True))
+        return self.host_chunks[c]
+
+    def _spill(self, n0: int, t: int) -> int:
+        """after the step of frames [n0, n0 + t): copy those at or past device_frames from the slot to the host chunks,
+        asynchronously on the current stream (ahead of the next step, which overwrites the slot).  The clip's frames are
+        contiguous in `frames` from row min(n0, device_frames) (frame_row, csrc/stream_kernels.cu).  Returns the bytes."""
+        if self.device_frames is None:
+            return 0
+        row0, nbytes = min(n0, self.device_frames), 0
+        for c, dst, s, cnt in HT.placement(n0, t, self.device_frames, self._per_chunk()):
+            if c >= 0:
+                src = self.frames[row0 + s:row0 + s + cnt]
+                self._chunk(c)[dst:dst + cnt].copy_(src, non_blocking=True)
+                nbytes += src.numel() * src.element_size()
+        return nbytes
 
     def _reserve_frames(self, t: int):
+        if self.device_frames is not None:    # fixed at creation: frames [0, N) and one clip's slot
+            return
         if self.bank.n_frames + t > self.frames.shape[0]:   # geometric growth of img_feature_buffer (device-resident)
             new = torch.empty(2 * (self.bank.n_frames + t), self.pa, self.D, dtype=self.frames.dtype, device=self.device)
             new[:self.bank.n_frames].copy_(self.frames[:self.bank.n_frames])
@@ -384,14 +470,18 @@ class StreamBank:
         b = self.bank
         counters = dict(n_tur=b.n_tur, n_long=b.n_long, n_cur=b.n_cur, n_frames=b.n_frames, step=b.step)
         with torch.cuda.device(self.device):
+            spilled = self.n_host() > 0     # frame_buffer() is then a pinned host tensor made for this checkpoint alone
+            frames = self.frame_buffer()
             ck = CK.llava(CK.star_config(self.cfg), counters, self.prefix(), self.long_work[:b.n_long],
-                          self.tur_work[:b.n_tur], self.frames[:b.n_frames], rng=rng)
+                          self.tur_work[:b.n_tur], None if spilled else frames, rng=rng,
+                          owned={"frames": frames} if spilled else None)
             torch.cuda.current_stream().synchronize()
         return ck
 
     def restore(self, ckpt):
-        """Continue the stream of `ckpt` in this bank (any device, any chunk_cap whose capacities hold it): same STAR
-        config or ValueError; the frame buffer grows as needed.  One fvs_bank_restore: the working sets and frames by copy
+        """Continue the stream of `ckpt` in this bank (any device, any chunk_cap whose capacities hold it, any
+        device_frames): same STAR config or ValueError; the frame buffer grows as needed, or, with device_frames, frames
+        [0, N) go to HBM and the rest to the host chunks.  One fvs_bank_restore: the working sets and frames by copy
         engine, the prefix and header under the seqlock, so readers that have this bank mapped never see a mix."""
         from . import checkpoint as CK
         CK.check_star(ckpt, self.cfg, "StreamBank.restore")
@@ -406,6 +496,11 @@ class StreamBank:
             L.check(self.lib.fvs_bank_restore(C.byref(self.cfg), C.byref(self.bank), n["n_tur"], n["n_long"], n["n_cur"],
                                               n["n_frames"], n["step"], *[t.data_ptr() if t.numel() else None for t in srcs],
                                               L.cur_stream()), "fvs_bank_restore")
+            self.host_chunks = []
+            frames, N = srcs[3], self.device_frames
+            for c, dst, s, cnt in HT.placement(0, n["n_frames"], N, self._per_chunk()):   # frames >= N: to the host tier
+                if c >= 0:
+                    self._chunk(c)[dst:dst + cnt].copy_(frames[s:s + cnt], non_blocking=True)
             self.ws.zero_()       # the step's arrival counters start at zero (a fresh bank's workspace is uninitialised)
             torch.cuda.current_stream().synchronize()    # the sources may be freed as soon as this returns
         self._last_T = 0
@@ -416,10 +511,11 @@ class StreamBank:
                              "reader its tensors (flash_vstream_b200.serve.export_bank)")
         c = self.cfg
         return {"cfg": {n: getattr(c, n) for n, _ in c._fields_}, "ntm": self._ntm_keep, "chunk_cap": self.chunk_cap,
-                "frames_cap": self.frames.shape[0], "device": str(self.device)}
+                "frames_cap": self.frames.shape[0], "device": str(self.device), "device_frames": self.device_frames}
 
     def __setstate__(self, st):
-        self.__init__(st["cfg"], st["ntm"], chunk_cap=st["chunk_cap"], frames_cap=st["frames_cap"], device=st["device"])
+        self.__init__(st["cfg"], st["ntm"], chunk_cap=st["chunk_cap"], frames_cap=st["frames_cap"], device=st["device"],
+                      device_frames=st.get("device_frames"))
 
     def needs_draws(self, t: int) -> bool:
         """does a step of t frames run the k-means (working set > long_len)?"""
@@ -502,10 +598,12 @@ def stream_step_many(banks, inputs, *, vit: Optional[VitEncoder] = None, draws=N
     else:
         kind, vh, vws, vwsn = L.INPUT_FEATURES, None, None, 0
     last_T = [bank.working_rows(inputs[i].shape[0]) for i, bank in enumerate(banks)]
+    first = [bank.bank.n_frames for bank in banks]
     L.check(b0.lib.fvs_stream_step_multi(C.byref(b0.cfg), jobs, len(banks), vh, L.ptr(inp), kind, vws, vwsn, int(max_blocks),
                                          L.cur_stream()), "fvs_stream_step_multi")
-    for bank, T in zip(banks, last_T):
+    for bank, T, n0, x in zip(banks, last_T, first, inputs):
         bank._last_T = T
+        bank._spill(n0, x.shape[0])     # frames past device_frames: slot -> host chunks, behind the step on this stream
 
 
 def bank_snapshot(prefix_buf: torch.Tensor, header: torch.Tensor, cur_size: int, long_size: int, out: Optional[torch.Tensor] = None,

@@ -23,6 +23,7 @@ from typing import List, Optional
 import torch
 import torch.nn as nn
 
+from . import host_tier as HT
 from . import ops
 from .compress_functions import (attention_feature, drop_feature, k_drop_feature, k_merge_feature, kmeans_draws,
                                  kmeans_feature, merge_feature, weighted_kmeans_device, weighted_kmeans_feature)
@@ -69,6 +70,8 @@ class VStreamMetaForCausalLM:
     fvs_fused_stream = True   # streaming steps run as fvs_stream_step on a persistent bank (ops.StreamBank) when the config
     #                           allows it; False = the op-by-op path below (same arithmetic, bit-identical state)
     fvs_chunk_cap = 32        # frames per embed_video_streaming call the bank is sized for (grown on demand)
+    fvs_bank_device_frames = None   # None: the bank's whole frame buffer in HBM; N: only frames [0, N) (N >= the long
+    #                                 working set's rows), later ones in pinned host memory (ops.StreamBank device_frames)
 
     # ---------------------------------------------------------------------------------------------- encoder
     def get_vision_tower(self):
@@ -264,12 +267,20 @@ class VStreamMetaForCausalLM:
     def _get_bank(self, cfg, t, device):
         bank = self.__dict__.get("_fvs_bank")
         key = tuple(sorted(cfg.items()))
-        if bank is None or self.__dict__.get("_fvs_bank_key") != key or bank.device != device or t > bank.chunk_cap:
-            if bank is not None and bank.steps > 0 and len(self.video_embedding_memory or []) > 0:
+        cap = HT.check_device_frames(self.fvs_bank_device_frames, "fvs_bank_device_frames")
+        mid_stream = bank is not None and bank.steps > 0 and len(self.video_embedding_memory or []) > 0
+        if mid_stream and cap != bank.device_frames:
+            raise ValueError(f"fvs_bank_device_frames changed from {bank.device_frames} to {cap} in the middle of a stream: "
+                             f"reset_video_stream() first, or save_video_stream() / load_video_stream() to move it")
+        if bank is None or self.__dict__.get("_fvs_bank_key") != key or bank.device != device or t > bank.chunk_cap or \
+                bank.device_frames != cap:
+            if mid_stream:
                 return None     # mid-stream change of shape: finish this stream op by op
             m = self.get_model().attention_model
             ntm = (m.q_proj.weight, m.q_proj.bias, m.k_proj.weight, m.k_proj.bias)
-            bank = ops.StreamBank(cfg, ntm, chunk_cap=max(int(self.fvs_chunk_cap), t), device=device)
+            chunk_cap = max(int(self.fvs_chunk_cap), t)
+            bank = ops.StreamBank(cfg, ntm, chunk_cap=chunk_cap, device=device,
+                                  device_frames=ops.device_window(cfg, chunk_cap, cap, "fvs_bank_device_frames"))
             self.__dict__["_fvs_bank"], self.__dict__["_fvs_bank_key"] = bank, key
         return bank
 
@@ -344,6 +355,11 @@ class VStreamMetaForCausalLM:
             bank = self._get_bank(cfg, image_features.shape[0], image_features.device) if cfg is not None else None
             if bank is not None and self._stream_step_fused(bank, image_features, None, draws):
                 return []
+        if self.fvs_bank_device_frames is not None:   # the op-by-op path keeps its own, device-resident frame buffer
+            knob = (self._fused_reject(s, g, image_features.shape[2], image_features.dtype) if image_features.is_cuda
+                    else "device") or "fvs_chunk_cap"
+            raise NotImplementedError(f"fvs_bank_device_frames bounds the frame buffer of the fused streaming step, and this "
+                                      f"stream runs op by op ({knob}): unset fvs_bank_device_frames or change {knob}")
         fused = ('mean' in (getattr(self.config, "compress_type", None) or '') and s.tur_size == 1
                  and g % s.compress_size == 0 and s.compress_size % s.long_size == 0 and g != s.compress_size
                  and s.long_size != s.compress_size and s.compress_size ** 2 <= 64 and image_features.shape[2] % 64 == 0

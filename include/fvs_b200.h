@@ -211,7 +211,12 @@ int fvs_gather_rows(const void* src, const int64_t* idx, void* out, int n, int64
  *   long_work  [long_work_rows, long_size^2 * D] — rows [0, n_long) = the long memory, then the incoming clip's rows
  *              (the k-means working set of vstream_arch.py:677-678 is built in place);
  *   tur_work   [tur_work_rows, D] — same for the abstract (Turing) memory (:690);
- *   frames     [frames_cap, cur_size^2 * D] — img_feature_buffer (:650,:676), appended in place; the caller grows it;
+ *   frames     [frames_cap, cur_size^2 * D] — img_feature_buffer (:650,:676), appended in place; the caller grows it.
+ *              With a device window (frames_window = N > 0) it holds only frames [0, N) plus a slot of chunk_cap rows
+ *              [N, N + chunk_cap) that receives the current clip's frames at or past N, in order, so frames_cap must be at
+ *              least N + chunk_cap and never grows.  A step reads only frames below N (key frames: frames[i] for a row i of
+ *              the long working set, so N must be >= fvs_bank_rows' long_work_rows) and the current clip's own frames, so
+ *              the caller may copy the slot's rows elsewhere (host memory) after the step and before the next one;
  *   header     8 x uint64 {seq, n_tur, n_long, n_cur, n_frames, step, 0, 0}: seq is odd while a step is writing the
  *              prefix, even otherwise — readers in other processes / on other GPUs (CUDA IPC) use fvs_bank_snapshot.
  * fvs_bank_rows gives the row capacities for a given maximum clip length (chunk_cap frames per call).
@@ -241,6 +246,8 @@ typedef struct fvs_bank {
   int32_t n_long, n_tur, n_cur;   /* host counters, maintained by the library */
   int64_t n_frames;
   uint64_t step;
+  int64_t frames_window; /* 0: `frames` holds every frame; N > 0: only frames [0, N) stay there, a clip's frames at or past
+                            N land in the slot [N, N + chunk_cap) (see `frames` above) */
 } fvs_bank;
 
 #define FVS_INPUT_PIXELS 0     /* input = [frames, 3, image, image] pixels; encoded with `vit`, pooled in the encoder's tail */
@@ -261,8 +268,9 @@ int fvs_bank_reset(fvs_bank* bank_h, fvs_stream_t stream);
  * kernel under the writer side of the seqlock (seq odd, copy, fence + grid barrier, counters, seq even), so a reader that
  * has the bank mapped sees the old prefix or the restored one, never a mix, and seq keeps growing.
  * Limits: n_long <= max(long_len, chunk_cap), n_tur <= max(tur_len, chunk_cap) (a first clip longer than a memory leaves
- * that many rows), n_cur <= key_len + cur_len, the prefix rows within fvs_bank_rows' capacity, n_frames <= frames_cap,
- * step == 0 exactly when n_frames == 0 (and then no memory rows), sources non-null where their count is non-zero.
+ * that many rows), n_cur <= key_len + cur_len, the prefix rows within fvs_bank_rows' capacity, n_frames <= frames_cap
+ * (with a device window N: any n_frames; only frames_src's first min(n_frames, N) rows are copied, the caller keeps the
+ * rest), step == 0 exactly when n_frames == 0 (and then no memory rows), sources non-null where their count is non-zero.
  * Validated before anything is enqueued; on FVS_EINVAL nothing was launched and no counter or header changed.
  * The next fvs_stream_step needs the bank's workspace arrival counters at zero: a workspace that completed a step, or
  * a zeroed one. */
