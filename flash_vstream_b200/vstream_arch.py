@@ -374,6 +374,10 @@ class VStreamMetaForCausalLM:
                 self.compress_spatial_features(image_feature, s.tur_size)
         cur_start = min(s.cur_len, image_feature.shape[0])
         cur_memory = image_feature[:0] if cur_start == 0 else image_feature[-cur_start:]
+        if s.long_len == 0:
+            # no long memory and no key retrieval from the first call on, as on the fused path and behind the guard of the
+            # offline path (:256-257); the reference's streaming branch has none (a K = 0 k-means on its second call)
+            long_new = long_new[:0]
         mem = self.video_embedding_memory
         first = mem is None or len(mem) == 0
         if first:
@@ -387,9 +391,12 @@ class VStreamMetaForCausalLM:
             old_long, old_tur = old_long.to(image_feature.device), old_tur.to(image_feature.device)
             assert old_long.shape[1:] == long_new.shape[1:]
             long_memory = torch.cat((old_long, long_new), dim=0)
-            long_c, min_indices, _, _ = self._compress_long(long_memory, s, draws, streaming=True)
-            key_memory = ops.gather_rows(buf, min_indices)   # global buffer, working-set indices (quirk of :687-688)
-            cur_memory = torch.cat([key_memory, cur_memory], dim=0)
+            if s.long_len == 0:
+                long_c = long_memory
+            else:
+                long_c, min_indices, _, _ = self._compress_long(long_memory, s, draws, streaming=True)
+                key_memory = ops.gather_rows(buf, min_indices)   # global buffer, working-set indices (quirk of :687-688)
+                cur_memory = torch.cat([key_memory, cur_memory], dim=0)
             Turing_memory = torch.cat((old_tur, tur_new), dim=0)
             tur_c, _ = attention_feature(Turing_memory, s.tur_len, self.attention, update_ratio=s.ratio)
         self._publish([cur_memory, long_c, tur_c, buf])

@@ -148,11 +148,16 @@ def spatial_pool3(feat: np.ndarray, a: int = 8, b: int = 4):
 # weighted k-means — model/compress_functions.py:130-169
 # ----------------------------------------------------------------------------------------------------------------
 def weighted_kmeans(X: np.ndarray, weights: Optional[np.ndarray], init_idx: Sequence[int], refill_idx: Sequence[int],
-                    K: int, max_iter: int = 10, tol: float = 1e-4):
+                    K: int, max_iter: int = 10, tol: float = 1e-4, *, trace: Optional[list] = None,
+                    chunk: Optional[int] = None):
     """Inner Lloyd loop `weighted_kmeans_torch` (compress_functions.py:133-157) on f16 data.
     X [T, PD] f16; weights [T] f16 or None (ones, :131-132); init_idx = randperm(T)[:K] (:134);
     refill_idx = the successive random.randint(0, T-1) draws (:152).
-    Returns (centroids [K,PD] f16, labels [T] int64, weights_sum [K] f16, exit_step i, refills_consumed)."""
+    Returns (centroids [K,PD] f16, labels [T] int64, weights_sum [K] f16, exit_step i, refills_consumed).
+    trace: a list that gets one dict per iteration — it, diff (the f16 value compared with tol), stop (the loop broke
+    there), empty (clusters refilled, in j order), refills (rows consumed), dist_inf / dist_nan (some distance was inf /
+    NaN), c_inf / c_nan (some new centroid element was).  chunk: rows per distance batch (memory only, same bits);
+    None keeps each batch's [rows, K, PD] fp32 terms near 64 MiB, at most 64 rows."""
     assert X.dtype == F16 and X.ndim == 2 and X.shape[1] % SLICE == 0
     T, PD = X.shape
     w = np.ones(T, F16) if weights is None else weights.astype(F16)
@@ -162,18 +167,21 @@ def weighted_kmeans(X: np.ndarray, weights: Optional[np.ndarray], init_idx: Sequ
     labels = np.zeros(T, np.int64)
     wsum = np.zeros(K, F16)
     it = 0
+    rows = chunk if chunk is not None else max(1, min(64, (1 << 24) // max(1, K * PD)))
     for it in range(max_iter):
         # dists = ((X[:,None] - C[None])**2).sum(2).sqrt()                                       (:138)
         dist = np.empty((T, K), F32)
-        for t0 in range(0, T, 64):                                    # chunked only to bound memory
-            terms = _sqdiff_f16(X[t0:t0 + 64, None, :], C[None, :, :])  # [t, K, PD]
+        for t0 in range(0, T, rows):                                  # chunked only to bound memory
+            terms = _sqdiff_f16(X[t0:t0 + rows, None, :], C[None, :, :])  # [t, K, PD]
             part = _slice_sum(terms)                                  # [t, K, S]
+            del terms
             tot = _seq_sum(part, -1).astype(F16)                      # f16(sum)
-            dist[t0:t0 + 64] = np.sqrt(tot.astype(F32)).astype(F16).astype(F32)
+            dist[t0:t0 + rows] = np.sqrt(tot.astype(F32)).astype(F16).astype(F32)
         labels = argmin_first_nan(dist, axis=1)                                                   # (:141)
         # weighted centroid update                                                               (:142-149)
         newC = np.empty_like(C)
         n_empty = 0
+        empty = []
         for j in range(K):
             members = np.nonzero(labels == j)[0]
             ws = F32(0)
@@ -189,11 +197,17 @@ def weighted_kmeans(X: np.ndarray, weights: Optional[np.ndarray], init_idx: Sequ
             else:                                                      # fix nan centroids          (:150-152)
                 newC[j] = X[int(refill_idx[pos + n_empty])]
                 n_empty += 1
+                empty.append(j)
         pos += n_empty
         # diff = torch.norm(C - newC, dim=1).sum()                                               (:153)
         d = (C.astype(F32) - newC.astype(F32)).astype(F16).astype(F32)
         nrm = np.sqrt(_seq_sum(_slice_sum(d * d), -1)).astype(F16)     # squares are NOT rounded to f16 by norm
         diff = F32(_seq_sum(nrm.astype(F32)[None, :], -1)[0].astype(F16))
+        if trace is not None:
+            nc = newC.astype(F32)
+            trace.append(dict(it=it, diff=float(diff), stop=bool(diff < tol_h), empty=empty, refills=n_empty,
+                              dist_inf=bool(np.isinf(dist).any()), dist_nan=bool(np.isnan(dist).any()),
+                              c_inf=bool(np.isinf(nc).any()), c_nan=bool(np.isnan(nc).any())))
         if diff < tol_h:                                                                          # (:154-155)
             break                                                      # centroids stay the OLD ones
         C = newC                                                                                  # (:156)
@@ -206,15 +220,19 @@ def step_indices_from_labels(labels: np.ndarray, K: int):
 
 
 def weighted_kmeans_feature(img_feature: np.ndarray, video_max_frames: int, weights=None, *, init_idx=None,
-                            refill_idx=None):
-    """compress_functions.py:130-169 incl. the T <= T0 pass-through (:160-161).  RNG draws are explicit inputs."""
+                            refill_idx=None, trace: Optional[list] = None, result: Optional[dict] = None):
+    """compress_functions.py:130-169 incl. the T <= T0 pass-through (:160-161).  RNG draws are explicit inputs.
+    trace: passed to weighted_kmeans; result: a dict that gets labels, exit_step and refills of the Lloyd loop."""
     T, P, D = img_feature.shape
     T0 = video_max_frames
     if weights is None:
         weights = np.ones(T, img_feature.dtype)
     if T <= T0:
         return img_feature, weights, [[[i] for i in range(T)]]
-    C, labels, wsum, _, _ = weighted_kmeans(img_feature.reshape(T, P * D), weights, init_idx, refill_idx, T0)
+    C, labels, wsum, it, used = weighted_kmeans(img_feature.reshape(T, P * D), weights, init_idx, refill_idx, T0,
+                                                trace=trace)
+    if result is not None:
+        result.update(labels=labels, exit_step=it, refills=used)
     return C.reshape(T0, P, D), wsum, step_indices_from_labels(labels, T0)
 
 
@@ -341,29 +359,52 @@ class StreamState:
 
 
 def stream_step(state: StreamState, feat_a: np.ndarray, cfg: StarConfig, ntm, *, init_idx=None, refill_idx=None,
-                order=None):
+                order=None, trace: Optional[list] = None):
     """One embed_video_streaming call after the encoder: feat_a [t, cur_size^2, D] f16 is the clip's pooled ViT
-    output (already `.to(float16)`, :649).  Mutates and returns `state`; returns a debug dict too."""
+    output (already `.to(float16)`, :649).  Mutates and returns `state`; returns a debug dict too.
+
+    long_len == 0 switches the long memory and the key retrieval off from the first call on, behind the guard of the
+    offline path (compress_temporal_features, :256-257); the reference's streaming branch has no such guard (its first
+    call publishes the clip's long rows, its second runs a k-means with K = 0 and raises).
+
+    trace: a list that gets one dict per call — T (long working-set rows), K, S (1024-element slices of a long row), kl
+    (key frames retrieved), kmeans (whether the Lloyd loop ran), chunks (rows of each abstract-memory chunk folded in) and
+    iters (the weighted_kmeans trace of the call)."""
     t = feat_a.shape[0]
     cur_start = min(cfg.cur_len, t)                                                       # :652
     cur = feat_a[:0] if cur_start == 0 else feat_a[-cur_start:]                           # :653-656
     long_new = spatial_pool(feat_a, cfg.long_size) if cfg.long_size ** 2 != feat_a.shape[1] else feat_a  # :659-660
     tur_new = spatial_pool(feat_a, cfg.tur_size) if cfg.tur_size ** 2 != feat_a.shape[1] else feat_a     # :661-662
+    if cfg.long_len == 0:
+        long_new = long_new[:0]
     dbg = {}
+    S = long_new.shape[1] * long_new.shape[2] // SLICE
     if state.buf is None:                                                                 # first call: :669-672 skipped
         state.cur, state.long, state.tur, state.buf = cur, long_new, tur_new, feat_a
+        if trace is not None:
+            trace.append(dict(T=long_new.shape[0], K=cfg.long_len, S=S, kl=0, kmeans=False, chunks=[], iters=[]))
         return state, dbg
     buf = np.concatenate([state.buf, feat_a], axis=0)                                     # :676
     L = np.concatenate([state.long, long_new], axis=0)                                    # :678
-    long_c, weight, _ = weighted_kmeans_feature(L, cfg.long_len, init_idx=init_idx, refill_idx=refill_idx)  # :679
-    if order is None:
-        order = argsort_desc_stable(weight)                                               # :681
-    idx = key_retrieve(L, order, cfg.key_length)                                          # :682-687
+    iters, res = [], {}
+    if cfg.long_len == 0:
+        long_c, idx = L, np.zeros(0, np.int64)
+    else:
+        long_c, weight, _ = weighted_kmeans_feature(L, cfg.long_len, init_idx=init_idx, refill_idx=refill_idx,
+                                                    trace=iters, result=res)              # :679
+        if order is None:
+            order = argsort_desc_stable(weight)                                           # :681
+        idx = key_retrieve(L, order, cfg.key_length)                                      # :682-687
+        dbg.update(weight=np.asarray(weight), order=np.asarray(order))
     key = buf[idx]                                    # global buffer indexed by working-set indices (:688, quirk)
     cur = np.concatenate([key, cur], axis=0)                                              # :689
     Tm = np.concatenate([state.tur, tur_new], axis=0)                                     # :690
     tur_c, _ = attention_feature(Tm, cfg.tur_len, ntm, cfg.update_ratio)                  # :691
-    dbg.update(weight=np.asarray(weight), order=np.asarray(order), key_idx=idx)
+    dbg.update(key_idx=idx, **res)
+    if trace is not None:
+        T1 = cfg.tur_len
+        chunks = [min(T1, Tm.shape[0] - i) for i in range(T1, Tm.shape[0], T1)] if Tm.shape[0] > T1 else []
+        trace.append(dict(T=L.shape[0], K=cfg.long_len, S=S, kl=len(idx), kmeans=bool(res), chunks=chunks, iters=iters))
     state.cur, state.long, state.tur, state.buf = cur, long_c, tur_c, buf                 # :693-695
     return state, dbg
 
