@@ -7,4 +7,5 @@ from .patch_merger import PatchMerger  # noqa: F401
 from .vstream_qwen2vl_model import (FlashMemory, get_real_grid_thw, get_real_grid_thws,  # noqa: F401
                                     get_spatial_real_grid_thw)
 from .stream_state import QwenStreamState  # noqa: F401
+from .multistream import QwenStreamPool  # noqa: F401
 from . import vstream_qwen2vl_realtime  # noqa: F401

@@ -13,15 +13,16 @@ import numpy as np
 import torch
 
 from . import ops as Q
-from ..draws import GLOBAL, to_device
+from ..draws import GLOBAL, DrawSource, to_device
 
 MAX_ITER = 10   # compress_functions.py:203 (max_iter=10)
 TOL = 1e-4      # compress_functions.py:203 (tol=1e-4)
 
 
 def weighted_kmeans_ordered_feature(img_feature: torch.Tensor, video_max_frames: int, weights: Optional[torch.Tensor] = None,
-                                    times=None, *, init_idx=None, refill_idx=None, order=None):
-    """compress_functions.py:181-298.  img_feature [T, P, D] (f16 / bf16 / f32, CUDA).  Returns
+                                    times=None, *, init_idx=None, refill_idx=None, order=None, source: DrawSource = GLOBAL):
+    """compress_functions.py:181-298.  img_feature [T, P, D] (f16 / bf16 / f32, CUDA); `source`: where the default draws
+    come from.  Returns
     (sorted_reduced_feature [T0, P, D] in the input dtype, sorted_weights fp32 [T0], centroids_timestamp fp32 [T0],
     sorted_step_indices) — or, like the reference, the 3-tuple (img_feature.float(), weights, [[[0], [1], ...]]) when
     T <= T0 (:265-266).  `order` replays the reference's (unstable) torch.argsort(centroids_timestamp) permutation; the
@@ -48,10 +49,10 @@ def weighted_kmeans_ordered_feature(img_feature: torch.Tensor, video_max_frames:
     else:
         K = T0
         if init_idx is None:
-            init_idx = GLOBAL.randperm(U, dev)[:K]                      # :218
+            init_idx = source.randperm(U, dev)[:K]                      # :218
         init_idx = torch.as_tensor(init_idx).to(device=dev, dtype=torch.int32)
         if refill_idx is None:
-            refill_dev, _ = GLOBAL.refill_candidates(T, MAX_ITER * K, dev)    # :258, drawn ahead
+            refill_dev, _ = source.refill_candidates(T, MAX_ITER * K, dev)    # :258, drawn ahead
         else:
             refill = list(int(v) for v in refill_idx)
             refill_dev = to_device(refill + [0] * (MAX_ITER * K - len(refill)), np.int32, dev)
@@ -60,7 +61,7 @@ def weighted_kmeans_ordered_feature(img_feature: torch.Tensor, video_max_frames:
         info_h = info.cpu().tolist()
         exit_step = info_h[0]
         if refill_idx is None:                                          # leave `random` where the reference would
-            GLOBAL.consume(T, info_h[1])
+            source.consume(T, info_h[1])
     step_indices = [[] for _ in range(K)]
     for j, l in enumerate(lab):                                         # :274-277
         step_indices[l].append(j)

@@ -1,0 +1,273 @@
+"""Many Qwen2-VL video streams on one GPU: `QwenStreamPool`, the Qwen2-VL counterpart of multistream.StreamPool
+(DESIGN.md §3.15).
+
+One `step` is one round over the listed streams, each with one clip:
+  1. every clip is validated before anything is enqueued;
+  2. temporal_pool builds each clip's half-resolution rows;
+  3. ONE fvs_qwen_vit_encode call (QwenVisionBlocksB200) encodes all clips: the segments of one (h, w) form one grid entry
+     whose t is their sum, so each resolution gets one attention launch.  A round that needs more than 16 grid entries or
+     more than `TOWER_ROWS` rows is split into several calls (plan_tower_calls);
+  4. ONE PatchMerger call merges every stream's new full-resolution frames;
+  5. each stream's memory step is enqueued (QwenStreamState.enqueue), the round waits ONCE for all their read-backs, and
+     each stream is completed (QwenStreamState.complete).
+
+Exact by construction: the tower is invariant to batch composition (§3.7) and the merger is row-wise (§3.5), so a pool
+stream gets the bits it gets alone through QwenStreamState with the same draws, however the round is composed or split.
+
+RNG: each stream owns a `draws.DrawSource` seeded by `open(seed)` (contract in draws.py), so a stream draws what the
+single-stream path draws after `torch.manual_seed(seed); random.seed(seed)` and never touches the global generators.
+"""
+from __future__ import annotations
+
+import os
+from typing import Optional
+
+import torch
+
+from .. import _lib as L
+from ..draws import DrawSource
+from .stream_state import _KMEANS_METHODS, QwenStreamState, check_device_frames
+from .vision_tower import QwenVisionBlocksB200
+
+MAX_GRIDS = 16            # grid entries one fvs_qwen_vit_encode call takes
+PATCH_DIM = 3 * 2 * 14 * 14
+
+
+def plan_tower_calls(clips, max_rows: int, max_grids: int = MAX_GRIDS):
+    """clips: per clip, its segments [(t, h, w), ...].  -> one (grids, places) per tower call: grids = [(t, h, w)] with
+    every (h, w) of the call once and t summed over its segments; places = [(clip index, [first output row of each of its
+    segments])].  Clips are taken in the order of their grids, so clips of one resolution share calls; a call takes
+    clips while it stays within `max_grids` entries and `max_rows` rows (a clip larger than `max_rows` goes alone)."""
+    order = sorted(range(len(clips)), key=lambda i: [(h, w) for _, h, w in clips[i]])
+    calls, cur, keys, rows = [], [], set(), 0
+    for i in order:
+        ck = {(h, w) for _, h, w in clips[i]}
+        n = sum(t * h * w for t, h, w in clips[i])
+        if cur and (len(keys | ck) > max_grids or rows + n > max_rows):
+            calls.append(cur)
+            cur, keys, rows = [], set(), 0
+        cur.append(i)
+        keys |= ck
+        rows += n
+    if cur:
+        calls.append(cur)
+    return [_call_layout(clips, members) for members in calls]
+
+
+def _call_layout(clips, members):
+    tsum = {}                                             # (h, w) -> summed t, in first-seen order
+    for i in members:
+        for t, h, w in clips[i]:
+            tsum[(h, w)] = tsum.get((h, w), 0) + t
+    base, r = {}, 0
+    for (h, w), t in tsum.items():
+        base[(h, w)] = r
+        r += t * h * w
+    places = []
+    for i in members:
+        offs = []
+        for t, h, w in clips[i]:
+            offs.append(base[(h, w)])
+            base[(h, w)] += t * h * w
+        places.append((i, offs))
+    return [(t, h, w) for (h, w), t in tsum.items()], places
+
+
+class _Stream:
+    """one pool stream; it has what qwen.serve.export_qwen_memory reads of a host (visual, stream_state), so it can be
+    exported like one"""
+
+    def __init__(self, visual, state: QwenStreamState):
+        self.visual, self.stream_state = visual, state
+
+
+class QwenStreamPool:
+    """A pool of Qwen2-VL streams sharing one realtime host's vision side (visual: VisualB200 with a QwenVisionBlocksB200
+    tower, its FlashMemory config and PatchMerger).
+
+    `open(seed)` -> sid; `step({sid: (pixel_values_videos, video_grid_thw), ...})` advances the listed streams by one clip
+    each (what the Qwen2-VL processor returns: patch rows [t*h*w, 1176] and one (t, h, w) grid); `state(sid)` is the
+    stream's QwenStreamState, `as_list(sid)` its 13-item list; `stream(sid)` can be handed to qwen.serve.export_qwen_memory.
+    `checkpoint(sid)` / `open(checkpoint=)` suspend and resume a stream; `close(sid)` drops it.  Configs and towers the
+    batched round does not cover raise NotImplementedError naming the knob: stream them through the host's single-stream
+    path.  `device_frames` applies to every stream, as `fvs_bank_device_frames` does to the host's stream (DESIGN.md
+    §3.13).  TOWER_ROWS bounds the rows of one tower call (its workspace is about 30 KB per row at 1280 wide)."""
+
+    TOWER_ROWS = 65536
+
+    def __init__(self, model, device_frames: Optional[int] = None, max_streams: Optional[int] = None):
+        visual = model.visual
+        flash, tower = visual.flash_memory, visual.encode_patches
+        if not isinstance(tower, QwenVisionBlocksB200):
+            raise NotImplementedError("QwenStreamPool: visual.encode_patches is not a QwenVisionBlocksB200 tower, which the "
+                                      "batched round encodes through; stream this host through its single-stream path")
+        if flash.temporal_method not in _KMEANS_METHODS:
+            raise NotImplementedError(f"QwenStreamPool: flash_memory_temporal_method={flash.temporal_method!r} is outside "
+                                      f"what the batched round covers ({', '.join(_KMEANS_METHODS)}); stream it through "
+                                      f"the host's single-stream path")
+        if flash.temporal_poolsize != 2:
+            raise NotImplementedError(f"QwenStreamPool: flash_memory_temporal_poolsize={flash.temporal_poolsize} is outside "
+                                      f"what the batched round covers (2); stream it through the host's single-stream path")
+        self.device = torch.device(visual.get_device())
+        if self.device.type != "cuda":
+            raise L.FvsError("QwenStreamPool needs the vision side on a CUDA device (no CPU fallback)")
+        if self.device.index is None:
+            self.device = torch.device("cuda", torch.cuda.current_device())
+        self.visual, self.flash, self.merger, self.tower = visual, flash, visual.merger, tower
+        self.device_frames = check_device_frames(device_frames, "device_frames")
+        self.max_streams = max_streams
+        self._streams: dict[int, _Stream] = {}
+        self._next = 0
+
+    # ---- streams -------------------------------------------------------------------------------------------------------
+    def open(self, seed: Optional[int] = None, *, checkpoint=None) -> int:
+        """A new stream -> its sid.  With `checkpoint` (of `checkpoint(sid)`, from this pool or another, on any device, or
+        of a host's save_video_stream()), the stream continues where the checkpoint left it: its state and, when the
+        checkpoint carries them, its generators.  A checkpoint without them (from the single-stream host, whose draws come
+        from the global generators) needs `seed=` for the generators the stream draws from from here on."""
+        if self.max_streams is not None and len(self._streams) >= self.max_streams:
+            raise RuntimeError(f"QwenStreamPool is full ({self.max_streams} streams)")
+        if checkpoint is not None and checkpoint.rng is None and seed is None:
+            raise ValueError("QwenStreamPool.open: this checkpoint carries no draw source (single-stream host): pass seed=")
+        if checkpoint is None:
+            state = QwenStreamState(self.flash, self.merger, device_frames=self.device_frames)
+        else:
+            state = QwenStreamState.restore(checkpoint, self.flash, self.merger, self.device, device_frames=self.device_frames)
+        if seed is None and checkpoint is None:
+            seed = int.from_bytes(os.urandom(8), "little") >> 1
+        rng = DrawSource(int(seed) if seed is not None else 0, self.device)
+        if checkpoint is not None and checkpoint.rng is not None:
+            r = checkpoint.rng
+            rng.cpu = r["cpu"].clone()
+            rng.cuda = r["cuda"].clone() if rng.cuda is not None and r["cuda"] is not None else rng.cuda
+            rng.py.setstate(r["py"])
+        state.rng = rng
+        sid = self._next
+        self._next += 1
+        self._streams[sid] = _Stream(self.visual, state)
+        return sid
+
+    def checkpoint(self, sid: int):
+        """The stream as a StreamCheckpoint in pinned host memory: its QwenStreamState and its draw source (settled first,
+        so no consumed refill count is lost or applied twice).  Suspend = checkpoint(sid) then close(sid); resume =
+        open(checkpoint=...) here or in another pool, or a host's load_video_stream()."""
+        from .. import checkpoint as CK
+        state = self._streams[sid].stream_state
+        state.rng.settle()
+        ck = state.checkpoint()
+        ck.rng = CK.rng_state(state.rng)
+        return ck
+
+    def close(self, sid: int):
+        del self._streams[sid]
+
+    def __len__(self):
+        return len(self._streams)
+
+    def stream(self, sid: int) -> _Stream:
+        return self._streams[sid]
+
+    def state(self, sid: int) -> QwenStreamState:
+        return self._streams[sid].stream_state
+
+    def as_list(self, sid: int):
+        """the stream's 13-item `video_embedding_memory` list (QwenStreamState.as_list)"""
+        return self._streams[sid].stream_state.as_list()
+
+    # ---- one round -----------------------------------------------------------------------------------------------------
+    def _validate(self, sid, clip):
+        """-> (pixel rows on the device in the tower's dtype, t, h, w); raises before anything is enqueued"""
+        if sid not in self._streams:
+            raise KeyError(f"QwenStreamPool.step: no stream {sid}")
+        pix, thw = clip
+        thw = torch.as_tensor(thw).reshape(-1, 3)
+        if thw.shape[0] != 1:
+            raise ValueError(f"QwenStreamPool.step: stream {sid}: one clip per stream (got {thw.shape[0]} grids)")
+        t, h, w = (int(v) for v in thw[0].tolist())
+        if t < 1 or h < 1 or w < 1 or h % 2 or w % 2:
+            raise ValueError(f"QwenStreamPool.step: stream {sid}: bad grid (t, h, w) = ({t}, {h}, {w})")
+        for name, side in (("pad_h", h), ("pad_w", w)):            # the reference's temporal_pool (pool size 2)
+            if (side // 2) % 2:
+                raise NotImplementedError(f"Performing temporal pool, {name} > 0, {name}={(side // 2) % 2}")
+        if pix.numel() != t * h * w * PATCH_DIM:
+            raise ValueError(f"QwenStreamPool.step: stream {sid}: {tuple(pix.shape)} pixels do not match the grid "
+                             f"({t}, {h}, {w})")
+        if pix.is_cuda and pix.device != self.device:
+            raise ValueError(f"QwenStreamPool.step: stream {sid}: pixels on {pix.device}, the pool is on {self.device}")
+        grid = self._streams[sid].stream_state.grid
+        if grid is not None and grid != (h, w):
+            raise ValueError(f"QwenStreamPool.step: stream {sid}: grid {(h, w)} differs from the stream's grid {grid}")
+        return pix, t, h, w
+
+    def _encode(self, items):
+        """items: [(pixels, t, h, w)] -> per item (x_new [t*h*w, D], small_new [t*h*w/4, D]) through as few tower calls
+        as plan_tower_calls allows"""
+        rows, segs = [], []
+        for pix, t, h, w in items:
+            full = pix.type(self.visual.get_dtype()).to(self.device, non_blocking=True).view(-1, PATCH_DIM)
+            small, _ = self.flash.temporal_pool(full, [t, h, w])
+            rows.append((full, small))
+            segs.append([(t, h, w), (t, h // 2, w // 2)])
+        out = [None] * len(items)
+        for grids, places in plan_tower_calls(segs, self.TOWER_ROWS):
+            pieces = sorted(((off, rows[i][k]) for i, offs in places for k, off in enumerate(offs)), key=lambda p: p[0])
+            feats = self.tower(torch.cat([p for _, p in pieces]) if len(pieces) > 1 else pieces[0][1], grids)
+            for i, offs in places:
+                out[i] = tuple(feats[off: off + r.shape[0]] for off, r in zip(offs, rows[i]))
+        return out
+
+    def step(self, clips: dict, draws: Optional[dict] = None):
+        """One round: one clip for every stream in `clips` ({sid: (pixel_values_videos, video_grid_thw)}); the other
+        streams do not move.  draws={sid: dict} replays a stream's draws (the `draws` of QwenStreamState.step).  A refused
+        round raises before anything is enqueued: no stream moves and no generator advances.  A stream whose clip raises
+        while being completed (ZeroDivisionError on an empty cluster, as the reference) is left as the single-stream
+        path leaves it; every other stream completes, and then the round raises one error naming the failing sids
+        (`.errors`: sid -> exception)."""
+        draws = draws or {}
+        sids = list(clips)
+        items = [self._validate(sid, clips[sid]) for sid in sids]
+        feats = self._encode(items)
+        merged = [None] * len(sids)
+        if self.flash.spatial_length > 0 and self.merger is not None:
+            xs = [x for x, _ in feats]
+            m = self.merger(torch.cat(xs) if len(xs) > 1 else xs[0])
+            r = 0
+            for k, x in enumerate(xs):
+                merged[k] = m[r: r + x.shape[0] // 4]
+                r += x.shape[0] // 4
+        pending = False
+        for k, sid in enumerate(sids):
+            st = self._streams[sid]
+            _, t, h, w = items[k]
+            pub = st.__dict__.get("_qwen_publication")
+            if pub is not None and st.stream_state.n_frames == 0:
+                pub.new_stream()
+            st.stream_state.enqueue(feats[k][0], feats[k][1], t, (h, w), (h // 2, w // 2), st.stream_state.n_frames,
+                                    draws=draws.get(sid), merged=merged[k])
+            pending = pending or bool(st.stream_state._pending)
+        if pending:                                    # the round's one host wait: every stream's read-back has landed
+            done = torch.cuda.Event()
+            done.record()
+            done.synchronize()
+        self._complete(sids)
+
+    def _complete(self, sids):
+        """complete every enqueued stream of the round and publish it; then raise one error for those that raised"""
+        errors = {}
+        for sid in sids:
+            st = self._streams[sid]
+            try:
+                st.stream_state.complete()
+            except Exception as e:                     # noqa: BLE001 - reported below, once every stream is completed
+                errors[sid] = e
+                continue
+            pub = st.__dict__.get("_qwen_publication")
+            if pub is not None:
+                pub.publish(st.stream_state)
+        if errors:
+            kinds = {type(e) for e in errors.values()}
+            cls = kinds.pop() if len(kinds) == 1 and ZeroDivisionError in kinds else RuntimeError
+            err = cls(f"QwenStreamPool.step: stream(s) {sorted(errors)} raised: "
+                      + "; ".join(f"{sid}: {type(e).__name__}: {e}" for sid, e in errors.items()))
+            err.errors = errors
+            raise err from next(iter(errors.values()))

@@ -73,6 +73,7 @@ class QwenStreamState:
     def __init__(self, flash, merger, device_frames=None):
         self.flash, self.merger = flash, merger
         self.device_frames = check_device_frames(device_frames)
+        self.rng = GLOBAL                     # the draws.DrawSource of every k-means draw (a QwenStreamPool stream owns one)
         self.reset()
 
     def reset(self):
@@ -92,14 +93,29 @@ class QwenStreamState:
         self.video_embeds = None
         self.tem_members = None
         self._readback = None                 # pinned int32 [8]: n_unique, info[4], flags
+        self._pending = None                  # what complete() needs of an enqueued clip ({} when nothing is read back)
         self.fast_steps = self.redone_steps = 0
         self.steps = 0                        # clips whose step completed (a clip that raises is not counted)
 
     # ------------------------------------------------------------------------------------------------ one clip
     def step(self, x_new: torch.Tensor, small_new: torch.Tensor, t: int, grid, small_grid, start_idx: int,
-             draws: Optional[dict] = None):
+             draws: Optional[dict] = None, merged: Optional[torch.Tensor] = None):
         """x_new [t * h * w, D] / small_new [t * hs * ws, D]: the tower's two-resolution features of the clip (device);
-        grid = (h, w), small_grid = (hs, ws) host integers.  Updates the state; returns nothing."""
+        grid = (h, w), small_grid = (hs, ws) host integers; merged: the PatchMerger rows of x_new, when the caller has
+        merged them already (None: merged here).  Updates the state.  enqueue(), one host wait, complete()."""
+        banks = self.enqueue(x_new, small_new, t, grid, small_grid, start_idx, draws, merged)
+        if self._pending:
+            done = torch.cuda.Event()
+            done.record()
+            done.synchronize()
+        self.complete()
+        return banks
+
+    def enqueue(self, x_new: torch.Tensor, small_new: torch.Tensor, t: int, grid, small_grid, start_idx: int,
+                draws: Optional[dict] = None, merged: Optional[torch.Tensor] = None):
+        """The first half of step(): the clip's work up to and including the copy of its 32-byte read-back, enqueued on
+        the current stream.  The caller waits until that copy has landed (an event recorded after it), then calls
+        complete().  Several states may be enqueued before one wait (QwenStreamPool)."""
         flash = self.flash
         dev, dt, D = x_new.device, x_new.dtype, x_new.shape[-1]
         h, w = grid
@@ -111,7 +127,10 @@ class QwenStreamState:
         # ---- banks (and, once per frame, the merged rows of the frame)
         self._prev_dam = self._dam()
         small_bank = self.bank_small.append(small_new.view(t, hs * ws, D))
-        merged = self.merger(x_new).view(t, h * w // 4, -1) if S0 > 0 and self.merger is not None else None
+        if S0 > 0 and self.merger is not None:
+            merged = (self.merger(x_new) if merged is None else merged).view(t, h * w // 4, -1)
+        else:
+            merged = None
         self._append_frames(x_new.view(t, h * w, D), merged, dev)
         bank = self.bank_x.rows() if self.bank_x.n else None
         self.n_frames += t
@@ -130,19 +149,20 @@ class QwenStreamState:
             cand_w = torch.ones(T, dtype=torch.float32, device=dev)
         d = draws or {}
         fast = T > T0 > 0 and flash.temporal_method in _KMEANS_METHODS
+        self._pending = {}
         if not fast:
             self._compress_sync(cand, cand_w, T, d, start_idx, t)
         else:
             snap = None
             init = d.get("init_idx")
             if init is None:
-                snap = GLOBAL.snapshot(dev)
-                init_dev = GLOBAL.randperm(T, dev)[:T0].to(torch.int32)          # randperm(n_unique), assuming n_unique == T
+                snap = self.rng.snapshot(dev)
+                init_dev = self.rng.randperm(T, dev)[:T0].to(torch.int32)        # randperm(n_unique), assuming n_unique == T
             else:
                 init_dev = to_device(np.asarray(init)[:T0], np.int32, dev)
             refill = d.get("refill_idx")
             if refill is None:
-                refill_dev, _ = GLOBAL.refill_candidates(T, CF.MAX_ITER * T0, dev)
+                refill_dev, _ = self.rng.refill_candidates(T, CF.MAX_ITER * T0, dev)
             else:
                 refill = list(int(v) for v in refill)
                 refill_dev = to_device(refill + [0] * (CF.MAX_ITER * T0 - len(refill)), np.int32, dev)
@@ -155,25 +175,33 @@ class QwenStreamState:
             if self._readback is None:
                 self._readback = torch.empty(8, dtype=torch.int32).pin_memory()
             self._readback[:6].copy_(torch.cat([km["n_unique"], km["info"], km["flags"]]), non_blocking=True)
-            done = torch.cuda.Event()
-            done.record()
-            done.synchronize()
+            self._pending = dict(cand=cand, cand_w=cand_w, T=T, d=d, start_idx=start_idx, t=t, snap=snap,
+                                 own_refills=refill is None)
+        return bank, small_bank
+
+    def complete(self):
+        """The second half of step(), once the read-back of enqueue() has landed: a valid fast-path clip is final (or raises
+        ZeroDivisionError on an empty cluster, as the reference does; the state is then left as that raise leaves it); a
+        clip with duplicate rows rewinds this state's draw source and is redone through the synchronous path."""
+        p, self._pending = self._pending, None
+        if p:
+            T0 = self.flash.temporal_length
+            T = p["T"]
             n_unique, _, consumed, _, _, empty = (int(v) for v in self._readback[:6])
-            valid = n_unique >= T0 and (snap is None or n_unique == T)
+            valid = n_unique >= T0 and (p["snap"] is None or n_unique == T)
             if valid:
                 if empty:
                     raise ZeroDivisionError("division by zero")          # sum(indices) / len(indices), compress_functions.py:279
-                if refill is None:
-                    GLOBAL.consume(T, consumed)                            # leave `random` where the reference would
+                if p["own_refills"]:
+                    self.rng.consume(T, consumed)                          # leave `random` where the reference would
                 self.fast_steps += 1
             else:                                                          # duplicates among the rows: the general path
-                if snap is not None:
-                    GLOBAL.rewind(snap)
+                if p["snap"] is not None:
+                    self.rng.rewind(p["snap"])
                 self.redone_steps += 1
-                self._compress_sync(cand, cand_w, T, d, start_idx, t)
+                self._compress_sync(p["cand"], p["cand_w"], T, p["d"], p["start_idx"], p["t"])
         self._prev_dam = None                 # the old DAM is the readers' now, not ours to keep alive
         self.steps += 1
-        return bank, small_bank
 
     # ------------------------------------------------------------------------------------------------ pieces
     def _thw(self, n, small=False):
@@ -300,7 +328,7 @@ class QwenStreamState:
         P, D = cand.shape[1], cand.shape[2]
         ts_in = torch.arange(T, device=cand.device, dtype=torch.float32)      # accepted and ignored by the reference (:279)
         tem_x, tem_thw, tem_w, tem_ts, members = flash.temporal_compress(
-            cand.reshape(T * P, D), self._thw(T, small=True), flash.temporal_length, cand_w, ts_in, draws=d)
+            cand.reshape(T * P, D), self._thw(T, small=True), flash.temporal_length, cand_w, ts_in, draws={**d, "source": self.rng})
         self._enqueue_rest(tem_x, tem_w, tem_ts, int(tem_thw[0]), members, d)
 
     # ------------------------------------------------------------------------------------------------ checkpoint / restore

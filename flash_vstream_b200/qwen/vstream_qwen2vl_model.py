@@ -19,6 +19,7 @@ import torch
 import torch.nn as nn
 
 from .. import ops as O
+from ..draws import GLOBAL
 from . import compress_functions as CF
 from . import ops as Q
 from .compress_functions import weighted_kmeans_ordered_feature
@@ -83,7 +84,8 @@ def get_spatial_real_grid_thw(thw, flash_memory_config):
 class FlashMemory(nn.Module):
     """vstream_qwen2vl_model.py:78-330.  `draws` (forward / temporal_compress / spatial_enhance) optionally replays the RNG
     draws and unstable-sort permutations recorded from a reference run: dict(init_idx=, refill_idx=, ts_order=,
-    weight_order=); by default the same generators as the reference are consumed and ties sort stably."""
+    weight_order=, source=); by default the same generators as the reference are consumed (source: a draws.DrawSource
+    to draw from instead) and ties sort stably."""
 
     def __init__(self, flash_memory_temporal_length=120, flash_memory_temporal_method='kmeans_ordered',
                  flash_memory_temporal_poolsize=2, flash_memory_temporal_pca_dim=32, flash_memory_spatial_length=60,
@@ -126,7 +128,8 @@ class FlashMemory(nn.Module):
         if method in ('kmeans_ordered', 'fast_kmeans_ordered'):      # same arithmetic (see CF.fast_weighted_kmeans_ordered_feature)
             d = draws or {}
             return weighted_kmeans_ordered_feature(frames, keep, weights, times, init_idx=d.get("init_idx"),
-                                                   refill_idx=d.get("refill_idx"), order=d.get("ts_order"))
+                                                   refill_idx=d.get("refill_idx"), order=d.get("ts_order"),
+                                                   source=d.get("source", GLOBAL))
         return getattr(CF, _ALTERNATE_TEMPORAL[method])(frames, keep)      # raises NotImplementedError (not built)
 
     def temporal_compress(self, x, thw, temporal_length, draws: Optional[dict] = None):

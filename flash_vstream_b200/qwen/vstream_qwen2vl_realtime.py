@@ -23,6 +23,7 @@ import torch
 import torch.nn as nn
 
 from .. import _lib as L
+from ..draws import GLOBAL
 from ..vstream_arch import _is_manager_proxy
 from . import vstream_qwen2vl_model as _offline
 from .compress_functions import weighted_kmeans_ordered_feature
@@ -36,7 +37,8 @@ class FlashMemory(_offline.FlashMemory):
     def temporal_compress(self, x, thw, temporal_length, temporal_weights, temporal_indices, draws: Optional[dict] = None):
         """:149-183.  temporal_weights are the carried cluster weights; temporal_indices (timestamps) are accepted and —
         exactly like the reference's weighted_kmeans_ordered_feature, which overwrites them with the mean member row index
-        (compress_functions.py:279) — do not influence the result."""
+        (compress_functions.py:279) — do not influence the result.  draws["source"] (a draws.DrawSource, default the global
+        generators) is where the draws not given in `draws` come from."""
         t, h, w = _offline._thw(thw)
         if t <= temporal_length:
             return (x, thw, torch.ones(t, device=x.device), torch.arange(t, device=x.device, dtype=torch.int32),
@@ -56,7 +58,7 @@ class FlashMemory(_offline.FlashMemory):
         d = draws or {}
         x, weights, timestamps, indices = weighted_kmeans_ordered_feature(
             x, temporal_length, temporal_weights, temporal_indices, init_idx=d.get("init_idx"),
-            refill_idx=d.get("refill_idx"), order=d.get("ts_order"))
+            refill_idx=d.get("refill_idx"), order=d.get("ts_order"), source=d.get("source", GLOBAL))
         tem_thw = thw.clone()
         tem_thw[0] = x.shape[0]
         return x.reshape(-1, x.shape[-1]), tem_thw, weights, timestamps, indices
