@@ -130,6 +130,8 @@ SIGNATURES = {
     "fvs_gather_rows_cast": (_i, [_vp, _vp, _vp, _i, C.c_int64, _i, _vp]),
     "fvs_qwen_klarge_workspace_bytes": (_sz, [_i, _i, _i]),
     "fvs_qwen_klarge_retrieve": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _sz, _vp]),
+    "fvs_qwen_klarge_retrieve_tiered": (_i, [_vp, _vp, _vp, _i, C.POINTER(_vp), _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _sz,
+                                             _vp]),
     "fvs_qwen_am_rope": (_i, [_vp, _i, _i, _i, _vp, _i, _i, _i, C.c_int64, _vp, _vp]),
     # two-tier feature bank of the Qwen2-VL streaming state
     "fvs_qwen_dam_gather": (_i, [_vp, _i, C.c_int64, _vp, _vp, C.c_int64, _vp, _i, _vp, _i, _vp, _vp, C.c_int64, C.c_int64,

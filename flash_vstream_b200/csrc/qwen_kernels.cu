@@ -617,10 +617,17 @@ __device__ __forceinline__ uint32_t pack2_16(float a, float b) {
   const __half2 h = __floats2half2_rn(a, b);
   return *reinterpret_cast<const uint32_t*>(&h);
 }
-template <bool kBF16, int kMode>
+// kRange: the launch sweeps bank rows [t_first, t_first + rows) of the t_total, row t_first at `bank` (one tier of a
+// two-tier bank, DESIGN.md §3.13: the HBM rows, or one pinned host chunk through its mapped pointer), and writes their
+// partials at the rows' global indices; the launch whose range starts at row 0 writes the |c|^2 partials.  A row's
+// partials do not depend on the block or launch that computes them, so any split of the rows gives the same bits.
+// Without kRange the launch sweeps the whole bank (t_first 0, rows t_total) and ignores the last two arguments.
+template <bool kBF16, int kMode, bool kRange>
 __global__ void __launch_bounds__(256) klarge_partial_kernel(const uint16_t* __restrict__ tem_x, const long long* __restrict__ klarge_idx,
                                                              const uint16_t* __restrict__ bank, float* __restrict__ part, int k,
-                                                             int t_total, int PD, const float* __restrict__ norms) {
+                                                             int t_total, int PD, const float* __restrict__ norms,
+                                                             int range_first, int range_rows) {
+  const int t_first = kRange ? range_first : 0, rows = kRange ? range_rows : t_total;
   extern __shared__ __align__(16) uint8_t smem_raw[];
   uint4* cs = reinterpret_cast<uint4*>(smem_raw);          // [k][128] uint4 = k rows of 1024 16-bit elements
   const int S = PD / SLICE, s = blockIdx.x;
@@ -644,9 +651,9 @@ __global__ void __launch_bounds__(256) klarge_partial_kernel(const uint16_t* __r
   float* p_ab = part;
   float* p_b2 = part + size_t(t_total) * k * S;
   float* p_a2 = p_b2 + size_t(t_total) * S;
-  const int rows_per = (t_total + gridDim.y - 1) / gridDim.y;      // bank rows of this block
-  const int t_beg = blockIdx.y * rows_per, t_end = min(t_total, t_beg + rows_per);
-  if (kMode != 2 && blockIdx.y == 0) {
+  const int rows_per = (rows + gridDim.y - 1) / gridDim.y;         // bank rows of this block
+  const int t_beg = t_first + blockIdx.y * rows_per, t_end = min(t_first + rows, t_beg + rows_per);
+  if (kMode != 2 && blockIdx.y == 0 && t_first == 0) {
     for (int kk = warp; kk < k; kk += 8) {                  // |c|^2 slice partials
       float acc = 0.f;
 #pragma unroll
@@ -666,8 +673,8 @@ __global__ void __launch_bounds__(256) klarge_partial_kernel(const uint16_t* __r
   for (int t0 = t_beg + warp * 2; t0 < t_end; t0 += 16) {
     const bool two = t0 + 1 < t_end;
     float x0[32], x1[32];
-    const uint4* src0 = reinterpret_cast<const uint4*>(bank + size_t(t0) * PD + size_t(s) * SLICE);
-    const uint4* src1 = reinterpret_cast<const uint4*>(bank + size_t(two ? t0 + 1 : t0) * PD + size_t(s) * SLICE);
+    const uint4* src0 = reinterpret_cast<const uint4*>(bank + size_t(t0 - t_first) * PD + size_t(s) * SLICE);
+    const uint4* src1 = reinterpret_cast<const uint4*>(bank + size_t((two ? t0 + 1 : t0) - t_first) * PD + size_t(s) * SLICE);
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
       unpack8<kBF16>(src0[i * 32 + lane], x0 + i * 8);
@@ -797,24 +804,102 @@ using namespace fvs;
 using namespace fvs::qwen;
 
 namespace {
-template <bool kBF16, int kMode>
+// the bank of a klarge retrieval, in two tiers: rows [0, n_dev) are contiguous at dev (HBM), row n_dev + c*chunk_frames + r
+// is row r of host chunk c (chunks: a host array of the chunks' mapped device pointers)
+struct KlargeBank {
+  const void* dev;
+  int n_dev;
+  const void* const* chunks;
+  int chunk_frames, t_total;
+};
+
+template <bool kBF16, int kMode, bool kRange>
 int klarge_partial_launch(const void* tem_x, const int64_t* klarge_idx, const void* bank, float* part, int k, int t_total,
-                          int PD, const float* norms, cudaStream_t stream) {
+                          int PD, const float* norms, int t_first, int rows, cudaStream_t stream) {
   using namespace fvs::qwen;
   static bool attr = false;   // per instantiation
-  auto kern = klarge_partial_kernel<kBF16, kMode>;
+  auto kern = klarge_partial_kernel<kBF16, kMode, kRange>;
   if (!attr) { FVS_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * SLICE * 2)); attr = true; }
-  const int nsplit = (t_total + 31) / 32;   // <= 32 bank rows per block: enough blocks to fill every SM from t ~ 32 up
+  const int nsplit = (rows + 31) / 32;      // <= 32 bank rows per block: enough blocks to fill every SM from t ~ 32 up
   kern<<<dim3(PD / SLICE, nsplit), 256, size_t(k) * SLICE * 2, stream>>>((const uint16_t*)tem_x, (const long long*)klarge_idx,
-                                                                       (const uint16_t*)bank, part, k, t_total, PD, norms);
+                                                                       (const uint16_t*)bank, part, k, t_total, PD, norms,
+                                                                       t_first, rows);
   FVS_CHECK_LAUNCH("klarge_partial_kernel");
   return FVS_OK;
 }
+// one sweep of the bank: a bank wholly in HBM is one launch over every row; otherwise one launch over the device rows and
+// one per host chunk, each reading its rows through the chunk's mapped pointer (PCIe)
+template <bool kBF16, int kMode>
+int klarge_sweep(const void* tem_x, const int64_t* klarge_idx, const KlargeBank& b, float* part, int k, int PD,
+                 const float* norms, cudaStream_t stream) {
+  if (b.n_dev == b.t_total)
+    return klarge_partial_launch<kBF16, kMode, false>(tem_x, klarge_idx, b.dev, part, k, b.t_total, PD, norms, 0, b.t_total,
+                                                      stream);
+  int r;
+  if (b.n_dev > 0 &&
+      (r = klarge_partial_launch<kBF16, kMode, true>(tem_x, klarge_idx, b.dev, part, k, b.t_total, PD, norms, 0, b.n_dev, stream)))
+    return r;
+  for (int c = 0, t = b.n_dev; t < b.t_total; ++c, t += b.chunk_frames)
+    if ((r = klarge_partial_launch<kBF16, kMode, true>(tem_x, klarge_idx, b.chunks[c], part, k, b.t_total, PD, norms, t,
+                                                       std::min(b.chunk_frames, b.t_total - t), stream)))
+      return r;
+  return FVS_OK;
+}
 template <int kMode>
-int klarge_partial(bool bf, const void* tem_x, const int64_t* klarge_idx, const void* bank, float* part, int k, int t_total,
-                   int PD, const float* norms, cudaStream_t stream) {
-  return bf ? klarge_partial_launch<true, kMode>(tem_x, klarge_idx, bank, part, k, t_total, PD, norms, stream)
-            : klarge_partial_launch<false, kMode>(tem_x, klarge_idx, bank, part, k, t_total, PD, norms, stream);
+int klarge_partial(bool bf, const void* tem_x, const int64_t* klarge_idx, const KlargeBank& b, float* part, int k, int PD,
+                   const float* norms, cudaStream_t stream) {
+  return bf ? klarge_sweep<true, kMode>(tem_x, klarge_idx, b, part, k, PD, norms, stream)
+            : klarge_sweep<false, kMode>(tem_x, klarge_idx, b, part, k, PD, norms, stream);
+}
+
+// fvs_qwen_klarge_retrieve and its tiered form: the checks (reported as `who`), the sweeps, the reductions and the tail
+int klarge_retrieve(const char* who, const void* tem_x, const int64_t* klarge_idx, const KlargeBank& b, int k, int PD, int dtype,
+                    int metric, int64_t* idx_out, float* dist_out, void* workspace, size_t workspace_bytes,
+                    fvs_stream_t stream_) {
+  const int t_total = b.t_total;
+  FVS_REQUIRE(tem_x && klarge_idx && idx_out && workspace && (b.dev || b.n_dev == 0), "%s: null pointer", who);
+  FVS_REQUIRE(dtype == FVS_F16 || dtype == FVS_BF16, "%s: dtype must be f16 or bf16", who);
+  FVS_REQUIRE(metric == FVS_KLARGE_EUCLIDEAN || metric == FVS_KLARGE_COSINE, "%s: unknown metric %d", who, metric);
+  FVS_REQUIRE(k > 0 && k <= 64 && t_total > 0, "%s: need 0 < k <= 64, t > 0 (k=%d t=%d)", who, k, t_total);
+  FVS_REQUIRE(PD % SLICE == 0, "%s: PD (%d) must be a multiple of %d", who, PD, SLICE);
+  FVS_REQUIRE(b.n_dev >= 0 && b.n_dev <= t_total, "%s: need 0 <= n_dev <= t_total (n_dev=%d t=%d)", who, b.n_dev, t_total);
+  if (b.n_dev < t_total) {
+    FVS_REQUIRE(b.chunks && b.chunk_frames > 0, "%s: host rows need a chunk table and chunk_frames > 0", who);
+    for (int c = 0; c * int64_t(b.chunk_frames) < t_total - b.n_dev; ++c)
+      FVS_REQUIRE(b.chunks[c], "%s: null pointer of host chunk %d", who, c);
+  }
+  FVS_REQUIRE(workspace_bytes >= fvs_qwen_klarge_workspace_bytes(k, t_total, PD), "%s: workspace too small", who);
+  cudaStream_t stream = (cudaStream_t)stream_;
+  const int S = PD / SLICE;
+  const bool bf = dtype == FVS_BF16;
+  const size_t n_ab = size_t(t_total) * k, n_norm = size_t(t_total) + k, units = n_ab + n_norm;
+  float* part = (float*)workspace;
+  float* tot = (float*)((uint8_t*)workspace + al(units * S * 4));
+  int r;
+  if (metric == FVS_KLARGE_EUCLIDEAN) {
+    if ((r = klarge_partial<0>(bf, tem_x, klarge_idx, b, part, k, PD, nullptr, stream))) return r;
+    seq_reduce_kernel<<<int((units + 7) / 8), 256, 0, stream>>>(part, tot, int(units), S, nullptr);
+    FVS_CHECK_LAUNCH("seq_reduce_kernel");
+    if (bf) klarge_tail_kernel<true><<<k, 32, 0, stream>>>(tot, k, t_total, (long long*)idx_out, dist_out);
+    else klarge_tail_kernel<false><<<k, 32, 0, stream>>>(tot, k, t_total, (long long*)idx_out, dist_out);
+    FVS_CHECK_LAUNCH("klarge_tail_kernel");
+    return FVS_OK;
+  }
+  // cosine: squared norms -> norms -> normalised dot products -> argmin of the similarity (the bank is swept twice)
+  float* norms = tot + n_ab;
+  if ((r = klarge_partial<1>(bf, tem_x, klarge_idx, b, part, k, PD, nullptr, stream))) return r;
+  seq_reduce_kernel<<<int((n_norm + 7) / 8), 256, 0, stream>>>(part + n_ab * S, norms, int(n_norm), S, nullptr);
+  FVS_CHECK_LAUNCH("seq_reduce_kernel");
+  if (bf) klcos_norm_kernel<true><<<int((n_norm + 255) / 256), 256, 0, stream>>>(norms, int(n_norm));
+  else klcos_norm_kernel<false><<<int((n_norm + 255) / 256), 256, 0, stream>>>(norms, int(n_norm));
+  FVS_CHECK_LAUNCH("klcos_norm_kernel");
+  if ((r = klarge_partial<2>(bf, tem_x, klarge_idx, b, part, k, PD, norms, stream))) return r;
+  seq_reduce_kernel<<<int((n_ab + 7) / 8), 256, 0, stream>>>(part, tot, int(n_ab), S, nullptr);
+  FVS_CHECK_LAUNCH("seq_reduce_kernel");
+  if (bf) klarge_cos_tail_kernel<true><<<k, 32, 0, stream>>>(tot, k, t_total, (long long*)idx_out, dist_out);
+  else klarge_cos_tail_kernel<false><<<k, 32, 0, stream>>>(tot, k, t_total, (long long*)idx_out, dist_out);
+  FVS_CHECK_LAUNCH("klarge_cos_tail_kernel");
+  return FVS_OK;
 }
 }  // namespace
 
@@ -955,44 +1040,20 @@ size_t fvs_qwen_klarge_workspace_bytes(int k, int t_total, int PD) {
 
 int fvs_qwen_klarge_retrieve(const void* tem_x, const int64_t* klarge_idx, const void* bank, int k, int t_total, int PD,
                              int dtype, int metric, int64_t* idx_out, float* dist_out, void* workspace,
-                             size_t workspace_bytes, fvs_stream_t stream_) {
-  FVS_REQUIRE(tem_x && klarge_idx && bank && idx_out && workspace, "fvs_qwen_klarge_retrieve: null pointer");
-  FVS_REQUIRE(dtype == FVS_F16 || dtype == FVS_BF16, "fvs_qwen_klarge_retrieve: dtype must be f16 or bf16");
-  FVS_REQUIRE(metric == FVS_KLARGE_EUCLIDEAN || metric == FVS_KLARGE_COSINE, "fvs_qwen_klarge_retrieve: unknown metric %d", metric);
-  FVS_REQUIRE(k > 0 && k <= 64 && t_total > 0, "fvs_qwen_klarge_retrieve: need 0 < k <= 64, t > 0 (k=%d t=%d)", k, t_total);
-  FVS_REQUIRE(PD % SLICE == 0, "fvs_qwen_klarge_retrieve: PD (%d) must be a multiple of %d", PD, SLICE);
-  FVS_REQUIRE(workspace_bytes >= fvs_qwen_klarge_workspace_bytes(k, t_total, PD), "fvs_qwen_klarge_retrieve: workspace too small");
-  cudaStream_t stream = (cudaStream_t)stream_;
-  const int S = PD / SLICE;
-  const bool bf = dtype == FVS_BF16;
-  const size_t n_ab = size_t(t_total) * k, n_norm = size_t(t_total) + k, units = n_ab + n_norm;
-  float* part = (float*)workspace;
-  float* tot = (float*)((uint8_t*)workspace + al(units * S * 4));
-  int r;
-  if (metric == FVS_KLARGE_EUCLIDEAN) {
-    if ((r = klarge_partial<0>(bf, tem_x, klarge_idx, bank, part, k, t_total, PD, nullptr, stream))) return r;
-    seq_reduce_kernel<<<int((units + 7) / 8), 256, 0, stream>>>(part, tot, int(units), S, nullptr);
-    FVS_CHECK_LAUNCH("seq_reduce_kernel");
-    if (bf) klarge_tail_kernel<true><<<k, 32, 0, stream>>>(tot, k, t_total, (long long*)idx_out, dist_out);
-    else klarge_tail_kernel<false><<<k, 32, 0, stream>>>(tot, k, t_total, (long long*)idx_out, dist_out);
-    FVS_CHECK_LAUNCH("klarge_tail_kernel");
-    return FVS_OK;
-  }
-  // cosine: squared norms -> norms -> normalised dot products -> argmin of the similarity
-  float* norms = tot + n_ab;
-  if ((r = klarge_partial<1>(bf, tem_x, klarge_idx, bank, part, k, t_total, PD, nullptr, stream))) return r;
-  seq_reduce_kernel<<<int((n_norm + 7) / 8), 256, 0, stream>>>(part + n_ab * S, norms, int(n_norm), S, nullptr);
-  FVS_CHECK_LAUNCH("seq_reduce_kernel");
-  if (bf) klcos_norm_kernel<true><<<int((n_norm + 255) / 256), 256, 0, stream>>>(norms, int(n_norm));
-  else klcos_norm_kernel<false><<<int((n_norm + 255) / 256), 256, 0, stream>>>(norms, int(n_norm));
-  FVS_CHECK_LAUNCH("klcos_norm_kernel");
-  if ((r = klarge_partial<2>(bf, tem_x, klarge_idx, bank, part, k, t_total, PD, norms, stream))) return r;
-  seq_reduce_kernel<<<int((n_ab + 7) / 8), 256, 0, stream>>>(part, tot, int(n_ab), S, nullptr);
-  FVS_CHECK_LAUNCH("seq_reduce_kernel");
-  if (bf) klarge_cos_tail_kernel<true><<<k, 32, 0, stream>>>(tot, k, t_total, (long long*)idx_out, dist_out);
-  else klarge_cos_tail_kernel<false><<<k, 32, 0, stream>>>(tot, k, t_total, (long long*)idx_out, dist_out);
-  FVS_CHECK_LAUNCH("klarge_cos_tail_kernel");
-  return FVS_OK;
+                             size_t workspace_bytes, fvs_stream_t stream) {
+  if (!bank) return set_error(FVS_EINVAL, "fvs_qwen_klarge_retrieve: null pointer");
+  const KlargeBank b{bank, t_total, nullptr, 0, t_total};
+  return klarge_retrieve("fvs_qwen_klarge_retrieve", tem_x, klarge_idx, b, k, PD, dtype, metric, idx_out, dist_out, workspace,
+                         workspace_bytes, stream);
+}
+
+int fvs_qwen_klarge_retrieve_tiered(const void* tem_x, const int64_t* klarge_idx, const void* dev_bank, int n_dev,
+                                    const void* const* host_chunks, int chunk_frames, int k, int t_total, int PD, int dtype,
+                                    int metric, int64_t* idx_out, float* dist_out, void* workspace, size_t workspace_bytes,
+                                    fvs_stream_t stream) {
+  const KlargeBank b{dev_bank, n_dev, host_chunks, chunk_frames, t_total};
+  return klarge_retrieve("fvs_qwen_klarge_retrieve_tiered", tem_x, klarge_idx, b, k, PD, dtype, metric, idx_out, dist_out,
+                         workspace, workspace_bytes, stream);
 }
 
 int fvs_qwen_am_rope(const int64_t* spa_positions, int spa_t, int spa_h, int spa_w, const int64_t* tem_positions, int tem_t,

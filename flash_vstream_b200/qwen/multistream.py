@@ -90,12 +90,14 @@ class QwenStreamPool:
     stream's QwenStreamState, `as_list(sid)` its 13-item list; `stream(sid)` can be handed to qwen.serve.export_qwen_memory.
     `checkpoint(sid)` / `open(checkpoint=)` suspend and resume a stream; `close(sid)` drops it.  Configs and towers the
     batched round does not cover raise NotImplementedError naming the knob: stream them through the host's single-stream
-    path.  `device_frames` applies to every stream, as `fvs_bank_device_frames` does to the host's stream (DESIGN.md
-    §3.13).  TOWER_ROWS bounds the rows of one tower call (its workspace is about 30 KB per row at 1280 wide)."""
+    path.  `device_frames` and `small_device_frames` apply to every stream, as `fvs_bank_device_frames` and
+    `fvs_bank_small_device_frames` do to the host's stream (DESIGN.md §3.13).  TOWER_ROWS bounds the rows of one tower
+    call (its workspace is about 30 KB per row at 1280 wide)."""
 
     TOWER_ROWS = 65536
 
-    def __init__(self, model, device_frames: Optional[int] = None, max_streams: Optional[int] = None):
+    def __init__(self, model, device_frames: Optional[int] = None, max_streams: Optional[int] = None,
+                 small_device_frames: Optional[int] = None):
         visual = model.visual
         flash, tower = visual.flash_memory, visual.encode_patches
         if not isinstance(tower, QwenVisionBlocksB200):
@@ -115,6 +117,7 @@ class QwenStreamPool:
             self.device = torch.device("cuda", torch.cuda.current_device())
         self.visual, self.flash, self.merger, self.tower = visual, flash, visual.merger, tower
         self.device_frames = check_device_frames(device_frames, "device_frames")
+        self.small_device_frames = check_device_frames(small_device_frames, "small_device_frames")
         self.max_streams = max_streams
         self._streams: dict[int, _Stream] = {}
         self._next = 0
@@ -130,9 +133,11 @@ class QwenStreamPool:
         if checkpoint is not None and checkpoint.rng is None and seed is None:
             raise ValueError("QwenStreamPool.open: this checkpoint carries no draw source (single-stream host): pass seed=")
         if checkpoint is None:
-            state = QwenStreamState(self.flash, self.merger, device_frames=self.device_frames)
+            state = QwenStreamState(self.flash, self.merger, device_frames=self.device_frames,
+                                    small_device_frames=self.small_device_frames)
         else:
-            state = QwenStreamState.restore(checkpoint, self.flash, self.merger, self.device, device_frames=self.device_frames)
+            state = QwenStreamState.restore(checkpoint, self.flash, self.merger, self.device, device_frames=self.device_frames,
+                                            small_device_frames=self.small_device_frames)
         if seed is None and checkpoint is None:
             seed = int.from_bytes(os.urandom(8), "little") >> 1
         rng = DrawSource(int(seed) if seed is not None else 0, self.device)

@@ -2,11 +2,12 @@
 from __future__ import annotations
 
 import ctypes as C
-from typing import Optional
+from typing import NamedTuple, Optional
 
 import torch
 
 from .. import _lib as L
+from ..host_tier import placement
 from ..ops import _c, _chk_cuda
 
 _ws_cache: dict = {}
@@ -101,25 +102,59 @@ def gather_rows_cast(src: torch.Tensor, idx: torch.Tensor, dtype: torch.dtype, o
     return out
 
 
-def klarge_retrieve(tem_x: torch.Tensor, klarge_idx: torch.Tensor, bank: torch.Tensor, want_dist: bool = False,
+class TieredBank(NamedTuple):
+    """A bank of t_total rows of PD 16-bit elements in two tiers (DESIGN.md §3.13): rows [0, n_dev) are `dev` (HBM,
+    [n_dev, PD], None when n_dev is 0); row n_dev + c * chunk_frames + r is row r of the pinned host chunk whose mapped
+    device pointer (host_device_ptr) is chunks[c]."""
+    dev: Optional[torch.Tensor]
+    n_dev: int
+    chunks: tuple
+    chunk_frames: int
+    t_total: int
+    dtype: torch.dtype
+    device: torch.device
+
+
+def klarge_plan(t_total: int, n_dev: int, chunk_frames: int):
+    """the row ranges a tiered klarge sweep launches over, as (chunk, t_first, rows): chunk -1 is the device rows (every
+    row when n_dev >= t_total), chunk c >= 0 the c-th host chunk"""
+    return [(c, s, cnt) for c, _, s, cnt in placement(0, t_total, n_dev, chunk_frames)]
+
+
+def klarge_retrieve(tem_x: torch.Tensor, klarge_idx: torch.Tensor, bank, want_dist: bool = False,
                     metric: str = "euclidean"):
-    """tem_x [st, PD], klarge_idx int64 [k], bank [t, PD] (16-bit) -> idx int64 [k] (and the rounded distances — or, with
-    metric="cosine" ('klarge_retrieve_cos'), similarities — fp32 [k, t])"""
+    """tem_x [st, PD], klarge_idx int64 [k], bank [t, PD] (16-bit) or a TieredBank of t rows -> idx int64 [k] (and the
+    rounded distances — or, with metric="cosine" ('klarge_retrieve_cos'), similarities — fp32 [k, t]).  A tiered bank's
+    host rows are read in place over PCIe (once per sweep; the cosine metric sweeps twice); the results are the bits of the
+    same rows in HBM."""
     code = {"euclidean": L.KLARGE_EUCLIDEAN, "cosine": L.KLARGE_COSINE}[metric]
-    _chk_cuda(tem_x, klarge_idx, bank)
-    tem_x, bank, klarge_idx = _c(tem_x), _c(bank), _c(klarge_idx)
-    assert klarge_idx.dtype == torch.int64 and tem_x.dtype == bank.dtype and tem_x.shape[1] == bank.shape[1]
-    k, (t, PD) = klarge_idx.numel(), bank.shape
+    tiered = isinstance(bank, TieredBank)
+    rows = bank.dev if tiered else bank
+    _chk_cuda(tem_x, klarge_idx, rows)
+    tem_x, klarge_idx, rows = _c(tem_x), _c(klarge_idx), None if rows is None else _c(rows)
+    assert klarge_idx.dtype == torch.int64 and tem_x.dtype == bank.dtype and (rows is None or tem_x.shape[1] == rows.shape[1])
+    assert not tiered or (0 if rows is None else rows.shape[0]) == bank.n_dev
+    k, t, PD = klarge_idx.numel(), bank.t_total if tiered else rows.shape[0], tem_x.shape[1]
     if k > 64:   # the kernel keeps <= 64 centroid slices in shared memory: sweep the bank once per group of 64
         parts = [klarge_retrieve(tem_x, klarge_idx[i:i + 64], bank, want_dist, metric) for i in range(0, k, 64)]
         return (torch.cat([p[0] for p in parts]), torch.cat([p[1] for p in parts])) if want_dist else torch.cat(parts)
     lib = L.load()
-    ws = _workspace(lib.fvs_qwen_klarge_workspace_bytes(k, t, PD), bank.device, "klarge")
-    idx = torch.empty(k, dtype=torch.int64, device=bank.device)
-    dist = torch.empty(k, t, dtype=torch.float32, device=bank.device) if want_dist else None
-    L.check(lib.fvs_qwen_klarge_retrieve(L.ptr(tem_x), L.ptr(klarge_idx), L.ptr(bank), k, t, PD, L.dtype_code(bank.dtype),
-                                         code, L.ptr(idx), L.ptr(dist), L.ptr(ws), ws.numel(), L.cur_stream()),
-            "fvs_qwen_klarge_retrieve")
+    dev = tem_x.device
+    ws = _workspace(lib.fvs_qwen_klarge_workspace_bytes(k, t, PD), dev, "klarge")
+    idx = torch.empty(k, dtype=torch.int64, device=dev)
+    dist = torch.empty(k, t, dtype=torch.float32, device=dev) if want_dist else None
+    if not tiered:
+        L.check(lib.fvs_qwen_klarge_retrieve(L.ptr(tem_x), L.ptr(klarge_idx), L.ptr(rows), k, t, PD, L.dtype_code(rows.dtype),
+                                             code, L.ptr(idx), L.ptr(dist), L.ptr(ws), ws.numel(), L.cur_stream()),
+                "fvs_qwen_klarge_retrieve")
+        return (idx, dist) if want_dist else idx
+    n_chunks = sum(1 for c, _, _ in klarge_plan(t, bank.n_dev, bank.chunk_frames) if c >= 0)
+    assert len(bank.chunks) >= n_chunks, f"a bank of {t} rows needs {n_chunks} host chunks, got {len(bank.chunks)}"
+    table = (C.c_void_p * n_chunks)(*bank.chunks[:n_chunks]) if n_chunks else None     # host array, read at launch
+    L.check(lib.fvs_qwen_klarge_retrieve_tiered(L.ptr(tem_x), L.ptr(klarge_idx), L.ptr(rows), int(bank.n_dev), table,
+                                                int(bank.chunk_frames), k, t, PD,
+                                                L.dtype_code(bank.dtype), code, L.ptr(idx), L.ptr(dist), L.ptr(ws),
+                                                ws.numel(), L.cur_stream()), "fvs_qwen_klarge_retrieve_tiered")
     return (idx, dist) if want_dist else idx
 
 

@@ -66,13 +66,17 @@ class QwenStreamState:
     """flash: the streaming FlashMemory (temporal_length / spatial_length in frames, methods); merger: PatchMerger.
     device_frames: how many frames of the full-resolution and merged banks stay in HBM (None: all of them).  Later frames
     are copied to pinned host chunks as they arrive and never move again; a step reads only its retrieved frames from
-    them (fvs_qwen_dam_gather).  The half-resolution bank, which the retrieval sweeps whole, always stays in HBM."""
+    them (fvs_qwen_dam_gather).
+    small_device_frames: how many frames of the half-resolution bank stay in HBM (None: all of them).  Later frames go to
+    pinned host chunks of their own; the klarge retrieval sweeps them in place over PCIe (fvs_qwen_klarge_retrieve_tiered),
+    once per step, twice with the cosine metric.  The two caps are independent; results are bit-identical either way."""
 
     CHUNK_BYTES = CHUNK_BYTES
 
-    def __init__(self, flash, merger, device_frames=None):
+    def __init__(self, flash, merger, device_frames=None, small_device_frames=None):
         self.flash, self.merger = flash, merger
         self.device_frames = check_device_frames(device_frames)
+        self.small_device_frames = check_device_frames(small_device_frames, "small_device_frames")
         self.rng = GLOBAL                     # the draws.DrawSource of every k-means draw (a QwenStreamPool stream owns one)
         self.reset()
 
@@ -84,6 +88,10 @@ class QwenStreamState:
         self._layout = None                   # (dtype, x row shape, merged row shape or None) of a bank frame
         self._prev_dam = None                 # (spa_positions, spa_x, DAM rows of video_embeds) before the current step
         self.host_fetches = None              # device int64 [1]: retrieved frames read from the host chunks so far
+        self.small_chunks = []                # pinned chunks of half-resolution frames >= small_device_frames: [F, hs*ws, D]
+        self._small_ptrs = []                 # their mapped device pointers
+        self.n_small_host = 0                 # half-resolution frames in those chunks
+        self._small_layout = None             # (dtype, row shape [hs*ws, D]) of a half-resolution frame
         self.n_frames = 0
         self.grid = None                      # (h, w) of a full-resolution frame; the half-resolution grid is (hs, ws)
         self.small_grid = None
@@ -126,7 +134,8 @@ class QwenStreamState:
         T0, S0 = flash.temporal_length, flash.spatial_length
         # ---- banks (and, once per frame, the merged rows of the frame)
         self._prev_dam = self._dam()
-        small_bank = self.bank_small.append(small_new.view(t, hs * ws, D))
+        self._append_small(small_new.view(t, hs * ws, D), dev)
+        small_bank = self.bank_small.rows() if self.bank_small.n else None
         if S0 > 0 and self.merger is not None:
             merged = (self.merger(x_new) if merged is None else merged).view(t, h * w // 4, -1)
         else:
@@ -215,12 +224,11 @@ class QwenStreamState:
         h, w = self.grid
         D = tem_x.shape[-1]
         n = self.n_frames
-        small_bank = self.bank_small.rows()
-        dt, dev = small_bank.dtype, small_bank.device
+        dt, dev = self._small_layout[0], tem_x.device
         self.tem_x, self.tem_weights, self.tem_timestamp, self.n_tem, self.tem_members = tem_x, tem_w, tem_ts, n_tem, members
         if flash.spatial_length > 0:
             tem_pos = torch.round(tem_ts.float()).to(torch.int64)
-            picks = flash.spatial_picks(small_bank.view(-1, D), n, tem_x, self._thw(n_tem, small=True), tem_w, tem_pos,
+            picks = flash.spatial_picks(self._small_bank(D, dev), n, tem_x, self._thw(n_tem, small=True), tem_w, tem_pos,
                                         draws=d)
             n_spa = picks.numel()                                   # min(n, spatial_length): known on the host
         else:
@@ -293,6 +301,38 @@ class QwenStreamState:
                 cm[dst: dst + cnt].copy_(m3[s: s + cnt], non_blocking=True)
             self.n_host += cnt
 
+    def _small_per_chunk(self) -> int:
+        dt, ps = self._small_layout
+        return chunk_frames(ps.numel() * dt.itemsize, self.CHUNK_BYTES)
+
+    def _append_small(self, s3, dev):
+        """half-resolution frames s3 [t, hs*ws, D], on the device or the host, appended to the two-tier half-resolution
+        bank; copies to its host chunks are asynchronous on the current stream, ordered before the retrieval that sweeps
+        them"""
+        if self._small_layout is None:
+            self._small_layout = (s3.dtype, torch.Size(s3.shape[1:]))
+        dt, ps = self._small_layout
+        F = self._small_per_chunk()
+        for c, dst, s, cnt in placement(self.bank_small.n + self.n_small_host, s3.shape[0], self.small_device_frames, F):
+            if c < 0:
+                self.bank_small.append(s3[s: s + cnt].to(dev, non_blocking=True))
+                continue
+            while len(self.small_chunks) <= c:
+                buf = torch.empty((F,) + tuple(ps), dtype=dt, pin_memory=True)
+                self.small_chunks.append(buf)
+                self._small_ptrs.append(Q.host_device_ptr(buf))
+            self.small_chunks[c][dst: dst + cnt].copy_(s3[s: s + cnt], non_blocking=True)
+            self.n_small_host += cnt
+
+    def _small_bank(self, D, dev):
+        """the half-resolution bank as the retrieval reads it: the HBM rows [n * hs*ws, D] while every frame is there, a
+        qwen.ops.TieredBank once frames have spilled"""
+        rb = self.bank_small
+        if self.n_small_host == 0:
+            return rb.rows().view(-1, D)
+        return Q.TieredBank(rb.rows().view(rb.n, -1) if rb.n else None, rb.n, tuple(self._small_ptrs),
+                            self._small_per_chunk(), rb.n + self.n_small_host, self._small_layout[0], dev)
+
     def _gather(self, picks, spa_x, merged, prev):
         dt, xs, ms = self._layout
         if self.host_fetches is None:
@@ -310,16 +350,13 @@ class QwenStreamState:
         """the whole full-resolution (or merged) bank as one pinned host tensor: device rows D2H, chunk rows H2H"""
         dt, xs, ms = self._layout
         rb = self.bank_merged if merged else self.bank_x
-        out = torch.empty((self.n_frames,) + tuple(ms if merged else xs), dtype=dt, pin_memory=True)
-        if rb.n:
-            out[: rb.n].copy_(rb.rows(), non_blocking=True)
-        torch.cuda.current_stream().synchronize()                    # the spills of the last steps have landed
-        s, F = rb.n, self._per_chunk()
-        for c in range(len(self.host_chunks)):
-            cnt = min(F, rb.n + self.n_host - s)
-            out[s: s + cnt].copy_(self._chunk(c, None)[int(merged)][:cnt])
-            s += cnt
-        return out
+        chunks = [self._chunk(c, None)[int(merged)] for c in range(len(self.host_chunks))]
+        return _on_host(rb, chunks, self.n_frames, ms if merged else xs, dt)
+
+    def _small_on_host(self) -> torch.Tensor:
+        """the whole half-resolution bank as one pinned host tensor: device rows D2H, chunk rows H2H"""
+        dt, ps = self._small_layout
+        return _on_host(self.bank_small, self.small_chunks, self.n_frames, ps, dt)
 
     def _compress_sync(self, cand, cand_w, T, d, start_idx, t):
         """every other branch of temporal_compress (:149-183): pass-through while the memory is filling, temporal_length 0,
@@ -354,15 +391,18 @@ class QwenStreamState:
                     "tem_timestamp_dtype": "float32" if n == 0 else CK.dtype_name(self.tem_timestamp.dtype)}
         if n == 0:
             return CK.qwen(self._config(0, "float16"), counters, {})
-        small = self.bank_small.rows()
-        tensors = {"bank_small": small, "tem_x": self.tem_x, "tem_timestamp": self.tem_timestamp,
-                   "spa_positions": self.spa_positions}
+        dt, ps = self._small_layout
+        tensors = {"tem_x": self.tem_x, "tem_timestamp": self.tem_timestamp, "spa_positions": self.spa_positions}
         if self.tem_weights is not None:          # temporal_method 'sample' keeps no weights
             tensors["tem_weights"] = self.tem_weights
         if self.merger is not None:
             tensors["video_embeds"] = self.video_embeds
-        with torch.cuda.device(small.device):
+        with torch.cuda.device(self.tem_x.device):
             owned = {}                            # spilled banks: assembled in pinned memory here, taken as they are
+            if self.n_small_host:
+                owned["bank_small"] = self._small_on_host()
+            else:
+                tensors["bank_small"] = self.bank_small.rows()
             for name, merged in (("bank_x", False), ("bank_merged", True)):
                 if merged and not counters["merged"]:
                     continue
@@ -370,15 +410,15 @@ class QwenStreamState:
                     owned[name] = self._bank_on_host(merged)
                 else:
                     tensors[name] = (self.bank_merged if merged else self.bank_x).rows()
-            ck = CK.qwen(self._config(int(small.shape[-1]), CK.dtype_name(small.dtype)), counters, tensors, owned=owned)
+            ck = CK.qwen(self._config(int(ps[-1]), CK.dtype_name(dt)), counters, tensors, owned=owned)
             torch.cuda.current_stream().synchronize()
         return ck
 
     @classmethod
-    def restore(cls, ckpt, flash, merger, device, device_frames=None) -> "QwenStreamState":
+    def restore(cls, ckpt, flash, merger, device, device_frames=None, small_device_frames=None) -> "QwenStreamState":
         """A state on `device` that continues `ckpt` bit for bit; `flash` / `merger` must have the configuration the
         checkpoint was taken with (ValueError naming the field otherwise).  The banks' frames are placed by this state's
-        `device_frames`, whatever the cap of the state that took the checkpoint."""
+        `device_frames` and `small_device_frames`, whatever the caps of the state that took the checkpoint."""
         from .. import checkpoint as CK
         if ckpt.family != CK.QWEN:
             raise ValueError(f"QwenStreamState.restore: a {ckpt.family!r} checkpoint is not a Qwen2-VL stream's")
@@ -391,14 +431,14 @@ class QwenStreamState:
         if n["n_frames"] and c["merger_dim"] != md:
             raise ValueError(f"QwenStreamState.restore: config.merger_dim of the checkpoint ({c['merger_dim']}) differs "
                              f"from the merger's ({md})")
-        st = cls(flash, merger, device_frames)
+        st = cls(flash, merger, device_frames, small_device_frames)
         if n["n_frames"] == 0:
             return st
         dev = torch.device(device)
         with torch.cuda.device(dev):
             get = lambda k: ckpt.tensor(k).to(dev, non_blocking=True)
             st._append_frames(ckpt.tensor("bank_x"), ckpt.tensor("bank_merged") if n["merged"] else None, dev)
-            st.bank_small.append(get("bank_small"))
+            st._append_small(ckpt.tensor("bank_small"), dev)
             st.n_frames, st.steps = n["n_frames"], n["steps"]
             st.fast_steps, st.redone_steps = n["fast_steps"], n["redone_steps"]
             st.grid, st.small_grid = tuple(c["grid"]), tuple(c["small_grid"])
@@ -418,12 +458,31 @@ class QwenStreamState:
     def as_list(self):
         """the 13 items of `video_embedding_memory` (:620-624); the thw entries are host tensors, everything else lives in HBM.
         Once frames have spilled to the host chunks, item 7 (the full-resolution bank, which no reader of the list uses) is
-        the zero-row stand-in x[:0]; its thw (item 8) stays exact."""
+        the zero-row stand-in x[:0]; its thw (item 8) stays exact.  Likewise item 9 (the half-resolution bank) once its
+        frames have spilled; item 10 stays exact."""
         n, h, w = self.n_frames, *self.grid
         n_spa = 0 if self.spa_positions is None else int(self.spa_positions.numel())
         ve = self.video_embeds
-        small = self.bank_small.rows().view(-1, self.tem_x.shape[-1])
-        x = self.bank_x.rows().view(n * h * w, -1) if self.n_host == 0 else small[:0]
+        D = self.tem_x.shape[-1]
+        # the stand-ins are zero-row device views of the banks' dtype (tem_x's when no half-resolution frame is in HBM)
+        rows = self.bank_small.rows().view(-1, D) if self.bank_small.n else self.tem_x.reshape(-1, D)
+        small = rows if self.n_small_host == 0 else rows[:0]
+        x = self.bank_x.rows().view(n * h * w, -1) if self.n_host == 0 else rows[:0]
         return [self.tem_x, self._thw(self.n_tem, small=True), self.tem_weights, self.tem_timestamp,
                 self.spa_x, self._thw(n_spa), self.spa_positions,
                 x, self._thw(n), small, self._thw(n, small=True), ve, None if ve is None else ve.shape]
+
+
+def _on_host(rb: RowBank, chunks, n: int, row_shape, dt) -> torch.Tensor:
+    """frames [0, n) of a two-tier bank as one pinned host tensor: the device rows of `rb` D2H, then the filled rows of
+    the host chunks (views [F, *row_shape], in order) H2H"""
+    out = torch.empty((n,) + tuple(row_shape), dtype=dt, pin_memory=True)
+    if rb.n:
+        out[: rb.n].copy_(rb.rows(), non_blocking=True)
+    torch.cuda.current_stream().synchronize()                    # the spills of the last steps have landed
+    s = rb.n
+    for c in chunks:
+        cnt = min(c.shape[0], n - s)
+        out[s: s + cnt].copy_(c[:cnt])
+        s += cnt
+    return out

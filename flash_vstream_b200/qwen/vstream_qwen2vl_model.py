@@ -162,7 +162,7 @@ class FlashMemory(nn.Module):
     def spatial_picks(self, small_x, t, tem_x, tem_thw, tem_weights, tem_positions, draws: Optional[dict] = None):
         """The frame indices spatial_enhance retrieves from a bank of t frames (int64 [min(t, spatial_length)], on
         small_x's device) without touching the full-resolution bank: a caller that keeps that bank elsewhere gathers
-        the frames itself (stream_state.QwenStreamState)."""
+        the frames itself (stream_state.QwenStreamState).  small_x may be a qwen.ops.TieredBank of the t frames."""
         dev = small_x.device
         if t <= self.spatial_length:
             return torch.arange(t, device=dev).long()
@@ -177,7 +177,8 @@ class FlashMemory(nn.Module):
         if self.spatial_method == 'nearest':
             return tem_positions[heaviest]                    # index plumbing only
         # 'klarge_retrieve' (Euclidean distance) / 'klarge_retrieve_cos' (argmin of the cosine similarity, :208-215)
-        return self._klarge_retrieve(tem_x.reshape(_ints(tem_thw)[0], -1), heaviest, small_x.reshape(t, -1),
+        bank = small_x if isinstance(small_x, Q.TieredBank) else small_x.reshape(t, -1)
+        return self._klarge_retrieve(tem_x.reshape(_ints(tem_thw)[0], -1), heaviest, bank,
                                      "cosine" if self.spatial_method == 'klarge_retrieve_cos' else "euclidean")
 
     def _klarge_retrieve(self, centroids, klarge_indices, bank, metric="euclidean"):

@@ -121,15 +121,26 @@ class RealtimeStreamingMixin:
     fvs_bank_device_frames: None (default: every bank frame in HBM) or an integer >= 0 — how many frames of the
     full-resolution and merged feature banks stay in HBM; later frames go to pinned host memory and a step reads back only
     the frames it retrieves (DESIGN.md §3.13).  Results are bit-identical either way.  It applies from the next stream
-    (and to load_video_stream); changing it in the middle of a stream raises ValueError."""
+    (and to load_video_stream); changing it in the middle of a stream raises ValueError.
+
+    fvs_bank_small_device_frames: the same for the half-resolution bank, whose later frames the retrieval sweeps in place
+    over PCIe every step (DESIGN.md §3.13).  With both caps set, a stream's HBM no longer grows with its length."""
 
     fvs_bank_device_frames = None
+    fvs_bank_small_device_frames = None
 
     def _bank_device_frames(self):
-        cap = check_device_frames(self.fvs_bank_device_frames, "fvs_bank_device_frames")
+        return self._cap("fvs_bank_device_frames", "device_frames")
+
+    def _bank_small_device_frames(self):
+        return self._cap("fvs_bank_small_device_frames", "small_device_frames")
+
+    def _cap(self, knob, attr):
+        """the validated value of the cap attribute `knob`, which the stream in progress (its state's `attr`) must share"""
+        cap = check_device_frames(getattr(self, knob), knob)
         st = self.__dict__.get("stream_state")
-        if st is not None and st.n_frames > 0 and self.video_embedding_memory and st.device_frames != cap:
-            raise ValueError(f"fvs_bank_device_frames changed from {st.device_frames} to {cap} in the middle of a stream: "
+        if st is not None and st.n_frames > 0 and self.video_embedding_memory and getattr(st, attr) != cap:
+            raise ValueError(f"{knob} changed from {getattr(st, attr)} to {cap} in the middle of a stream: "
                              f"it takes effect with the next stream (init_streaming())")
         return cap
 
@@ -163,7 +174,7 @@ class RealtimeStreamingMixin:
         with the read-back ("temporal_compress" .. "merger" of the reference's meter are one bucket here: time_3..time_6)."""
         time_0 = time.perf_counter()
         assert self.use_video_streaming_mode
-        cap = self._bank_device_frames()
+        cap, small_cap = self._bank_device_frames(), self._bank_small_device_frames()
         grid_host = video_grid_thw.cpu()          # the grid stays on the host: every shape below comes from it (a CUDA grid
         t, h, w = (int(v) for v in grid_host.reshape(-1, 3)[0].tolist())   # costs one sync here, a host grid none)
         pixel_values_videos = pixel_values_videos.type(self.visual.get_dtype()).to(self.visual.get_device(), non_blocking=True)
@@ -178,7 +189,8 @@ class RealtimeStreamingMixin:
             x_new = small_new = feats
         pub = self.__dict__.get("_qwen_publication")              # set by qwen.serve.export_qwen_memory (opt-in)
         if self.stream_state is None or not self.video_embedding_memory:
-            self.stream_state = QwenStreamState(self.visual.flash_memory, self.visual.merger, device_frames=cap)
+            self.stream_state = QwenStreamState(self.visual.flash_memory, self.visual.merger, device_frames=cap,
+                                                small_device_frames=small_cap)
             if pub is not None:
                 pub.new_stream()
         time_3 = time.perf_counter()
@@ -215,8 +227,9 @@ class RealtimeStreamingMixin:
             raise ValueError(f"load_video_stream: config.grid {ckpt.config['grid']} / {ckpt.config['small_grid']} is not "
                              f"the exported grid {pub.grid} / {pub.small_grid}")
         cap = check_device_frames(self.fvs_bank_device_frames, "fvs_bank_device_frames")
+        small_cap = check_device_frames(self.fvs_bank_small_device_frames, "fvs_bank_small_device_frames")
         state = QwenStreamState.restore(ckpt, self.visual.flash_memory, self.visual.merger, self.visual.get_device(),
-                                        device_frames=cap)
+                                        device_frames=cap, small_device_frames=small_cap)
         if state.n_frames == 0:
             self.stream_state = None
             self._publish([])

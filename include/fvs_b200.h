@@ -454,6 +454,18 @@ size_t fvs_qwen_klarge_workspace_bytes(int k, int t_total, int PD);
 int fvs_qwen_klarge_retrieve(const void* tem_x, const int64_t* klarge_idx, const void* bank, int k, int t_total, int PD,
                              int dtype, int metric, int64_t* idx_out, float* dist_out, void* workspace,
                              size_t workspace_bytes, fvs_stream_t stream);
+/* The same retrieval over a two-tier bank (DESIGN.md §3.13): rows [0, n_dev) are contiguous device rows dev_bank (may be
+ * NULL when n_dev == 0); row n_dev + c*chunk_frames + r is row r of pinned host chunk c, read in place through its mapped
+ * device pointer host_chunks[c] (a HOST array of ceil((t_total - n_dev) / chunk_frames) pointers, fvs_host_device_ptr).
+ * One sweep launch covers the device rows and one each host chunk; the reductions and the tail run once over all t_total
+ * rows, so the results are bit-identical to fvs_qwen_klarge_retrieve on the same rows.  Each step reads the host rows
+ * over PCIe once (Euclidean) or twice (cosine).  With n_dev == t_total it launches exactly what fvs_qwen_klarge_retrieve
+ * launches.  FVS_EINVAL with nothing launched on a bad argument (n_dev outside [0, t_total], a NULL chunk table or chunk
+ * pointer, or chunk_frames <= 0 while host rows exist). */
+int fvs_qwen_klarge_retrieve_tiered(const void* tem_x, const int64_t* klarge_idx, const void* dev_bank, int n_dev,
+                                    const void* const* host_chunks, int chunk_frames, int k, int t_total, int PD, int dtype,
+                                    int metric, int64_t* idx_out, float* dist_out, void* workspace, size_t workspace_bytes,
+                                    fvs_stream_t stream);
 
 /* FlashMemory.calc_am_rope (vstream_qwen2vl_model.py:254-277): out [3, n] int64 position ids of the n = spa_t*spa_h*spa_w
  * + tem_t*tem_h*tem_w memory tokens (DAM rows first, then CSM rows offset by the DAM size), plus visual_start_id. */
