@@ -65,6 +65,11 @@ class ResampleAxis(C.Structure):  # fvs_resample_axis
                [("bounds", C.c_void_p), ("coeffs", C.c_void_p)]
 
 
+class PreprocessJob(C.Structure):  # fvs_preprocess_job
+    _fields_ = [("frames", C.c_void_p)] + [(n, C.c_int) for n in ("T", "H", "W", "C")] + \
+               [("x", ResampleAxis), ("y", ResampleAxis)]
+
+
 PRE_CLIP, PRE_QWEN = 0, 1
 KLARGE_EUCLIDEAN, KLARGE_COSINE = 0, 1
 INPUT_PIXELS, INPUT_FEATURES = 0, 1
@@ -147,6 +152,8 @@ SIGNATURES = {
     "fvs_preprocess_workspace_bytes": (_sz, [C.POINTER(ResampleAxis), C.POINTER(ResampleAxis), _i]),
     "fvs_preprocess": (_i, [_vp, _i, _i, _i, _i, C.POINTER(ResampleAxis), C.POINTER(ResampleAxis), _vp, _i, _i, _vp, _vp, _sz,
                             _vp]),
+    "fvs_preprocess_plan": (_i, [C.POINTER(PreprocessJob), _i, _i, _i, _i64p, _i64p]),
+    "fvs_preprocess_multi": (_i, [C.POINTER(PreprocessJob), _i, _vp, _i, _i, _vp, _vp, _sz, _vp]),
 }
 
 _lib = None

@@ -1,5 +1,6 @@
-// preprocess_kernels.cu — fvs_resample_plan / fvs_preprocess_workspace_bytes / fvs_preprocess: decoded uint8 RGB frames
-// -> the pixels the vision towers take, bit-identical to the reference's CPU image processors.
+// preprocess_kernels.cu — fvs_resample_plan / fvs_preprocess_workspace_bytes / fvs_preprocess / fvs_preprocess_plan /
+// fvs_preprocess_multi: decoded uint8 RGB frames -> the pixels the vision towers take, bit-identical to the reference's
+// CPU image processors.
 //
 // Both reference processors resize with Pillow's BICUBIC resample of an 8-bit RGB image (transformers'
 // image_transforms.resize), which is fixed-point: per-axis int32 coefficients with 22 fractional bits, a horizontal pass
@@ -7,13 +8,18 @@
 // normalize are a function of one byte per channel, so the host hands in a float32 [3, 256] table built with the numpy
 // operations of transformers, and the device only looks values up.
 //
-// Two launches per call: resample_rows_kernel (horizontal pass into a planar uint8 workspace [T, 3, rows, cols]) and
-// resample_cols_kernel (vertical pass, table lookup, and the layout write).  Only the window of the resized image the
+// A call is a table of jobs (clips of any size; fvs_preprocess is the one-job case) and two launches per 32 jobs:
+// resample_rows_kernel (horizontal pass into a planar uint8 workspace [T, 3, rows, cols] per job) and resample_cols_kernel
+// (vertical pass, table lookup, and the layout write).  Both grids are flat: a block finds its job in the block-offset
+// table, so the per-element code is the same whatever the jobs next to it.  Only the window of the resized image the
 // caller asks for is computed (the CLIP center crop): the outputs of the window are the same integers the full resize
 // computes there, because every output depends only on its own taps.
 #include <cuda_fp16.h>
 
+#include <algorithm>
 #include <cmath>
+#include <cstdio>
+#include <vector>
 
 #include "fvs_common.h"
 
@@ -129,26 +135,45 @@ __device__ __forceinline__ int clip8(int acc) {
   return acc < 0 ? 0 : (acc > 255 ? 255 : acc);
 }
 
-struct RowArgs {
+// One clip of a launch: its frames, its slice of the workspace and of the output, and its two axis plans.
+struct Job {
   const uint8_t* src;       // [T, H, W, 3]
   uint8_t* tmp;             // [T, 3, rows, cols]
-  const int2* bounds;       // [cols] {xmin, n}
-  const int* coeffs;        // [cols, taps]
-  int H, W, taps, cols, rows, row0, span0, span;
+  void* out;
+  const int2* xb;           // [cols] {xmin, n}
+  const int* xk;            // [cols, xtaps]
+  const int2* yb;           // [out_rows] {ymin, n}
+  const int* yk;            // [out_rows, ytaps]
+  int H, W, T, xtaps, ytaps, cols, rows, row0, span0, span, out_rows;
 };
 
-// Horizontal pass: block (r, t) stages source row row0 + r of frame t (the columns the window reads) in shared memory
-// and writes its `cols` outputs per channel, clipped to uint8, channel-planar.
-__global__ void __launch_bounds__(kThreads) resample_rows_kernel(const __grid_constant__ RowArgs a) {
-  extern __shared__ uint8_t row[];
-  const int r = blockIdx.x, t = blockIdx.y;
+// Up to kMaxJobs clips per launch pair, in a kernel parameter (no allocation, no copy).  Block b of the rows launch
+// belongs to the job j with row_block0[j] <= b < row_block0[j + 1]; likewise for the cols launch.
+constexpr int kMaxJobs = 32;
+struct MultiArgs {
+  Job job[kMaxJobs];
+  int row_block0[kMaxJobs + 1];
+  int col_block0[kMaxJobs + 1];
+  const float* table;       // [3, 256]
+  int n;
+};
+
+__device__ __forceinline__ int find_job(const int* block0, int n, int b) {
+  int j = 0;
+  while (j + 1 < n && b >= block0[j + 1]) ++j;
+  return j;
+}
+
+// Horizontal pass: row row0 + r of frame t (the columns the window reads) staged in shared memory, `cols` outputs per
+// channel, clipped to uint8, channel-planar.
+__device__ __forceinline__ void resample_row(const Job& a, int r, int t, uint8_t* row) {
   const uint8_t* src = a.src + ((size_t(t) * a.H + a.row0 + r) * a.W + a.span0) * 3;
   for (int i = threadIdx.x; i < a.span * 3; i += blockDim.x) row[i] = src[i];
   __syncthreads();
   for (int i = threadIdx.x; i < 3 * a.cols; i += blockDim.x) {
     const int c = i / a.cols, x = i - c * a.cols;
-    const int2 b = a.bounds[x];
-    const int* k = a.coeffs + size_t(x) * a.taps;
+    const int2 b = a.xb[x];
+    const int* k = a.xk + size_t(x) * a.xtaps;
     const uint8_t* p = row + (b.x - a.span0) * 3 + c;
     int acc = 1 << (kBits - 1);
     for (int j = 0; j < b.y; ++j) acc += int(p[3 * j]) * k[j];
@@ -156,27 +181,14 @@ __global__ void __launch_bounds__(kThreads) resample_rows_kernel(const __grid_co
   }
 }
 
-struct ColArgs {
-  const uint8_t* tmp;       // [T, 3, rows, cols]
-  void* out;
-  const int2* bounds;       // [out_rows] {ymin, n}
-  const int* coeffs;        // [out_rows, taps]
-  const float* table;       // [3, 256]
-  int T, taps, cols, rows, row0, out_rows;
-};
-
 // Vertical pass over output row y of frame t, then the table lookup and the layout write:
 //   FVS_PRE_CLIP  f16 [T, 3, out_rows, cols];
 //   FVS_PRE_QWEN  fp32 [T/2 * gh * gw, 1176], row ((ti*gh/2 + bh)*gw/2 + bw)*4 + mh*2 + mw, column ((c*2 + tp)*14 + py)*14
 //                 + px; a one-frame clip fills both temporal slots.
 template <int kLayout>
-__global__ void __launch_bounds__(kThreads) resample_cols_kernel(const __grid_constant__ ColArgs a) {
-  __shared__ float lut[3 * 256];
-  for (int i = threadIdx.x; i < 3 * 256; i += blockDim.x) lut[i] = a.table[i];
-  __syncthreads();
-  const int y = blockIdx.x, t = blockIdx.y;
-  const int2 b = a.bounds[y];
-  const int* k = a.coeffs + size_t(y) * a.taps;
+__device__ __forceinline__ void resample_col(const Job& a, int y, int t, const float* lut) {
+  const int2 b = a.yb[y];
+  const int* k = a.yk + size_t(y) * a.ytaps;
   for (int i = threadIdx.x; i < 3 * a.cols; i += blockDim.x) {
     const int c = i / a.cols, x = i - c * a.cols;
     const uint8_t* p = a.tmp + ((size_t(t) * 3 + c) * a.rows + (b.x - a.row0)) * a.cols + x;
@@ -196,6 +208,146 @@ __global__ void __launch_bounds__(kThreads) resample_cols_kernel(const __grid_co
       if (a.T == 1) o[(1 - tp) * kPatch * kPatch] = v;
     }
   }
+}
+
+// Flat grids: job j owns blocks [block0[j], block0[j + 1]); its block (t * rows + r) is row r of frame t.
+__global__ void __launch_bounds__(kThreads) resample_rows_kernel(const __grid_constant__ MultiArgs m) {
+  extern __shared__ uint8_t row[];
+  const int j = find_job(m.row_block0, m.n, blockIdx.x);
+  const Job& a = m.job[j];
+  const int b = blockIdx.x - m.row_block0[j], t = b / a.rows;
+  resample_row(a, b - t * a.rows, t, row);
+}
+
+template <int kLayout>
+__global__ void __launch_bounds__(kThreads) resample_cols_kernel(const __grid_constant__ MultiArgs m) {
+  __shared__ float lut[3 * 256];
+  for (int i = threadIdx.x; i < 3 * 256; i += blockDim.x) lut[i] = m.table[i];
+  __syncthreads();
+  const int j = find_job(m.col_block0, m.n, blockIdx.x);
+  const Job& a = m.job[j];
+  const int b = blockIdx.x - m.col_block0[j], t = b / a.out_rows;
+  resample_col<kLayout>(a, b - t * a.out_rows, t, lut);
+}
+
+// ---- host: validation and the plan of a job table -------------------------------------------------------------------
+struct JobPlan {
+  int64_t row_block, col_block;   // first block of the job in its launch pair
+  int64_t out_off, ws_off;        // output elements / workspace bytes before the job
+};
+
+// every check fvs_preprocess makes of one clip; `api` names the job
+int check_job(const fvs_preprocess_job& jb, int layout, int pool, const char* api) {
+  FVS_REQUIRE(jb.frames, "%s: null frames", api);
+  FVS_REQUIRE(jb.C == 3, "%s: %d channels (RGB frames have 3)", api, jb.C);
+  FVS_REQUIRE(jb.T > 0 && jb.H > 0 && jb.W > 0, "%s: empty input [%d, %d, %d, 3]", api, jb.T, jb.H, jb.W);
+  FVS_REQUIRE(jb.T <= 65535, "%s: %d frames in one call (at most 65535)", api, jb.T);
+  int r;
+  if ((r = check_axis(&jb.x, jb.W, "x", api)) || (r = check_axis(&jb.y, jb.H, "y", api))) return r;
+  FVS_REQUIRE(size_t(jb.x.span_count) * 3 <= kRowSmemMax, "%s: a window reading %d source columns is wider than the %zu "
+              "supported", api, jb.x.span_count, kRowSmemMax / 3);
+  FVS_REQUIRE(layout == FVS_PRE_CLIP || layout == FVS_PRE_QWEN, "%s: unknown layout %d", api, layout);
+  if (layout == FVS_PRE_QWEN) {
+    FVS_REQUIRE(jb.T == 1 || jb.T % kTemporal == 0, "%s: Qwen2-VL clips hold 1 or an even number of frames, not %d", api,
+                jb.T);
+    FVS_REQUIRE(pool >= 1, "%s: pool %d < 1", api, pool);
+    const int f = kPatch * kMerge * pool;
+    FVS_REQUIRE(jb.x.first == 0 && jb.x.count == jb.x.out_size && jb.y.first == 0 && jb.y.count == jb.y.out_size,
+                "%s: the Qwen2-VL layout takes the whole resized frame (no crop)", api);
+    FVS_REQUIRE(jb.y.count % f == 0 && jb.x.count % f == 0, "%s: resized %dx%d is not a multiple of %d (patch %d x merge "
+                "%d x pool %d)", api, jb.y.count, jb.x.count, f, kPatch, kMerge, pool);
+  }
+  return FVS_OK;
+}
+
+int64_t out_elements(const fvs_preprocess_job& jb, int layout) {
+  if (layout == FVS_PRE_CLIP) return int64_t(jb.T) * 3 * jb.y.count * jb.x.count;
+  return int64_t(jb.T > 1 ? jb.T / kTemporal : 1) * (jb.y.count / kPatch) * (jb.x.count / kPatch) * kQwenCols;
+}
+
+// Validates every job (the error names the first bad one) and lays them out; returns the number of launch pairs.
+// `one` keeps fvs_preprocess's own messages for its single clip.
+int plan_jobs(const fvs_preprocess_job* jobs, int n, int layout, int pool, JobPlan* plan, int64_t* out_total,
+              int64_t* ws_total, const char* api, bool one) {
+  FVS_REQUIRE(jobs && n > 0, "%s: no jobs", api);
+  int64_t out = 0, ws = 0, rows = 0, cols = 0;
+  char name[96];
+  for (int i = 0; i < n; ++i) {
+    const fvs_preprocess_job& jb = jobs[i];
+    if (one) {
+      std::snprintf(name, sizeof name, "%s", api);
+    } else {
+      std::snprintf(name, sizeof name, "%s: job %d", api, i);
+    }
+    int r = check_job(jb, layout, pool, name);
+    if (r) return r;
+    if (i % kMaxJobs == 0) rows = cols = 0;
+    plan[i] = {rows, cols, out, ws};
+    rows += int64_t(jb.y.span_count) * jb.T;
+    cols += int64_t(jb.y.count) * jb.T;
+    FVS_REQUIRE(rows <= INT32_MAX && cols <= INT32_MAX, "%s: more than %d blocks in one launch", name, INT32_MAX);
+    out += out_elements(jb, layout);
+    ws += int64_t(workspace_bytes(jb.x, jb.y, jb.T));
+  }
+  *out_total = out;
+  *ws_total = ws;
+  return (n + kMaxJobs - 1) / kMaxJobs;
+}
+
+int preprocess_jobs(const fvs_preprocess_job* jobs, int n, const float* table, int layout, int pool, void* out,
+                    void* workspace, size_t workspace_bytes_, cudaStream_t st, const char* api, bool one) {
+  FVS_REQUIRE(jobs && table && out && workspace, "%s: null pointer", api);
+  FVS_REQUIRE(n > 0 && n <= (1 << 20), "%s: %d jobs", api, n);
+  std::vector<JobPlan> plan(n);
+  int64_t out_total = 0, ws_total = 0;
+  const int launches = plan_jobs(jobs, n, layout, pool, plan.data(), &out_total, &ws_total, api, one);
+  if (launches < 0) return launches;
+  FVS_REQUIRE(workspace_bytes_ >= size_t(ws_total), "%s: workspace of %zu bytes < %zu", api, workspace_bytes_,
+              size_t(ws_total));
+  const size_t esize = layout == FVS_PRE_CLIP ? sizeof(__half) : sizeof(float);
+  for (int g = 0; g < launches; ++g) {
+    MultiArgs m = {};
+    m.table = table;
+    m.n = std::min(kMaxJobs, n - g * kMaxJobs);
+    size_t row_smem = 0;
+    for (int k = 0; k < m.n; ++k) {
+      const fvs_preprocess_job& jb = jobs[g * kMaxJobs + k];
+      const JobPlan& p = plan[g * kMaxJobs + k];
+      Job& a = m.job[k];
+      a.src = jb.frames;
+      a.tmp = static_cast<uint8_t*>(workspace) + p.ws_off;
+      a.out = static_cast<char*>(out) + p.out_off * esize;
+      a.xb = reinterpret_cast<const int2*>(jb.x.bounds);
+      a.xk = jb.x.coeffs;
+      a.yb = reinterpret_cast<const int2*>(jb.y.bounds);
+      a.yk = jb.y.coeffs;
+      a.H = jb.H;
+      a.W = jb.W;
+      a.T = jb.T;
+      a.xtaps = jb.x.taps;
+      a.ytaps = jb.y.taps;
+      a.cols = jb.x.count;
+      a.rows = jb.y.span_count;
+      a.row0 = jb.y.span_first;
+      a.span0 = jb.x.span_first;
+      a.span = jb.x.span_count;
+      a.out_rows = jb.y.count;
+      m.row_block0[k] = int(p.row_block);
+      m.col_block0[k] = int(p.col_block);
+      m.row_block0[k + 1] = int(p.row_block + int64_t(a.rows) * a.T);
+      m.col_block0[k + 1] = int(p.col_block + int64_t(a.out_rows) * a.T);
+      row_smem = std::max(row_smem, size_t(a.span) * 3);
+    }
+    resample_rows_kernel<<<m.row_block0[m.n], kThreads, row_smem, st>>>(m);
+    FVS_CHECK_LAUNCH("resample_rows_kernel");
+    if (layout == FVS_PRE_CLIP) {
+      resample_cols_kernel<FVS_PRE_CLIP><<<m.col_block0[m.n], kThreads, 0, st>>>(m);
+    } else {
+      resample_cols_kernel<FVS_PRE_QWEN><<<m.col_block0[m.n], kThreads, 0, st>>>(m);
+    }
+    FVS_CHECK_LAUNCH("resample_cols_kernel");
+  }
+  return FVS_OK;
 }
 
 }  // namespace pre
@@ -234,61 +386,30 @@ int fvs_preprocess(const uint8_t* frames, int T, int H, int W, int C, const fvs_
                    size_t workspace_bytes_, fvs_stream_t stream) {
   const char* api = "fvs_preprocess";
   FVS_REQUIRE(frames && x_h && y_h && table && out && workspace, "%s: null pointer", api);
-  FVS_REQUIRE(C == 3, "%s: %d channels (RGB frames have 3)", api, C);
-  FVS_REQUIRE(T > 0 && H > 0 && W > 0, "%s: empty input [%d, %d, %d, 3]", api, T, H, W);
-  FVS_REQUIRE(T <= 65535, "%s: %d frames in one call (at most 65535)", api, T);
-  int r;
-  if ((r = check_axis(x_h, W, "x", api)) || (r = check_axis(y_h, H, "y", api))) return r;
-  const size_t need = workspace_bytes(*x_h, *y_h, T);
-  FVS_REQUIRE(workspace_bytes_ >= need, "%s: workspace of %zu bytes < %zu", api, workspace_bytes_, need);
-  const size_t row_smem = size_t(x_h->span_count) * 3;
-  FVS_REQUIRE(row_smem <= kRowSmemMax, "%s: a window reading %d source columns is wider than the %zu supported", api,
-              x_h->span_count, kRowSmemMax / 3);
-  FVS_REQUIRE(layout == FVS_PRE_CLIP || layout == FVS_PRE_QWEN, "%s: unknown layout %d", api, layout);
-  if (layout == FVS_PRE_QWEN) {
-    FVS_REQUIRE(T == 1 || T % kTemporal == 0, "%s: Qwen2-VL clips hold 1 or an even number of frames, not %d", api, T);
-    FVS_REQUIRE(pool >= 1, "%s: pool %d < 1", api, pool);
-    const int f = kPatch * kMerge * pool;
-    FVS_REQUIRE(x_h->first == 0 && x_h->count == x_h->out_size && y_h->first == 0 && y_h->count == y_h->out_size,
-                "%s: the Qwen2-VL layout takes the whole resized frame (no crop)", api);
-    FVS_REQUIRE(y_h->count % f == 0 && x_h->count % f == 0, "%s: resized %dx%d is not a multiple of %d (patch %d x merge %d x pool %d)",
-                api, y_h->count, x_h->count, f, kPatch, kMerge, pool);
+  fvs_preprocess_job jb = {frames, T, H, W, C, *x_h, *y_h};
+  return preprocess_jobs(&jb, 1, table, layout, pool, out, workspace, workspace_bytes_, (cudaStream_t)stream, api, true);
+}
+
+int fvs_preprocess_plan(const fvs_preprocess_job* jobs_h, int n_jobs, int layout, int pool, int64_t* plan_h,
+                        int64_t* totals_h) {
+  const char* api = "fvs_preprocess_plan";
+  FVS_REQUIRE(jobs_h && plan_h && totals_h && n_jobs > 0, "%s: null pointer or no jobs", api);
+  std::vector<JobPlan> plan(n_jobs);
+  const int launches = plan_jobs(jobs_h, n_jobs, layout, pool, plan.data(), &totals_h[0], &totals_h[1], api, false);
+  if (launches < 0) return launches;
+  for (int i = 0; i < n_jobs; ++i) {
+    plan_h[4 * i + 0] = plan[i].row_block;
+    plan_h[4 * i + 1] = plan[i].col_block;
+    plan_h[4 * i + 2] = plan[i].out_off;
+    plan_h[4 * i + 3] = plan[i].ws_off;
   }
-  RowArgs ra = {};
-  ra.src = frames;
-  ra.tmp = static_cast<uint8_t*>(workspace);
-  ra.bounds = reinterpret_cast<const int2*>(x_h->bounds);
-  ra.coeffs = x_h->coeffs;
-  ra.H = H;
-  ra.W = W;
-  ra.taps = x_h->taps;
-  ra.cols = x_h->count;
-  ra.rows = y_h->span_count;
-  ra.row0 = y_h->span_first;
-  ra.span0 = x_h->span_first;
-  ra.span = x_h->span_count;
-  cudaStream_t st = (cudaStream_t)stream;
-  resample_rows_kernel<<<dim3(ra.rows, T), kThreads, row_smem, st>>>(ra);
-  FVS_CHECK_LAUNCH("resample_rows_kernel");
-  ColArgs ca = {};
-  ca.tmp = ra.tmp;
-  ca.out = out;
-  ca.bounds = reinterpret_cast<const int2*>(y_h->bounds);
-  ca.coeffs = y_h->coeffs;
-  ca.table = table;
-  ca.T = T;
-  ca.taps = y_h->taps;
-  ca.cols = x_h->count;
-  ca.rows = y_h->span_count;
-  ca.row0 = y_h->span_first;
-  ca.out_rows = y_h->count;
-  if (layout == FVS_PRE_CLIP) {
-    resample_cols_kernel<FVS_PRE_CLIP><<<dim3(ca.out_rows, T), kThreads, 0, st>>>(ca);
-  } else {
-    resample_cols_kernel<FVS_PRE_QWEN><<<dim3(ca.out_rows, T), kThreads, 0, st>>>(ca);
-  }
-  FVS_CHECK_LAUNCH("resample_cols_kernel");
-  return FVS_OK;
+  return launches;
+}
+
+int fvs_preprocess_multi(const fvs_preprocess_job* jobs_h, int n_jobs, const float* table, int layout, int pool, void* out,
+                         void* workspace, size_t workspace_bytes_, fvs_stream_t stream) {
+  return preprocess_jobs(jobs_h, n_jobs, table, layout, pool, out, workspace, workspace_bytes_, (cudaStream_t)stream,
+                         "fvs_preprocess_multi", false);
 }
 
 }  // extern "C"

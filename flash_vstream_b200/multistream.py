@@ -13,6 +13,7 @@ from __future__ import annotations
 import os
 from typing import Optional
 
+import numpy as np
 import torch
 
 from . import ops
@@ -36,10 +37,13 @@ class StreamPool:
     serve.export_bank / MemoryReader).  `close(sid)` resets the bank and keeps it for the next `open`.  Configs the
     fused streaming step does not cover raise NotImplementedError: stream them through the model's single-stream path.
     `device_frames` (ops.StreamBank): every bank of the pool keeps only that many frames of its frame buffer in HBM, the
-    later ones in pinned host memory, so a stream's HBM stays what it was when the bank was made."""
+    later ones in pinned host memory, so a stream's HBM stays what it was when the bank was made.
+    `preprocess` (a preprocess.CLIPFramePreprocessor whose crop is the tower's image size): `step` also takes decoded
+    uint8 frames [t, H, W, 3] per stream (any mix of sizes, host or device); the round's clips go through ONE
+    `preprocess.many` call, whose contiguous output the step reads as it is (no concatenation)."""
 
     def __init__(self, model, *, chunk_cap: int = 1, max_streams: Optional[int] = None,
-                 device_frames: Optional[int] = None):
+                 device_frames: Optional[int] = None, preprocess=None):
         host = model.get_model()
         ntm = host.attention_model
         D = ntm.q_proj.weight.shape[1]
@@ -62,6 +66,7 @@ class StreamPool:
         self.chunk_cap = int(chunk_cap)
         self.device_frames = ops.device_window(self.cfg, self.chunk_cap, device_frames)
         self.max_streams = max_streams
+        self.preprocess = preprocess
         self._streams: dict[int, _Stream] = {}
         self._free: list[ops.StreamBank] = []
         self._next = 0
@@ -130,17 +135,30 @@ class StreamPool:
     # ---- one batched step ----------------------------------------------------------------------------------------------
     def step(self, clips: dict, draws: Optional[dict] = None, *, max_blocks: int = 0):
         """One step of every stream in `clips` ({sid: clip}); the others do not move.  draws={sid: (init_idx, refill_idx)}
-        bypasses a stream's generators.  If any stream's step is refused, no stream moves and no generator advances."""
+        bypasses a stream's generators.  If any stream's step is refused, no stream moves and no generator advances.
+        With `preprocess`, a round of uint8 frames is pre-processed in one call first; a round mixing them with pixels or
+        features is refused."""
         draws = draws or {}
         sids = list(clips)
         streams = [self._streams[sid] for sid in sids]
-        inputs = []
-        for sid in sids:
-            x = clips[sid]
-            if x.ndim == 5:
-                assert x.shape[0] == 1, "one clip per stream"
-                x = x[0]
-            inputs.append(x)
+        frames = {_is_frames(clips[sid]) for sid in sids}
+        if len(frames) > 1:
+            raise ValueError("one step takes uint8 frames, pixels or features for every stream, not a mix")
+        packed = None
+        if frames == {True}:
+            if self.preprocess is None:
+                raise ValueError("uint8 frames need a pool made with preprocess=CLIPFramePreprocessor(...)")
+            packed, inputs = self.preprocess.many([clips[sid] for sid in sids])
+            if packed.dim() != 4:
+                raise ValueError("the preprocessor made crops of different sizes for this round")
+        else:
+            inputs = []
+            for sid in sids:
+                x = clips[sid]
+                if x.ndim == 5:
+                    assert x.shape[0] == 1, "one clip per stream"
+                    x = x[0]
+                inputs.append(x)
         pixels = {x.ndim == 4 and x.shape[1] == 3 for x in inputs}
         if len(pixels) != 1:
             raise ValueError("one step takes either pixels or features for every stream")
@@ -159,7 +177,8 @@ class StreamPool:
                     *d, r = kmeans_draws(st.rng, st.bank.working_rows(t), st.bank.cfg.long_len, self.device)
                 dr.append(d)
                 refills.append(r)
-            ops.stream_step_many([st.bank for st in streams], inputs, vit=vit, draws=dr, max_blocks=max_blocks)
+            ops.stream_step_many([st.bank for st in streams], inputs, vit=vit, draws=dr, max_blocks=max_blocks,
+                                 _packed=packed)
         except BaseException:
             for st, snap in zip(streams, snaps):
                 st.rng.rewind(snap)
@@ -167,3 +186,8 @@ class StreamPool:
         for st, r in zip(streams, refills):
             if r is not None:          # learn (asynchronously) how many refill candidates the device consumed
                 r.consumed_from(st.bank.info()[1])
+
+
+def _is_frames(clip) -> bool:
+    """decoded frames (uint8 [t, H, W, 3], tensor or array), as opposed to pixels or features"""
+    return clip.dtype == (torch.uint8 if isinstance(clip, torch.Tensor) else np.uint8)

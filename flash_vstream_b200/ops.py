@@ -545,11 +545,14 @@ class StreamBank:
         return lab, info, key, wsum
 
 
-def stream_step_many(banks, inputs, *, vit: Optional[VitEncoder] = None, draws=None, max_blocks: int = 0):
+def stream_step_many(banks, inputs, *, vit: Optional[VitEncoder] = None, draws=None, max_blocks: int = 0,
+                     _packed: Optional[torch.Tensor] = None):
     """One step for many streams (fvs_stream_step_multi): banks[i] takes clip inputs[i] — pixels [t_i,3,S,S] (with `vit`)
     or finished ViT features [t_i, grid*grid, D] f16.  Bit-identical to banks[0].step(inputs[0], ...), then banks[1]...,
     with the same draws.  draws: None or a list with (init_idx, refill_idx) | None per bank.  max_blocks caps the blocks
-    of one consolidation launch (0 = the device's co-residency limit).  If any bank's step is refused, no bank moves."""
+    of one consolidation launch (0 = the device's co-residency limit).  If any bank's step is refused, no bank moves.
+    _packed: the clips already back to back in one contiguous tensor (inputs[i] its consecutive slices, e.g. the views
+    of a preprocessor's many()), which the step then reads in place of their concatenation."""
     banks, inputs = list(banks), list(inputs)
     if not banks or len(banks) != len(inputs):
         raise ValueError(f"{len(banks)} banks for {len(inputs)} clips")
@@ -585,7 +588,18 @@ def stream_step_many(banks, inputs, *, vit: Optional[VitEncoder] = None, draws=N
     else:
         for x in inputs:
             assert x.dtype == torch.float16 and x.shape[1] == b0.cfg.grid ** 2 and x.shape[2] == b0.D, x.shape
-    inp = _c(torch.cat(inputs, dim=0)) if len(inputs) > 1 else _c(inputs[0])
+    if _packed is not None:
+        if (not _packed.is_contiguous() or _packed.dtype != inputs[0].dtype or tuple(_packed.shape[1:]) != tuple(inputs[0].shape[1:])
+                or _packed.shape[0] != sum(x.shape[0] for x in inputs)):
+            raise ValueError(f"packed clips {_packed.dtype} {tuple(_packed.shape)} are not the {len(inputs)} clips back to back")
+        row, off = _packed[0].numel() * _packed.element_size(), 0
+        for x in inputs:
+            if x.data_ptr() != _packed.data_ptr() + off * row:
+                raise ValueError("packed clips: the clips are not consecutive slices of the packed tensor")
+            off += x.shape[0]
+        inp = _packed
+    else:
+        inp = _c(torch.cat(inputs, dim=0)) if len(inputs) > 1 else _c(inputs[0])
     for i, bank in enumerate(banks):
         t = inputs[i].shape[0]
         bank._reserve_frames(t)

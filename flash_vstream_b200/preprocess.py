@@ -137,14 +137,19 @@ class _FramePreprocessor:
             t = self._tables[device] = torch.from_numpy(self.table).to(device)
         return t
 
-    def _frames(self, frames):
+    @staticmethod
+    def _tensor(frames, what="frames"):
         import torch
         if isinstance(frames, np.ndarray):
             frames = torch.from_numpy(frames)
         if not isinstance(frames, torch.Tensor):
-            raise TypeError(f"frames must be a uint8 tensor or array [T, H, W, 3], got {type(frames).__name__}")
+            raise TypeError(f"{what} must be a uint8 tensor or array [T, H, W, 3], got {type(frames).__name__}")
         if frames.dtype != torch.uint8 or frames.dim() != 4:
-            raise ValueError(f"frames must be uint8 [T, H, W, 3], got {frames.dtype} {tuple(frames.shape)}")
+            raise ValueError(f"{what} must be uint8 [T, H, W, 3], got {frames.dtype} {tuple(frames.shape)}")
+        return frames
+
+    def _frames(self, frames):
+        frames = self._tensor(frames)
         device = self._device(frames)
         if not frames.is_cuda:
             frames = frames.to(device, non_blocking=True)
@@ -180,6 +185,54 @@ class _FramePreprocessor:
                                                   workspace.data_ptr(), workspace.numel() * workspace.element_size(),
                                                   _lib.cur_stream()), "fvs_preprocess")
         return out
+
+    def _many(self, clips, out=None, workspace=None):
+        """-> (out, one view of `out` per clip): every clip through one fvs_preprocess_multi call"""
+        import torch
+        if not isinstance(clips, (list, tuple)):
+            raise TypeError(f"clips must be a list of uint8 [T, H, W, 3] clips, got {type(clips).__name__}")
+        if not clips:
+            raise ValueError("clips is empty")
+        clips = [self._tensor(f, f"clip {i}") for i, f in enumerate(clips)]
+        devices = {f.device for f in clips if f.is_cuda}
+        if len(devices) > 1:
+            raise ValueError(f"the clips are on more than one device: {sorted(map(str, devices))}")
+        device = devices.pop() if devices else self._device()
+        n = len(clips)
+        jobs = (_lib.PreprocessJob * n)()
+        for i, f in enumerate(clips):           # planned from the shapes: a refused call copies nothing to the device
+            T, H, W, ch = f.shape
+            x, y, pool, _ = self._plan(device, H, W)
+            jobs[i] = _lib.PreprocessJob(f.data_ptr(), T, H, W, ch, x, y)
+        lib = _lib.load()
+        plan, totals = (C.c_int64 * (4 * n))(), (C.c_int64 * 2)()
+        launches = lib.fvs_preprocess_plan(jobs, n, self._layout, pool, plan, totals)
+        if launches < 0:
+            _lib.check(launches, "fvs_preprocess_plan")
+        frames = [(f if f.is_cuda else f.to(device, non_blocking=True)).contiguous() for f in clips]
+        for i, f in enumerate(frames):
+            jobs[i].frames = f.data_ptr()
+        shapes = [self.output_shape(*(int(v) for v in f.shape[:3])) for f in frames]
+        if len({s[1:] for s in shapes}) == 1:       # CLIP with one crop, and every Qwen2-VL call: one stacked tensor
+            shape = (sum(s[0] for s in shapes),) + shapes[0][1:]
+        else:
+            shape = (int(totals[0]),)
+        dtype = torch.float16 if self._layout == _lib.PRE_CLIP else torch.float32
+        if out is None:
+            out = torch.empty(shape, dtype=dtype, device=device)
+        elif tuple(out.shape) != shape or out.dtype != dtype or out.device != device or not out.is_contiguous():
+            raise ValueError(f"out must be a contiguous {dtype} {shape} tensor on {device}")
+        if workspace is None:
+            workspace = torch.empty(int(totals[1]), dtype=torch.uint8, device=device)
+        elif workspace.device != device:
+            raise ValueError(f"workspace must be on {device}")
+        with torch.cuda.device(device):
+            _lib.check(lib.fvs_preprocess_multi(jobs, n, self._table(device).data_ptr(), self._layout, pool, out.data_ptr(),
+                                                workspace.data_ptr(), workspace.numel() * workspace.element_size(),
+                                                _lib.cur_stream()), "fvs_preprocess_multi")
+        flat = out.view(-1)
+        views = [flat[plan[4 * i + 2]: plan[4 * i + 2] + math.prod(s)].view(s) for i, s in enumerate(shapes)]
+        return out, views
 
 
 class CLIPFramePreprocessor(_FramePreprocessor):
@@ -228,6 +281,13 @@ class CLIPFramePreprocessor(_FramePreprocessor):
     def __call__(self, frames, out=None, workspace=None):
         return self._run(frames, out, workspace)
 
+    def many(self, clips, out=None, workspace=None):
+        """Many clips (a list of uint8 [T, H, W, 3], host or device, any mix of sizes) in one launch pair per 32 clips ->
+        (out, views): out f16 [sum T, 3, crop, crop] (1-D when the clips' crops differ), views[i] the [T_i, 3, h, w] slice
+        of clip i, bit-identical to self(clips[i]).  out and workspace (the sum of workspace_bytes
+        over the clips) may be given."""
+        return self._many(clips, out, workspace)
+
 
 class Qwen2VLFramePreprocessor(_FramePreprocessor):
     """Qwen2-VL side: frames -> {'pixel_values_videos': fp32 [t*gh*gw, 1176] on the device, 'video_grid_thw': int64
@@ -262,3 +322,13 @@ class Qwen2VLFramePreprocessor(_FramePreprocessor):
         pixels = self._run(frames, out, workspace)
         T, H, W = (int(v) for v in frames.shape[:3])
         return {"pixel_values_videos": pixels, "video_grid_thw": torch.tensor([self.grid_thw(T, H, W)], dtype=torch.int64)}
+
+    def many(self, clips, out=None, workspace=None):
+        """Many clips (a list of uint8 [T, H, W, 3], host or device, any mix of sizes) in one launch pair per 32 clips ->
+        (out, views, grids): out fp32 [sum t*gh*gw, 1176], views[i] clip i's rows and grids[i] its int64 [[t, gh, gw]]
+        (host), bit-identical to self(clips[i]).  out and workspace (the sum of workspace_bytes
+        over the clips) may be given."""
+        import torch
+        out, views = self._many(clips, out, workspace)
+        grids = [torch.tensor([self.grid_thw(*(int(v) for v in f.shape[:3]))], dtype=torch.int64) for f in clips]
+        return out, views, grids

@@ -92,12 +92,15 @@ class QwenStreamPool:
     batched round does not cover raise NotImplementedError naming the knob: stream them through the host's single-stream
     path.  `device_frames` and `small_device_frames` apply to every stream, as `fvs_bank_device_frames` and
     `fvs_bank_small_device_frames` do to the host's stream (DESIGN.md §3.13).  TOWER_ROWS bounds the rows of one tower
-    call (its workspace is about 30 KB per row at 1280 wide)."""
+    call (its workspace is about 30 KB per row at 1280 wide).  `preprocess` (a preprocess.Qwen2VLFramePreprocessor):
+    `step` also takes decoded uint8 frames [T, H, W, 3] per stream (any mix of sizes, host or device); the round's clips
+    go through ONE `preprocess.many` call, and each stream's rows and grid then make its (pixel_values_videos,
+    video_grid_thw)."""
 
     TOWER_ROWS = 65536
 
     def __init__(self, model, device_frames: Optional[int] = None, max_streams: Optional[int] = None,
-                 small_device_frames: Optional[int] = None):
+                 small_device_frames: Optional[int] = None, preprocess=None):
         visual = model.visual
         flash, tower = visual.flash_memory, visual.encode_patches
         if not isinstance(tower, QwenVisionBlocksB200):
@@ -119,6 +122,7 @@ class QwenStreamPool:
         self.device_frames = check_device_frames(device_frames, "device_frames")
         self.small_device_frames = check_device_frames(small_device_frames, "small_device_frames")
         self.max_streams = max_streams
+        self.preprocess = preprocess
         self._streams: dict[int, _Stream] = {}
         self._next = 0
 
@@ -227,9 +231,23 @@ class QwenStreamPool:
         round raises before anything is enqueued: no stream moves and no generator advances.  A stream whose clip raises
         while being completed (ZeroDivisionError on an empty cluster, as the reference) is left as the single-stream
         path leaves it; every other stream completes, and then the round raises one error naming the failing sids
-        (`.errors`: sid -> exception)."""
+        (`.errors`: sid -> exception).  With `preprocess`, a round of uint8 frames ({sid: [T, H, W, 3]}) is pre-processed
+        in one call first; a round mixing them with (pixels, grid) clips is refused."""
         draws = draws or {}
         sids = list(clips)
+        frames = {not isinstance(clips[sid], (tuple, list)) for sid in sids}
+        if len(frames) > 1:
+            raise ValueError("QwenStreamPool.step: one round takes uint8 frames or (pixels, grid) clips for every stream, "
+                             "not a mix")
+        if frames == {True}:
+            if self.preprocess is None:
+                raise ValueError("QwenStreamPool.step: uint8 frames need a pool made with "
+                                 "preprocess=Qwen2VLFramePreprocessor(...)")
+            for sid in sids:
+                if sid not in self._streams:
+                    raise KeyError(f"QwenStreamPool.step: no stream {sid}")
+            _, rows, grids = self.preprocess.many([clips[sid] for sid in sids])
+            clips = dict(zip(sids, zip(rows, grids)))
         items = [self._validate(sid, clips[sid]) for sid in sids]
         feats = self._encode(items)
         merged = [None] * len(sids)

@@ -24,7 +24,7 @@ import torch
 
 from .. import _lib as L
 from ..ops import _chk_cuda
-from ..serve import MetricMeter
+from ..serve import MetricMeter, serve_pool
 
 HEADER_FIELDS = ("seq", "epoch", "clips", "n_frames", "n_tem", "n_spa", "rows", "grid")
 STATUS_FIELDS = ("seq0", "seq1") + HEADER_FIELDS[1:]
@@ -227,3 +227,22 @@ def frame_memory_manager(model, frame_queue, *, preprocess=None, time_meter: Opt
         if on_clip is not None:
             on_clip(frame_cnt)
     return frame_cnt
+
+
+def pool_memory_manager(pool, queues, *, time_meter: Optional[dict] = None, on_round=None, meter_device_time: bool = True):
+    """frame_memory_manager for many streams of one QwenStreamPool.  `queues` maps the sid of each stream (opened in
+    `pool` with its own seed) to its frame queue; None on a queue ends that stream only, its publication keeps the last
+    memory, and the loop returns {sid: frames embedded} once every queue has ended.  Each round takes at most one clip
+    from every queue that has one (later clips wait, in order, for later rounds), blocks for the next clip when none has
+    one, and runs ONE pool.step: uint8 frames [T, H, W, 3] when the pool has a preprocessor (one pre-processing call per
+    round), else the video_inputs dicts of embed_new_video_clip.  Frames are counted as frame_memory_manager counts them.
+    'memory_latency' is metered per stream into time_meter[sid] (a MetricMeter; a stream's first clip not logged),
+    waiting on an event with meter_device_time.  Readers attach at any time, before the first frame too:
+    QwenMemoryReader(*export_qwen_memory(pool.stream(sid), grid=(h, w))).  on_round({sid: frames}) runs after each
+    round.  Each queue is read by one thread that holds at most one of its clips, so a bounded queue still holds its
+    producer back; the threads end with their queue's None, or when the loop raises, and the exception's `unconsumed`
+    then gives back, per stream, the clips taken from its queue that were not embedded."""
+    def step(clips):
+        pool.step({k: (c["pixel_values_videos"], c["video_grid_thw"]) if isinstance(c, dict) else c for k, c in clips.items()})
+    return serve_pool(queues, step, _clip_frames, time_meter=time_meter, on_round=on_round,
+                      meter_device_time=meter_device_time)

@@ -17,9 +17,14 @@ The Manager-list protocol of the unmodified CLI keeps working too: embed_video_s
 `video_embedding_memory` is a Manager proxy (see VStreamMetaForCausalLM._publish), which is the reference's own cost model.
 
 MetricMeter mirrors the reference's meter (cli_video_stream.py:33-99) with the same bucket names
-('memory_latency' in the memory manager, :194-196)."""
+('memory_latency' in the memory manager, :194-196).
+
+pool_memory_manager is the same loop for many streams of one multistream.StreamPool: one frame queue per stream, one
+pool step per round (DESIGN.md §3.9)."""
 from __future__ import annotations
 
+import queue as _queue
+import threading
 import time
 from typing import Optional
 
@@ -138,3 +143,158 @@ def frame_memory_manager(model, frame_queue, *, preprocess=None, time_meter: Opt
         if on_step is not None:
             on_step(frame_cnt)
     return frame_cnt
+
+
+# ---- many streams: one pool, one queue per stream ---------------------------------------------------------------------
+def form_round(keys, ready, ended):
+    """The next round of a pool serve loop, from which streams have a clip at the head of their queue (`ready`) and which
+    have ended (`ended`: their None was taken).  -> (take, done): take = the live streams with a clip ready, in `keys`
+    order, one clip each; done = every stream has ended.  take == [] and not done: wait for the next clip."""
+    take = [k for k in keys if k in ready and k not in ended]
+    return take, all(k in ended for k in keys)
+
+
+class _Inbox:
+    """One thread per queue hands the loop that queue's next item, and holds at most one item at a time: the others stay
+    in the caller's queue, so a bounded queue (the reference's Queue(maxsize=10)) still holds its producer back.  After
+    the loop takes a stream's item, that stream's thread looks at its queue without blocking ("fetching"), and the loop
+    forms its next round only once every such look is done, so a round has every stream whose queue has a clip.  The
+    loop waits on a condition for whichever thread delivers next.  A thread ends after handing over its queue's None, or
+    at close(); it waits in q.get with a timeout only so that close() is seen, and an item is handed over as soon as it
+    is put."""
+    STOP_CHECK_S = 0.05
+
+    def __init__(self, queues):
+        self.cv = threading.Condition()
+        self.held = {}                                    # key -> the item taken from its queue, not yet given out
+        self.fetching = set(queues)                       # keys whose thread has not looked at its queue yet
+        self.stop = False
+        self.threads = [threading.Thread(target=self._forward, args=(k, q), name=f"pool-queue-{k}", daemon=True)
+                        for k, q in queues.items()]
+        for t in self.threads:
+            t.start()
+
+    def _get(self, key, q):
+        """the queue's next item, or _STOP once close() was called"""
+        try:
+            return q.get_nowait()
+        except _queue.Empty:
+            pass
+        with self.cv:
+            self.fetching.discard(key)                    # looked: empty for now
+            self.cv.notify_all()
+        while True:
+            try:
+                return q.get(timeout=self.STOP_CHECK_S)
+            except _queue.Empty:
+                with self.cv:
+                    if self.stop:
+                        return _STOP
+
+    def _forward(self, key, q):
+        while True:
+            with self.cv:
+                while key in self.held and not self.stop:
+                    self.cv.wait()
+                if self.stop:
+                    return
+            item = self._get(key, q)
+            if item is _STOP:
+                return
+            with self.cv:                                 # kept even after close(): close() returns it
+                self.held[key] = item
+                self.fetching.discard(key)
+                self.cv.notify_all()
+            if item is None:
+                return
+
+    def ready(self, block: bool) -> set:
+        """the keys whose next item is held, once every thread has looked at its queue; with `block`, wait until there
+        is one"""
+        with self.cv:
+            while self.fetching or (block and not self.held):
+                self.cv.wait()
+            return set(self.held)
+
+    def take(self, key):
+        with self.cv:
+            item = self.held.pop(key)
+            if item is not None:                          # the thread of an ended stream has returned
+                self.fetching.add(key)
+            self.cv.notify_all()
+            return item
+
+    def close(self) -> dict:
+        """stop and join every thread; -> the items taken from the queues and not given out"""
+        with self.cv:
+            self.stop = True
+            self.cv.notify_all()
+        for t in self.threads:
+            t.join()
+        return self.held
+
+
+_STOP = object()
+
+
+def serve_pool(queues, step, frames_of, *, time_meter=None, on_round=None, meter_device_time: bool = True):
+    """The loop of both families' pool_memory_manager: rounds from form_round, one `step({key: clip})` per round.  If the
+    loop raises, its queue threads are stopped first, and the exception's `unconsumed` maps each stream to the items
+    taken from its queue that no completed round embedded, in queue order (the failed round's clip, then the one item
+    held for the next round; a None among them is the stream's end)."""
+    keys = list(queues)
+    inbox = _Inbox(queues)
+    meters = time_meter if time_meter is not None else {}
+    ended, counts, wait, clips = set(), {k: 0 for k in keys}, False, {}
+    try:
+        while True:
+            ready = inbox.ready(block=wait)
+            for k in ready:                               # None at the head of a queue ends that stream only
+                if k not in ended and inbox.held[k] is None:
+                    inbox.take(k)
+                    ended.add(k)
+            take, done = form_round(keys, ready - ended, ended)
+            if done:
+                return counts
+            wait = not take
+            if wait:
+                continue
+            clips = {k: inbox.take(k) for k in take}
+            start_time = time.perf_counter()
+            with torch.no_grad():
+                step(clips)
+            if meter_device_time:
+                ev = torch.cuda.Event()
+                ev.record()
+                ev.synchronize()
+            latency = time.perf_counter() - start_time
+            for k in take:
+                if counts[k] > 0:                         # a stream's first clip is not logged (cli_video_stream.py:193)
+                    meters.setdefault(k, MetricMeter()).add('memory_latency', latency)
+                counts[k] += frames_of(clips[k])
+            clips = {}
+            if on_round is not None:
+                on_round(dict(counts))
+    except BaseException as e:
+        held = inbox.close()
+        e.unconsumed = {k: [c for c in ((clips[k],) if k in clips else ()) + ((held[k],) if k in held else ())]
+                        for k in keys if k in clips or k in held}
+        raise
+    finally:
+        inbox.close()
+
+
+def pool_memory_manager(pool, queues, *, time_meter: Optional[dict] = None, on_round=None, meter_device_time: bool = True):
+    """frame_memory_manager for many streams of one multistream.StreamPool.  `queues` maps the sid of each stream (opened
+    in `pool` with its own seed) to its frame queue; None on a queue ends that stream only, its bank keeps the last
+    memory, and the loop returns {sid: frames embedded} once every queue has ended.  Each round takes at most one clip
+    from every queue that has one (later clips wait, in order, for later rounds), blocks for the next clip when none has
+    one, and runs ONE pool.step: uint8 frames [t, H, W, 3] when the pool has a preprocessor (one pre-processing call per
+    round), else pixels [t, 3, S, S].  'memory_latency' is metered per stream into time_meter[sid] (a MetricMeter; a
+    stream's first clip not logged), waiting on an event with meter_device_time like frame_memory_manager.  Readers
+    attach at any time, before the first frame too: MemoryReader(*export_bank(pool.bank(sid))).  on_round({sid: frames})
+    runs after each round.  Each queue is read by one thread that holds at most one of its clips, so a bounded queue
+    still holds its producer back; the threads end with their queue's None, or when the loop raises, and the
+    exception's `unconsumed` then gives back, per stream, the clips taken from its queue that were not embedded."""
+    return serve_pool(queues, pool.step, lambda clip: int(clip.shape[0]), time_meter=time_meter, on_round=on_round,
+                      meter_device_time=meter_device_time)

@@ -556,6 +556,26 @@ size_t fvs_preprocess_workspace_bytes(const fvs_resample_axis* x_h, const fvs_re
 int fvs_preprocess(const uint8_t* frames, int T, int H, int W, int C, const fvs_resample_axis* x_h,
                    const fvs_resample_axis* y_h, const float* table, int layout, int pool, void* out, void* workspace,
                    size_t workspace_bytes, fvs_stream_t stream);
+/* Many clips, one configuration (table, layout, pool), one contiguous output.  Job i is clip i with its own frames, size
+ * and axis plans (host structs of fvs_resample_plan with device tables).  Each job writes at its own offset: the outputs
+ * of the jobs lie back to back in job order (CLIP: f16 [sum T, 3, y.count, x.count] when every job has the same window;
+ * Qwen2-VL: fp32 rows [sum t * gh * gw, 1176]), and each takes its own slice of one workspace.  Every job's bits equal
+ * fvs_preprocess on that clip alone (it is the one-job case of the same code).  One launch pair per 32 jobs: a flat grid
+ * whose blocks find their job in a block-offset table passed as a kernel parameter.  Every job is checked as
+ * fvs_preprocess checks its clip before anything is launched; FVS_EINVAL names the first bad job. */
+typedef struct fvs_preprocess_job {
+  const uint8_t* frames;        /* device uint8 [T, H, W, C = 3] */
+  int T, H, W, C;
+  fvs_resample_axis x, y;
+} fvs_preprocess_job;
+/* Host plan of a job table (pure host arithmetic, validates like fvs_preprocess_multi, no CUDA call): plan_h [n_jobs, 4] =
+ * {first block of the job in its rows launch, in its cols launch, output elements before it, workspace bytes before it};
+ * totals_h [2] = {output elements, workspace bytes}.  Returns the number of launch pairs (>= 1) or a negative error. */
+int fvs_preprocess_plan(const fvs_preprocess_job* jobs_h, int n_jobs, int layout, int pool, int64_t* plan_h,
+                        int64_t* totals_h);
+/* workspace: at least totals_h[1] bytes of fvs_preprocess_plan; out: totals_h[0] elements. */
+int fvs_preprocess_multi(const fvs_preprocess_job* jobs_h, int n_jobs, const float* table, int layout, int pool, void* out,
+                         void* workspace, size_t workspace_bytes, fvs_stream_t stream);
 
 #ifdef __cplusplus
 }
