@@ -25,6 +25,7 @@ import torch.nn as nn
 from .. import _lib as L
 from ..draws import GLOBAL
 from ..vstream_arch import _is_manager_proxy
+from . import offline as _offline_pass
 from . import vstream_qwen2vl_model as _offline
 from .compress_functions import weighted_kmeans_ordered_feature
 from .patch_merger import PatchMerger
@@ -65,13 +66,37 @@ class FlashMemory(_offline.FlashMemory):
 
 
 class VisualB200(nn.Module):
-    """The `self.visual` object of the streaming model for this path: flash_memory + merger + the injected ViT blocks."""
+    """The `self.visual` object of the streaming model for this path: flash_memory + merger + the injected ViT blocks.
+    `forward` is the offline pass of the same object (qwen/offline.py); offline_max_rows bounds the tower rows of one of
+    its calls (whole temporal patches per call, DESIGN.md §3.16)."""
 
     def __init__(self, flash_memory: FlashMemory, merger: PatchMerger, encode_patches: Optional[Callable] = None,
-                 dtype=torch.bfloat16, device="cuda"):
+                 dtype=torch.bfloat16, device="cuda", offline_max_rows: int = _offline_pass.DEFAULT_MAX_ROWS):
         super().__init__()
         self.flash_memory, self.merger, self.encode_patches = flash_memory, merger, encode_patches
         self._dtype, self._device = dtype, torch.device(device)
+        self.offline_max_rows = _offline_pass.check_max_rows(offline_max_rows)
+
+    @classmethod
+    def from_reference(cls, visual, *, dtype=None, device="cuda", offline_max_rows: int = _offline_pass.DEFAULT_MAX_ROWS,
+                       **tower_kw):
+        """From the reference's FlashVStreamQwen2VisionTransformerPretrainedModel: its blocks (QwenVisionBlocksB200),
+        the mirror FlashMemory of its flash_memory.config and its merger, in `dtype` (default: the module's)."""
+        from .vision_tower import QwenVisionBlocksB200
+        dtype = dtype or next(visual.parameters()).dtype
+        tower = QwenVisionBlocksB200.from_module(visual, dtype=dtype, device=device, **tower_kw)
+        m = visual.merger
+        merger = PatchMerger.from_weights({k: v.detach().to(dtype) for k, v in (
+            ("ln_w", m.ln_q.weight), ("ln_b", m.ln_q.bias), ("fc1_w", m.mlp[0].weight), ("fc1_b", m.mlp[0].bias),
+            ("fc2_w", m.mlp[2].weight), ("fc2_b", m.mlp[2].bias))}, device=device)
+        return cls(FlashMemory(**visual.flash_memory.config), merger, encode_patches=tower, dtype=dtype, device=device,
+                   offline_max_rows=offline_max_rows)
+
+    def forward(self, hidden_states, grid_thw, position_ids, visual_position_ids, draws: Optional[list] = None):
+        """vstream_qwen2vl_model.py:388-428: (video_embeds, position_ids).  The full-resolution tower runs only on the
+        frames the memory keeps, in chunks of at most offline_max_rows rows; the bits are the unpruned pass's."""
+        return _offline_pass.forward(self, hidden_states, grid_thw, position_ids, visual_position_ids, draws=draws,
+                                     max_rows=self.offline_max_rows)
 
     def _apply(self, fn, recurse=True):
         """.cuda() / .to(device) of this module or of its host also move the injected tower (QwenVisionBlocksB200.to), so
