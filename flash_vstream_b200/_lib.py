@@ -70,6 +70,30 @@ class PreprocessJob(C.Structure):  # fvs_preprocess_job
                [("x", ResampleAxis), ("y", ResampleAxis)]
 
 
+class QwenMemJob(C.Structure):  # fvs_qwen_mem_job
+    _fields_ = [("X", C.c_void_p)] + [(n, C.c_int) for n in ("T", "K", "PD", "x_dtype")] + \
+               [(n, C.c_void_p) for n in ("w", "init_idx", "refill_idx")] + [("max_iter", C.c_int), ("tol", C.c_float)] + \
+               [(n, C.c_void_p) for n in ("uniq_idx", "n_unique", "uniq_workspace")] + [("uniq_workspace_bytes", C.c_size_t)] + \
+               [(n, C.c_void_p) for n in ("C", "wsum", "labels", "info", "km_workspace")] + \
+               [("km_workspace_bytes", C.c_size_t)] + \
+               [(n, C.c_void_p) for n in ("order_in", "sorted_idx", "ts", "w_sorted", "flags", "out")] + [("out_dtype", C.c_int)]
+
+
+class QwenRetrieveJob(C.Structure):  # fvs_qwen_retrieve_job
+    _fields_ = [(n, C.c_void_p) for n in ("tem_x", "klarge_idx", "bank")] + \
+               [(n, C.c_int) for n in ("k", "t_total", "n_dev", "PD")] + \
+               [(n, C.c_void_p) for n in ("idx_out", "dist_out", "workspace")] + [("workspace_bytes", C.c_size_t)]
+
+
+class QwenGatherJob(C.Structure):  # fvs_qwen_gather_job
+    _fields_ = [("picks", C.c_void_p), ("n", C.c_int), ("n_frames", C.c_int64), ("dev_x", C.c_void_p),
+                ("dev_merged", C.c_void_p), ("n_dev", C.c_int64), ("host_chunks", C.c_void_p), ("chunk_frames", C.c_int),
+                ("prev_picks", C.c_void_p), ("m", C.c_int), ("prev_x", C.c_void_p), ("prev_merged", C.c_void_p),
+                ("x_frame_elems", C.c_int64), ("merged_frame_elems", C.c_int64), ("spa_x_out", C.c_void_p),
+                ("merged_out", C.c_void_p), ("host_fetches", C.c_void_p)]
+
+
+QWEN_MEM_JOBS_PER_LAUNCH = 16
 PRE_CLIP, PRE_QWEN = 0, 1
 KLARGE_EUCLIDEAN, KLARGE_COSINE = 0, 1
 INPUT_PIXELS, INPUT_FEATURES = 0, 1
@@ -133,6 +157,13 @@ SIGNATURES = {
     "fvs_qwen_kmeans": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _f, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "fvs_qwen_kmeans_finalize": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
     "fvs_gather_rows_cast": (_i, [_vp, _vp, _vp, _i, C.c_int64, _i, _vp]),
+    "fvs_qwen_mem_plan": (_i, [C.POINTER(QwenMemJob), _i, _i, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
+    "fvs_qwen_unique_rows_multi": (_i, [C.POINTER(QwenMemJob), _i, _i, _vp]),
+    "fvs_qwen_kmeans_multi": (_i, [C.POINTER(QwenMemJob), _i, _i, _vp]),
+    "fvs_qwen_kmeans_finalize_multi": (_i, [C.POINTER(QwenMemJob), _i, _i, _vp]),
+    "fvs_gather_rows_cast_multi": (_i, [C.POINTER(QwenMemJob), _i, _i, _vp]),
+    "fvs_qwen_klarge_retrieve_multi": (_i, [C.POINTER(QwenRetrieveJob), _i, _i, _i, _vp]),
+    "fvs_qwen_dam_gather_multi": (_i, [C.POINTER(QwenGatherJob), _i, _i, _vp]),
     "fvs_qwen_klarge_workspace_bytes": (_sz, [_i, _i, _i]),
     "fvs_qwen_klarge_retrieve": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _sz, _vp]),
     "fvs_qwen_klarge_retrieve_tiered": (_i, [_vp, _vp, _vp, _i, C.POINTER(_vp), _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _sz,

@@ -8,6 +8,9 @@
 // expression trees: one rounding per op in the op's dtype, fp32 accumulation inside reductions in the canonical slice order
 // of mem_device.cuh (fp32 products are rounded before they are added — no FMA — and 16-bit x 16-bit products are exact,
 // so oracle/qwen_oracle.py reproduces every bit with numpy).
+#include <algorithm>
+#include <vector>
+
 #include "fvs_common.h"
 #include "fvs_ptx.cuh"
 #include "mem_device.cuh"
@@ -87,9 +90,8 @@ __global__ void __launch_bounds__(196) temporal_pool_kernel(const uint16_t* __re
 
 // ------------------------------------------------------------------------------------------------ unique(X, dim=0)
 // cmp[i*T+j] = sign of the lexicographic comparison row i vs row j (-1, 0, +1); one block per pair, early exit.
-__global__ void __launch_bounds__(256) lex_compare_kernel(const void* __restrict__ X, int T, int PD, int dt,
-                                                          signed char* __restrict__ cmp) {
-  const int i = blockIdx.x, j = blockIdx.y;
+__device__ __forceinline__ void lex_compare_body(int i, int j, const void* __restrict__ X, int T, int PD, int dt,
+                                                 signed char* __restrict__ cmp) {
   if (j <= i) {
     if (j == i && threadIdx.x == 0) cmp[i * T + i] = 0;
     return;
@@ -123,10 +125,13 @@ __global__ void __launch_bounds__(256) lex_compare_kernel(const void* __restrict
     cmp[j * T + i] = (signed char)(-result);
   }
 }
+__global__ void __launch_bounds__(256) lex_compare_kernel(const void* __restrict__ X, int T, int PD, int dt,
+                                                          signed char* __restrict__ cmp) {
+  lex_compare_body(blockIdx.x, blockIdx.y, X, T, PD, dt, cmp);
+}
 // single block: rows that are the first of their duplicate class, in ascending lexicographic order
-__global__ void unique_order_kernel(const signed char* __restrict__ cmp, int T, int* __restrict__ uniq_idx,
-                                    int* __restrict__ n_unique) {
-  extern __shared__ int is_first[];
+__device__ __forceinline__ void unique_order_body(const signed char* __restrict__ cmp, int T, int* __restrict__ uniq_idx,
+                                                  int* __restrict__ n_unique, int* is_first) {
   for (int i = threadIdx.x; i < T; i += blockDim.x) {
     int f = 1;
     for (int j = 0; j < i; ++j)
@@ -146,6 +151,11 @@ __global__ void unique_order_kernel(const signed char* __restrict__ cmp, int T, 
     for (int i = 0; i < T; ++i) n += is_first[i];
     *n_unique = n;
   }
+}
+__global__ void unique_order_kernel(const signed char* __restrict__ cmp, int T, int* __restrict__ uniq_idx,
+                                    int* __restrict__ n_unique) {
+  extern __shared__ int is_first[];
+  unique_order_body(cmp, T, uniq_idx, n_unique, is_first);
 }
 
 // ------------------------------------------------------------------------------------------------ fp32 k-means
@@ -170,10 +180,10 @@ struct KO {             // device state + buffers of one weighted_kmeans_ordered
 
 // tot[u] = part[u, 0] + part[u, 1] + ... sequentially (the oracle's _seq_sum over slices); one warp per unit: coalesced
 // loads of 32 partials, then a broadcast chain so the dependent adds run at register speed
-__global__ void __launch_bounds__(256) seq_reduce_kernel(const float* __restrict__ part, float* __restrict__ tot, int units,
-                                                         int S, const int* __restrict__ done) {
+__device__ __forceinline__ void seq_reduce_body(unsigned bid, const float* __restrict__ part, float* __restrict__ tot, int units,
+                                                int S, const int* __restrict__ done) {
   if (done && *done) return;
-  const int u = blockIdx.x * 8 + (threadIdx.x >> 5);
+  const int u = bid * 8 + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
   if (u >= units) return;
   float acc = 0.f;
@@ -183,6 +193,10 @@ __global__ void __launch_bounds__(256) seq_reduce_kernel(const float* __restrict
     for (int i = 0; i < n; ++i) acc = __fadd_rn(acc, __shfl_sync(0xffffffffu, v, i));
   }
   if (lane == 0) tot[u] = acc;
+}
+__global__ void __launch_bounds__(256) seq_reduce_kernel(const float* __restrict__ part, float* __restrict__ tot, int units,
+                                                         int S, const int* __restrict__ done) {
+  seq_reduce_body(blockIdx.x, part, tot, units, S, done);
 }
 
 // one 1024-element slice of a row -> 32 fp32 registers in the canonical ownership (lane l: elements i*256 + l*8 + e),
@@ -226,9 +240,9 @@ __device__ __forceinline__ void store_slice_f32(float* __restrict__ dst, int lan
 }
 
 // |x_t|^2 slice partials: warp per (t, slice)
-__global__ void __launch_bounds__(256) ko_xnorm_kernel(KO B, const void* __restrict__ X, int dt, int T, int PD) {
+__device__ __forceinline__ void ko_xnorm_body(unsigned bid, KO B, const void* __restrict__ X, int dt, int T, int PD) {
   const int S = PD / SLICE;
-  const int unit = blockIdx.x * 8 + (threadIdx.x >> 5);
+  const int unit = bid * 8 + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
   if (unit >= T * S) return;
   float x[32];
@@ -239,11 +253,14 @@ __global__ void __launch_bounds__(256) ko_xnorm_kernel(KO B, const void* __restr
   acc = butterfly_sum(acc);
   if (lane == 0) B.a2[unit] = acc;
 }
+__global__ void __launch_bounds__(256) ko_xnorm_kernel(KO B, const void* __restrict__ X, int dt, int T, int PD) {
+  ko_xnorm_body(blockIdx.x, B, X, dt, T, PD);
+}
 
 // initial centroids = unique_X[indices] widened to fp32, and their |c|^2 slice partials: warp per (k, slice)
-__global__ void __launch_bounds__(256) ko_init_kernel(KO B, const void* __restrict__ X, int dt, const int* __restrict__ uniq_idx,
+__device__ __forceinline__ void ko_init_body(unsigned bid, KO B, const void* __restrict__ X, int dt, const int* __restrict__ uniq_idx,
                                                       const int* __restrict__ init_idx, int T, int K, int PD) {
-  if (blockIdx.x == 0) {
+  if (bid == 0) {
     if (threadIdx.x == 0) {
       B.state[0] = 0; B.state[1] = 0; B.state[2] = 0; B.state[3] = 0; B.state[4] = 0;
       B.chg_list[0] = K;
@@ -252,7 +269,7 @@ __global__ void __launch_bounds__(256) ko_init_kernel(KO B, const void* __restri
     for (int t = threadIdx.x; t < T; t += blockDim.x) B.labels[t] = -1;
   }
   const int S = PD / SLICE;
-  const int unit = blockIdx.x * 8 + (threadIdx.x >> 5);
+  const int unit = bid * 8 + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
   if (unit >= K * S) return;
   const int k = unit / S, s = unit % S;
@@ -265,6 +282,10 @@ __global__ void __launch_bounds__(256) ko_init_kernel(KO B, const void* __restri
   for (int q = 0; q < 32; ++q) acc = __fadd_rn(acc, __fmul_rn(x[q], x[q]));
   acc = butterfly_sum(acc);
   if (lane == 0) B.b2[unit] = acc;
+}
+__global__ void __launch_bounds__(256) ko_init_kernel(KO B, const void* __restrict__ X, int dt, const int* __restrict__ uniq_idx,
+                                                      const int* __restrict__ init_idx, int T, int K, int PD) {
+  ko_init_body(blockIdx.x, B, X, dt, uniq_idx, init_idx, T, K, PD);
 }
 
 // canonical slice partial of sum(a*b): lane l owns elements i*256 + l*8 + e, products rounded, sequential adds, butterfly.
@@ -288,13 +309,12 @@ __device__ __forceinline__ float slice_dot_smem(const float (&a)[32], const floa
 // of the previous iteration, which are exactly what a recomputation would produce.
 constexpr int KO_KC = 8;
 constexpr int KO_PARTIAL_SMEM = 2 * KO_KC * SLICE * 4;
-__global__ void __launch_bounds__(256) ko_partial_kernel(KO B, const void* __restrict__ X, int dt, int T, int K, int PD) {
+__device__ __forceinline__ void ko_partial_body(unsigned bid, float4* cs, KO B, const void* __restrict__ X, int dt, int T, int K,
+                                                int PD) {
   if (B.state[0]) return;
-  extern __shared__ __align__(16) uint8_t ko_smem[];
-  float4* cs = reinterpret_cast<float4*>(ko_smem);          // [2][KO_KC][256] float4
-  const int S = PD / SLICE;
-  const int s = blockIdx.x % S;
-  const int t_raw = (blockIdx.x / S) * 8 + (threadIdx.x >> 5);
+  const int S = PD / SLICE;                                 // cs: [2][KO_KC][256] float4 of dynamic shared memory
+  const int s = bid % S;
+  const int t_raw = (bid / S) * 8 + (threadIdx.x >> 5);
   const int t = min(t_raw, T - 1);
   const int lane = threadIdx.x & 31;
   const float* C = B.C[0] + size_t(s) * SLICE;
@@ -336,11 +356,15 @@ __global__ void __launch_bounds__(256) ko_partial_kernel(KO B, const void* __res
     __syncthreads();
   }
 }
+__global__ void __launch_bounds__(256) ko_partial_kernel(KO B, const void* __restrict__ X, int dt, int T, int K, int PD) {
+  extern __shared__ __align__(16) uint8_t ko_smem[];
+  ko_partial_body(blockIdx.x, reinterpret_cast<float4*>(ko_smem), B, X, dt, T, K, PD);
+}
 // dists = sqrt((A_2 + B_2^T) - 2*AB); labels = argmin (first index, NaN wins); warp per row.  A row whose label moved marks
 // both clusters dirty: only dirty clusters are recomputed by ko_update.
-__global__ void __launch_bounds__(256) ko_assign_kernel(KO B, int T, int K, int PD) {
+__device__ __forceinline__ void ko_assign_body(unsigned bid, KO B, int T, int K, int PD) {
   if (B.state[0]) return;
-  const int t = blockIdx.x * 8 + (threadIdx.x >> 5);
+  const int t = bid * 8 + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
   if (t >= T) return;
   const float a2 = B.a2t[t];
@@ -361,16 +385,19 @@ __global__ void __launch_bounds__(256) ko_assign_kernel(KO B, int T, int K, int 
     }
   }
 }
+__global__ void __launch_bounds__(256) ko_assign_kernel(KO B, int T, int K, int PD) {
+  ko_assign_body(blockIdx.x, B, T, K, PD);
+}
 // warp per (cluster j, slice): weighted mean (sequential in t), refill of empty clusters, ||c_old - c_new||^2 partial.
 // A cluster whose member set did not change since the previous iteration (and that was not empty, i.e. not refilled from
 // a fresh random draw) would reproduce its centroid bit for bit: it is skipped (norm partial 0, weight sum unchanged).
 // New values go to the staging buffer C[1]; ko_commit copies the changed rows into C[0] unless the loop stopped on the
 // tolerance (the reference then keeps the OLD centroids).
-__global__ void __launch_bounds__(256) ko_update_kernel(KO B, const void* __restrict__ X, int dt, const float* __restrict__ w,
+__device__ __forceinline__ void ko_update_body(unsigned bid, KO B, const void* __restrict__ X, int dt, const float* __restrict__ w,
                                                         const int* __restrict__ refill_idx, int T, int K, int PD, int iter) {
   if (B.state[0]) return;
   const int S = PD / SLICE;
-  const int unit = blockIdx.x * 8 + (threadIdx.x >> 5);
+  const int unit = bid * 8 + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
   if (unit >= K * S) return;
   const int j = unit / S, s = unit % S;
@@ -427,9 +454,13 @@ __global__ void __launch_bounds__(256) ko_update_kernel(KO B, const void* __rest
     if (s == 0) B.wsum[j] = wsum_j;
   }
 }
+__global__ void __launch_bounds__(256) ko_update_kernel(KO B, const void* __restrict__ X, int dt, const float* __restrict__ w,
+                                                        const int* __restrict__ refill_idx, int T, int K, int PD, int iter) {
+  ko_update_body(blockIdx.x, B, X, dt, w, refill_idx, T, K, PD, iter);
+}
 // one block: per-cluster norms (slices added in order: warp per cluster, coalesced loads + shuffle chain), then thread 0
 // forms diff = sum_k ||c_k - c'_k||, takes the break decision and builds the change list of the next iteration
-__global__ void __launch_bounds__(1024) ko_converge_kernel(KO B, int K, int PD, int iter, int max_iter, float tol) {
+__device__ __forceinline__ void ko_converge_body(KO B, int K, int PD, int iter, int max_iter, float tol) {
   if (B.state[0]) return;
   const int S = PD / SLICE;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -466,11 +497,14 @@ __global__ void __launch_bounds__(1024) ko_converge_kernel(KO B, int K, int PD, 
     if (iter == max_iter - 1) B.state[0] = 1;
   }
 }
+__global__ void __launch_bounds__(1024) ko_converge_kernel(KO B, int K, int PD, int iter, int max_iter, float tol) {
+  ko_converge_body(B, K, PD, iter, max_iter, tol);
+}
 // centroids = new_centroids for the rows that changed, plus their |c|^2 slice partials: warp per (list entry, slice)
-__global__ void __launch_bounds__(256) ko_commit_kernel(KO B, int K, int PD, int iter, int max_iter) {
+__device__ __forceinline__ void ko_commit_body(unsigned bid, KO B, int K, int PD, int iter, int max_iter) {
   if (B.state[1] != iter + 1) return;          // loop already over, or this iteration stopped on the tolerance
   const int S = PD / SLICE;
-  const int unit = blockIdx.x * 8 + (threadIdx.x >> 5);
+  const int unit = bid * 8 + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
   const int n_list = B.chg_list[0];
   if (unit < n_list * S) {
@@ -485,14 +519,17 @@ __global__ void __launch_bounds__(256) ko_commit_kernel(KO B, int K, int PD, int
     if (lane == 0) B.b2[size_t(k) * S + s] = acc;
   }
 }
-__global__ void __launch_bounds__(256) ko_finish_kernel(KO B, float* __restrict__ C_out, float* __restrict__ wsum_out,
-                                                        int* __restrict__ labels_out, int* __restrict__ info_out, int T, int K,
-                                                        int PD) {
+__global__ void __launch_bounds__(256) ko_commit_kernel(KO B, int K, int PD, int iter, int max_iter) {
+  ko_commit_body(blockIdx.x, B, K, PD, iter, max_iter);
+}
+// a plain copy: the result does not depend on how many blocks (nblk) share it
+__device__ __forceinline__ void ko_finish_body(unsigned bid, unsigned nblk, KO B, float* __restrict__ C_out, float* __restrict__ wsum_out,
+                                               int* __restrict__ labels_out, int* __restrict__ info_out, int T, int K, int PD) {
   const float4* src = reinterpret_cast<const float4*>(B.C[0]);
   float4* dst = reinterpret_cast<float4*>(C_out);
   const size_t n4 = size_t(K) * PD / 4;
-  for (size_t i = blockIdx.x * size_t(blockDim.x) + threadIdx.x; i < n4; i += size_t(gridDim.x) * blockDim.x) dst[i] = src[i];
-  if (blockIdx.x == 0) {
+  for (size_t i = bid * size_t(blockDim.x) + threadIdx.x; i < n4; i += size_t(nblk) * blockDim.x) dst[i] = src[i];
+  if (bid == 0) {
     for (int i = threadIdx.x; i < K; i += blockDim.x) wsum_out[i] = B.wsum[i];
     for (int i = threadIdx.x; i < T; i += blockDim.x) labels_out[i] = B.labels[i];
     if (threadIdx.x == 0) {
@@ -500,13 +537,19 @@ __global__ void __launch_bounds__(256) ko_finish_kernel(KO B, float* __restrict_
     }
   }
 }
+__global__ void __launch_bounds__(256) ko_finish_kernel(KO B, float* __restrict__ C_out, float* __restrict__ wsum_out,
+                                                        int* __restrict__ labels_out, int* __restrict__ info_out, int T, int K,
+                                                        int PD) {
+  ko_finish_body(blockIdx.x, gridDim.x, B, C_out, wsum_out, labels_out, info_out, T, K, PD);
+}
 
-// out[i, :] = cast(src_f32[idx[i], :]) ; idx int64; blockIdx.y = output row, 4 elements per thread (row % 4 == 0)
-__global__ void __launch_bounds__(256) gather_cast_kernel(const float* __restrict__ src, const long long* __restrict__ idx,
-                                                          void* __restrict__ out, size_t row, int out_dt) {
-  const size_t i = blockIdx.y;
+// out[i, :] = cast(src_f32[idx[i], :]) ; idx int64; block bx of nbx covers a strided share of output row i, 4 elements per
+// thread (row % 4 == 0)
+__device__ __forceinline__ void gather_cast_body(unsigned bx, unsigned nbx, size_t i, const float* __restrict__ src,
+                                                 const long long* __restrict__ idx, void* __restrict__ out, size_t row,
+                                                 int out_dt) {
   const float4* s = reinterpret_cast<const float4*>(src + size_t(idx[i]) * row);
-  for (size_t c = blockIdx.x * size_t(blockDim.x) + threadIdx.x; c < row / 4; c += size_t(gridDim.x) * blockDim.x) {
+  for (size_t c = bx * size_t(blockDim.x) + threadIdx.x; c < row / 4; c += size_t(nbx) * blockDim.x) {
     const float4 v = s[c];
     if (out_dt == FVS_F32) {
       reinterpret_cast<float4*>(static_cast<float*>(out) + i * row)[c] = v;
@@ -521,6 +564,10 @@ __global__ void __launch_bounds__(256) gather_cast_kernel(const float* __restric
     }
   }
 }
+__global__ void __launch_bounds__(256) gather_cast_kernel(const float* __restrict__ src, const long long* __restrict__ idx,
+                                                          void* __restrict__ out, size_t row, int out_dt) {
+  gather_cast_body(blockIdx.x, gridDim.x, blockIdx.y, src, idx, out, row, out_dt);
+}
 
 // ------------------------------------------------------------------------------------------------ k-means bookkeeping
 // What weighted_kmeans_ordered_feature does on the host after the Lloyd loop (compress_functions.py:274-290), on the device:
@@ -529,10 +576,10 @@ __global__ void __launch_bounds__(256) gather_cast_kernel(const float* __restric
 // timestamps permuted accordingly.  flags[0] = number of empty clusters (the reference raises ZeroDivisionError there).
 // One block; integer atomics, so the result does not depend on thread order.
 constexpr int kMaxFinalizeK = 1024;
-__global__ void __launch_bounds__(256) ko_finalize_kernel(const int* __restrict__ labels, const float* __restrict__ wsum, int T,
-                                                          int K, const long long* __restrict__ order_in,
-                                                          long long* __restrict__ sorted_idx, float* __restrict__ ts_sorted,
-                                                          float* __restrict__ w_sorted, int* __restrict__ flags) {
+__device__ __forceinline__ void ko_finalize_body(const int* __restrict__ labels, const float* __restrict__ wsum, int T, int K,
+                                                 const long long* __restrict__ order_in, long long* __restrict__ sorted_idx,
+                                                 float* __restrict__ ts_sorted, float* __restrict__ w_sorted,
+                                                 int* __restrict__ flags) {
   __shared__ unsigned long long s_sum[kMaxFinalizeK];
   __shared__ int s_cnt[kMaxFinalizeK];
   __shared__ float s_ts[kMaxFinalizeK];
@@ -569,6 +616,12 @@ __global__ void __launch_bounds__(256) ko_finalize_kernel(const int* __restrict_
     w_sorted[dst] = wsum[src];
   }
   if (threadIdx.x == 0) flags[0] = s_empty;
+}
+__global__ void __launch_bounds__(256) ko_finalize_kernel(const int* __restrict__ labels, const float* __restrict__ wsum, int T,
+                                                          int K, const long long* __restrict__ order_in,
+                                                          long long* __restrict__ sorted_idx, float* __restrict__ ts_sorted,
+                                                          float* __restrict__ w_sorted, int* __restrict__ flags) {
+  ko_finalize_body(labels, wsum, T, K, order_in, sorted_idx, ts_sorted, w_sorted, flags);
 }
 
 // ------------------------------------------------------------------------------------------------ spatial_enhance
@@ -622,15 +675,16 @@ __device__ __forceinline__ uint32_t pack2_16(float a, float b) {
 // partials at the rows' global indices; the launch whose range starts at row 0 writes the |c|^2 partials.  A row's
 // partials do not depend on the block or launch that computes them, so any split of the rows gives the same bits.
 // Without kRange the launch sweeps the whole bank (t_first 0, rows t_total) and ignores the last two arguments.
+// (s, by, ny): the slice, the row split and the number of row splits of the block (blockIdx.x, blockIdx.y, gridDim.y)
 template <bool kBF16, int kMode, bool kRange>
-__global__ void __launch_bounds__(256) klarge_partial_kernel(const uint16_t* __restrict__ tem_x, const long long* __restrict__ klarge_idx,
-                                                             const uint16_t* __restrict__ bank, float* __restrict__ part, int k,
-                                                             int t_total, int PD, const float* __restrict__ norms,
-                                                             int range_first, int range_rows) {
+__device__ __forceinline__ void klarge_partial_body(unsigned s_, unsigned by, unsigned ny, uint4* cs,
+                                                    const uint16_t* __restrict__ tem_x, const long long* __restrict__ klarge_idx,
+                                                    const uint16_t* __restrict__ bank, float* __restrict__ part, int k,
+                                                    int t_total, int PD, const float* __restrict__ norms, int range_first,
+                                                    int range_rows) {
   const int t_first = kRange ? range_first : 0, rows = kRange ? range_rows : t_total;
-  extern __shared__ __align__(16) uint8_t smem_raw[];
-  uint4* cs = reinterpret_cast<uint4*>(smem_raw);          // [k][128] uint4 = k rows of 1024 16-bit elements
-  const int S = PD / SLICE, s = blockIdx.x;
+  // cs: [k][128] uint4 of dynamic shared memory = k rows of 1024 16-bit elements
+  const int S = PD / SLICE, s = s_;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   // norms (kMode 2): [t_total] bank norms then [k] centroid norms, fp32 holding the dtype-rounded values
   for (int i = threadIdx.x; i < k * 128; i += 256) {
@@ -651,9 +705,9 @@ __global__ void __launch_bounds__(256) klarge_partial_kernel(const uint16_t* __r
   float* p_ab = part;
   float* p_b2 = part + size_t(t_total) * k * S;
   float* p_a2 = p_b2 + size_t(t_total) * S;
-  const int rows_per = (rows + gridDim.y - 1) / gridDim.y;         // bank rows of this block
-  const int t_beg = t_first + blockIdx.y * rows_per, t_end = min(t_first + rows, t_beg + rows_per);
-  if (kMode != 2 && blockIdx.y == 0 && t_first == 0) {
+  const int rows_per = (rows + ny - 1) / ny;                       // bank rows of this block
+  const int t_beg = t_first + by * rows_per, t_end = min(t_first + rows, t_beg + rows_per);
+  if (kMode != 2 && by == 0 && t_first == 0) {
     for (int kk = warp; kk < k; kk += 8) {                  // |c|^2 slice partials
       float acc = 0.f;
 #pragma unroll
@@ -730,11 +784,20 @@ __global__ void __launch_bounds__(256) klarge_partial_kernel(const uint16_t* __r
     }
   }
 }
+template <bool kBF16, int kMode, bool kRange>
+__global__ void __launch_bounds__(256) klarge_partial_kernel(const uint16_t* __restrict__ tem_x, const long long* __restrict__ klarge_idx,
+                                                             const uint16_t* __restrict__ bank, float* __restrict__ part, int k,
+                                                             int t_total, int PD, const float* __restrict__ norms,
+                                                             int range_first, int range_rows) {
+  extern __shared__ __align__(16) uint8_t smem_raw[];
+  klarge_partial_body<kBF16, kMode, kRange>(blockIdx.x, blockIdx.y, gridDim.y, reinterpret_cast<uint4*>(smem_raw), tem_x,
+                                            klarge_idx, bank, part, k, t_total, PD, norms, range_first, range_rows);
+}
 // warp per centroid: distances over the bank (lane-strided) and argmin (NaN from a negative radicand wins, as in torch)
 template <bool kBF16>
-__global__ void klarge_tail_kernel(const float* __restrict__ tot, int k, int t_total, long long* __restrict__ idx,
-                                   float* __restrict__ dist_out) {
-  const int kk = blockIdx.x, lane = threadIdx.x;
+__device__ __forceinline__ void klarge_tail_body(unsigned kk_, const float* __restrict__ tot, int k, int t_total,
+                                                 long long* __restrict__ idx, float* __restrict__ dist_out) {
+  const int kk = kk_, lane = threadIdx.x;
   const float* ab = tot;
   const float* b2 = tot + size_t(t_total) * k;
   const float* a2 = b2 + t_total;
@@ -751,18 +814,27 @@ __global__ void klarge_tail_kernel(const float* __restrict__ tot, int k, int t_t
   warp_argmin(best, besti);
   if (lane == 0) idx[kk] = besti;
 }
+template <bool kBF16>
+__global__ void klarge_tail_kernel(const float* __restrict__ tot, int k, int t_total, long long* __restrict__ idx,
+                                   float* __restrict__ dist_out) {
+  klarge_tail_body<kBF16>(blockIdx.x, tot, k, t_total, idx, dist_out);
+}
 
 // norms[i] = dt(sqrt(sumsq[i])) for the t bank rows followed by the k centroids (in place over the reduced totals)
 template <bool kBF16>
-__global__ void klcos_norm_kernel(float* __restrict__ v, int n) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+__device__ __forceinline__ void klcos_norm_body(unsigned bid, float* __restrict__ v, int n) {
+  const int i = bid * blockDim.x + threadIdx.x;
   if (i < n) v[i] = round16<kBF16>(sqrtf(v[i]));
+}
+template <bool kBF16>
+__global__ void klcos_norm_kernel(float* __restrict__ v, int n) {
+  klcos_norm_body<kBF16>(blockIdx.x, v, n);
 }
 // warp per centroid: similarities over the bank and their argmin (a zero row gives 0/0 = NaN, which wins as in torch)
 template <bool kBF16>
-__global__ void klarge_cos_tail_kernel(const float* __restrict__ ab, int k, int t_total, long long* __restrict__ idx,
-                                       float* __restrict__ sim_out) {
-  const int kk = blockIdx.x, lane = threadIdx.x;
+__device__ __forceinline__ void klarge_cos_tail_body(unsigned kk_, const float* __restrict__ ab, int k, int t_total,
+                                                     long long* __restrict__ idx, float* __restrict__ sim_out) {
+  const int kk = kk_, lane = threadIdx.x;
   float best = INFINITY;
   int besti = 0x7fffffff;
   for (int t = lane; t < t_total; t += 32) {
@@ -772,6 +844,11 @@ __global__ void klarge_cos_tail_kernel(const float* __restrict__ ab, int k, int 
   }
   warp_argmin(best, besti);
   if (lane == 0) idx[kk] = besti;
+}
+template <bool kBF16>
+__global__ void klarge_cos_tail_kernel(const float* __restrict__ ab, int k, int t_total, long long* __restrict__ idx,
+                                       float* __restrict__ sim_out) {
+  klarge_cos_tail_body<kBF16>(blockIdx.x, ab, k, t_total, idx, sim_out);
 }
 
 // ------------------------------------------------------------------------------------------------ AM-RoPE
@@ -795,7 +872,32 @@ __global__ void am_rope_kernel(const long long* __restrict__ spa_pos, int spa_t,
   }
 }
 
-inline size_t al(size_t v) { return (v + 255) & ~size_t(255); }
+__host__ __device__ inline size_t al(size_t v) { return (v + 255) & ~size_t(255); }
+
+// the device state of one fvs_qwen_kmeans call, carved from its workspace (fvs_qwen_kmeans_workspace_bytes)
+__host__ __device__ inline KO ko_carve(void* workspace, int T, int K, int PD) {
+  const size_t S = size_t(PD) / SLICE, TK = size_t(T) * K + K;
+  uint8_t* p = (uint8_t*)workspace;
+  KO B;
+  B.state = (int*)p; p += al(32);
+  B.C[0] = (float*)p; p += al(size_t(K) * PD * 4);
+  B.C[1] = (float*)p; p += al(size_t(K) * PD * 4);
+  B.ab = (float*)p; p += al(TK * S * 4);
+  B.b2 = B.ab + size_t(T) * K * S;
+  B.abt = (float*)p; p += al(TK * 4);
+  B.b2t = B.abt + size_t(T) * K;
+  B.a2 = (float*)p; p += al(size_t(T) * S * 4);
+  B.a2t = (float*)p; p += al(size_t(T) * 4);
+  B.normpart = (float*)p; p += al(size_t(K) * S * 4);
+  B.normt = (float*)p; p += al(size_t(K) * 4);
+  B.wsum = (float*)p; p += al(size_t(K) * 4);
+  B.labels = (int*)p; p += al(size_t(T) * 4);
+  B.chg_flag = (int*)p; p += al((size_t(K) + 1) * 4);
+  B.chg_list = (int*)p; p += al((size_t(K) + 1) * 4);
+  B.dirty = (int*)p; p += al((size_t(K) + 1) * 4);
+  B.wprev = (float*)p;
+  return B;
+}
 
 }  // namespace qwen
 }  // namespace fvs
@@ -903,6 +1005,360 @@ int klarge_retrieve(const char* who, const void* tem_x, const int64_t* klarge_id
 }
 }  // namespace
 
+// ------------------------------------------------------------------------------------------------ many streams, one launch
+// The CSM chain of many streams (DESIGN.md §3.17): every kernel of the single-stream chain becomes one flat grid in which
+// job j owns blocks [first[j], first[j+1]) — exactly the blocks its single call launches, in the same order — and calls
+// the same per-block body with its local block index.  A job's reductions therefore run in the same order whatever the
+// other jobs are and however the jobs are grouped into launches.  The job table travels as a __grid_constant__ kernel
+// parameter (at most FVS_QWEN_MEM_JOBS_PER_LAUNCH jobs, under 3 KB).
+namespace fvs {
+namespace qwen {
+
+constexpr int kMemJobs = FVS_QWEN_MEM_JOBS_PER_LAUNCH;
+struct MemJobDev {
+  const void* X;
+  const float* w;
+  const int* init_idx;
+  const int* refill_idx;
+  int* uniq_idx;
+  int* n_unique;
+  void* uniq_ws;
+  float* C;
+  float* wsum;
+  int* labels;
+  int* info;
+  void* km_ws;
+  const long long* order_in;
+  long long* sorted_idx;
+  float* ts;
+  float* w_sorted;
+  int* flags;
+  void* out;
+  int T, K, PD, dt, max_iter, out_dt;
+  float tol;
+};
+struct MemLaunch {
+  MemJobDev job[kMemJobs];
+  int first[kMemJobs + 1];   // block offsets of the launched kernel
+  int n, it, finish_blocks;
+};
+enum MemStage { kLex, kOrder, kInit, kXnorm, kA2, kPartial, kReduce, kAssign, kUpdate, kConverge, kCommit, kFinish, kFinalize,
+                kGather };
+
+// blocks of job J in stage st (iteration it): the grid of the single-stream launch, flattened; 0 once the job's loop is over
+__host__ __device__ inline int gather_bx(int PD) { const int bx = (PD / 4 + 255) / 256; return bx > 64 ? 64 : bx; }
+inline int mem_stage_blocks(const MemJobDev& J, int st, int it, int finish_blocks) {
+  const int S = J.PD / SLICE, iters = J.max_iter == 0 ? 1 : J.max_iter;
+  const bool loop = it < iters, upd = J.max_iter > 0 && it < J.max_iter;
+  switch (st) {
+    case kLex: return J.T * J.T;
+    case kOrder: case kFinalize: return 1;
+    case kInit: return (J.K * S + 7) / 8;
+    case kXnorm: return (J.T * S + 7) / 8;
+    case kA2: return (J.T + 7) / 8;
+    case kPartial: return loop ? ((J.T + 7) / 8) * S : 0;
+    case kReduce: return loop ? int((size_t(J.T) * J.K + J.K + 7) / 8) : 0;
+    case kAssign: return loop ? (J.T + 7) / 8 : 0;
+    case kUpdate: case kCommit: return upd ? (J.K * S + 7) / 8 : 0;
+    case kConverge: return upd ? 1 : 0;
+    case kFinish: return finish_blocks;
+    case kGather: return gather_bx(J.PD) * J.K;
+  }
+  return 0;
+}
+
+template <int kStage>
+__global__ void __launch_bounds__(kStage == kConverge ? 1024 : 256) mem_multi_kernel(const __grid_constant__ MemLaunch L) {
+  extern __shared__ __align__(16) uint8_t mm_smem[];
+  int j = 0;
+  while (j + 1 < L.n && blockIdx.x >= unsigned(L.first[j + 1])) ++j;
+  const MemJobDev& J = L.job[j];
+  const unsigned b = blockIdx.x - unsigned(L.first[j]);
+  if constexpr (kStage == kLex) {
+    lex_compare_body(int(b % unsigned(J.T)), int(b / unsigned(J.T)), J.X, J.T, J.PD, J.dt, (signed char*)J.uniq_ws);
+  } else if constexpr (kStage == kOrder) {
+    unique_order_body((const signed char*)J.uniq_ws, J.T, J.uniq_idx, J.n_unique, reinterpret_cast<int*>(mm_smem));
+  } else if constexpr (kStage == kFinalize) {
+    ko_finalize_body(J.labels, J.wsum, J.T, J.K, J.order_in, J.sorted_idx, J.ts, J.w_sorted, J.flags);
+  } else if constexpr (kStage == kGather) {
+    const unsigned bx = gather_bx(J.PD);
+    gather_cast_body(b % bx, bx, b / bx, J.C, J.sorted_idx, J.out, size_t(J.PD), J.out_dt);
+  } else {
+    const KO B = ko_carve(J.km_ws, J.T, J.K, J.PD);
+    const int S = J.PD / SLICE;
+    if constexpr (kStage == kInit) ko_init_body(b, B, J.X, J.dt, J.uniq_idx, J.init_idx, J.T, J.K, J.PD);
+    else if constexpr (kStage == kXnorm) ko_xnorm_body(b, B, J.X, J.dt, J.T, J.PD);
+    else if constexpr (kStage == kA2) seq_reduce_body(b, B.a2, B.a2t, J.T, S, nullptr);
+    else if constexpr (kStage == kPartial) ko_partial_body(b, reinterpret_cast<float4*>(mm_smem), B, J.X, J.dt, J.T, J.K, J.PD);
+    else if constexpr (kStage == kReduce) seq_reduce_body(b, B.ab, B.abt, J.T * J.K + J.K, S, B.state);
+    else if constexpr (kStage == kAssign) ko_assign_body(b, B, J.T, J.K, J.PD);
+    else if constexpr (kStage == kUpdate) ko_update_body(b, B, J.X, J.dt, J.w, J.refill_idx, J.T, J.K, J.PD, L.it);
+    else if constexpr (kStage == kConverge) ko_converge_body(B, J.K, J.PD, L.it, J.max_iter, J.tol);
+    else if constexpr (kStage == kCommit) ko_commit_body(b, B, J.K, J.PD, L.it, J.max_iter);
+    else if constexpr (kStage == kFinish) ko_finish_body(b, L.finish_blocks, B, J.C, J.wsum, J.labels, J.info, J.T, J.K, J.PD);
+  }
+}
+
+// the klarge retrieval of many jobs: the single call's launches, each one flat grid over the jobs' blocks
+struct KlJobDev {
+  const uint16_t* tem_x;
+  const long long* klarge_idx;
+  const uint16_t* bank;
+  float* part;
+  float* tot;
+  long long* idx;
+  float* dist;
+  int k, t_total, PD, nsplit;
+};
+struct KlLaunch {
+  KlJobDev job[kMemJobs];
+  int first[kMemJobs + 1];
+  int n;
+};
+enum KlStage { kKlSweep0, kKlSweep1, kKlSweep2, kKlReduceAll, kKlReduceNorms, kKlNorms, kKlReduceAb, kKlTail, kKlCosTail };
+inline int kl_stage_blocks(const KlJobDev& J, int st) {
+  const int S = J.PD / SLICE;
+  const size_t n_ab = size_t(J.t_total) * J.k, n_norm = size_t(J.t_total) + J.k;
+  switch (st) {
+    case kKlSweep0: case kKlSweep1: case kKlSweep2: return S * J.nsplit;
+    case kKlReduceAll: return int((n_ab + n_norm + 7) / 8);
+    case kKlReduceNorms: return int((n_norm + 7) / 8);
+    case kKlNorms: return int((n_norm + 255) / 256);
+    case kKlReduceAb: return int((n_ab + 7) / 8);
+    case kKlTail: case kKlCosTail: return J.k;
+  }
+  return 0;
+}
+template <bool kBF16, int kStage>
+__global__ void __launch_bounds__(256) klarge_multi_kernel(const __grid_constant__ KlLaunch L) {
+  extern __shared__ __align__(16) uint8_t kl_smem[];
+  int j = 0;
+  while (j + 1 < L.n && blockIdx.x >= unsigned(L.first[j + 1])) ++j;
+  const KlJobDev& J = L.job[j];
+  const unsigned b = blockIdx.x - unsigned(L.first[j]);
+  const unsigned S = J.PD / SLICE;
+  const size_t n_ab = size_t(J.t_total) * J.k, n_norm = size_t(J.t_total) + J.k;
+  uint4* cs = reinterpret_cast<uint4*>(kl_smem);
+  if constexpr (kStage == kKlSweep0 || kStage == kKlSweep1 || kStage == kKlSweep2) {
+    constexpr int kMode = kStage - kKlSweep0;
+    klarge_partial_body<kBF16, kMode, false>(b % S, b / S, J.nsplit, cs, J.tem_x, J.klarge_idx, J.bank, J.part, J.k,
+                                             J.t_total, J.PD, kMode == 2 ? J.tot + n_ab : nullptr, 0, J.t_total);
+  } else if constexpr (kStage == kKlReduceAll) {
+    seq_reduce_body(b, J.part, J.tot, int(n_ab + n_norm), S, nullptr);
+  } else if constexpr (kStage == kKlReduceNorms) {
+    seq_reduce_body(b, J.part + n_ab * S, J.tot + n_ab, int(n_norm), S, nullptr);
+  } else if constexpr (kStage == kKlNorms) {
+    klcos_norm_body<kBF16>(b, J.tot + n_ab, int(n_norm));
+  } else if constexpr (kStage == kKlReduceAb) {
+    seq_reduce_body(b, J.part, J.tot, int(n_ab), S, nullptr);
+  } else if constexpr (kStage == kKlTail) {
+    klarge_tail_body<kBF16>(b, J.tot, J.k, J.t_total, J.idx, J.dist);
+  } else {
+    klarge_cos_tail_body<kBF16>(b, J.tot, J.k, J.t_total, J.idx, J.dist);
+  }
+}
+
+}  // namespace qwen
+}  // namespace fvs
+
+namespace {
+using fvs::qwen::MemJobDev;
+using fvs::qwen::MemLaunch;
+
+enum MemCall { kCallUnique, kCallKmeans, kCallFinalize, kCallGather };
+
+int lloyd_blocks(const fvs_qwen_mem_job& j) { return ((j.T + 7) / 8) * (j.PD / SLICE); }
+
+// the checks of the single-stream entry point of `call`, per job, and no output byte shared by two jobs
+int check_mem_jobs(const char* api, const fvs_qwen_mem_job* jobs, int n, int budget, int call) {
+  FVS_REQUIRE(jobs && n > 0 && budget >= 0, "%s: need a job table, n_jobs > 0 and budget >= 0", api);
+  struct Range { uintptr_t lo, hi; int job; };
+  std::vector<Range> out;
+  auto add = [&](const void* p, size_t bytes, int i) { out.push_back({uintptr_t(p), uintptr_t(p) + bytes, i}); };
+  for (int i = 0; i < n; ++i) {
+    const fvs_qwen_mem_job& j = jobs[i];
+    FVS_REQUIRE(j.T > 0 && j.T <= 4096 && j.K > 0 && j.K <= j.T && j.K <= kMaxFinalizeK,
+                "%s: job %d: need 0 < T <= 4096, 0 < K <= min(T, %d) (T=%d K=%d)", api, i, kMaxFinalizeK, j.T, j.K);
+    FVS_REQUIRE(j.PD > 0 && j.PD % SLICE == 0, "%s: job %d: PD (%d) must be a positive multiple of %d", api, i, j.PD, SLICE);
+    if (call == kCallUnique || call == kCallKmeans)
+      FVS_REQUIRE(j.X && (j.x_dtype == FVS_F16 || j.x_dtype == FVS_BF16 || j.x_dtype == FVS_F32),
+                  "%s: job %d: null X or bad x dtype", api, i);
+    if (call == kCallUnique) {
+      FVS_REQUIRE(j.uniq_idx && j.n_unique && j.uniq_workspace, "%s: job %d: null pointer", api, i);
+      FVS_REQUIRE(j.uniq_workspace_bytes >= fvs_qwen_unique_workspace_bytes(j.T), "%s: job %d: workspace too small", api, i);
+      add(j.uniq_idx, size_t(j.T) * 4, i);
+      add(j.n_unique, 4, i);
+      add(j.uniq_workspace, fvs_qwen_unique_workspace_bytes(j.T), i);
+    } else if (call == kCallKmeans) {
+      FVS_REQUIRE(j.w && j.init_idx && j.refill_idx && j.C && j.wsum && j.labels && j.info && j.km_workspace,
+                  "%s: job %d: null pointer", api, i);
+      FVS_REQUIRE(j.max_iter >= 0 && j.max_iter <= 1000, "%s: job %d: bad max_iter", api, i);
+      const size_t ws = fvs_qwen_kmeans_workspace_bytes(j.T, j.K, j.PD);
+      FVS_REQUIRE(j.km_workspace_bytes >= ws, "%s: job %d: workspace too small", api, i);
+      add(j.C, size_t(j.K) * j.PD * 4, i);
+      add(j.wsum, size_t(j.K) * 4, i);
+      add(j.labels, size_t(j.T) * 4, i);
+      add(j.info, 16, i);
+      add(j.km_workspace, ws, i);
+    } else if (call == kCallFinalize) {
+      FVS_REQUIRE(j.labels && j.wsum && j.sorted_idx && j.ts && j.w_sorted && j.flags, "%s: job %d: null pointer", api, i);
+      add(j.sorted_idx, size_t(j.K) * 8, i);
+      add(j.ts, size_t(j.K) * 4, i);
+      add(j.w_sorted, size_t(j.K) * 4, i);
+      add(j.flags, 4, i);
+    } else {
+      FVS_REQUIRE(j.C && j.sorted_idx && j.out, "%s: job %d: null pointer", api, i);
+      FVS_REQUIRE(j.out_dtype == FVS_F16 || j.out_dtype == FVS_BF16 || j.out_dtype == FVS_F32, "%s: job %d: bad out dtype",
+                  api, i);
+      add(j.out, size_t(j.K) * j.PD * (j.out_dtype == FVS_F32 ? 4 : 2), i);
+    }
+  }
+  for (size_t a = 0; a < out.size(); ++a)
+    for (size_t b = a + 1; b < out.size(); ++b)
+      FVS_REQUIRE(out[a].job == out[b].job || out[a].hi <= out[b].lo || out[b].hi <= out[a].lo,
+                  "%s: jobs %d and %d share an output", api, out[a].job, out[b].job);
+  return FVS_OK;
+}
+
+// jobs in order, at most kMemJobs per group and, with budget > 0, at most `budget` Lloyd-sweep blocks (a larger job alone)
+int mem_groups(const fvs_qwen_mem_job* jobs, int n, int budget, int32_t* blocks, int32_t* groups) {
+  int g = 0, in_group = 0;
+  long long sum = 0;
+  for (int i = 0; i < n; ++i) {
+    const int b = lloyd_blocks(jobs[i]);
+    if (in_group && (in_group == fvs::qwen::kMemJobs || (budget > 0 && sum + b > budget))) {
+      ++g;
+      in_group = 0;
+      sum = 0;
+    }
+    blocks[i] = b;
+    groups[i] = g;
+    ++in_group;
+    sum += b;
+  }
+  return g + 1;
+}
+
+MemJobDev mem_job_dev(const fvs_qwen_mem_job& j) {
+  return MemJobDev{j.X, j.w, j.init_idx, j.refill_idx, j.uniq_idx, j.n_unique, j.uniq_workspace, j.C, j.wsum, j.labels,
+                   j.info, j.km_workspace, (const long long*)j.order_in, (long long*)j.sorted_idx, j.ts, j.w_sorted, j.flags,
+                   j.out, j.T, j.K, j.PD, j.x_dtype, j.max_iter, j.out_dtype, j.tol};
+}
+
+// one launch of stage kStage over the group in L (skipped when no job has blocks in it)
+template <int kStage>
+int mem_launch(MemLaunch& L, int threads, size_t smem, cudaStream_t stream, const char* name) {
+  using namespace fvs::qwen;
+  L.first[0] = 0;
+  for (int j = 0; j < L.n; ++j) L.first[j + 1] = L.first[j] + mem_stage_blocks(L.job[j], kStage, L.it, L.finish_blocks);
+  if (L.first[L.n] == 0) return FVS_OK;
+  mem_multi_kernel<kStage><<<L.first[L.n], threads, smem, stream>>>(L);
+  FVS_CHECK_LAUNCH(name);
+  return FVS_OK;
+}
+
+int run_mem_multi(const char* api, const fvs_qwen_mem_job* jobs, int n, int budget, fvs_stream_t stream_, int call) {
+  using namespace fvs::qwen;
+  int r = check_mem_jobs(api, jobs, n, budget, call);
+  if (r) return r;
+  std::vector<int32_t> blocks(n), groups(n);
+  const int n_groups = mem_groups(jobs, n, budget, blocks.data(), groups.data());
+  cudaStream_t stream = (cudaStream_t)stream_;
+  if (call == kCallKmeans) {
+    static bool attr_done = false;
+    if (!attr_done) {
+      FVS_CUDA_OK(cudaFuncSetAttribute(mem_multi_kernel<kPartial>, cudaFuncAttributeMaxDynamicSharedMemorySize, KO_PARTIAL_SMEM));
+      attr_done = true;
+    }
+  }
+  const int sm8 = device_sm_count() * 8;
+  for (int g = 0, i0 = 0; g < n_groups; ++g) {
+    MemLaunch L;
+    L.n = 0;
+    L.it = 0;
+    L.finish_blocks = 1;
+    int max_T = 1, iters = 0;
+    size_t max_row4 = 1;
+    for (; i0 < n && groups[i0] == g; ++i0) {
+      const fvs_qwen_mem_job& j = jobs[i0];
+      L.job[L.n++] = mem_job_dev(j);
+      max_T = std::max(max_T, j.T);
+      iters = std::max(iters, j.max_iter == 0 ? 1 : j.max_iter);
+      max_row4 = std::max(max_row4, size_t(j.K) * j.PD / 4);
+    }
+    if (call == kCallUnique) {
+      if ((r = mem_launch<kLex>(L, 256, 0, stream, "mem_multi_kernel<lex_compare>"))) return r;
+      if ((r = mem_launch<kOrder>(L, 256, size_t(max_T) * sizeof(int), stream, "mem_multi_kernel<unique_order>"))) return r;
+    } else if (call == kCallFinalize) {
+      if ((r = mem_launch<kFinalize>(L, 256, 0, stream, "mem_multi_kernel<ko_finalize>"))) return r;
+    } else if (call == kCallGather) {
+      if ((r = mem_launch<kGather>(L, 256, 0, stream, "mem_multi_kernel<gather_cast>"))) return r;
+    } else {
+      // the single call's launch sequence, each launch covering the whole group; a job whose loop is over has no blocks
+      if ((r = mem_launch<kInit>(L, 256, 0, stream, "mem_multi_kernel<ko_init>"))) return r;
+      if ((r = mem_launch<kXnorm>(L, 256, 0, stream, "mem_multi_kernel<ko_xnorm>"))) return r;
+      if ((r = mem_launch<kA2>(L, 256, 0, stream, "mem_multi_kernel<seq_reduce>"))) return r;
+      for (int it = 0; it < iters; ++it) {
+        L.it = it;
+        if ((r = mem_launch<kPartial>(L, 256, KO_PARTIAL_SMEM, stream, "mem_multi_kernel<ko_partial>"))) return r;
+        if ((r = mem_launch<kReduce>(L, 256, 0, stream, "mem_multi_kernel<seq_reduce>"))) return r;
+        if ((r = mem_launch<kAssign>(L, 256, 0, stream, "mem_multi_kernel<ko_assign>"))) return r;
+        if ((r = mem_launch<kUpdate>(L, 256, 0, stream, "mem_multi_kernel<ko_update>"))) return r;
+        if ((r = mem_launch<kConverge>(L, 1024, 0, stream, "mem_multi_kernel<ko_converge>"))) return r;
+        if ((r = mem_launch<kCommit>(L, 256, 0, stream, "mem_multi_kernel<ko_commit>"))) return r;
+      }
+      // the result copy is split evenly: its bits do not depend on the number of blocks
+      L.finish_blocks = int(std::min<size_t>(std::max(1, sm8 / L.n), (max_row4 + 255) / 256));
+      if ((r = mem_launch<kFinish>(L, 256, 0, stream, "mem_multi_kernel<ko_finish>"))) return r;
+    }
+  }
+  return FVS_OK;
+}
+}  // namespace
+
+namespace {
+using fvs::qwen::KlJobDev;
+using fvs::qwen::KlLaunch;
+
+template <bool kBF16, int kStage>
+int kl_launch(KlLaunch& L, int threads, size_t smem, cudaStream_t stream, const char* name) {
+  using namespace fvs::qwen;
+  L.first[0] = 0;
+  for (int j = 0; j < L.n; ++j) L.first[j + 1] = L.first[j] + kl_stage_blocks(L.job[j], kStage);
+  if (L.first[L.n] == 0) return FVS_OK;
+  if (smem > 48 * 1024) {
+    static bool attr = false;   // per instantiation
+    if (!attr) {
+      FVS_CUDA_OK(cudaFuncSetAttribute(klarge_multi_kernel<kBF16, kStage>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       64 * SLICE * 2));
+      attr = true;
+    }
+  }
+  klarge_multi_kernel<kBF16, kStage><<<L.first[L.n], threads, smem, stream>>>(L);
+  FVS_CHECK_LAUNCH(name);
+  return FVS_OK;
+}
+
+template <bool kBF16>
+int kl_group(KlLaunch& L, int metric, cudaStream_t stream) {
+  using namespace fvs::qwen;
+  int max_k = 1, r;
+  for (int j = 0; j < L.n; ++j) max_k = std::max(max_k, L.job[j].k);
+  const size_t smem = size_t(max_k) * SLICE * 2;
+  if (metric == FVS_KLARGE_EUCLIDEAN) {
+    if ((r = kl_launch<kBF16, kKlSweep0>(L, 256, smem, stream, "klarge_multi_kernel<sweep>"))) return r;
+    if ((r = kl_launch<kBF16, kKlReduceAll>(L, 256, 0, stream, "klarge_multi_kernel<seq_reduce>"))) return r;
+    return kl_launch<kBF16, kKlTail>(L, 32, 0, stream, "klarge_multi_kernel<tail>");
+  }
+  if ((r = kl_launch<kBF16, kKlSweep1>(L, 256, smem, stream, "klarge_multi_kernel<sweep norms>"))) return r;
+  if ((r = kl_launch<kBF16, kKlReduceNorms>(L, 256, 0, stream, "klarge_multi_kernel<seq_reduce>"))) return r;
+  if ((r = kl_launch<kBF16, kKlNorms>(L, 256, 0, stream, "klarge_multi_kernel<norms>"))) return r;
+  if ((r = kl_launch<kBF16, kKlSweep2>(L, 256, smem, stream, "klarge_multi_kernel<sweep cos>"))) return r;
+  if ((r = kl_launch<kBF16, kKlReduceAb>(L, 256, 0, stream, "klarge_multi_kernel<seq_reduce>"))) return r;
+  return kl_launch<kBF16, kKlCosTail>(L, 32, 0, stream, "klarge_multi_kernel<cos tail>");
+}
+}  // namespace
+
 extern "C" {
 
 int fvs_qwen_temporal_pool(const void* x, void* out, int t, int h, int w, int dtype, fvs_stream_t stream) {
@@ -958,26 +1414,8 @@ int fvs_qwen_kmeans(const void* X, int x_dtype, const float* w, const int32_t* u
   FVS_REQUIRE(workspace_bytes >= fvs_qwen_kmeans_workspace_bytes(T, K, PD), "fvs_qwen_kmeans: workspace too small");
   cudaStream_t stream = (cudaStream_t)stream_;
   const int S = PD / SLICE;
-  uint8_t* p = (uint8_t*)workspace;
-  KO B;
-  B.state = (int*)p; p += al(32);
-  B.C[0] = (float*)p; p += al(size_t(K) * PD * 4);
-  B.C[1] = (float*)p; p += al(size_t(K) * PD * 4);
+  const KO B = ko_carve(workspace, T, K, PD);
   const size_t TK = size_t(T) * K + K;
-  B.ab = (float*)p; p += al(TK * S * 4);
-  B.b2 = B.ab + size_t(T) * K * S;
-  B.abt = (float*)p; p += al(TK * 4);
-  B.b2t = B.abt + size_t(T) * K;
-  B.a2 = (float*)p; p += al(size_t(T) * S * 4);
-  B.a2t = (float*)p; p += al(size_t(T) * 4);
-  B.normpart = (float*)p; p += al(size_t(K) * S * 4);
-  B.normt = (float*)p; p += al(size_t(K) * 4);
-  B.wsum = (float*)p; p += al(size_t(K) * 4);
-  B.labels = (int*)p; p += al(size_t(T) * 4);
-  B.chg_flag = (int*)p; p += al((size_t(K) + 1) * 4);
-  B.chg_list = (int*)p; p += al((size_t(K) + 1) * 4);
-  B.dirty = (int*)p; p += al((size_t(K) + 1) * 4);
-  B.wprev = (float*)p;
   static bool attr_done = false;
   if (!attr_done) {
     FVS_CUDA_OK(cudaFuncSetAttribute(ko_partial_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, KO_PARTIAL_SMEM));
@@ -1054,6 +1492,75 @@ int fvs_qwen_klarge_retrieve_tiered(const void* tem_x, const int64_t* klarge_idx
   const KlargeBank b{dev_bank, n_dev, host_chunks, chunk_frames, t_total};
   return klarge_retrieve("fvs_qwen_klarge_retrieve_tiered", tem_x, klarge_idx, b, k, PD, dtype, metric, idx_out, dist_out,
                          workspace, workspace_bytes, stream);
+}
+
+int fvs_qwen_mem_plan(const fvs_qwen_mem_job* jobs_h, int n_jobs, int budget, int32_t* blocks_h, int32_t* groups_h) {
+  const char* api = "fvs_qwen_mem_plan";
+  FVS_REQUIRE(jobs_h && n_jobs > 0 && budget >= 0 && blocks_h && groups_h, "%s: need jobs, n_jobs > 0, budget >= 0, outputs",
+              api);
+  for (int i = 0; i < n_jobs; ++i) {
+    const fvs_qwen_mem_job& j = jobs_h[i];
+    FVS_REQUIRE(j.T > 0 && j.T <= 4096 && j.K > 0 && j.K <= j.T && j.PD > 0 && j.PD % SLICE == 0,
+                "%s: job %d: bad shape T=%d K=%d PD=%d", api, i, j.T, j.K, j.PD);
+  }
+  return mem_groups(jobs_h, n_jobs, budget, blocks_h, groups_h);
+}
+
+int fvs_qwen_unique_rows_multi(const fvs_qwen_mem_job* jobs_h, int n_jobs, int budget, fvs_stream_t stream) {
+  return run_mem_multi("fvs_qwen_unique_rows_multi", jobs_h, n_jobs, budget, stream, kCallUnique);
+}
+int fvs_qwen_kmeans_multi(const fvs_qwen_mem_job* jobs_h, int n_jobs, int budget, fvs_stream_t stream) {
+  return run_mem_multi("fvs_qwen_kmeans_multi", jobs_h, n_jobs, budget, stream, kCallKmeans);
+}
+int fvs_qwen_kmeans_finalize_multi(const fvs_qwen_mem_job* jobs_h, int n_jobs, int budget, fvs_stream_t stream) {
+  return run_mem_multi("fvs_qwen_kmeans_finalize_multi", jobs_h, n_jobs, budget, stream, kCallFinalize);
+}
+int fvs_gather_rows_cast_multi(const fvs_qwen_mem_job* jobs_h, int n_jobs, int budget, fvs_stream_t stream) {
+  return run_mem_multi("fvs_gather_rows_cast_multi", jobs_h, n_jobs, budget, stream, kCallGather);
+}
+
+int fvs_qwen_klarge_retrieve_multi(const fvs_qwen_retrieve_job* jobs_h, int n_jobs, int dtype, int metric,
+                                   fvs_stream_t stream) {
+  const char* api = "fvs_qwen_klarge_retrieve_multi";
+  FVS_REQUIRE(jobs_h && n_jobs > 0, "%s: need a job table and n_jobs > 0", api);
+  FVS_REQUIRE(dtype == FVS_F16 || dtype == FVS_BF16, "%s: dtype must be f16 or bf16", api);
+  FVS_REQUIRE(metric == FVS_KLARGE_EUCLIDEAN || metric == FVS_KLARGE_COSINE, "%s: unknown metric %d", api, metric);
+  struct Range { uintptr_t lo, hi; int job; };
+  std::vector<Range> out;
+  for (int i = 0; i < n_jobs; ++i) {          // the checks of fvs_qwen_klarge_retrieve, per job
+    const fvs_qwen_retrieve_job& j = jobs_h[i];
+    FVS_REQUIRE(j.tem_x && j.klarge_idx && j.bank && j.idx_out && j.workspace, "%s: job %d: null pointer", api, i);
+    FVS_REQUIRE(j.k > 0 && j.k <= 64 && j.t_total > 0, "%s: job %d: need 0 < k <= 64, t > 0 (k=%d t=%d)", api, i, j.k,
+                j.t_total);
+    FVS_REQUIRE(j.PD > 0 && j.PD % SLICE == 0, "%s: job %d: PD (%d) must be a positive multiple of %d", api, i, j.PD, SLICE);
+    FVS_REQUIRE(j.n_dev == j.t_total, "%s: job %d: %d of its %d bank rows are in host memory: step it through "
+                "fvs_qwen_klarge_retrieve_tiered", api, i, j.t_total - j.n_dev, j.t_total);
+    const size_t ws = fvs_qwen_klarge_workspace_bytes(j.k, j.t_total, j.PD);
+    FVS_REQUIRE(j.workspace_bytes >= ws, "%s: job %d: workspace too small", api, i);
+    out.push_back({uintptr_t(j.idx_out), uintptr_t(j.idx_out) + size_t(j.k) * 8, i});
+    out.push_back({uintptr_t(j.workspace), uintptr_t(j.workspace) + ws, i});
+    if (j.dist_out) out.push_back({uintptr_t(j.dist_out), uintptr_t(j.dist_out) + size_t(j.k) * j.t_total * 4, i});
+  }
+  for (size_t a = 0; a < out.size(); ++a)
+    for (size_t b = a + 1; b < out.size(); ++b)
+      FVS_REQUIRE(out[a].job == out[b].job || out[a].hi <= out[b].lo || out[b].hi <= out[a].lo,
+                  "%s: jobs %d and %d share an output", api, out[a].job, out[b].job);
+  for (int i0 = 0; i0 < n_jobs; i0 += kMemJobs) {
+    KlLaunch L;
+    L.n = std::min(kMemJobs, n_jobs - i0);
+    for (int q = 0; q < L.n; ++q) {
+      const fvs_qwen_retrieve_job& j = jobs_h[i0 + q];
+      const size_t units = size_t(j.t_total) * j.k + j.t_total + j.k;
+      float* part = (float*)j.workspace;
+      float* tot = (float*)((uint8_t*)j.workspace + al(units * (j.PD / SLICE) * 4));
+      L.job[q] = KlJobDev{(const uint16_t*)j.tem_x, (const long long*)j.klarge_idx, (const uint16_t*)j.bank, part, tot,
+                          (long long*)j.idx_out, j.dist_out, j.k, j.t_total, j.PD, (j.t_total + 31) / 32};
+    }
+    const int r = dtype == FVS_BF16 ? kl_group<true>(L, metric, (cudaStream_t)stream)
+                                    : kl_group<false>(L, metric, (cudaStream_t)stream);
+    if (r) return r;
+  }
+  return FVS_OK;
 }
 
 int fvs_qwen_am_rope(const int64_t* spa_positions, int spa_t, int spa_h, int spa_w, const int64_t* tem_positions, int tem_t,

@@ -13,6 +13,7 @@ import numpy as np
 import torch
 
 from . import ops as Q
+from .. import _lib as L
 from ..draws import GLOBAL, DrawSource, to_device
 
 MAX_ITER = 10   # compress_functions.py:203 (max_iter=10)
@@ -137,6 +138,56 @@ def ordered_kmeans_enqueue(img_feature: torch.Tensor, video_max_frames: int, wei
     feat = Q.gather_rows_cast(C.view(T0, P, D), sorted_idx, img_feature.dtype, out=out)
     return dict(feat=feat, weights=w_sorted, timestamps=ts, members=LazyMembers(labels, sorted_idx), n_unique=n_unique,
                 info=info, flags=flags)
+
+
+def ordered_kmeans_enqueue_multi(reqs, video_max_frames: int, budget: int = 0):
+    """ordered_kmeans_enqueue for many streams at once (DESIGN.md §3.17): reqs = [(img_feature [T, P, D], weights [T],
+    init_idx, refill_idx, order or None)], each as ordered_kmeans_enqueue takes it.  The four kernels of the chain (unique
+    rows, Lloyd loop, finalize, ordered cast) run once per launch group for all streams; stream i gets the bits
+    ordered_kmeans_enqueue gives it.  Returns (per stream the dict of ordered_kmeans_enqueue, readback) where readback is
+    a device int32 [n, 8] holding each stream's n_unique, info[4] and flags in columns 0, 1-4 and 5 (the dicts' n_unique,
+    info and flags are views of it), so the caller copies every stream's read-back at once."""
+    n, K = len(reqs), int(video_max_frames)
+    dev = reqs[0][0].device
+    Ts = [r[0].shape[0] for r in reqs]
+    rb = torch.zeros(n, 8, dtype=torch.int32, device=dev)
+    uniq = torch.zeros(sum(Ts), dtype=torch.int32, device=dev)      # zero-filled, as unique_rows (ops.py) leaves it
+    labels = torch.empty(sum(Ts), dtype=torch.int32, device=dev)
+    small = torch.empty(n, 3, K, dtype=torch.float32, device=dev)     # wsum, timestamps, sorted weights
+    sorted_idx = torch.empty(n, K, dtype=torch.int64, device=dev)
+    lib = L.load()
+    sizes = []
+    for (x, *_), T in zip(reqs, Ts):
+        PD = x[0].numel()
+        sizes.append((Q._al(K * PD * 4), Q._al(lib.fvs_qwen_unique_workspace_bytes(T)),
+                      Q._al(lib.fvs_qwen_kmeans_workspace_bytes(T, K, PD))))
+    ws = Q._workspace(sum(map(sum, sizes)), dev, "mem_multi")
+    jobs, outs, keep, o, t0 = [], [], [], 0, 0           # keep: converted inputs, alive until the calls are enqueued
+    for i, ((x, w, init_idx, refill_idx, order), T, (nc, nu, nk)) in enumerate(zip(reqs, Ts, sizes)):
+        assert T > K and init_idx.dtype == torch.int32 and refill_idx.dtype == torch.int32
+        X, w32 = Q._c(x.reshape(T, -1)), Q._c(w.to(torch.float32))
+        order = None if order is None else Q._c(order)
+        init_idx, refill_idx = Q._c(init_idx), Q._c(refill_idx)
+        keep.append((X, w32, order, init_idx, refill_idx))
+        PD = X.shape[1]
+        C = ws[o: o + K * PD * 4].view(torch.float32).view(K, PD)
+        feat = torch.empty((K,) + tuple(x.shape[1:]), dtype=x.dtype, device=dev)
+        lab = labels[t0: t0 + T]
+        jobs.append(Q.mem_job(X, K, w=w32, init_idx=init_idx, refill_idx=refill_idx,
+                              max_iter=MAX_ITER, tol=TOL, uniq_idx=uniq[t0: t0 + T], n_unique=rb[i, 0:1],
+                              uniq_ws=ws[o + nc: o + nc + nu], C=C, wsum=small[i, 0], labels=lab, info=rb[i, 1:5],
+                              km_ws=ws[o + nc + nu: o + nc + nu + nk], order=order,
+                              sorted_idx=sorted_idx[i], ts=small[i, 1], w_sorted=small[i, 2], flags=rb[i, 5:6], out=feat))
+        outs.append(dict(feat=feat, weights=small[i, 2], timestamps=small[i, 1], members=LazyMembers(lab, sorted_idx[i]),
+                         n_unique=rb[i, 0:1], info=rb[i, 1:5], flags=rb[i, 5:6]))
+        o += nc + nu + nk
+        t0 += T
+    arr = Q.mem_jobs(jobs)
+    Q.unique_rows_multi(arr, budget)
+    Q.kmeans_multi(arr, budget)
+    Q.kmeans_finalize_multi(arr, budget)
+    Q.gather_rows_cast_multi(arr, budget)
+    return outs, rb
 
 
 def fast_weighted_kmeans_ordered_feature(img_feature, video_max_frames, weights=None, *, init_idx=None, refill_idx=None,

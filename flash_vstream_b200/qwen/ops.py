@@ -102,6 +102,132 @@ def gather_rows_cast(src: torch.Tensor, idx: torch.Tensor, dtype: torch.dtype, o
     return out
 
 
+# ---- the CSM chain of many streams (fvs_qwen_*_multi, DESIGN.md §3.17) ----------------------------------------------------
+def mem_job(X: torch.Tensor, K: int, *, w=None, init_idx=None, refill_idx=None, max_iter: int = 10, tol: float = 1e-4,
+            uniq_idx=None, n_unique=None, uniq_ws=None, C=None, wsum=None, labels=None, info=None, km_ws=None, order=None,
+            sorted_idx=None, ts=None, w_sorted=None, flags=None, out=None) -> L.QwenMemJob:
+    """one fvs_qwen_mem_job: X [T, PD] (contiguous, device) and whichever device tensors the calls it goes to read or write
+    (workspaces: uint8 views of at least the fvs_qwen_*_workspace_bytes); the tensors must outlive the calls' enqueue"""
+    _chk_cuda(X, w, init_idx, refill_idx, uniq_idx, n_unique, uniq_ws, C, wsum, labels, info, km_ws, order, sorted_idx, ts,
+              w_sorted, flags, out)
+    assert X.is_contiguous() and X.dim() == 2
+    T, PD = X.shape
+    nb = lambda t: 0 if t is None else t.numel() * t.element_size()
+    return L.QwenMemJob(
+        X=X.data_ptr(), T=T, K=int(K), PD=PD, x_dtype=L.dtype_code(X.dtype), w=L.ptr(w), init_idx=L.ptr(init_idx),
+        refill_idx=L.ptr(refill_idx), max_iter=int(max_iter), tol=float(tol), uniq_idx=L.ptr(uniq_idx),
+        n_unique=L.ptr(n_unique), uniq_workspace=L.ptr(uniq_ws), uniq_workspace_bytes=nb(uniq_ws), C=L.ptr(C),
+        wsum=L.ptr(wsum), labels=L.ptr(labels), info=L.ptr(info), km_workspace=L.ptr(km_ws), km_workspace_bytes=nb(km_ws),
+        order_in=L.ptr(order), sorted_idx=L.ptr(sorted_idx), ts=L.ptr(ts), w_sorted=L.ptr(w_sorted), flags=L.ptr(flags),
+        out=L.ptr(out), out_dtype=L.dtype_code(out.dtype) if out is not None else 0)
+
+
+def mem_jobs(jobs) -> "C.Array":
+    return (L.QwenMemJob * len(jobs))(*jobs)
+
+
+def mem_plan(jobs, budget: int = 0):
+    """fvs_qwen_mem_plan (host arithmetic): -> (Lloyd-sweep blocks per job, launch group per job, number of groups)"""
+    n = len(jobs)
+    blocks, groups = (C.c_int32 * n)(), (C.c_int32 * n)()
+    r = L.load().fvs_qwen_mem_plan(mem_jobs(jobs) if not isinstance(jobs, C.Array) else jobs, n, int(budget), blocks, groups)
+    if r < 0:
+        L.check(r, "fvs_qwen_mem_plan")
+    return list(blocks), list(groups), r
+
+
+def _multi(name: str, jobs, budget: int):
+    arr = jobs if isinstance(jobs, C.Array) else mem_jobs(jobs)
+    L.check(getattr(L.load(), name)(arr, len(arr), int(budget), L.cur_stream()), name)
+
+
+def unique_rows_multi(jobs, budget: int = 0):
+    """fvs_qwen_unique_rows per job (uniq_idx, n_unique, uniq_ws), in one launch pair per launch group"""
+    _multi("fvs_qwen_unique_rows_multi", jobs, budget)
+
+
+def kmeans_multi(jobs, budget: int = 0):
+    """fvs_qwen_kmeans per job (C, wsum, labels, info, km_ws), each kernel of the Lloyd loop once per launch group"""
+    _multi("fvs_qwen_kmeans_multi", jobs, budget)
+
+
+def kmeans_finalize_multi(jobs, budget: int = 0):
+    """fvs_qwen_kmeans_finalize per job (sorted_idx, ts, w_sorted, flags)"""
+    _multi("fvs_qwen_kmeans_finalize_multi", jobs, budget)
+
+
+def gather_rows_cast_multi(jobs, budget: int = 0):
+    """fvs_gather_rows_cast(C, sorted_idx, out) per job"""
+    _multi("fvs_gather_rows_cast_multi", jobs, budget)
+
+
+def klarge_retrieve_multi(items, metric: str = "euclidean", want_dist: bool = False):
+    """fvs_qwen_klarge_retrieve_multi: items = [(tem_x [st, PD], klarge_idx int64 [k <= 64], bank [t, PD])], every bank
+    wholly in HBM and of one 16-bit dtype -> per item idx int64 [k] (and dist fp32 [k, t]), the bits klarge_retrieve
+    gives each item alone"""
+    code = {"euclidean": L.KLARGE_EUCLIDEAN, "cosine": L.KLARGE_COSINE}[metric]
+    lib = L.load()
+    keep, sizes = [], []
+    for tem_x, klarge_idx, bank in items:
+        _chk_cuda(tem_x, klarge_idx, bank)
+        tem_x, klarge_idx, bank = _c(tem_x), _c(klarge_idx), _c(bank)
+        assert klarge_idx.dtype == torch.int64 and tem_x.dtype == bank.dtype == items[0][2].dtype
+        assert tem_x.shape[1] == bank.shape[1]
+        keep.append((tem_x, klarge_idx, bank))
+        sizes.append(_al(lib.fvs_qwen_klarge_workspace_bytes(klarge_idx.numel(), bank.shape[0], bank.shape[1])))
+    dev = keep[0][0].device
+    ws = _workspace(sum(sizes), dev, "klarge_multi")
+    jobs, outs, o = [], [], 0
+    for (tem_x, klarge_idx, bank), nb in zip(keep, sizes):
+        k, t = klarge_idx.numel(), bank.shape[0]
+        idx = torch.empty(k, dtype=torch.int64, device=dev)
+        dist = torch.empty(k, t, dtype=torch.float32, device=dev) if want_dist else None
+        jobs.append(L.QwenRetrieveJob(tem_x=tem_x.data_ptr(), klarge_idx=klarge_idx.data_ptr(), bank=bank.data_ptr(), k=k,
+                                      t_total=t, n_dev=t, PD=bank.shape[1], idx_out=idx.data_ptr(), dist_out=L.ptr(dist),
+                                      workspace=ws.data_ptr() + o, workspace_bytes=nb))
+        outs.append((idx, dist) if want_dist else idx)
+        o += nb
+    arr = (L.QwenRetrieveJob * len(jobs))(*jobs)
+    L.check(lib.fvs_qwen_klarge_retrieve_multi(arr, len(jobs), L.dtype_code(keep[0][2].dtype), code, L.cur_stream()),
+            "fvs_qwen_klarge_retrieve_multi")
+    return outs
+
+
+def dam_gather_multi(calls):
+    """fvs_qwen_dam_gather_multi: calls = [dict of dam_gather's keyword arguments], one per stream, all outputs of one
+    dtype; each stream gets the bits (and host_fetches count) of its own dam_gather call"""
+    jobs, keep = [], []
+    for a in calls:
+        picks, prev, sx, mo = _c(a["picks"]), a.get("prev"), a.get("spa_x_out"), a.get("merged_out")
+        _chk_cuda(picks, a["dev_x"], a["dev_merged"], a["chunks"], sx, mo, a.get("host_fetches"))
+        m, pp, px, pm = 0, None, None, None
+        if prev is not None and prev[0] is not None and prev[0].numel():
+            pp, px, pm = prev
+            pp = _c(pp)
+            m = pp.numel()
+        keep.append((picks, pp))
+        jobs.append(L.QwenGatherJob(
+            picks=picks.data_ptr(), n=picks.numel(), n_frames=int(a["n_frames"]), dev_x=L.ptr(a["dev_x"]),
+            dev_merged=L.ptr(a["dev_merged"]), n_dev=int(a["n_dev"]), host_chunks=L.ptr(a["chunks"]),
+            chunk_frames=int(a["chunk_frames"]), prev_picks=L.ptr(pp), m=m, prev_x=L.ptr(px), prev_merged=L.ptr(pm),
+            x_frame_elems=int(a["x_frame_elems"]), merged_frame_elems=int(a["merged_frame_elems"]), spa_x_out=L.ptr(sx),
+            merged_out=L.ptr(mo), host_fetches=L.ptr(a.get("host_fetches"))))
+    out0 = calls[0].get("spa_x_out") if calls[0].get("spa_x_out") is not None else calls[0].get("merged_out")
+    arr = (L.QwenGatherJob * len(jobs))(*jobs)
+    L.check(L.load().fvs_qwen_dam_gather_multi(arr, len(jobs), L.dtype_code(out0.dtype), L.cur_stream()),
+            "fvs_qwen_dam_gather_multi")
+
+
+def mem_workspace_bytes(T: int, K: int, PD: int) -> int:
+    """bytes one job of the CSM chain needs besides its outputs: fp32 centroids, unique-rows and k-means workspaces"""
+    lib = L.load()
+    return _al(K * PD * 4) + _al(lib.fvs_qwen_unique_workspace_bytes(T)) + _al(lib.fvs_qwen_kmeans_workspace_bytes(T, K, PD))
+
+
+def _al(v: int) -> int:
+    return (v + 255) & ~255
+
+
 class TieredBank(NamedTuple):
     """A bank of t_total rows of PD 16-bit elements in two tiers (DESIGN.md §3.13): rows [0, n_dev) are `dev` (HBM,
     [n_dev, PD], None when n_dev is 0); row n_dev + c * chunk_frames + r is row r of the pinned host chunk whose mapped

@@ -33,6 +33,7 @@ import torch
 
 from . import compress_functions as CF
 from . import ops as Q
+from .. import ops as O
 from ..draws import GLOBAL, to_device
 from ..host_tier import CHUNK_BYTES, check_device_frames, chunk_frames, placement  # noqa: F401
 
@@ -123,7 +124,20 @@ class QwenStreamState:
                 draws: Optional[dict] = None, merged: Optional[torch.Tensor] = None):
         """The first half of step(): the clip's work up to and including the copy of its 32-byte read-back, enqueued on
         the current stream.  The caller waits until that copy has landed (an event recorded after it), then calls
-        complete().  Several states may be enqueued before one wait (QwenStreamPool)."""
+        complete().  Several states may be enqueued before one wait (QwenStreamPool).  = enqueue_input(), the CSM
+        k-means of its request (ordered_kmeans_enqueue), enqueue_csm()."""
+        banks, req = self.enqueue_input(x_new, small_new, t, grid, small_grid, start_idx, draws, merged)
+        if req is not None:
+            self.enqueue_csm(req, CF.ordered_kmeans_enqueue(req["cand"], self.flash.temporal_length, req["cand_w"],
+                                                            req["init"], req["refill"], req["order"]))
+        return banks
+
+    def enqueue_input(self, x_new: torch.Tensor, small_new: torch.Tensor, t: int, grid, small_grid, start_idx: int,
+                      draws: Optional[dict] = None, merged: Optional[torch.Tensor] = None):
+        """The clip up to the CSM k-means: banks, candidates and the k-means draws, taken from this state's draw source
+        in the order step() takes them.  -> ((bank, small_bank), req): req is None when the clip needs no fast-path
+        k-means (memory still filling, or a branch the synchronous path runs, which is then already enqueued); otherwise
+        the k-means to run (cand [T, P, D], cand_w, init, refill, order) before enqueue_csm(req, result)."""
         flash = self.flash
         dev, dt, D = x_new.device, x_new.dtype, x_new.shape[-1]
         h, w = grid
@@ -161,32 +175,47 @@ class QwenStreamState:
         self._pending = {}
         if not fast:
             self._compress_sync(cand, cand_w, T, d, start_idx, t)
+            return (bank, small_bank), None
+        snap = None
+        init = d.get("init_idx")
+        if init is None:
+            snap = self.rng.snapshot(dev)
+            init_dev = self.rng.randperm(T, dev)[:T0].to(torch.int32)        # randperm(n_unique), assuming n_unique == T
         else:
-            snap = None
-            init = d.get("init_idx")
-            if init is None:
-                snap = self.rng.snapshot(dev)
-                init_dev = self.rng.randperm(T, dev)[:T0].to(torch.int32)        # randperm(n_unique), assuming n_unique == T
-            else:
-                init_dev = to_device(np.asarray(init)[:T0], np.int32, dev)
-            refill = d.get("refill_idx")
-            if refill is None:
-                refill_dev, _ = self.rng.refill_candidates(T, CF.MAX_ITER * T0, dev)
-            else:
-                refill = list(int(v) for v in refill)
-                refill_dev = to_device(refill + [0] * (CF.MAX_ITER * T0 - len(refill)), np.int32, dev)
-            order = d.get("ts_order")
-            order_dev = None if order is None else to_device(order, np.int64, dev)
-            km = CF.ordered_kmeans_enqueue(cand, T0, cand_w, init_dev, refill_dev, order_dev)
-            tem_x, tem_w, tem_ts = km["feat"].view(T0 * P, D), km["weights"], km["timestamps"]
-            self._enqueue_rest(tem_x, tem_w, tem_ts, T0, km["members"], d)
-            # ---- the one read-back of the step
+            init_dev = to_device(np.asarray(init)[:T0], np.int32, dev)
+        refill = d.get("refill_idx")
+        if refill is None:
+            refill_dev, _ = self.rng.refill_candidates(T, CF.MAX_ITER * T0, dev)
+        else:
+            refill = list(int(v) for v in refill)
+            refill_dev = to_device(refill + [0] * (CF.MAX_ITER * T0 - len(refill)), np.int32, dev)
+        order = d.get("ts_order")
+        order_dev = None if order is None else to_device(order, np.int64, dev)
+        req = dict(cand=cand, cand_w=cand_w, T=T, d=d, start_idx=start_idx, t=t, snap=snap, own_refills=refill is None,
+                   init=init_dev, refill=refill_dev, order=order_dev)
+        return (bank, small_bank), req
+
+    def enqueue_csm(self, req: dict, km: dict, readback: Optional[torch.Tensor] = None):
+        """The rest of the clip once the CSM k-means of enqueue_input's `req` is enqueued (km: the dict of
+        ordered_kmeans_enqueue): DAM retrieval, merged memory and the read-back.  readback: a pinned int32 [8] row the
+        caller fills itself with km's n_unique, info and flags after its last kernel (QwenStreamPool copies every
+        stream's at once); None: this state copies its own."""
+        T0, P = self.flash.temporal_length, req["cand"].shape[1]
+        D = req["cand"].shape[2]
+        tem_x, tem_w, tem_ts = km["feat"].view(T0 * P, D), km["weights"], km["timestamps"]
+        self._enqueue_rest(tem_x, tem_w, tem_ts, T0, km["members"], req["d"])
+        # ---- the one read-back of the step
+        if readback is None:
             if self._readback is None:
                 self._readback = torch.empty(8, dtype=torch.int32).pin_memory()
             self._readback[:6].copy_(torch.cat([km["n_unique"], km["info"], km["flags"]]), non_blocking=True)
-            self._pending = dict(cand=cand, cand_w=cand_w, T=T, d=d, start_idx=start_idx, t=t, snap=snap,
-                                 own_refills=refill is None)
-        return bank, small_bank
+            readback = self._readback
+        self._set_pending(req, readback)
+
+    def _set_pending(self, req: dict, readback: torch.Tensor):
+        """what complete() needs of the enqueued fast-path clip; readback: the row it reads"""
+        keep = ("cand", "cand_w", "T", "d", "start_idx", "t", "snap", "own_refills")
+        self._pending = dict({k: req[k] for k in keep}, readback=readback)
 
     def complete(self):
         """The second half of step(), once the read-back of enqueue() has landed: a valid fast-path clip is final (or raises
@@ -196,7 +225,7 @@ class QwenStreamState:
         if p:
             T0 = self.flash.temporal_length
             T = p["T"]
-            n_unique, _, consumed, _, _, empty = (int(v) for v in self._readback[:6])
+            n_unique, _, consumed, _, _, empty = (int(v) for v in p.get("readback", self._readback)[:6])
             valid = n_unique >= T0 and (p["snap"] is None or n_unique == T)
             if valid:
                 if empty:
@@ -219,21 +248,53 @@ class QwenStreamState:
 
     def _enqueue_rest(self, tem_x, tem_w, tem_ts, n_tem, members, d):
         """DAM retrieval and the merged memory for a CSM that is already (being) computed; no host round trip for the
-        default spatial methods."""
+        default spatial methods.  = _rest_retrieval, the retrieval it asks for, _rest_outputs, the gather and the merger
+        (QwenStreamPool runs the middle three as one job table each for all its streams)."""
+        ctx = self._rest_retrieval(tem_x, tem_w, tem_ts, n_tem, members, d)
+        if ctx["retrieve"] is not None:
+            centroids, heaviest, bank, metric = ctx["retrieve"]
+            ctx["picks"] = Q.klarge_retrieve(centroids, heaviest, bank, metric=metric)
+        gather, merge = self._rest_outputs(ctx)
+        if gather is not None:
+            Q.dam_gather(**gather)
+        if merge is not None:
+            self.merger(merge[0], out=merge[1])
+
+    def _rest_retrieval(self, tem_x, tem_w, tem_ts, n_tem, members, d):
+        """the CSM fields, and the DAM picks or, for a klarge retrieval over a bank wholly in HBM (k <= 64), what it
+        needs: ctx["retrieve"] = (centroids [st, PD], heaviest int64 [k], bank [n, PD], metric); picks are then set by
+        the caller"""
         flash = self.flash
-        h, w = self.grid
         D = tem_x.shape[-1]
         n = self.n_frames
-        dt, dev = self._small_layout[0], tem_x.device
+        dev = tem_x.device
         self.tem_x, self.tem_weights, self.tem_timestamp, self.n_tem, self.tem_members = tem_x, tem_w, tem_ts, n_tem, members
-        if flash.spatial_length > 0:
-            tem_pos = torch.round(tem_ts.float()).to(torch.int64)
-            picks = flash.spatial_picks(self._small_bank(D, dev), n, tem_x, self._thw(n_tem, small=True), tem_w, tem_pos,
-                                        draws=d)
-            n_spa = picks.numel()                                   # min(n, spatial_length): known on the host
+        ctx = dict(tem_x=tem_x, d=d, picks=None, retrieve=None)
+        if flash.spatial_length <= 0:
+            ctx["picks"], ctx["n_spa"] = torch.empty(0, dtype=torch.int64, device=dev), 0
+            return ctx
+        n_spa = min(n, flash.spatial_length)                            # known on the host
+        ctx["n_spa"] = n_spa
+        tem_pos = torch.round(tem_ts.float()).to(torch.int64)
+        klarge = flash.spatial_method in ("klarge_retrieve", "klarge_retrieve_cos")
+        if (klarge and n > flash.spatial_length and self.n_small_host == 0 and n_spa <= 64
+                and (d or {}).get("weight_order") is None and self._small_layout[0] in (torch.float16, torch.bfloat16)):
+            heaviest = O.argsort_desc(tem_w)[:n_spa]                   # spatial_picks' ranking
+            ctx["retrieve"] = (tem_x.reshape(n_tem, -1), heaviest, self.bank_small.rows().view(n, -1),
+                               "cosine" if flash.spatial_method == "klarge_retrieve_cos" else "euclidean")
         else:
-            picks, n_spa = torch.empty(0, dtype=torch.int64, device=dev), 0
-        whole = n_spa == n and self.n_host == 0           # memory still filling: the DAM is the whole bank, a view of it
+            ctx["picks"] = flash.spatial_picks(self._small_bank(D, dev), n, tem_x, self._thw(n_tem, small=True), tem_w,
+                                               tem_pos, draws=d)
+        return ctx
+
+    def _rest_outputs(self, ctx):
+        """the DAM and video_embeds tensors for the picks of ctx -> (keyword arguments of the dam_gather that fills them,
+        or None; (CSM rows, the slice of video_embeds their merged rows go to), or None)"""
+        h, w = self.grid
+        tem_x, picks, n_spa = ctx["tem_x"], ctx["picks"], ctx["n_spa"]
+        D = tem_x.shape[-1]
+        dt, dev = self._small_layout[0], tem_x.device
+        whole = n_spa == self.n_frames and self.n_host == 0   # memory still filling: the DAM is the whole bank, a view of it
         spa_x = self.bank_x.rows() if whole else torch.empty(n_spa, h * w, D, dtype=dt, device=dev)
         self.spa_x, self.spa_positions = spa_x, picks
         pm = h * w // 4                                               # merged tokens of a retrieved frame
@@ -243,12 +304,13 @@ class QwenStreamState:
         # one launch writes the retrieved frames and their merged rows (fresh tensors: readers may hold the old ones)
         gather_x = n_spa > 0 and not whole
         gather_m = n_spa > 0 and out is not None
+        gather = None
         if gather_x or gather_m:
-            self._gather(picks, spa_x if gather_x else None, out[: n_spa * pm].view(n_spa, pm, -1) if gather_m else None,
-                         self._prev_dam)
-        if out is not None and out.shape[0] > n_spa * pm:
-            self.merger(tem_x, out=out[n_spa * pm:])
+            gather = self._gather_args(picks, spa_x if gather_x else None,
+                                       out[: n_spa * pm].view(n_spa, pm, -1) if gather_m else None, self._prev_dam)
+        merge = (tem_x, out[n_spa * pm:]) if out is not None and out.shape[0] > n_spa * pm else None
         self.video_embeds = out
+        return gather, merge
 
     # ------------------------------------------------------------------------------------------------ two-tier bank
     def _dam(self):
@@ -334,13 +396,18 @@ class QwenStreamState:
                             self._small_per_chunk(), rb.n + self.n_small_host, self._small_layout[0], dev)
 
     def _gather(self, picks, spa_x, merged, prev):
+        Q.dam_gather(**self._gather_args(picks, spa_x, merged, prev))
+
+    def _gather_args(self, picks, spa_x, merged, prev) -> dict:
+        """the keyword arguments of the Q.dam_gather that writes spa_x / merged for `picks` from this state's banks"""
         dt, xs, ms = self._layout
         if self.host_fetches is None:
             self.host_fetches = torch.zeros(1, dtype=torch.int64, device=picks.device)
-        Q.dam_gather(picks, self.bank_x.n + self.n_host, self.bank_x.buf if self.bank_x.n else None,
-                     self.bank_merged.buf if self.bank_merged.n else None, self.bank_x.n, self._chunk_table,
-                     self._per_chunk(), xs.numel(), 0 if ms is None else ms.numel(), prev=prev, spa_x_out=spa_x,
-                     merged_out=merged, host_fetches=self.host_fetches)
+        return dict(picks=picks, n_frames=self.bank_x.n + self.n_host, dev_x=self.bank_x.buf if self.bank_x.n else None,
+                    dev_merged=self.bank_merged.buf if self.bank_merged.n else None, n_dev=self.bank_x.n,
+                    chunks=self._chunk_table, chunk_frames=self._per_chunk(), x_frame_elems=xs.numel(),
+                    merged_frame_elems=0 if ms is None else ms.numel(), prev=prev, spa_x_out=spa_x, merged_out=merged,
+                    host_fetches=self.host_fetches)
 
     def host_fetch_count(self) -> int:
         """retrieved frames read from the host chunks since the stream started here (synchronises; tests and timing)"""

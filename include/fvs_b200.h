@@ -438,6 +438,58 @@ int fvs_qwen_kmeans_finalize(const int32_t* labels, const float* wsum, int T, in
 int fvs_gather_rows_cast(const float* src, const int64_t* idx, void* out, int n, int64_t row_elems, int out_dtype,
                          fvs_stream_t stream);
 
+/* ---- the CSM chain of many Qwen2-VL streams in one launch per kernel (DESIGN.md §3.17) -------------------------------
+ * One fvs_qwen_mem_job per stream: its candidates X [T, PD] (x_dtype), draws and outputs, all device pointers.  Each
+ * *_multi call below gives job i exactly the bits the single-stream call gives it, whatever the other jobs are: a job
+ * always gets the blocks its single call launches, laid end to end with the other jobs' blocks in one flat grid (a block
+ * finds its job in a block-offset table passed as a kernel parameter), so no reduction of a job depends on its
+ * neighbours or on the budget.  Jobs go into launches in order, at most FVS_QWEN_MEM_JOBS_PER_LAUNCH per launch and, when
+ * budget > 0, at most `budget` Lloyd-sweep blocks per launch (a larger job goes alone); every kernel of a call is then
+ * launched once per launch group.  Every job is validated before anything is enqueued: on FVS_EINVAL (a bad shape or
+ * pointer, a workspace too small, an output range shared by two jobs) nothing was launched.  No allocation, no host sync.
+ *   fvs_qwen_unique_rows_multi:     fvs_qwen_unique_rows(X, T, PD, x_dtype, uniq_idx, n_unique, uniq_workspace, ...)
+ *   fvs_qwen_kmeans_multi:          fvs_qwen_kmeans(X, x_dtype, w, uniq_idx, init_idx, refill_idx, T, K, PD, max_iter, tol,
+ *                                                   C, wsum, labels, info, km_workspace, ...); each job keeps its own
+ *                                   max_iter and tolerance exit (a job that has stopped skips the remaining iterations)
+ *   fvs_qwen_kmeans_finalize_multi: fvs_qwen_kmeans_finalize(labels, wsum, T, K, order_in, sorted_idx, ts, w_sorted, flags)
+ *   fvs_gather_rows_cast_multi:     fvs_gather_rows_cast(C, sorted_idx, out, K, PD, out_dtype)
+ * Fields a call does not read may be anything. */
+#define FVS_QWEN_MEM_JOBS_PER_LAUNCH 16
+typedef struct fvs_qwen_mem_job {
+  const void* X;                   /* [T, PD] candidate rows */
+  int T, K, PD, x_dtype;           /* T <= 4096, 0 < K <= min(T, 1024), PD % 1024 == 0 */
+  const float* w;                  /* [T] fp32 weights */
+  const int32_t* init_idx;         /* [K] */
+  const int32_t* refill_idx;       /* [max(1, max_iter * K)] */
+  int max_iter;
+  float tol;
+  int32_t* uniq_idx;               /* [T]: written by unique_rows, read by kmeans (NULL there: X[init_idx[k]]) */
+  int32_t* n_unique;               /* [1] */
+  void* uniq_workspace;            /* fvs_qwen_unique_workspace_bytes(T) */
+  size_t uniq_workspace_bytes;
+  float* C;                        /* [K, PD] fp32 centroids */
+  float* wsum;                     /* [K] */
+  int32_t* labels;                 /* [T] */
+  int32_t* info;                   /* [4] */
+  void* km_workspace;              /* fvs_qwen_kmeans_workspace_bytes(T, K, PD) */
+  size_t km_workspace_bytes;
+  const int64_t* order_in;         /* [K] permutation to replay, or NULL (stable order) */
+  int64_t* sorted_idx;             /* [K] */
+  float* ts;                       /* [K] */
+  float* w_sorted;                 /* [K] */
+  int32_t* flags;                  /* [1] */
+  void* out;                       /* [K, PD] out_dtype: the ordered, cast centroids */
+  int out_dtype;
+} fvs_qwen_mem_job;
+/* The launch plan of the *_multi calls for `budget` (pure host arithmetic, no CUDA call): job i gets blocks_h[i] Lloyd-
+ * sweep blocks ((T+7)/8 * PD/1024, the widest grid of its chain) in launch group groups_h[i].  Returns the number of
+ * launch groups (>= 1) or a negative error code. */
+int fvs_qwen_mem_plan(const fvs_qwen_mem_job* jobs_h, int n_jobs, int budget, int32_t* blocks_h, int32_t* groups_h);
+int fvs_qwen_unique_rows_multi(const fvs_qwen_mem_job* jobs_h, int n_jobs, int budget, fvs_stream_t stream);
+int fvs_qwen_kmeans_multi(const fvs_qwen_mem_job* jobs_h, int n_jobs, int budget, fvs_stream_t stream);
+int fvs_qwen_kmeans_finalize_multi(const fvs_qwen_mem_job* jobs_h, int n_jobs, int budget, fvs_stream_t stream);
+int fvs_gather_rows_cast_multi(const fvs_qwen_mem_job* jobs_h, int n_jobs, int budget, fvs_stream_t stream);
+
 /* spatial_enhance with spatial_method='klarge_retrieve' (vstream_qwen2vl_model.py:197-207, 229-238): for the k centroids
  * c_i = tem_x[klarge_idx[i]] (tem_x [st, PD], klarge_idx int64 [k] = the k heaviest clusters) and the bank [t_total, PD] of
  * half-resolution frames, idx_out[i] = argmin_t sqrt((|c_i|^2 + |b_t|^2) - 2 c_i.b_t) with every op rounded to the 16-bit
@@ -467,6 +519,26 @@ int fvs_qwen_klarge_retrieve_tiered(const void* tem_x, const int64_t* klarge_idx
                                     int metric, int64_t* idx_out, float* dist_out, void* workspace, size_t workspace_bytes,
                                     fvs_stream_t stream);
 
+/* The klarge retrieval of many streams in one launch per kernel (DESIGN.md §3.17): job i gets exactly the bits of
+ * fvs_qwen_klarge_retrieve(tem_x, klarge_idx, bank, k, t_total, PD, dtype, metric, idx_out, dist_out, workspace, ...)
+ * whatever the other jobs are: its sweep keeps the single call's split-K partition (PD/1024 slices x ceil(t_total/32)
+ * row splits), laid end to end with the other jobs' blocks.  dtype and metric are the call's; k, t_total, PD, the bank
+ * and klarge_idx are each job's.  The bank must be wholly in HBM: a job with n_dev != t_total (host rows, which the
+ * tiered sweep reads through fvs_qwen_klarge_retrieve_tiered) is refused.  At most FVS_QWEN_MEM_JOBS_PER_LAUNCH jobs per
+ * launch; FVS_EINVAL with nothing launched on a bad job or an output shared by two jobs. */
+typedef struct fvs_qwen_retrieve_job {
+  const void* tem_x;               /* [st, PD] centroids */
+  const int64_t* klarge_idx;       /* [k] */
+  const void* bank;                /* [t_total, PD] half-resolution frames, device rows */
+  int k, t_total, n_dev, PD;       /* 0 < k <= 64; n_dev must equal t_total */
+  int64_t* idx_out;                /* [k] */
+  float* dist_out;                 /* [k, t_total] or NULL */
+  void* workspace;                 /* fvs_qwen_klarge_workspace_bytes(k, t_total, PD) */
+  size_t workspace_bytes;
+} fvs_qwen_retrieve_job;
+int fvs_qwen_klarge_retrieve_multi(const fvs_qwen_retrieve_job* jobs_h, int n_jobs, int dtype, int metric,
+                                   fvs_stream_t stream);
+
 /* FlashMemory.calc_am_rope (vstream_qwen2vl_model.py:254-277): out [3, n] int64 position ids of the n = spa_t*spa_h*spa_w
  * + tem_t*tem_h*tem_w memory tokens (DAM rows first, then CSM rows offset by the DAM size), plus visual_start_id. */
 int fvs_qwen_am_rope(const int64_t* spa_positions, int spa_t, int spa_h, int spa_w, const int64_t* tem_positions, int tem_t,
@@ -489,6 +561,29 @@ int fvs_qwen_dam_gather(const int64_t* picks, int n, int64_t n_frames, const voi
                         int64_t n_dev, const void* const* host_chunks, int chunk_frames, const int64_t* prev_picks, int m,
                         const void* prev_x, const void* prev_merged, int64_t x_frame_elems, int64_t merged_frame_elems,
                         int dtype, void* spa_x_out, void* merged_out, uint64_t* host_fetches, fvs_stream_t stream);
+/* fvs_qwen_dam_gather of many streams in one launch: job i gets exactly the bits (and host_fetches count) of the single
+ * call with its own arguments — its own two-tier bank, previous DAM and chunk table.  dtype is the call's.  At most
+ * FVS_QWEN_MEM_JOBS_PER_LAUNCH jobs per launch; every job gets the single call's checks, and no output (spa_x_out,
+ * merged_out, host_fetches) may be shared by two jobs: FVS_EINVAL with nothing launched otherwise. */
+typedef struct fvs_qwen_gather_job {
+  const int64_t* picks;
+  int n;
+  int64_t n_frames;
+  const void* dev_x;
+  const void* dev_merged;
+  int64_t n_dev;
+  const void* const* host_chunks;  /* DEVICE table, as for fvs_qwen_dam_gather */
+  int chunk_frames;
+  const int64_t* prev_picks;
+  int m;
+  const void* prev_x;
+  const void* prev_merged;
+  int64_t x_frame_elems, merged_frame_elems;
+  void* spa_x_out;
+  void* merged_out;
+  uint64_t* host_fetches;
+} fvs_qwen_gather_job;
+int fvs_qwen_dam_gather_multi(const fvs_qwen_gather_job* jobs_h, int n_jobs, int dtype, fvs_stream_t stream);
 /* *dev_out = the device address of pinned host memory `host` (cudaHostGetDevicePointer); FVS_EINVAL if it is not pinned */
 int fvs_host_device_ptr(const void* host, void** dev_out);
 
