@@ -45,8 +45,8 @@ def check(name, got, ref, bound, rounding=None):
     ratio = err / bound
     worst = float(ratio.max())
     i = int(ratio.argmax())
-    pre = "" if rounding is None else \
-        f", before the output rounding {float(((err - rounding).clamp(min=0) / (bound - rounding)).max()):.3f}"
+    pre = "" if rounding is None else ", before the output rounding " \
+        f"{float(((err - rounding).clamp(min=0) / (bound - rounding)).nan_to_num(nan=0.0, posinf=math.inf).max()):.3f}"
     print(f"\n[{name}] max err/bound {worst:.3f} (err {float(err.flatten()[i]):.3e}, bound {float(bound.flatten()[i]):.3e})"
           f"{pre}")
     assert torch.isfinite(got).all(), name
@@ -67,12 +67,17 @@ ATTN_CASES = [(n, 16) for n in ATTN_TOKENS] + [(577, 1), (864, 3), (129, 3), (65
 
 
 def attention_bound_check(name, nat, out, frames, tokens, heads, hd, scale):
+    ref, bound, rounding = attention_bound(nat, frames, tokens, heads, hd, scale)
+    return check(name, out.view(frames, tokens, heads, hd), ref, bound, rounding)
+
+
+def attention_bound(nat, frames, tokens, heads, hd, scale):
+    """fp64 reference, element-wise bound and its output-rounding part, each [frames, tokens, heads, hd], for the
+    attention of the natural-layout qkv rows `nat` [frames * tokens, 3 * heads * hd]"""
     dt = nat.dtype
     u, s_p = U16[dt], (2.0 ** -25 if dt == torch.float16 else 0.0)
     q, k, v = nat.double().view(frames, tokens, 3, heads, hd).unbind(2)
-    got = out.view(frames, tokens, heads, hd)
-    worst = 0.0
-    ref_all = torch.empty(frames, tokens, heads, hd, dtype=torch.float64, device=out.device)
+    ref_all = torch.empty(frames, tokens, heads, hd, dtype=torch.float64, device=nat.device)
     bound_all, round_all = torch.empty_like(ref_all), torch.empty_like(ref_all)
     for f in range(frames):
         for h in range(heads):
@@ -87,7 +92,7 @@ def attention_bound_check(name, nat, out, frames, tokens, heads, hd, scale):
                 b[r0:r1] = (w[r0:r1, :, None] * (vh[None] - o[r0:r1, None, :]).abs()).sum(1)
             b += u * o.abs() + 2.0 ** -20 * vh.abs().amax(0)
             ref_all[f, :, h], bound_all[f, :, h], round_all[f, :, h] = o, b, u * o.abs()
-    return check(name, got, ref_all, bound_all, round_all)
+    return ref_all, bound_all, round_all
 
 
 @pytest.mark.parametrize("dt", list(DTYPES))
@@ -179,6 +184,27 @@ def gemm_case(L, epi, dtype, M, N, K, pad, g, tails):
         aux = (torch.randn(period, N, generator=g)).to(dtype).cuda()
     aux_in = aux.double().clone() if aux is not None else None
     linear_raw(L, A, W, bias, aux, out, code, period)
+    parts = {}
+    y, bound, rounding = linear_bound(A, W, bias, epi, aux_in, out, parts)
+    name = f"linear {epi} {str(dtype)[6:]} M{M} N{N} K{K}{' pitched' if pad else ''}"
+    worst = check(name, out, y, bound, rounding)
+    if epi == "quickgelu":
+        x, tanh_term = parts["x"], parts["tanh_term"]
+        tail = (x >= -6) & (x <= -1)
+        if bool(tail.any()):
+            err = (out.double() - y).abs()
+            tails.append((float(err[tail].max()), float(tanh_term[tail].min()), float((err / bound)[tail].max())))
+    return worst
+
+
+def linear_bound(A, W, bias, epi, aux, out, parts=None):
+    """fp64 reference, element-wise bound and its output-rounding part (None for an fp32 out) of fvs_linear with the
+    epilogue `epi` (an EPI name) on the 16-bit A [M, K], W [N, K], bias [N] or None and the epilogue's aux input as it was
+    before the call: the residual [M, N] (fp32 for the _f32 epilogues) or the row table [period, N].  `out` is what the
+    kernel wrote; its dtype selects the output rounding.  `parts`, a dict, receives the fp64 pre-activation "x" and the
+    quick-GELU "tanh_term"."""
+    M, K = A.shape
+    f32_out = out.dtype == torch.float32
     Ad, Wd = A.double(), W.double()
     acc = Ad @ Wd.T
     e = K * 2.0 ** -23 * (Ad.abs() @ Wd.abs().T)                  # accumulation
@@ -187,6 +213,9 @@ def gemm_case(L, epi, dtype, M, N, K, pad, g, tails):
         e = e + U32 * (x.abs() + e)                               # fl(acc + bias)
     else:
         x = acc                                                   # acc + 0.f: exact
+    aux_in = aux.double() if aux is not None else None
+    if parts is not None:
+        parts["x"] = x
     if epi == "quickgelu":
         xa = x.abs() + e
         y = x * torch.sigmoid(1.702 * x)                          # = 0.5 x (1 + tanh(0.851 x))
@@ -194,6 +223,8 @@ def gemm_case(L, epi, dtype, M, N, K, pad, g, tails):
         tanh_term = 0.5 * xa * EPS_TANH
         e = LIP_QUICKGELU * e + tanh_term + 0.5 * xa * dz         # tanh.approx error; tanh is 1-Lipschitz
         e = e + U32 * (y.abs() + e)                               # fmaf(h, t, h)
+        if parts is not None:
+            parts["tanh_term"] = tanh_term
     elif epi == "gelu":
         xa = x.abs() + e
         y = 0.5 * x * (1 + torch.erf(x / math.sqrt(2)))
@@ -202,7 +233,7 @@ def gemm_case(L, epi, dtype, M, N, K, pad, g, tails):
         e = LIP_GELU * e + 0.5 * xa * (d_erf + 2 * U32)           # fl(1 + erf), |1 + erf| <= 2: one rounding
         e = e + U32 * (y.abs() + e)                               # (0.5 x) * (1 + erf): one rounding
     elif epi == "rowtable":
-        y = x + aux_in[torch.arange(M, device=x.device) % period]
+        y = x + aux_in[torch.arange(M, device=x.device) % aux_in.shape[0]]
         e = e + U32 * (y.abs() + e)
     elif aux is not None:
         y = x + aux_in
@@ -211,14 +242,7 @@ def gemm_case(L, epi, dtype, M, N, K, pad, g, tails):
         y = x
     rounding = None if f32_out else half_ulp(out)
     bound = e if f32_out else e + rounding
-    name = f"linear {epi} {str(dtype)[6:]} M{M} N{N} K{K}{' pitched' if pad else ''}"
-    worst = check(name, out, y, bound, rounding)
-    if epi == "quickgelu":
-        tail = (x >= -6) & (x <= -1)
-        if bool(tail.any()):
-            err = (out.double() - y).abs()
-            tails.append((float(err[tail].max()), float(tanh_term[tail].min()), float((err / bound)[tail].max())))
-    return worst
+    return y, bound, rounding
 
 
 @pytest.mark.parametrize("dt", list(DTYPES))

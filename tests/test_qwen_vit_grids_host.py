@@ -50,11 +50,41 @@ def grid_positions(h, w, mutation=None):
     return torch.stack([hp, wp], dim=-1)
 
 
+# Localised rotary mistakes (rope_mutation of vit_forward / rope_apply), each touching a few percent of q and k or less:
+#   'sin_sign'        the sign of sin flipped in one 8-dim group (dims 8g..8g+7 and their partners +40) of one head;
+#   'extra_unrotated' dims 32..39 and 72..79 of every head (the 16-dim "extra" block of the kernel's layout) not rotated;
+#   'partner_shift'   every dim rotated against partner d + 39 (d < 40) / d - 39 instead of d + 40 / d - 40.
+ROPE_MUTATIONS = ("sin_sign", "extra_unrotated", "partner_shift")
+SIN_SIGN_HEAD, SIN_SIGN_GROUP = 5, 2
+
+
+def rope_apply(v, cos, sin, rope_mutation=None):
+    """apply_rotary_pos_emb_vision: v * cos + rotate_half(v) * sin on v [rows, heads, hd], cos / sin [rows, 1, hd]
+    (cat([angles, angles])), optionally with one of ROPE_MUTATIONS"""
+    hd = v.shape[-1]
+    half = hd // 2
+    if rope_mutation == "partner_shift":
+        rot = torch.cat([-v[..., half - 1:hd - 1], v[..., 1:half + 1]], dim=-1)
+    else:
+        rot = torch.cat([-v[..., half:], v[..., :half]], dim=-1)
+    if rope_mutation == "sin_sign":
+        sin = sin.expand(-1, v.shape[1], -1).clone()
+        for d0 in (8 * SIN_SIGN_GROUP, half + 8 * SIN_SIGN_GROUP):
+            sin[:, SIN_SIGN_HEAD, d0:d0 + 8] *= -1
+    elif rope_mutation == "extra_unrotated":
+        cos, sin = cos.clone(), sin.clone()
+        for d0 in (half - 8, hd - 8):
+            cos[..., d0:d0 + 8], sin[..., d0:d0 + 8] = 1, 0
+    else:
+        assert rope_mutation in (None, "partner_shift"), rope_mutation
+    return v * cos + rot * sin
+
+
 def vit_forward(patch_rows, grids, sd, *, depth, heads=16, eps=1e-6, dtype=torch.float64, device="cpu", mutation=None,
-                head_chunk=4):
+                head_chunk=4, rope_mutation=None):
     """QO.qwen_vit_forward in any precision on any device (test_oracle_restatement_is_the_oracle pins the two), with
-    the rotary positions optionally mutated (see grid_positions).  Attention runs per segment and `head_chunk` heads at
-    a time, so that a 4784-token segment fits on the GPU in fp64."""
+    the rotary positions optionally mutated (see grid_positions) or the rotary itself (one of ROPE_MUTATIONS).
+    Attention runs per segment and `head_chunk` heads at a time, so that a 4784-token segment fits on the GPU in fp64."""
     f = lambda k: sd[k].to(device=device, dtype=dtype)
     E = sd["patch_embed.proj.weight"].shape[0]
     hd = E // heads
@@ -72,8 +102,7 @@ def vit_forward(patch_rows, grids, sd, *, depth, heads=16, eps=1e-6, dtype=torch
     cos, sin = emb.cos()[:, None, :], emb.sin()[:, None, :]
 
     def rope(v):
-        v1, v2 = v[..., : hd // 2], v[..., hd // 2:]
-        return v * cos + torch.cat([-v2, v1], dim=-1) * sin
+        return rope_apply(v, cos, sin, rope_mutation)
 
     ln = torch.nn.functional.layer_norm
     for i in range(depth):
