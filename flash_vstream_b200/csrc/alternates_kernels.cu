@@ -357,7 +357,8 @@ __global__ void __launch_bounds__(256) kmf_dist_kernel(KM B, const __half* __res
   const __half* c = (B.state[1] ? B.C[1] : B.C[0]) + size_t(k) * PD;
   const float ab = warp_row_sum([&](int e) { return __fmul_rn(__fmul_rn(-2.0f, h2f(x[e])), h2f(c[e])); }, PD, lane);
   const float tot = rh(__fadd_rn(__fadd_rn(ab, B.xn[t]), B.cn[k]));
-  if (lane == 0) B.dist[u] = rh(sqrtf(fmaxf(tot, 0.0f)));
+  // clamp_min(0) keeps a NaN (-inf + inf once |x|^2 saturates); fmaxf(NaN, 0) would return 0, the nearest distance
+  if (lane == 0) B.dist[u] = rh(sqrtf(tot < 0.0f ? 0.0f : tot));
 }
 __global__ void __launch_bounds__(256) kmf_assign_kernel(KM B, int T, int K) {
   if (B.state[0]) return;

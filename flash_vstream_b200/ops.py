@@ -273,6 +273,12 @@ def abstract_update(M, F, Wq, bq, Wk, bk, ratio=0.2, out=None):
 
 
 def argsort_desc(w: torch.Tensor) -> torch.Tensor:
+    """stable descending argsort of a 1-D weight vector.  Anything else is refused: the flattened order of a [n, n] matrix
+    holds indices up to n² - 1, which key_retrieve would read as rows of the long memory."""
+    if not isinstance(w, torch.Tensor):
+        raise TypeError(f"argsort_desc: the weight must be a tensor, got {type(w).__name__}")
+    if w.dim() != 1:
+        raise ValueError(f"argsort_desc: the weight must be 1-D, got shape {tuple(w.shape)}")
     _chk_cuda(w)
     w = _c(w)
     out = torch.empty(w.numel(), dtype=torch.int64, device=w.device)

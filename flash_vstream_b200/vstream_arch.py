@@ -32,6 +32,32 @@ from .draws import GLOBAL
 KEY_LENGTH = 3  # hard-coded in the reference (vstream_arch.py:263, :683)
 
 
+_ALTERNATES = (drop_feature, merge_feature, k_drop_feature, kmeans_feature, k_merge_feature)
+
+
+def _refuse_alternate_weight(fn, T: int, T0: int, sample_type: str):
+    """Raise where the reference's key retrieval raises on the weight an alternate compressor returns for T long rows
+    (vstream_arch.py:258-266, :679-686).  The callers run this before the pooling of the call, its frame buffer append and
+    any launch:
+      * None -> TypeError from torch.argsort(None): kdrop and kmeans never return a weight, drop / merge / kmerge return
+        None on their T <= T0 pass-through;
+      * k_merge's [T0, T0] similarity matrix -> long_memory[argsort(weight)] is [T0, T0, P, D], and the distance to the
+        long memory does not broadcast (T > T0 >= 2) -> RuntimeError.  Sorting that matrix flat instead would give indices
+        up to T0² - 1, far past the T rows key retrieval reads.
+    Draws: kdrop first draws its T - T0 coin flips, as the reference's k_drop_feature does before it returns; a refused
+    kmeans draws nothing, while the reference draws its randperm and the refills of a Lloyd loop that would have to run."""
+    if fn not in _ALTERNATES:
+        return
+    if fn is k_drop_feature and T > T0:
+        GLOBAL.randints(0, 1, T - T0)
+    if fn in (k_drop_feature, kmeans_feature) or T <= T0:
+        raise TypeError(f"argsort(): video_sample_type = {sample_type} returns no weight for {T} long-memory rows "
+                        f"and video_long_memory_length = {T0}, and the key retrieval sorts that weight")
+    if fn is k_merge_feature:
+        raise RuntimeError(f"video_sample_type = {sample_type} returns its [{T0}, {T0}] similarity matrix as the weight; "
+                           f"the key centroids it selects do not broadcast against the {T} long-memory rows")
+
+
 def _is_manager_proxy(obj) -> bool:
     try:
         from multiprocessing.managers import BaseProxy
@@ -149,7 +175,9 @@ class VStreamMetaForCausalLM:
             init_idx, refill_idx = draws if draws is not None else (None, None)
             long_c, weight, _, _ = weighted_kmeans_device(long_memory, s.long_len, None, init_idx, refill_idx)
         else:   # the streaming table also knows the *_kmerge aliases (vstream_arch.py:626-637)
-            long_c, weight, _ = self._compress_fn(s.sample_type, streaming=streaming)(long_memory, s.long_len)
+            fn = self._compress_fn(s.sample_type, streaming=streaming)
+            _refuse_alternate_weight(fn, long_memory.shape[0], s.long_len, s.sample_type)   # the callers checked already
+            long_c, weight, _ = fn(long_memory, s.long_len)
         order = self._order(weight)
         return long_c, ops.key_retrieve(long_memory, order, KEY_LENGTH), order, weight
 
@@ -161,6 +189,9 @@ class VStreamMetaForCausalLM:
         new_image_features = []
         for img_feature in image_features:
             cur_start = min(s.cur_len, img_feature.shape[0])
+            n_long = img_feature.shape[0] - cur_start
+            if s.long_len != 0 and n_long > 0:     # before this video's pooling launches
+                _refuse_alternate_weight(self._compress_fn(s.sample_type), n_long, s.long_len, s.sample_type)
             if cur_start == 0:
                 cur_memory, long_memory, Turing_memory = img_feature[:0], img_feature, img_feature
             else:
@@ -342,13 +373,24 @@ class VStreamMetaForCausalLM:
             bank = self._get_bank(cfg, concat_images.shape[0], concat_images.device) if cfg is not None else None
             if bank is not None and self._stream_step_fused(bank, concat_images, engine, draws):
                 return []
+        self._refuse_stream(s, concat_images.shape[0])
         image_features = self.encode_images(concat_images)                           # [t, P, D]
         return self.consolidate_streaming(image_features, draws=draws)
+
+    def _refuse_stream(self, s, t):
+        """_refuse_alternate_weight for a streaming call of t frames, before its encoder, pooling and buffer append: its
+        compression sees the published long rows plus t (the reference publishes only at the end of a call, :693-695,
+        so a refused call leaves the stream as it was)"""
+        fn = self._compress_fn(s.sample_type, streaming=True)
+        mem = self.video_embedding_memory
+        if fn in _ALTERNATES and s.long_len != 0 and mem is not None and len(mem) > 0:
+            _refuse_alternate_weight(fn, mem[1].shape[0] + t, s.long_len, s.sample_type)
 
     def consolidate_streaming(self, image_features, draws=None):
         """Everything of embed_video_streaming after the encoder (vstream_arch.py:644-697)."""
         s = self._star_cfg()
         self._compress_fn(s.sample_type, streaming=True)   # unknown video_sample_type raises like the reference (:663-664)
+        self._refuse_stream(s, image_features.shape[0])
         g = round(math.sqrt(image_features.shape[1]))
         if image_features.is_cuda and g * g == image_features.shape[1]:
             cfg = self._fused_cfg(s, g, image_features.shape[2], image_features.dtype)

@@ -17,7 +17,7 @@ RNG: random.randint coin flips (drop variants) and torch.randperm / random.randi
 """
 from __future__ import annotations
 
-from typing import List, Sequence
+from typing import List, Optional, Sequence
 
 import numpy as np
 
@@ -133,13 +133,17 @@ def merge_feature(img_feature: np.ndarray, video_max_frames: int, img_similarity
 
 
 # ---------------------------------------------------------------------------------------------------- kmeans_feature (:91-127)
-def cdist16(X: np.ndarray, C: np.ndarray) -> np.ndarray:
+def cdist16(X: np.ndarray, C: np.ndarray, stats: Optional[list] = None) -> np.ndarray:
     """torch.cdist(X, C, p=2) on f16 with more than 25 rows on either side: ATen's matmul form (_euclidean_dist):
     [-2x, |x|^2, 1] . [c, 1, |c|^2] accumulated in fp32 as ONE dot product, rounded to f16, clamp_min(0), sqrt.
-    |v|^2 = f16(sum_f32(f16(v_i^2))) (v.pow(2).sum(-1) on f16)."""
+    |v|^2 = f16(sum_f32(f16(v_i^2))) (v.pow(2).sum(-1) on f16): +inf once the row's mean square passes 65504 / PD or
+    one |v_i| >= 256, and then every distance of that row is inf (or NaN, which clamp_min keeps).
+    stats: a list that gets the fraction of rows of X whose |x|^2 is inf."""
     Xf, Cf = X.astype(F32), C.astype(F32)
     xn = _h(_sum(_h(Xf * Xf)))
     cn = _h(_sum(_h(Cf * Cf)))
+    if stats is not None:
+        stats.append(float(np.isinf(xn).mean()))
     out = np.empty((X.shape[0], C.shape[0]), F32)
     for t in range(X.shape[0]):
         part = _seq_sum(_slice_sum((F32(-2.0) * Xf[t])[None, :] * Cf), -1)     # slices sequential
@@ -149,7 +153,9 @@ def cdist16(X: np.ndarray, C: np.ndarray) -> np.ndarray:
 
 
 def kmeans_feature(img_feature: np.ndarray, video_max_frames: int, img_similarity=None, *, init_idx: Sequence[int] = (),
-                   refill_idx: Sequence[int] = (), max_iter: int = 10, tol: float = 1e-4):
+                   refill_idx: Sequence[int] = (), max_iter: int = 10, tol: float = 1e-4, result: Optional[dict] = None):
+    """result: a dict that gets labels, exit_step, refills and converged of the Lloyd loop, and per iteration whether some
+    |x|^2 was inf (xn_inf) and some distance NaN (dist_nan)"""
     T, P, D = img_feature.shape
     T0 = video_max_frames
     if T <= T0:
@@ -159,8 +165,11 @@ def kmeans_feature(img_feature: np.ndarray, video_max_frames: int, img_similarit
     tol_h = F32(F16(tol))
     pos = 0
     labels = np.zeros(T, np.int64)
-    for _ in range(max_iter):
-        labels = argmin_first_nan(cdist16(X, C), axis=1)
+    it, converged, xn_inf, dist_nan = 0, False, [], []
+    for it in range(max_iter):
+        dist = cdist16(X, C, stats=xn_inf)
+        dist_nan.append(bool(np.isnan(dist).any()))
+        labels = argmin_first_nan(dist, axis=1)
         new = np.empty_like(C)
         for j in range(T0):
             members = np.nonzero(labels == j)[0]
@@ -176,8 +185,11 @@ def kmeans_feature(img_feature: np.ndarray, video_max_frames: int, img_similarit
         nrm = _h(np.sqrt(_sum(d * d)))
         diff = _h(_seq_sum(nrm[None, :], -1)[0])
         if diff < tol_h:
+            converged = True
             break
         C = new
+    if result is not None:
+        result.update(labels=labels, exit_step=it, refills=pos, converged=converged, xn_inf=xn_inf, dist_nan=dist_nan)
     return C.reshape(T0, P, D), img_similarity, step_indices_from_labels(labels, T0)
 
 

@@ -310,9 +310,33 @@ class StarConfig:
         self.update_ratio, self.key_length = update_ratio, key_length
 
 
-def compress_temporal_features(feat: np.ndarray, cfg: StarConfig, ntm, *, init_idx=None, refill_idx=None, order=None):
+def _compress_long(long_: np.ndarray, cfg: StarConfig, compressor, init_idx, refill_idx, **kmeans_kw):
+    """compress_fn(long_memory, video_long_memory_length) (:258, :679): weighted_kmeans_feature by default, or
+    `compressor(long_, long_len) -> (long_c, weight, steps)`, e.g. an alternates_oracle function with its draws bound"""
+    if compressor is None:
+        return weighted_kmeans_feature(long_, cfg.long_len, init_idx=init_idx, refill_idx=refill_idx, **kmeans_kw)
+    return compressor(long_, cfg.long_len)
+
+
+def _weight_order(weight) -> np.ndarray:
+    """sorted_indices = torch.argsort(weight, descending=True) followed by long_memory[sorted_indices] and the distance
+    broadcast (:261-266, :681-686), raising where they raise for the weights the alternate compressors return: None
+    (kdrop and kmeans always, every compressor's T <= T0 pass-through) -> TypeError from torch.argsort; k_merge's
+    [T0, T0] similarity matrix -> long_memory[sorted_indices] is [T0, T0, P, D] and (long[:, None] - key[None]) does not
+    broadcast for T > T0 >= 2 -> RuntimeError"""
+    if weight is None:
+        raise TypeError("argsort(): got (NoneType, descending=bool) as the weight to sort")
+    w = np.asarray(weight)
+    if w.ndim != 1:
+        raise RuntimeError(f"a weight of shape {w.shape} gives key centroids that do not broadcast against the long memory")
+    return argsort_desc_stable(w)
+
+
+def compress_temporal_features(feat: np.ndarray, cfg: StarConfig, ntm, *, init_idx=None, refill_idx=None, order=None,
+                               compressor=None):
     """feat [T, cur_size^2, D] f16 (already pooled to compress_size) -> (memory [<=681, D], debug dict).
-    `order` optionally overrides the descending weight argsort (to replay the reference's unstable tie order)."""
+    `order` optionally overrides the descending weight argsort (to replay the reference's unstable tie order).
+    `compressor` replaces weighted_kmeans_feature (see _compress_long); its weight feeds the key retrieval."""
     T = feat.shape[0]
     cur_start = min(cfg.cur_len, T)                                                       # :240
     if cur_start == 0:
@@ -327,9 +351,9 @@ def compress_temporal_features(feat: np.ndarray, cfg: StarConfig, ntm, *, init_i
     if cfg.long_len == 0 or long_.shape[0] == 0:
         long_c = long_[:0]                                                                # :256-257
     else:
-        long_c, weight, _ = weighted_kmeans_feature(long_, cfg.long_len, init_idx=init_idx, refill_idx=refill_idx)
+        long_c, weight, _ = _compress_long(long_, cfg, compressor, init_idx, refill_idx)  # :258
         if order is None:
-            order = argsort_desc_stable(weight)                                           # :261
+            order = _weight_order(weight)                                                 # :261
         idx = key_retrieve(long_, order, cfg.key_length)                                  # :262-267
         cur = np.concatenate([feat[idx], cur], axis=0)                                    # :268-269
         dbg.update(weight=np.asarray(weight), order=np.asarray(order), key_idx=idx)
@@ -359,9 +383,11 @@ class StreamState:
 
 
 def stream_step(state: StreamState, feat_a: np.ndarray, cfg: StarConfig, ntm, *, init_idx=None, refill_idx=None,
-                order=None, trace: Optional[list] = None):
+                order=None, trace: Optional[list] = None, compressor=None):
     """One embed_video_streaming call after the encoder: feat_a [t, cur_size^2, D] f16 is the clip's pooled ViT
     output (already `.to(float16)`, :649).  Mutates and returns `state`; returns a debug dict too.
+    `compressor` replaces weighted_kmeans_feature as in compress_temporal_features; where the key retrieval raises on its
+    weight, `state` is left as it was (the reference publishes at the end of the call, :693-695).
 
     long_len == 0 switches the long memory and the key retrieval off from the first call on, behind the guard of the
     offline path (compress_temporal_features, :256-257); the reference's streaming branch has no such guard (its first
@@ -390,10 +416,10 @@ def stream_step(state: StreamState, feat_a: np.ndarray, cfg: StarConfig, ntm, *,
     if cfg.long_len == 0:
         long_c, idx = L, np.zeros(0, np.int64)
     else:
-        long_c, weight, _ = weighted_kmeans_feature(L, cfg.long_len, init_idx=init_idx, refill_idx=refill_idx,
-                                                    trace=iters, result=res)              # :679
+        kw = dict(trace=iters, result=res) if compressor is None else {}
+        long_c, weight, _ = _compress_long(L, cfg, compressor, init_idx, refill_idx, **kw)  # :679
         if order is None:
-            order = argsort_desc_stable(weight)                                           # :681
+            order = _weight_order(weight)                                                 # :681
         idx = key_retrieve(L, order, cfg.key_length)                                      # :682-687
         dbg.update(weight=np.asarray(weight), order=np.asarray(order))
     key = buf[idx]                                    # global buffer indexed by working-set indices (:688, quirk)
