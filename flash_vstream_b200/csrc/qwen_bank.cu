@@ -12,10 +12,10 @@
 namespace fvs {
 namespace qwen {
 
-// gridDim.y = picks; every block copies a strided share of the pick's 16-byte words: x words first, then merged words.
+// Every block copies a strided share of one pick's 16-byte words: x words first, then merged words.
 // Sources, in order: the device tier, the same frame in the previous step's DAM (prev_x / prev_m), the host chunk.
 // A pick outside [0, n_frames) writes zeros (the host validates nothing on the device's behalf).
-// (bx, nbx, i): the block's share of pick i and the number of blocks per pick (blockIdx.x, gridDim.x, blockIdx.y)
+// (bx, nbx, i): the block's share of pick i and the number of blocks per pick
 __device__ __forceinline__ void dam_gather_body(
     unsigned bx, unsigned nbx, unsigned i_, const long long* __restrict__ picks, long long n_frames, const uint4* dev_x,
     const uint4* dev_m, long long n_dev, const uint4* const* __restrict__ chunks, long long chunk_frames,
@@ -71,15 +71,6 @@ __device__ __forceinline__ void dam_gather_body(
     }
   }
 }
-__global__ void __launch_bounds__(256) dam_gather_kernel(
-    const long long* __restrict__ picks, long long n_frames, const uint4* dev_x, const uint4* dev_m, long long n_dev,
-    const uint4* const* __restrict__ chunks, long long chunk_frames, const long long* __restrict__ prev_picks, int m,
-    const uint4* prev_x, const uint4* prev_m, long long fx, long long fm, uint4* out_x, uint4* out_m,
-    unsigned long long* host_fetches) {
-  dam_gather_body(blockIdx.x, gridDim.x, blockIdx.y, picks, n_frames, dev_x, dev_m, n_dev, chunks, chunk_frames, prev_picks,
-                  m, prev_x, prev_m, fx, fm, out_x, out_m, host_fetches);
-}
-
 }  // namespace qwen
 }  // namespace fvs
 
@@ -104,23 +95,53 @@ struct GatherJobDev {
   long long n_frames, n_dev, chunk_frames, fx, fm;
   int m, bx;
 };
+template <int kJobs>
 struct GatherLaunch {
-  GatherJobDev job[kGatherJobs];
-  int first[kGatherJobs + 1];
+  GatherJobDev job[kJobs];
+  int first[kJobs + 1];
   int n;
 };
-// one flat grid over the jobs: job j's block b is block (b % bx, b / bx) of its single-call grid (bx, n)
-__global__ void __launch_bounds__(256) dam_gather_multi_kernel(const __grid_constant__ GatherLaunch L) {
+// one flat grid over the jobs (a single call is the one-job grid): job j's block b copies share b % bx of pick b / bx
+template <int kJobs>
+__global__ void __launch_bounds__(256) dam_gather_multi_kernel(const __grid_constant__ GatherLaunch<kJobs> L) {
   int j = 0;
-  while (j + 1 < L.n && blockIdx.x >= unsigned(L.first[j + 1])) ++j;
+  if constexpr (kJobs > 1)
+    while (j + 1 < L.n && blockIdx.x >= unsigned(L.first[j + 1])) ++j;
   const GatherJobDev& J = L.job[j];
   const unsigned b = blockIdx.x - unsigned(L.first[j]), bx = J.bx;
   dam_gather_body(b % bx, bx, b / bx, J.picks, J.n_frames, J.dev_x, J.dev_m, J.n_dev, J.chunks, J.chunk_frames, J.prev_picks,
                   J.m, J.prev_x, J.prev_m, J.fx, J.fm, J.out_x, J.out_m, J.host_fetches);
 }
 
-// the checks of fvs_qwen_dam_gather for every job, then (multi) no output shared by two jobs, then the launches: the
-// single call launches its own grid (bx, n); the multi call one flat grid per kGatherJobs jobs
+GatherJobDev gather_job_dev(const fvs_qwen_gather_job& j) {
+  const long long fx = j.x_frame_elems * 2 / 16, fm = j.merged_frame_elems * 2 / 16;
+  const long long words = (j.spa_x_out ? fx : 0) + (j.merged_out ? fm : 0);
+  long long bx = (words + 4 * 256 - 1) / (4 * 256);
+  if (bx > 64) bx = 64;
+  if (bx < 1) bx = 1;
+  return GatherJobDev{(const long long*)j.picks, (const uint4*)j.dev_x, (const uint4*)j.dev_merged,
+                      (const uint4* const*)j.host_chunks, (const long long*)j.prev_picks, (const uint4*)j.prev_x,
+                      (const uint4*)j.prev_merged, (uint4*)j.spa_x_out, (uint4*)j.merged_out,
+                      (unsigned long long*)j.host_fetches, (long long)j.n_frames, (long long)j.n_dev,
+                      (long long)j.chunk_frames, fx, fm, j.m, int(bx)};
+}
+
+template <int kJobs>
+int dam_gather_launch(const fvs_qwen_gather_job* jobs, int n, cudaStream_t stream) {
+  GatherLaunch<kJobs> L;
+  L.n = n;
+  L.first[0] = 0;
+  for (int q = 0; q < n; ++q) {
+    L.job[q] = gather_job_dev(jobs[q]);
+    L.first[q + 1] = L.first[q] + L.job[q].bx * jobs[q].n;
+  }
+  dam_gather_multi_kernel<kJobs><<<L.first[n], 256, 0, stream>>>(L);
+  FVS_CHECK_LAUNCH("dam_gather_multi_kernel");
+  return FVS_OK;
+}
+
+// the checks of fvs_qwen_dam_gather for every job, then (multi) no output shared by two jobs, then one flat grid per
+// kGatherJobs jobs (a single call: the one-job grid)
 int dam_gather_jobs(const char* api, const fvs_qwen_gather_job* jobs, int n_jobs, int dtype, cudaStream_t stream, bool multi) {
   FVS_REQUIRE(jobs && n_jobs > 0, "%s: need a job table and n_jobs > 0", api);
   FVS_REQUIRE(dtype == FVS_F16 || dtype == FVS_BF16, "%s: dtype must be f16 or bf16", api);
@@ -159,36 +180,10 @@ int dam_gather_jobs(const char* api, const fvs_qwen_gather_job* jobs, int n_jobs
     for (size_t b = a + 1; b < out.size(); ++b)
       FVS_REQUIRE(out[a].job == out[b].job || out[a].hi <= out[b].lo || out[b].hi <= out[a].lo,
                   "%s: jobs %d and %d share an output", api, out[a].job, out[b].job);
-  auto dev_job = [](const fvs_qwen_gather_job& j) {
-    const long long fx = j.x_frame_elems * 2 / 16, fm = j.merged_frame_elems * 2 / 16;
-    const long long words = (j.spa_x_out ? fx : 0) + (j.merged_out ? fm : 0);
-    long long bx = (words + 4 * 256 - 1) / (4 * 256);
-    if (bx > 64) bx = 64;
-    if (bx < 1) bx = 1;
-    return GatherJobDev{(const long long*)j.picks, (const uint4*)j.dev_x, (const uint4*)j.dev_merged,
-                        (const uint4* const*)j.host_chunks, (const long long*)j.prev_picks, (const uint4*)j.prev_x,
-                        (const uint4*)j.prev_merged, (uint4*)j.spa_x_out, (uint4*)j.merged_out,
-                        (unsigned long long*)j.host_fetches, (long long)j.n_frames, (long long)j.n_dev,
-                        (long long)j.chunk_frames, fx, fm, j.m, int(bx)};
-  };
-  if (!multi) {
-    const GatherJobDev J = dev_job(jobs[0]);
-    dam_gather_kernel<<<dim3(unsigned(J.bx), unsigned(jobs[0].n)), 256, 0, stream>>>(
-        J.picks, J.n_frames, J.dev_x, J.dev_m, J.n_dev, J.chunks, J.chunk_frames, J.prev_picks, J.m, J.prev_x, J.prev_m, J.fx,
-        J.fm, J.out_x, J.out_m, J.host_fetches);
-    FVS_CHECK_LAUNCH("dam_gather_kernel");
-    return FVS_OK;
-  }
   for (int i0 = 0; i0 < n_jobs; i0 += kGatherJobs) {
-    GatherLaunch L;
-    L.n = std::min(kGatherJobs, n_jobs - i0);
-    L.first[0] = 0;
-    for (int q = 0; q < L.n; ++q) {
-      L.job[q] = dev_job(jobs[i0 + q]);
-      L.first[q + 1] = L.first[q] + L.job[q].bx * jobs[i0 + q].n;
-    }
-    dam_gather_multi_kernel<<<L.first[L.n], 256, 0, stream>>>(L);
-    FVS_CHECK_LAUNCH("dam_gather_multi_kernel");
+    const int n = std::min(kGatherJobs, n_jobs - i0);
+    const int r = n == 1 ? dam_gather_launch<1>(jobs + i0, 1, stream) : dam_gather_launch<kGatherJobs>(jobs + i0, n, stream);
+    if (r) return r;
   }
   return FVS_OK;
 }

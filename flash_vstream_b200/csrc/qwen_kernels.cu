@@ -125,10 +125,6 @@ __device__ __forceinline__ void lex_compare_body(int i, int j, const void* __res
     cmp[j * T + i] = (signed char)(-result);
   }
 }
-__global__ void __launch_bounds__(256) lex_compare_kernel(const void* __restrict__ X, int T, int PD, int dt,
-                                                          signed char* __restrict__ cmp) {
-  lex_compare_body(blockIdx.x, blockIdx.y, X, T, PD, dt, cmp);
-}
 // single block: rows that are the first of their duplicate class, in ascending lexicographic order
 __device__ __forceinline__ void unique_order_body(const signed char* __restrict__ cmp, int T, int* __restrict__ uniq_idx,
                                                   int* __restrict__ n_unique, int* is_first) {
@@ -151,11 +147,6 @@ __device__ __forceinline__ void unique_order_body(const signed char* __restrict_
     for (int i = 0; i < T; ++i) n += is_first[i];
     *n_unique = n;
   }
-}
-__global__ void unique_order_kernel(const signed char* __restrict__ cmp, int T, int* __restrict__ uniq_idx,
-                                    int* __restrict__ n_unique) {
-  extern __shared__ int is_first[];
-  unique_order_body(cmp, T, uniq_idx, n_unique, is_first);
 }
 
 // ------------------------------------------------------------------------------------------------ fp32 k-means
@@ -193,10 +184,6 @@ __device__ __forceinline__ void seq_reduce_body(unsigned bid, const float* __res
     for (int i = 0; i < n; ++i) acc = __fadd_rn(acc, __shfl_sync(0xffffffffu, v, i));
   }
   if (lane == 0) tot[u] = acc;
-}
-__global__ void __launch_bounds__(256) seq_reduce_kernel(const float* __restrict__ part, float* __restrict__ tot, int units,
-                                                         int S, const int* __restrict__ done) {
-  seq_reduce_body(blockIdx.x, part, tot, units, S, done);
 }
 
 // one 1024-element slice of a row -> 32 fp32 registers in the canonical ownership (lane l: elements i*256 + l*8 + e),
@@ -253,9 +240,6 @@ __device__ __forceinline__ void ko_xnorm_body(unsigned bid, KO B, const void* __
   acc = butterfly_sum(acc);
   if (lane == 0) B.a2[unit] = acc;
 }
-__global__ void __launch_bounds__(256) ko_xnorm_kernel(KO B, const void* __restrict__ X, int dt, int T, int PD) {
-  ko_xnorm_body(blockIdx.x, B, X, dt, T, PD);
-}
 
 // initial centroids = unique_X[indices] widened to fp32, and their |c|^2 slice partials: warp per (k, slice)
 __device__ __forceinline__ void ko_init_body(unsigned bid, KO B, const void* __restrict__ X, int dt, const int* __restrict__ uniq_idx,
@@ -282,10 +266,6 @@ __device__ __forceinline__ void ko_init_body(unsigned bid, KO B, const void* __r
   for (int q = 0; q < 32; ++q) acc = __fadd_rn(acc, __fmul_rn(x[q], x[q]));
   acc = butterfly_sum(acc);
   if (lane == 0) B.b2[unit] = acc;
-}
-__global__ void __launch_bounds__(256) ko_init_kernel(KO B, const void* __restrict__ X, int dt, const int* __restrict__ uniq_idx,
-                                                      const int* __restrict__ init_idx, int T, int K, int PD) {
-  ko_init_body(blockIdx.x, B, X, dt, uniq_idx, init_idx, T, K, PD);
 }
 
 // canonical slice partial of sum(a*b): lane l owns elements i*256 + l*8 + e, products rounded, sequential adds, butterfly.
@@ -356,10 +336,6 @@ __device__ __forceinline__ void ko_partial_body(unsigned bid, float4* cs, KO B, 
     __syncthreads();
   }
 }
-__global__ void __launch_bounds__(256) ko_partial_kernel(KO B, const void* __restrict__ X, int dt, int T, int K, int PD) {
-  extern __shared__ __align__(16) uint8_t ko_smem[];
-  ko_partial_body(blockIdx.x, reinterpret_cast<float4*>(ko_smem), B, X, dt, T, K, PD);
-}
 // dists = sqrt((A_2 + B_2^T) - 2*AB); labels = argmin (first index, NaN wins); warp per row.  A row whose label moved marks
 // both clusters dirty: only dirty clusters are recomputed by ko_update.
 __device__ __forceinline__ void ko_assign_body(unsigned bid, KO B, int T, int K, int PD) {
@@ -384,9 +360,6 @@ __device__ __forceinline__ void ko_assign_body(unsigned bid, KO B, int T, int K,
       B.labels[t] = besti;
     }
   }
-}
-__global__ void __launch_bounds__(256) ko_assign_kernel(KO B, int T, int K, int PD) {
-  ko_assign_body(blockIdx.x, B, T, K, PD);
 }
 // warp per (cluster j, slice): weighted mean (sequential in t), refill of empty clusters, ||c_old - c_new||^2 partial.
 // A cluster whose member set did not change since the previous iteration (and that was not empty, i.e. not refilled from
@@ -454,10 +427,6 @@ __device__ __forceinline__ void ko_update_body(unsigned bid, KO B, const void* _
     if (s == 0) B.wsum[j] = wsum_j;
   }
 }
-__global__ void __launch_bounds__(256) ko_update_kernel(KO B, const void* __restrict__ X, int dt, const float* __restrict__ w,
-                                                        const int* __restrict__ refill_idx, int T, int K, int PD, int iter) {
-  ko_update_body(blockIdx.x, B, X, dt, w, refill_idx, T, K, PD, iter);
-}
 // one block: per-cluster norms (slices added in order: warp per cluster, coalesced loads + shuffle chain), then thread 0
 // forms diff = sum_k ||c_k - c'_k||, takes the break decision and builds the change list of the next iteration
 __device__ __forceinline__ void ko_converge_body(KO B, int K, int PD, int iter, int max_iter, float tol) {
@@ -497,9 +466,6 @@ __device__ __forceinline__ void ko_converge_body(KO B, int K, int PD, int iter, 
     if (iter == max_iter - 1) B.state[0] = 1;
   }
 }
-__global__ void __launch_bounds__(1024) ko_converge_kernel(KO B, int K, int PD, int iter, int max_iter, float tol) {
-  ko_converge_body(B, K, PD, iter, max_iter, tol);
-}
 // centroids = new_centroids for the rows that changed, plus their |c|^2 slice partials: warp per (list entry, slice)
 __device__ __forceinline__ void ko_commit_body(unsigned bid, KO B, int K, int PD, int iter, int max_iter) {
   if (B.state[1] != iter + 1) return;          // loop already over, or this iteration stopped on the tolerance
@@ -519,9 +485,6 @@ __device__ __forceinline__ void ko_commit_body(unsigned bid, KO B, int K, int PD
     if (lane == 0) B.b2[size_t(k) * S + s] = acc;
   }
 }
-__global__ void __launch_bounds__(256) ko_commit_kernel(KO B, int K, int PD, int iter, int max_iter) {
-  ko_commit_body(blockIdx.x, B, K, PD, iter, max_iter);
-}
 // a plain copy: the result does not depend on how many blocks (nblk) share it
 __device__ __forceinline__ void ko_finish_body(unsigned bid, unsigned nblk, KO B, float* __restrict__ C_out, float* __restrict__ wsum_out,
                                                int* __restrict__ labels_out, int* __restrict__ info_out, int T, int K, int PD) {
@@ -536,11 +499,6 @@ __device__ __forceinline__ void ko_finish_body(unsigned bid, unsigned nblk, KO B
       info_out[0] = B.state[2]; info_out[1] = B.state[3]; info_out[2] = B.state[4]; info_out[3] = 0;
     }
   }
-}
-__global__ void __launch_bounds__(256) ko_finish_kernel(KO B, float* __restrict__ C_out, float* __restrict__ wsum_out,
-                                                        int* __restrict__ labels_out, int* __restrict__ info_out, int T, int K,
-                                                        int PD) {
-  ko_finish_body(blockIdx.x, gridDim.x, B, C_out, wsum_out, labels_out, info_out, T, K, PD);
 }
 
 // out[i, :] = cast(src_f32[idx[i], :]) ; idx int64; block bx of nbx covers a strided share of output row i, 4 elements per
@@ -563,10 +521,6 @@ __device__ __forceinline__ void gather_cast_body(unsigned bx, unsigned nbx, size
           make_uint2(*reinterpret_cast<const uint32_t*>(&a), *reinterpret_cast<const uint32_t*>(&b));
     }
   }
-}
-__global__ void __launch_bounds__(256) gather_cast_kernel(const float* __restrict__ src, const long long* __restrict__ idx,
-                                                          void* __restrict__ out, size_t row, int out_dt) {
-  gather_cast_body(blockIdx.x, gridDim.x, blockIdx.y, src, idx, out, row, out_dt);
 }
 
 // ------------------------------------------------------------------------------------------------ k-means bookkeeping
@@ -617,12 +571,6 @@ __device__ __forceinline__ void ko_finalize_body(const int* __restrict__ labels,
   }
   if (threadIdx.x == 0) flags[0] = s_empty;
 }
-__global__ void __launch_bounds__(256) ko_finalize_kernel(const int* __restrict__ labels, const float* __restrict__ wsum, int T,
-                                                          int K, const long long* __restrict__ order_in,
-                                                          long long* __restrict__ sorted_idx, float* __restrict__ ts_sorted,
-                                                          float* __restrict__ w_sorted, int* __restrict__ flags) {
-  ko_finalize_body(labels, wsum, T, K, order_in, sorted_idx, ts_sorted, w_sorted, flags);
-}
 
 // ------------------------------------------------------------------------------------------------ spatial_enhance
 // klarge_retrieve (vstream_qwen2vl_model.py:197-207, 231-238): for the k heaviest centroids c (rows klarge_idx of tem_x) and
@@ -631,7 +579,7 @@ __global__ void __launch_bounds__(256) ko_finalize_kernel(const int* __restrict_
 // Both sums run in the canonical slice order, so the oracle reproduces every bit.  The contraction is HBM-bound (k <= 64
 // rows against t bank rows of P*D elements: ~0.5 flop/byte), so it runs as a split-K sweep on the CUDA cores: one block per
 // 1024-element slice keeps the centroid slice in shared memory, streams the bank slice once and emits fp32 slice partials;
-// seq_reduce_kernel adds the slices in order; the tail kernel rounds, forms the distances and takes the argmin.
+// seq_reduce adds the slices in order; the tail rounds, forms the distances and takes the argmin.
 template <bool kBF16>
 __device__ __forceinline__ void unpack8(const uint4 v, float* f) {
   const uint32_t w[4] = {v.x, v.y, v.z, v.w};
@@ -657,7 +605,7 @@ __device__ __forceinline__ float round16(float v) {
 //   |v| = dt( sqrt( sum_f32(v_i^2) ) )   (Tensor.norm accumulates the exact products in fp32),   vn_i = dt(v_i / |v|),
 //   cos = dt( sum_f32( cn_i bn_i ) ),   all sums in the canonical slice order.
 // Same sweep in two passes: kMode 1 emits the slice partials of the squared norms (unrounded products), the norms are
-// finalised by klcos_norm_kernel, kMode 2 normalises both operands on the fly (centroids when they are staged in shared
+// finalised by klcos_norm, kMode 2 normalises both operands on the fly (centroids when they are staged in shared
 // memory, bank rows after the unpack) and emits the dot-product partials.  kMode 0 is the Euclidean form.
 //
 // partial layout [units, S]: unit t*k + kk = c_kk . b_t, unit t_total*k + t = |b_t|^2, unit t_total*k + t_total + kk = |c_kk|^2
@@ -675,7 +623,7 @@ __device__ __forceinline__ uint32_t pack2_16(float a, float b) {
 // partials at the rows' global indices; the launch whose range starts at row 0 writes the |c|^2 partials.  A row's
 // partials do not depend on the block or launch that computes them, so any split of the rows gives the same bits.
 // Without kRange the launch sweeps the whole bank (t_first 0, rows t_total) and ignores the last two arguments.
-// (s, by, ny): the slice, the row split and the number of row splits of the block (blockIdx.x, blockIdx.y, gridDim.y)
+// (s, by, ny): the slice, the row split and the number of row splits of the block
 template <bool kBF16, int kMode, bool kRange>
 __device__ __forceinline__ void klarge_partial_body(unsigned s_, unsigned by, unsigned ny, uint4* cs,
                                                     const uint16_t* __restrict__ tem_x, const long long* __restrict__ klarge_idx,
@@ -784,14 +732,16 @@ __device__ __forceinline__ void klarge_partial_body(unsigned s_, unsigned by, un
     }
   }
 }
-template <bool kBF16, int kMode, bool kRange>
+// one tier of a bank with host rows: bank rows [range_first, range_first + range_rows) (a bank wholly in HBM is swept by
+// klarge_multi_kernel)
+template <bool kBF16, int kMode>
 __global__ void __launch_bounds__(256) klarge_partial_kernel(const uint16_t* __restrict__ tem_x, const long long* __restrict__ klarge_idx,
                                                              const uint16_t* __restrict__ bank, float* __restrict__ part, int k,
                                                              int t_total, int PD, const float* __restrict__ norms,
                                                              int range_first, int range_rows) {
   extern __shared__ __align__(16) uint8_t smem_raw[];
-  klarge_partial_body<kBF16, kMode, kRange>(blockIdx.x, blockIdx.y, gridDim.y, reinterpret_cast<uint4*>(smem_raw), tem_x,
-                                            klarge_idx, bank, part, k, t_total, PD, norms, range_first, range_rows);
+  klarge_partial_body<kBF16, kMode, true>(blockIdx.x, blockIdx.y, gridDim.y, reinterpret_cast<uint4*>(smem_raw), tem_x,
+                                          klarge_idx, bank, part, k, t_total, PD, norms, range_first, range_rows);
 }
 // warp per centroid: distances over the bank (lane-strided) and argmin (NaN from a negative radicand wins, as in torch)
 template <bool kBF16>
@@ -814,21 +764,12 @@ __device__ __forceinline__ void klarge_tail_body(unsigned kk_, const float* __re
   warp_argmin(best, besti);
   if (lane == 0) idx[kk] = besti;
 }
-template <bool kBF16>
-__global__ void klarge_tail_kernel(const float* __restrict__ tot, int k, int t_total, long long* __restrict__ idx,
-                                   float* __restrict__ dist_out) {
-  klarge_tail_body<kBF16>(blockIdx.x, tot, k, t_total, idx, dist_out);
-}
 
 // norms[i] = dt(sqrt(sumsq[i])) for the t bank rows followed by the k centroids (in place over the reduced totals)
 template <bool kBF16>
 __device__ __forceinline__ void klcos_norm_body(unsigned bid, float* __restrict__ v, int n) {
   const int i = bid * blockDim.x + threadIdx.x;
   if (i < n) v[i] = round16<kBF16>(sqrtf(v[i]));
-}
-template <bool kBF16>
-__global__ void klcos_norm_kernel(float* __restrict__ v, int n) {
-  klcos_norm_body<kBF16>(blockIdx.x, v, n);
 }
 // warp per centroid: similarities over the bank and their argmin (a zero row gives 0/0 = NaN, which wins as in torch)
 template <bool kBF16>
@@ -844,11 +785,6 @@ __device__ __forceinline__ void klarge_cos_tail_body(unsigned kk_, const float* 
   }
   warp_argmin(best, besti);
   if (lane == 0) idx[kk] = besti;
-}
-template <bool kBF16>
-__global__ void klarge_cos_tail_kernel(const float* __restrict__ ab, int k, int t_total, long long* __restrict__ idx,
-                                       float* __restrict__ sim_out) {
-  klarge_cos_tail_body<kBF16>(blockIdx.x, ab, k, t_total, idx, sim_out);
 }
 
 // ------------------------------------------------------------------------------------------------ AM-RoPE
@@ -899,121 +835,13 @@ __host__ __device__ inline KO ko_carve(void* workspace, int T, int K, int PD) {
   return B;
 }
 
-}  // namespace qwen
-}  // namespace fvs
-
-using namespace fvs;
-using namespace fvs::qwen;
-
-namespace {
-// the bank of a klarge retrieval, in two tiers: rows [0, n_dev) are contiguous at dev (HBM), row n_dev + c*chunk_frames + r
-// is row r of host chunk c (chunks: a host array of the chunks' mapped device pointers)
-struct KlargeBank {
-  const void* dev;
-  int n_dev;
-  const void* const* chunks;
-  int chunk_frames, t_total;
-};
-
-template <bool kBF16, int kMode, bool kRange>
-int klarge_partial_launch(const void* tem_x, const int64_t* klarge_idx, const void* bank, float* part, int k, int t_total,
-                          int PD, const float* norms, int t_first, int rows, cudaStream_t stream) {
-  using namespace fvs::qwen;
-  static bool attr = false;   // per instantiation
-  auto kern = klarge_partial_kernel<kBF16, kMode, kRange>;
-  if (!attr) { FVS_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * SLICE * 2)); attr = true; }
-  const int nsplit = (rows + 31) / 32;      // <= 32 bank rows per block: enough blocks to fill every SM from t ~ 32 up
-  kern<<<dim3(PD / SLICE, nsplit), 256, size_t(k) * SLICE * 2, stream>>>((const uint16_t*)tem_x, (const long long*)klarge_idx,
-                                                                       (const uint16_t*)bank, part, k, t_total, PD, norms,
-                                                                       t_first, rows);
-  FVS_CHECK_LAUNCH("klarge_partial_kernel");
-  return FVS_OK;
-}
-// one sweep of the bank: a bank wholly in HBM is one launch over every row; otherwise one launch over the device rows and
-// one per host chunk, each reading its rows through the chunk's mapped pointer (PCIe)
-template <bool kBF16, int kMode>
-int klarge_sweep(const void* tem_x, const int64_t* klarge_idx, const KlargeBank& b, float* part, int k, int PD,
-                 const float* norms, cudaStream_t stream) {
-  if (b.n_dev == b.t_total)
-    return klarge_partial_launch<kBF16, kMode, false>(tem_x, klarge_idx, b.dev, part, k, b.t_total, PD, norms, 0, b.t_total,
-                                                      stream);
-  int r;
-  if (b.n_dev > 0 &&
-      (r = klarge_partial_launch<kBF16, kMode, true>(tem_x, klarge_idx, b.dev, part, k, b.t_total, PD, norms, 0, b.n_dev, stream)))
-    return r;
-  for (int c = 0, t = b.n_dev; t < b.t_total; ++c, t += b.chunk_frames)
-    if ((r = klarge_partial_launch<kBF16, kMode, true>(tem_x, klarge_idx, b.chunks[c], part, k, b.t_total, PD, norms, t,
-                                                       std::min(b.chunk_frames, b.t_total - t), stream)))
-      return r;
-  return FVS_OK;
-}
-template <int kMode>
-int klarge_partial(bool bf, const void* tem_x, const int64_t* klarge_idx, const KlargeBank& b, float* part, int k, int PD,
-                   const float* norms, cudaStream_t stream) {
-  return bf ? klarge_sweep<true, kMode>(tem_x, klarge_idx, b, part, k, PD, norms, stream)
-            : klarge_sweep<false, kMode>(tem_x, klarge_idx, b, part, k, PD, norms, stream);
-}
-
-// fvs_qwen_klarge_retrieve and its tiered form: the checks (reported as `who`), the sweeps, the reductions and the tail
-int klarge_retrieve(const char* who, const void* tem_x, const int64_t* klarge_idx, const KlargeBank& b, int k, int PD, int dtype,
-                    int metric, int64_t* idx_out, float* dist_out, void* workspace, size_t workspace_bytes,
-                    fvs_stream_t stream_) {
-  const int t_total = b.t_total;
-  FVS_REQUIRE(tem_x && klarge_idx && idx_out && workspace && (b.dev || b.n_dev == 0), "%s: null pointer", who);
-  FVS_REQUIRE(dtype == FVS_F16 || dtype == FVS_BF16, "%s: dtype must be f16 or bf16", who);
-  FVS_REQUIRE(metric == FVS_KLARGE_EUCLIDEAN || metric == FVS_KLARGE_COSINE, "%s: unknown metric %d", who, metric);
-  FVS_REQUIRE(k > 0 && k <= 64 && t_total > 0, "%s: need 0 < k <= 64, t > 0 (k=%d t=%d)", who, k, t_total);
-  FVS_REQUIRE(PD % SLICE == 0, "%s: PD (%d) must be a multiple of %d", who, PD, SLICE);
-  FVS_REQUIRE(b.n_dev >= 0 && b.n_dev <= t_total, "%s: need 0 <= n_dev <= t_total (n_dev=%d t=%d)", who, b.n_dev, t_total);
-  if (b.n_dev < t_total) {
-    FVS_REQUIRE(b.chunks && b.chunk_frames > 0, "%s: host rows need a chunk table and chunk_frames > 0", who);
-    for (int c = 0; c * int64_t(b.chunk_frames) < t_total - b.n_dev; ++c)
-      FVS_REQUIRE(b.chunks[c], "%s: null pointer of host chunk %d", who, c);
-  }
-  FVS_REQUIRE(workspace_bytes >= fvs_qwen_klarge_workspace_bytes(k, t_total, PD), "%s: workspace too small", who);
-  cudaStream_t stream = (cudaStream_t)stream_;
-  const int S = PD / SLICE;
-  const bool bf = dtype == FVS_BF16;
-  const size_t n_ab = size_t(t_total) * k, n_norm = size_t(t_total) + k, units = n_ab + n_norm;
-  float* part = (float*)workspace;
-  float* tot = (float*)((uint8_t*)workspace + al(units * S * 4));
-  int r;
-  if (metric == FVS_KLARGE_EUCLIDEAN) {
-    if ((r = klarge_partial<0>(bf, tem_x, klarge_idx, b, part, k, PD, nullptr, stream))) return r;
-    seq_reduce_kernel<<<int((units + 7) / 8), 256, 0, stream>>>(part, tot, int(units), S, nullptr);
-    FVS_CHECK_LAUNCH("seq_reduce_kernel");
-    if (bf) klarge_tail_kernel<true><<<k, 32, 0, stream>>>(tot, k, t_total, (long long*)idx_out, dist_out);
-    else klarge_tail_kernel<false><<<k, 32, 0, stream>>>(tot, k, t_total, (long long*)idx_out, dist_out);
-    FVS_CHECK_LAUNCH("klarge_tail_kernel");
-    return FVS_OK;
-  }
-  // cosine: squared norms -> norms -> normalised dot products -> argmin of the similarity (the bank is swept twice)
-  float* norms = tot + n_ab;
-  if ((r = klarge_partial<1>(bf, tem_x, klarge_idx, b, part, k, PD, nullptr, stream))) return r;
-  seq_reduce_kernel<<<int((n_norm + 7) / 8), 256, 0, stream>>>(part + n_ab * S, norms, int(n_norm), S, nullptr);
-  FVS_CHECK_LAUNCH("seq_reduce_kernel");
-  if (bf) klcos_norm_kernel<true><<<int((n_norm + 255) / 256), 256, 0, stream>>>(norms, int(n_norm));
-  else klcos_norm_kernel<false><<<int((n_norm + 255) / 256), 256, 0, stream>>>(norms, int(n_norm));
-  FVS_CHECK_LAUNCH("klcos_norm_kernel");
-  if ((r = klarge_partial<2>(bf, tem_x, klarge_idx, b, part, k, PD, norms, stream))) return r;
-  seq_reduce_kernel<<<int((n_ab + 7) / 8), 256, 0, stream>>>(part, tot, int(n_ab), S, nullptr);
-  FVS_CHECK_LAUNCH("seq_reduce_kernel");
-  if (bf) klarge_cos_tail_kernel<true><<<k, 32, 0, stream>>>(tot, k, t_total, (long long*)idx_out, dist_out);
-  else klarge_cos_tail_kernel<false><<<k, 32, 0, stream>>>(tot, k, t_total, (long long*)idx_out, dist_out);
-  FVS_CHECK_LAUNCH("klarge_cos_tail_kernel");
-  return FVS_OK;
-}
-}  // namespace
-
-// ------------------------------------------------------------------------------------------------ many streams, one launch
-// The CSM chain of many streams (DESIGN.md §3.17): every kernel of the single-stream chain becomes one flat grid in which
-// job j owns blocks [first[j], first[j+1]) — exactly the blocks its single call launches, in the same order — and calls
-// the same per-block body with its local block index.  A job's reductions therefore run in the same order whatever the
-// other jobs are and however the jobs are grouped into launches.  The job table travels as a __grid_constant__ kernel
-// parameter (at most FVS_QWEN_MEM_JOBS_PER_LAUNCH jobs, under 3 KB).
-namespace fvs {
-namespace qwen {
-
+// ------------------------------------------------------------------------------------------------ job tables
+// Every kernel of the CSM chain and of the klarge retrieval is launched over a job table (DESIGN.md §3.17): job j owns
+// blocks [first[j], first[j+1]) of one flat grid and calls the per-block body with its local block index.  A job gets the
+// same blocks in the same order whatever the other jobs are, so its reductions run in the same order however the jobs are
+// grouped into launches.  A single call is the one-job table: kJobs = 1 has no job scan and a small parameter block; a
+// group of more jobs runs the kJobs = FVS_QWEN_MEM_JOBS_PER_LAUNCH instantiation.  The table travels as a
+// __grid_constant__ kernel parameter (under 4 KB).
 constexpr int kMemJobs = FVS_QWEN_MEM_JOBS_PER_LAUNCH;
 struct MemJobDev {
   const void* X;
@@ -1036,17 +864,19 @@ struct MemJobDev {
   void* out;
   int T, K, PD, dt, max_iter, out_dt;
   float tol;
+  long long row_elems;     // gather: elements per row of C and out (PD in a table)
 };
+template <int kJobs>
 struct MemLaunch {
-  MemJobDev job[kMemJobs];
-  int first[kMemJobs + 1];   // block offsets of the launched kernel
+  MemJobDev job[kJobs];
+  int first[kJobs + 1];    // block offsets of the launched kernel
   int n, it, finish_blocks;
 };
 enum MemStage { kLex, kOrder, kInit, kXnorm, kA2, kPartial, kReduce, kAssign, kUpdate, kConverge, kCommit, kFinish, kFinalize,
                 kGather };
 
-// blocks of job J in stage st (iteration it): the grid of the single-stream launch, flattened; 0 once the job's loop is over
-__host__ __device__ inline int gather_bx(int PD) { const int bx = (PD / 4 + 255) / 256; return bx > 64 ? 64 : bx; }
+// blocks of job J in stage st (iteration it); 0 once the job's loop is over
+__host__ __device__ inline int gather_bx(long long row) { const long long bx = (row / 4 + 255) / 256; return bx > 64 ? 64 : int(bx); }
 inline int mem_stage_blocks(const MemJobDev& J, int st, int it, int finish_blocks) {
   const int S = J.PD / SLICE, iters = J.max_iter == 0 ? 1 : J.max_iter;
   const bool loop = it < iters, upd = J.max_iter > 0 && it < J.max_iter;
@@ -1062,16 +892,22 @@ inline int mem_stage_blocks(const MemJobDev& J, int st, int it, int finish_block
     case kUpdate: case kCommit: return upd ? (J.K * S + 7) / 8 : 0;
     case kConverge: return upd ? 1 : 0;
     case kFinish: return finish_blocks;
-    case kGather: return gather_bx(J.PD) * J.K;
+    case kGather: return gather_bx(J.row_elems) * J.K;
   }
   return 0;
 }
 
-template <int kStage>
-__global__ void __launch_bounds__(kStage == kConverge ? 1024 : 256) mem_multi_kernel(const __grid_constant__ MemLaunch L) {
+// Blocks of 256 per SM that the heaviest one-job stages keep: without a bound a one-job kernel spends extra registers on
+// its job descriptor and loses blocks per SM.  The Lloyd update runs at most 80 registers (3 blocks); the klarge bank
+// sweeps are bounded by kl_min_blocks.  A minBlocks of 0 leaves an instantiation unbounded, as every many-job one is.
+constexpr int mem_min_blocks(int jobs, int stage) { return jobs == 1 && stage == kUpdate ? 3 : 0; }
+template <int kJobs, int kStage>
+__global__ void __launch_bounds__(kStage == kConverge ? 1024 : 256, mem_min_blocks(kJobs, kStage))
+    mem_multi_kernel(const __grid_constant__ MemLaunch<kJobs> L) {
   extern __shared__ __align__(16) uint8_t mm_smem[];
   int j = 0;
-  while (j + 1 < L.n && blockIdx.x >= unsigned(L.first[j + 1])) ++j;
+  if constexpr (kJobs > 1)
+    while (j + 1 < L.n && blockIdx.x >= unsigned(L.first[j + 1])) ++j;
   const MemJobDev& J = L.job[j];
   const unsigned b = blockIdx.x - unsigned(L.first[j]);
   if constexpr (kStage == kLex) {
@@ -1081,8 +917,8 @@ __global__ void __launch_bounds__(kStage == kConverge ? 1024 : 256) mem_multi_ke
   } else if constexpr (kStage == kFinalize) {
     ko_finalize_body(J.labels, J.wsum, J.T, J.K, J.order_in, J.sorted_idx, J.ts, J.w_sorted, J.flags);
   } else if constexpr (kStage == kGather) {
-    const unsigned bx = gather_bx(J.PD);
-    gather_cast_body(b % bx, bx, b / bx, J.C, J.sorted_idx, J.out, size_t(J.PD), J.out_dt);
+    const unsigned bx = gather_bx(J.row_elems);
+    gather_cast_body(b % bx, bx, b / bx, J.C, J.sorted_idx, J.out, size_t(J.row_elems), J.out_dt);
   } else {
     const KO B = ko_carve(J.km_ws, J.T, J.K, J.PD);
     const int S = J.PD / SLICE;
@@ -1099,7 +935,7 @@ __global__ void __launch_bounds__(kStage == kConverge ? 1024 : 256) mem_multi_ke
   }
 }
 
-// the klarge retrieval of many jobs: the single call's launches, each one flat grid over the jobs' blocks
+// the klarge retrieval: a sweep of the bank, the slice reductions and the tail, each one flat grid over the jobs
 struct KlJobDev {
   const uint16_t* tem_x;
   const long long* klarge_idx;
@@ -1110,12 +946,20 @@ struct KlJobDev {
   float* dist;
   int k, t_total, PD, nsplit;
 };
+template <int kJobs>
 struct KlLaunch {
-  KlJobDev job[kMemJobs];
-  int first[kMemJobs + 1];
+  KlJobDev job[kJobs];
+  int first[kJobs + 1];
   int n;
 };
 enum KlStage { kKlSweep0, kKlSweep1, kKlSweep2, kKlReduceAll, kKlReduceNorms, kKlNorms, kKlReduceAb, kKlTail, kKlCosTail };
+// launch bounds of the one-job Euclidean and cosine bank sweeps (see mem_min_blocks): bf16 Euclidean at most 64
+// registers (4 blocks of 256 per SM), the others at most 96 (2 blocks of up to 320 threads per SM; a 256-thread sweep
+// runs 2 blocks per SM either way, and a bound of 80 would spill)
+constexpr int kl_min_blocks(int jobs, bool bf16, int stage) {
+  return jobs > 1 || (stage != kKlSweep0 && stage != kKlSweep2) ? 0 : bf16 && stage == kKlSweep0 ? 4 : 2;
+}
+constexpr int kl_max_threads(int jobs, bool bf16, int stage) { return kl_min_blocks(jobs, bf16, stage) == 2 ? 320 : 256; }
 inline int kl_stage_blocks(const KlJobDev& J, int st) {
   const int S = J.PD / SLICE;
   const size_t n_ab = size_t(J.t_total) * J.k, n_norm = size_t(J.t_total) + J.k;
@@ -1129,11 +973,13 @@ inline int kl_stage_blocks(const KlJobDev& J, int st) {
   }
   return 0;
 }
-template <bool kBF16, int kStage>
-__global__ void __launch_bounds__(256) klarge_multi_kernel(const __grid_constant__ KlLaunch L) {
+template <int kJobs, bool kBF16, int kStage>
+__global__ void __launch_bounds__(kl_max_threads(kJobs, kBF16, kStage), kl_min_blocks(kJobs, kBF16, kStage))
+    klarge_multi_kernel(const __grid_constant__ KlLaunch<kJobs> L) {
   extern __shared__ __align__(16) uint8_t kl_smem[];
   int j = 0;
-  while (j + 1 < L.n && blockIdx.x >= unsigned(L.first[j + 1])) ++j;
+  if constexpr (kJobs > 1)
+    while (j + 1 < L.n && blockIdx.x >= unsigned(L.first[j + 1])) ++j;
   const KlJobDev& J = L.job[j];
   const unsigned b = blockIdx.x - unsigned(L.first[j]);
   const unsigned S = J.PD / SLICE;
@@ -1161,64 +1007,57 @@ __global__ void __launch_bounds__(256) klarge_multi_kernel(const __grid_constant
 }  // namespace qwen
 }  // namespace fvs
 
-namespace {
-using fvs::qwen::MemJobDev;
-using fvs::qwen::MemLaunch;
+using namespace fvs;
+using namespace fvs::qwen;
 
+namespace {
+// the output byte ranges of a job table: no byte may belong to two jobs
+struct JobOutputs {
+  struct Range { uintptr_t lo, hi; int job; };
+  std::vector<Range> r;
+  void add(const void* p, size_t bytes, int job) { r.push_back({uintptr_t(p), uintptr_t(p) + bytes, job}); }
+  int check(const char* api) const {
+    for (size_t a = 0; a < r.size(); ++a)
+      for (size_t b = a + 1; b < r.size(); ++b)
+        FVS_REQUIRE(r[a].job == r[b].job || r[a].hi <= r[b].lo || r[b].hi <= r[a].lo, "%s: jobs %d and %d share an output",
+                    api, r[a].job, r[b].job);
+    return FVS_OK;
+  }
+};
+
+// ---- the CSM chain
 enum MemCall { kCallUnique, kCallKmeans, kCallFinalize, kCallGather };
 
-int lloyd_blocks(const fvs_qwen_mem_job& j) { return ((j.T + 7) / 8) * (j.PD / SLICE); }
+bool known_dtype(int dt) { return dt == FVS_F16 || dt == FVS_BF16 || dt == FVS_F32; }
 
-// the checks of the single-stream entry point of `call`, per job, and no output byte shared by two jobs
-int check_mem_jobs(const char* api, const fvs_qwen_mem_job* jobs, int n, int budget, int call) {
-  FVS_REQUIRE(jobs && n > 0 && budget >= 0, "%s: need a job table, n_jobs > 0 and budget >= 0", api);
-  struct Range { uintptr_t lo, hi; int job; };
-  std::vector<Range> out;
-  auto add = [&](const void* p, size_t bytes, int i) { out.push_back({uintptr_t(p), uintptr_t(p) + bytes, i}); };
-  for (int i = 0; i < n; ++i) {
-    const fvs_qwen_mem_job& j = jobs[i];
-    FVS_REQUIRE(j.T > 0 && j.T <= 4096 && j.K > 0 && j.K <= j.T && j.K <= kMaxFinalizeK,
-                "%s: job %d: need 0 < T <= 4096, 0 < K <= min(T, %d) (T=%d K=%d)", api, i, kMaxFinalizeK, j.T, j.K);
-    FVS_REQUIRE(j.PD > 0 && j.PD % SLICE == 0, "%s: job %d: PD (%d) must be a positive multiple of %d", api, i, j.PD, SLICE);
-    if (call == kCallUnique || call == kCallKmeans)
-      FVS_REQUIRE(j.X && (j.x_dtype == FVS_F16 || j.x_dtype == FVS_BF16 || j.x_dtype == FVS_F32),
-                  "%s: job %d: null X or bad x dtype", api, i);
-    if (call == kCallUnique) {
-      FVS_REQUIRE(j.uniq_idx && j.n_unique && j.uniq_workspace, "%s: job %d: null pointer", api, i);
-      FVS_REQUIRE(j.uniq_workspace_bytes >= fvs_qwen_unique_workspace_bytes(j.T), "%s: job %d: workspace too small", api, i);
-      add(j.uniq_idx, size_t(j.T) * 4, i);
-      add(j.n_unique, 4, i);
-      add(j.uniq_workspace, fvs_qwen_unique_workspace_bytes(j.T), i);
-    } else if (call == kCallKmeans) {
-      FVS_REQUIRE(j.w && j.init_idx && j.refill_idx && j.C && j.wsum && j.labels && j.info && j.km_workspace,
-                  "%s: job %d: null pointer", api, i);
-      FVS_REQUIRE(j.max_iter >= 0 && j.max_iter <= 1000, "%s: job %d: bad max_iter", api, i);
-      const size_t ws = fvs_qwen_kmeans_workspace_bytes(j.T, j.K, j.PD);
-      FVS_REQUIRE(j.km_workspace_bytes >= ws, "%s: job %d: workspace too small", api, i);
-      add(j.C, size_t(j.K) * j.PD * 4, i);
-      add(j.wsum, size_t(j.K) * 4, i);
-      add(j.labels, size_t(j.T) * 4, i);
-      add(j.info, 16, i);
-      add(j.km_workspace, ws, i);
-    } else if (call == kCallFinalize) {
-      FVS_REQUIRE(j.labels && j.wsum && j.sorted_idx && j.ts && j.w_sorted && j.flags, "%s: job %d: null pointer", api, i);
-      add(j.sorted_idx, size_t(j.K) * 8, i);
-      add(j.ts, size_t(j.K) * 4, i);
-      add(j.w_sorted, size_t(j.K) * 4, i);
-      add(j.flags, 4, i);
-    } else {
-      FVS_REQUIRE(j.C && j.sorted_idx && j.out, "%s: job %d: null pointer", api, i);
-      FVS_REQUIRE(j.out_dtype == FVS_F16 || j.out_dtype == FVS_BF16 || j.out_dtype == FVS_F32, "%s: job %d: bad out dtype",
-                  api, i);
-      add(j.out, size_t(j.K) * j.PD * (j.out_dtype == FVS_F32 ? 4 : 2), i);
-    }
+// the checks of one call of the chain, reported as `who` ("fvs_qwen_kmeans", or "fvs_qwen_kmeans_multi: job 3");
+// ws_bytes: the call's workspace (unique rows, k-means)
+int check_mem_call(const char* who, const MemJobDev& J, size_t ws_bytes, int call) {
+  if (call == kCallUnique) {
+    FVS_REQUIRE(J.X && J.uniq_idx && J.n_unique && J.uniq_ws, "%s: null pointer", who);
+    FVS_REQUIRE(J.T > 0 && J.T <= 4096 && J.PD > 0, "%s: bad shape T=%d PD=%d", who, J.T, J.PD);
+    FVS_REQUIRE(ws_bytes >= fvs_qwen_unique_workspace_bytes(J.T), "%s: workspace too small", who);
+  } else if (call == kCallKmeans) {
+    FVS_REQUIRE(J.X && J.w && J.init_idx && J.refill_idx && J.C && J.wsum && J.labels && J.info && J.km_ws,
+                "%s: null pointer", who);
+    FVS_REQUIRE(known_dtype(J.dt), "%s: bad x dtype", who);
+    FVS_REQUIRE(J.T > 0 && J.K > 0 && J.K <= J.T, "%s: need 0 < K <= T (T=%d K=%d)", who, J.T, J.K);
+    FVS_REQUIRE(J.PD > 0 && J.PD % SLICE == 0, "%s: PD (%d) must be a positive multiple of %d", who, J.PD, SLICE);
+    FVS_REQUIRE(J.max_iter >= 0 && J.max_iter <= 1000, "%s: bad max_iter", who);
+    FVS_REQUIRE(ws_bytes >= fvs_qwen_kmeans_workspace_bytes(J.T, J.K, J.PD), "%s: workspace too small", who);
+  } else if (call == kCallFinalize) {
+    FVS_REQUIRE(J.labels && J.wsum && J.sorted_idx && J.ts && J.w_sorted && J.flags, "%s: null pointer", who);
+    FVS_REQUIRE(J.T > 0 && J.K > 0 && J.K <= kMaxFinalizeK, "%s: need T > 0, 0 < K <= %d (T=%d K=%d)", who, kMaxFinalizeK,
+                J.T, J.K);
+  } else {
+    FVS_REQUIRE(J.C && J.sorted_idx && J.out, "%s: null pointer", who);
+    FVS_REQUIRE(J.K > 0 && J.K <= 65535 && J.row_elems > 0, "%s: need 0 < n <= 65535 rows, row_elems > 0 (n=%d)", who, J.K);
+    FVS_REQUIRE(J.row_elems % 4 == 0, "%s: row_elems must be a multiple of 4", who);
   }
-  for (size_t a = 0; a < out.size(); ++a)
-    for (size_t b = a + 1; b < out.size(); ++b)
-      FVS_REQUIRE(out[a].job == out[b].job || out[a].hi <= out[b].lo || out[b].hi <= out[a].lo,
-                  "%s: jobs %d and %d share an output", api, out[a].job, out[b].job);
   return FVS_OK;
 }
+
+int lloyd_blocks(const fvs_qwen_mem_job& j) { return ((j.T + 7) / 8) * (j.PD / SLICE); }
 
 // jobs in order, at most kMemJobs per group and, with budget > 0, at most `budget` Lloyd-sweep blocks (a larger job alone)
 int mem_groups(const fvs_qwen_mem_job* jobs, int n, int budget, int32_t* blocks, int32_t* groups) {
@@ -1226,7 +1065,7 @@ int mem_groups(const fvs_qwen_mem_job* jobs, int n, int budget, int32_t* blocks,
   long long sum = 0;
   for (int i = 0; i < n; ++i) {
     const int b = lloyd_blocks(jobs[i]);
-    if (in_group && (in_group == fvs::qwen::kMemJobs || (budget > 0 && sum + b > budget))) {
+    if (in_group && (in_group == kMemJobs || (budget > 0 && sum + b > budget))) {
       ++g;
       in_group = 0;
       sum = 0;
@@ -1242,120 +1081,247 @@ int mem_groups(const fvs_qwen_mem_job* jobs, int n, int budget, int32_t* blocks,
 MemJobDev mem_job_dev(const fvs_qwen_mem_job& j) {
   return MemJobDev{j.X, j.w, j.init_idx, j.refill_idx, j.uniq_idx, j.n_unique, j.uniq_workspace, j.C, j.wsum, j.labels,
                    j.info, j.km_workspace, (const long long*)j.order_in, (long long*)j.sorted_idx, j.ts, j.w_sorted, j.flags,
-                   j.out, j.T, j.K, j.PD, j.x_dtype, j.max_iter, j.out_dtype, j.tol};
+                   j.out, j.T, j.K, j.PD, j.x_dtype, j.max_iter, j.out_dtype, j.tol, j.PD};
 }
 
 // one launch of stage kStage over the group in L (skipped when no job has blocks in it)
-template <int kStage>
-int mem_launch(MemLaunch& L, int threads, size_t smem, cudaStream_t stream, const char* name) {
-  using namespace fvs::qwen;
+template <int kJobs, int kStage>
+int mem_launch(MemLaunch<kJobs>& L, int threads, size_t smem, cudaStream_t stream, const char* name) {
   L.first[0] = 0;
   for (int j = 0; j < L.n; ++j) L.first[j + 1] = L.first[j] + mem_stage_blocks(L.job[j], kStage, L.it, L.finish_blocks);
   if (L.first[L.n] == 0) return FVS_OK;
-  mem_multi_kernel<kStage><<<L.first[L.n], threads, smem, stream>>>(L);
+  if constexpr (kStage == kPartial) {
+    static bool attr = false;   // per instantiation
+    if (!attr) {
+      FVS_CUDA_OK(cudaFuncSetAttribute(mem_multi_kernel<kJobs, kPartial>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       KO_PARTIAL_SMEM));
+      attr = true;
+    }
+  }
+  mem_multi_kernel<kJobs, kStage><<<L.first[L.n], threads, smem, stream>>>(L);
   FVS_CHECK_LAUNCH(name);
   return FVS_OK;
 }
 
-int run_mem_multi(const char* api, const fvs_qwen_mem_job* jobs, int n, int budget, fvs_stream_t stream_, int call) {
-  using namespace fvs::qwen;
-  int r = check_mem_jobs(api, jobs, n, budget, call);
+// the launch sequence of `call` for one group of n <= kJobs jobs
+template <int kJobs>
+int mem_group(const MemJobDev* jobs, int n, int call, cudaStream_t stream) {
+  MemLaunch<kJobs> L;
+  L.n = n;
+  L.it = 0;
+  L.finish_blocks = 1;
+  int max_T = 1, iters = 0, r;
+  size_t max_row4 = 1;
+  for (int j = 0; j < n; ++j) {
+    L.job[j] = jobs[j];
+    max_T = std::max(max_T, jobs[j].T);
+    iters = std::max(iters, jobs[j].max_iter == 0 ? 1 : jobs[j].max_iter);
+    max_row4 = std::max(max_row4, size_t(jobs[j].K) * jobs[j].PD / 4);
+  }
+  if (call == kCallUnique) {
+    if ((r = mem_launch<kJobs, kLex>(L, 256, 0, stream, "mem_multi_kernel<lex_compare>"))) return r;
+    return mem_launch<kJobs, kOrder>(L, 256, size_t(max_T) * sizeof(int), stream, "mem_multi_kernel<unique_order>");
+  }
+  if (call == kCallFinalize) return mem_launch<kJobs, kFinalize>(L, 256, 0, stream, "mem_multi_kernel<ko_finalize>");
+  if (call == kCallGather) return mem_launch<kJobs, kGather>(L, 256, 0, stream, "mem_multi_kernel<gather_cast>");
+  if ((r = mem_launch<kJobs, kInit>(L, 256, 0, stream, "mem_multi_kernel<ko_init>"))) return r;
+  if ((r = mem_launch<kJobs, kXnorm>(L, 256, 0, stream, "mem_multi_kernel<ko_xnorm>"))) return r;
+  if ((r = mem_launch<kJobs, kA2>(L, 256, 0, stream, "mem_multi_kernel<seq_reduce>"))) return r;
+  // 6 launches per iteration, all early-exit once a job's device-side loop is over; a job whose host-side loop is over
+  // (max_iter == 0: one assignment, no update) has no blocks
+  for (int it = 0; it < iters; ++it) {
+    L.it = it;
+    if ((r = mem_launch<kJobs, kPartial>(L, 256, KO_PARTIAL_SMEM, stream, "mem_multi_kernel<ko_partial>"))) return r;
+    if ((r = mem_launch<kJobs, kReduce>(L, 256, 0, stream, "mem_multi_kernel<seq_reduce>"))) return r;
+    if ((r = mem_launch<kJobs, kAssign>(L, 256, 0, stream, "mem_multi_kernel<ko_assign>"))) return r;
+    if ((r = mem_launch<kJobs, kUpdate>(L, 256, 0, stream, "mem_multi_kernel<ko_update>"))) return r;
+    if ((r = mem_launch<kJobs, kConverge>(L, 1024, 0, stream, "mem_multi_kernel<ko_converge>"))) return r;
+    if ((r = mem_launch<kJobs, kCommit>(L, 256, 0, stream, "mem_multi_kernel<ko_commit>"))) return r;
+  }
+  // the result copy is split evenly: its bits do not depend on the number of blocks
+  L.finish_blocks = int(std::min<size_t>(std::max(1, device_sm_count() * 8 / n), (max_row4 + 255) / 256));
+  return mem_launch<kJobs, kFinish>(L, 256, 0, stream, "mem_multi_kernel<ko_finish>");
+}
+int mem_run(const MemJobDev* jobs, int n, int call, cudaStream_t stream) {
+  return n == 1 ? mem_group<1>(jobs, 1, call, stream) : mem_group<kMemJobs>(jobs, n, call, stream);
+}
+
+// a single call of the chain: the one-job table
+int mem_single(const char* who, const MemJobDev& J, size_t ws_bytes, int call, fvs_stream_t stream) {
+  const int r = check_mem_call(who, J, ws_bytes, call);
+  return r ? r : mem_run(&J, 1, call, (cudaStream_t)stream);
+}
+
+int mem_table(const char* api, const fvs_qwen_mem_job* jobs, int n, int budget, fvs_stream_t stream, int call) {
+  FVS_REQUIRE(jobs && n > 0 && budget >= 0, "%s: need a job table, n_jobs > 0 and budget >= 0", api);
+  std::vector<MemJobDev> dev(n);
+  JobOutputs out;
+  for (int i = 0; i < n; ++i) {
+    const fvs_qwen_mem_job& j = jobs[i];
+    char who[96];
+    snprintf(who, sizeof who, "%s: job %d", api, i);
+    // the table's own limits: the shapes fvs_qwen_mem_plan takes, and the dtypes the single calls leave unchecked
+    FVS_REQUIRE(j.T > 0 && j.T <= 4096 && j.K > 0 && j.K <= j.T && j.K <= kMaxFinalizeK,
+                "%s: need 0 < T <= 4096, 0 < K <= min(T, %d) (T=%d K=%d)", who, kMaxFinalizeK, j.T, j.K);
+    FVS_REQUIRE(j.PD > 0 && j.PD % SLICE == 0, "%s: PD (%d) must be a positive multiple of %d", who, j.PD, SLICE);
+    FVS_REQUIRE(call != kCallUnique || known_dtype(j.x_dtype), "%s: bad x dtype", who);
+    FVS_REQUIRE(call != kCallGather || known_dtype(j.out_dtype), "%s: bad out dtype", who);
+    dev[i] = mem_job_dev(j);
+    const int r = check_mem_call(who, dev[i], call == kCallUnique ? j.uniq_workspace_bytes : j.km_workspace_bytes, call);
+    if (r) return r;
+    if (call == kCallUnique) {
+      out.add(j.uniq_idx, size_t(j.T) * 4, i);
+      out.add(j.n_unique, 4, i);
+      out.add(j.uniq_workspace, fvs_qwen_unique_workspace_bytes(j.T), i);
+    } else if (call == kCallKmeans) {
+      out.add(j.C, size_t(j.K) * j.PD * 4, i);
+      out.add(j.wsum, size_t(j.K) * 4, i);
+      out.add(j.labels, size_t(j.T) * 4, i);
+      out.add(j.info, 16, i);
+      out.add(j.km_workspace, fvs_qwen_kmeans_workspace_bytes(j.T, j.K, j.PD), i);
+    } else if (call == kCallFinalize) {
+      out.add(j.sorted_idx, size_t(j.K) * 8, i);
+      out.add(j.ts, size_t(j.K) * 4, i);
+      out.add(j.w_sorted, size_t(j.K) * 4, i);
+      out.add(j.flags, 4, i);
+    } else {
+      out.add(j.out, size_t(j.K) * j.PD * (j.out_dtype == FVS_F32 ? 4 : 2), i);
+    }
+  }
+  int r = out.check(api);
   if (r) return r;
   std::vector<int32_t> blocks(n), groups(n);
   const int n_groups = mem_groups(jobs, n, budget, blocks.data(), groups.data());
-  cudaStream_t stream = (cudaStream_t)stream_;
-  if (call == kCallKmeans) {
-    static bool attr_done = false;
-    if (!attr_done) {
-      FVS_CUDA_OK(cudaFuncSetAttribute(mem_multi_kernel<kPartial>, cudaFuncAttributeMaxDynamicSharedMemorySize, KO_PARTIAL_SMEM));
-      attr_done = true;
-    }
-  }
-  const int sm8 = device_sm_count() * 8;
   for (int g = 0, i0 = 0; g < n_groups; ++g) {
-    MemLaunch L;
-    L.n = 0;
-    L.it = 0;
-    L.finish_blocks = 1;
-    int max_T = 1, iters = 0;
-    size_t max_row4 = 1;
-    for (; i0 < n && groups[i0] == g; ++i0) {
-      const fvs_qwen_mem_job& j = jobs[i0];
-      L.job[L.n++] = mem_job_dev(j);
-      max_T = std::max(max_T, j.T);
-      iters = std::max(iters, j.max_iter == 0 ? 1 : j.max_iter);
-      max_row4 = std::max(max_row4, size_t(j.K) * j.PD / 4);
-    }
-    if (call == kCallUnique) {
-      if ((r = mem_launch<kLex>(L, 256, 0, stream, "mem_multi_kernel<lex_compare>"))) return r;
-      if ((r = mem_launch<kOrder>(L, 256, size_t(max_T) * sizeof(int), stream, "mem_multi_kernel<unique_order>"))) return r;
-    } else if (call == kCallFinalize) {
-      if ((r = mem_launch<kFinalize>(L, 256, 0, stream, "mem_multi_kernel<ko_finalize>"))) return r;
-    } else if (call == kCallGather) {
-      if ((r = mem_launch<kGather>(L, 256, 0, stream, "mem_multi_kernel<gather_cast>"))) return r;
-    } else {
-      // the single call's launch sequence, each launch covering the whole group; a job whose loop is over has no blocks
-      if ((r = mem_launch<kInit>(L, 256, 0, stream, "mem_multi_kernel<ko_init>"))) return r;
-      if ((r = mem_launch<kXnorm>(L, 256, 0, stream, "mem_multi_kernel<ko_xnorm>"))) return r;
-      if ((r = mem_launch<kA2>(L, 256, 0, stream, "mem_multi_kernel<seq_reduce>"))) return r;
-      for (int it = 0; it < iters; ++it) {
-        L.it = it;
-        if ((r = mem_launch<kPartial>(L, 256, KO_PARTIAL_SMEM, stream, "mem_multi_kernel<ko_partial>"))) return r;
-        if ((r = mem_launch<kReduce>(L, 256, 0, stream, "mem_multi_kernel<seq_reduce>"))) return r;
-        if ((r = mem_launch<kAssign>(L, 256, 0, stream, "mem_multi_kernel<ko_assign>"))) return r;
-        if ((r = mem_launch<kUpdate>(L, 256, 0, stream, "mem_multi_kernel<ko_update>"))) return r;
-        if ((r = mem_launch<kConverge>(L, 1024, 0, stream, "mem_multi_kernel<ko_converge>"))) return r;
-        if ((r = mem_launch<kCommit>(L, 256, 0, stream, "mem_multi_kernel<ko_commit>"))) return r;
-      }
-      // the result copy is split evenly: its bits do not depend on the number of blocks
-      L.finish_blocks = int(std::min<size_t>(std::max(1, sm8 / L.n), (max_row4 + 255) / 256));
-      if ((r = mem_launch<kFinish>(L, 256, 0, stream, "mem_multi_kernel<ko_finish>"))) return r;
-    }
+    int i1 = i0;
+    while (i1 < n && groups[i1] == g) ++i1;
+    if ((r = mem_run(dev.data() + i0, i1 - i0, call, (cudaStream_t)stream))) return r;
+    i0 = i1;
   }
   return FVS_OK;
 }
-}  // namespace
 
-namespace {
-using fvs::qwen::KlJobDev;
-using fvs::qwen::KlLaunch;
+// ---- the klarge retrieval
+// the bank of a klarge retrieval, in two tiers: rows [0, n_dev) are contiguous at dev (HBM), row n_dev + c*chunk_frames + r
+// is row r of host chunk c (chunks: a host array of the chunks' mapped device pointers)
+struct KlargeBank {
+  const void* dev;
+  int n_dev;
+  const void* const* chunks;
+  int chunk_frames, t_total;
+};
 
-template <bool kBF16, int kStage>
-int kl_launch(KlLaunch& L, int threads, size_t smem, cudaStream_t stream, const char* name) {
-  using namespace fvs::qwen;
+// the checks of fvs_qwen_klarge_retrieve and its tiered form, reported as `who`
+int check_klarge(const char* who, const void* tem_x, const int64_t* klarge_idx, const KlargeBank& b, int k, int PD, int dtype,
+                 int metric, const int64_t* idx_out, const void* workspace, size_t workspace_bytes) {
+  const int t_total = b.t_total;
+  FVS_REQUIRE(tem_x && klarge_idx && idx_out && workspace && (b.dev || b.n_dev == 0), "%s: null pointer", who);
+  FVS_REQUIRE(dtype == FVS_F16 || dtype == FVS_BF16, "%s: dtype must be f16 or bf16", who);
+  FVS_REQUIRE(metric == FVS_KLARGE_EUCLIDEAN || metric == FVS_KLARGE_COSINE, "%s: unknown metric %d", who, metric);
+  FVS_REQUIRE(k > 0 && k <= 64 && t_total > 0, "%s: need 0 < k <= 64, t > 0 (k=%d t=%d)", who, k, t_total);
+  FVS_REQUIRE(PD > 0 && PD % SLICE == 0, "%s: PD (%d) must be a positive multiple of %d", who, PD, SLICE);
+  FVS_REQUIRE(b.n_dev >= 0 && b.n_dev <= t_total, "%s: need 0 <= n_dev <= t_total (n_dev=%d t=%d)", who, b.n_dev, t_total);
+  if (b.n_dev < t_total) {
+    FVS_REQUIRE(b.chunks && b.chunk_frames > 0, "%s: host rows need a chunk table and chunk_frames > 0", who);
+    for (int c = 0; c * int64_t(b.chunk_frames) < t_total - b.n_dev; ++c)
+      FVS_REQUIRE(b.chunks[c], "%s: null pointer of host chunk %d", who, c);
+  }
+  FVS_REQUIRE(workspace_bytes >= fvs_qwen_klarge_workspace_bytes(k, t_total, PD), "%s: workspace too small", who);
+  return FVS_OK;
+}
+
+KlJobDev kl_job_dev(const void* tem_x, const int64_t* klarge_idx, const void* bank, int k, int t_total, int PD,
+                    int64_t* idx_out, float* dist_out, void* workspace) {
+  const size_t units = size_t(t_total) * k + t_total + k;
+  float* part = (float*)workspace;
+  float* tot = (float*)((uint8_t*)workspace + al(units * (PD / SLICE) * 4));
+  // <= 32 bank rows per block: enough blocks to fill every SM from t ~ 32 up
+  return KlJobDev{(const uint16_t*)tem_x, (const long long*)klarge_idx, (const uint16_t*)bank, part, tot,
+                  (long long*)idx_out, dist_out, k, t_total, PD, (t_total + 31) / 32};
+}
+
+template <int kJobs, bool kBF16, int kStage>
+int kl_launch(KlLaunch<kJobs>& L, int threads, size_t smem, cudaStream_t stream, const char* name) {
   L.first[0] = 0;
   for (int j = 0; j < L.n; ++j) L.first[j + 1] = L.first[j] + kl_stage_blocks(L.job[j], kStage);
   if (L.first[L.n] == 0) return FVS_OK;
   if (smem > 48 * 1024) {
     static bool attr = false;   // per instantiation
     if (!attr) {
-      FVS_CUDA_OK(cudaFuncSetAttribute(klarge_multi_kernel<kBF16, kStage>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+      FVS_CUDA_OK(cudaFuncSetAttribute(klarge_multi_kernel<kJobs, kBF16, kStage>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                        64 * SLICE * 2));
       attr = true;
     }
   }
-  klarge_multi_kernel<kBF16, kStage><<<L.first[L.n], threads, smem, stream>>>(L);
+  klarge_multi_kernel<kJobs, kBF16, kStage><<<L.first[L.n], threads, smem, stream>>>(L);
   FVS_CHECK_LAUNCH(name);
   return FVS_OK;
 }
 
-template <bool kBF16>
-int kl_group(KlLaunch& L, int metric, cudaStream_t stream) {
-  using namespace fvs::qwen;
+// sweep kMode of a bank with host rows (one job): one range launch over the device rows and one per host chunk, each
+// reading its rows through the chunk's mapped pointer (PCIe)
+template <bool kBF16, int kMode>
+int klarge_tier_sweep(const KlJobDev& J, const KlargeBank& b, cudaStream_t stream) {
+  static bool attr = false;   // per instantiation
+  auto kern = klarge_partial_kernel<kBF16, kMode>;
+  if (!attr) { FVS_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * SLICE * 2)); attr = true; }
+  const float* norms = kMode == 2 ? J.tot + size_t(J.t_total) * J.k : nullptr;
+  auto launch = [&](const void* rows_at, int t_first, int rows) {
+    kern<<<dim3(J.PD / SLICE, (rows + 31) / 32), 256, size_t(J.k) * SLICE * 2, stream>>>(
+        J.tem_x, J.klarge_idx, (const uint16_t*)rows_at, J.part, J.k, J.t_total, J.PD, norms, t_first, rows);
+    FVS_CHECK_LAUNCH("klarge_partial_kernel");
+    return FVS_OK;
+  };
+  int r;
+  if (b.n_dev > 0 && (r = launch(b.dev, 0, b.n_dev))) return r;
+  for (int c = 0, t = b.n_dev; t < b.t_total; ++c, t += b.chunk_frames)
+    if ((r = launch(b.chunks[c], t, std::min(b.chunk_frames, b.t_total - t)))) return r;
+  return FVS_OK;
+}
+
+// sweep kMode: one launch over every job's whole bank, or the range launches of `tiers` (a one-job group with host rows)
+template <int kJobs, bool kBF16, int kMode>
+int kl_sweep(KlLaunch<kJobs>& L, const KlargeBank* tiers, size_t smem, cudaStream_t stream, const char* name) {
+  if (tiers) return klarge_tier_sweep<kBF16, kMode>(L.job[0], *tiers, stream);
+  return kl_launch<kJobs, kBF16, kKlSweep0 + kMode>(L, 256, smem, stream, name);
+}
+
+template <int kJobs, bool kBF16>
+int kl_group(KlLaunch<kJobs>& L, int metric, const KlargeBank* tiers, cudaStream_t stream) {
   int max_k = 1, r;
   for (int j = 0; j < L.n; ++j) max_k = std::max(max_k, L.job[j].k);
   const size_t smem = size_t(max_k) * SLICE * 2;
   if (metric == FVS_KLARGE_EUCLIDEAN) {
-    if ((r = kl_launch<kBF16, kKlSweep0>(L, 256, smem, stream, "klarge_multi_kernel<sweep>"))) return r;
-    if ((r = kl_launch<kBF16, kKlReduceAll>(L, 256, 0, stream, "klarge_multi_kernel<seq_reduce>"))) return r;
-    return kl_launch<kBF16, kKlTail>(L, 32, 0, stream, "klarge_multi_kernel<tail>");
+    if ((r = kl_sweep<kJobs, kBF16, 0>(L, tiers, smem, stream, "klarge_multi_kernel<sweep>"))) return r;
+    if ((r = kl_launch<kJobs, kBF16, kKlReduceAll>(L, 256, 0, stream, "klarge_multi_kernel<seq_reduce>"))) return r;
+    return kl_launch<kJobs, kBF16, kKlTail>(L, 32, 0, stream, "klarge_multi_kernel<tail>");
   }
-  if ((r = kl_launch<kBF16, kKlSweep1>(L, 256, smem, stream, "klarge_multi_kernel<sweep norms>"))) return r;
-  if ((r = kl_launch<kBF16, kKlReduceNorms>(L, 256, 0, stream, "klarge_multi_kernel<seq_reduce>"))) return r;
-  if ((r = kl_launch<kBF16, kKlNorms>(L, 256, 0, stream, "klarge_multi_kernel<norms>"))) return r;
-  if ((r = kl_launch<kBF16, kKlSweep2>(L, 256, smem, stream, "klarge_multi_kernel<sweep cos>"))) return r;
-  if ((r = kl_launch<kBF16, kKlReduceAb>(L, 256, 0, stream, "klarge_multi_kernel<seq_reduce>"))) return r;
-  return kl_launch<kBF16, kKlCosTail>(L, 32, 0, stream, "klarge_multi_kernel<cos tail>");
+  // cosine: squared norms -> norms -> normalised dot products -> argmin of the similarity (the bank is swept twice)
+  if ((r = kl_sweep<kJobs, kBF16, 1>(L, tiers, smem, stream, "klarge_multi_kernel<sweep norms>"))) return r;
+  if ((r = kl_launch<kJobs, kBF16, kKlReduceNorms>(L, 256, 0, stream, "klarge_multi_kernel<seq_reduce>"))) return r;
+  if ((r = kl_launch<kJobs, kBF16, kKlNorms>(L, 256, 0, stream, "klarge_multi_kernel<norms>"))) return r;
+  if ((r = kl_sweep<kJobs, kBF16, 2>(L, tiers, smem, stream, "klarge_multi_kernel<sweep cos>"))) return r;
+  if ((r = kl_launch<kJobs, kBF16, kKlReduceAb>(L, 256, 0, stream, "klarge_multi_kernel<seq_reduce>"))) return r;
+  return kl_launch<kJobs, kBF16, kKlCosTail>(L, 32, 0, stream, "klarge_multi_kernel<cos tail>");
+}
+
+// one launch group of n <= kJobs retrieval jobs
+template <int kJobs>
+int kl_run(const KlJobDev* jobs, int n, bool bf, int metric, const KlargeBank* tiers, cudaStream_t stream) {
+  KlLaunch<kJobs> L;
+  L.n = n;
+  for (int j = 0; j < n; ++j) L.job[j] = jobs[j];
+  return bf ? kl_group<kJobs, true>(L, metric, tiers, stream) : kl_group<kJobs, false>(L, metric, tiers, stream);
+}
+
+// fvs_qwen_klarge_retrieve and its tiered form: the one-job table, with the tiers' range sweeps for a bank with host rows
+int klarge_retrieve(const char* who, const void* tem_x, const int64_t* klarge_idx, const KlargeBank& b, int k, int PD, int dtype,
+                    int metric, int64_t* idx_out, float* dist_out, void* workspace, size_t workspace_bytes,
+                    fvs_stream_t stream) {
+  const int r = check_klarge(who, tem_x, klarge_idx, b, k, PD, dtype, metric, idx_out, workspace, workspace_bytes);
+  if (r) return r;
+  const KlJobDev J = kl_job_dev(tem_x, klarge_idx, b.dev, k, b.t_total, PD, idx_out, dist_out, workspace);
+  return kl_run<1>(&J, 1, dtype == FVS_BF16, metric, b.n_dev < b.t_total ? &b : nullptr, (cudaStream_t)stream);
 }
 }  // namespace
 
@@ -1382,17 +1348,11 @@ int fvs_qwen_temporal_pool(const void* x, void* out, int t, int h, int w, int dt
 size_t fvs_qwen_unique_workspace_bytes(int T) { return T > 0 ? al(size_t(T) * T) : 0; }
 
 int fvs_qwen_unique_rows(const void* X, int T, int PD, int dtype, int32_t* uniq_idx_out, int32_t* n_unique_out,
-                         void* workspace, size_t workspace_bytes, fvs_stream_t stream_) {
-  FVS_REQUIRE(X && uniq_idx_out && n_unique_out && workspace, "fvs_qwen_unique_rows: null pointer");
-  FVS_REQUIRE(T > 0 && T <= 4096 && PD > 0, "fvs_qwen_unique_rows: bad shape T=%d PD=%d", T, PD);
-  FVS_REQUIRE(workspace_bytes >= fvs_qwen_unique_workspace_bytes(T), "fvs_qwen_unique_rows: workspace too small");
-  cudaStream_t stream = (cudaStream_t)stream_;
-  signed char* cmp = (signed char*)workspace;
-  lex_compare_kernel<<<dim3(T, T), 256, 0, stream>>>(X, T, PD, dtype, cmp);
-  FVS_CHECK_LAUNCH("lex_compare_kernel");
-  unique_order_kernel<<<1, 256, T * sizeof(int), stream>>>(cmp, T, uniq_idx_out, n_unique_out);
-  FVS_CHECK_LAUNCH("unique_order_kernel");
-  return FVS_OK;
+                         void* workspace, size_t workspace_bytes, fvs_stream_t stream) {
+  MemJobDev J{};
+  J.X = X; J.T = T; J.PD = PD; J.dt = dtype;
+  J.uniq_idx = uniq_idx_out; J.n_unique = n_unique_out; J.uniq_ws = workspace;
+  return mem_single("fvs_qwen_unique_rows", J, workspace_bytes, kCallUnique, stream);
 }
 
 size_t fvs_qwen_kmeans_workspace_bytes(int T, int K, int PD) {
@@ -1404,70 +1364,29 @@ size_t fvs_qwen_kmeans_workspace_bytes(int T, int K, int PD) {
 
 int fvs_qwen_kmeans(const void* X, int x_dtype, const float* w, const int32_t* uniq_idx, const int32_t* init_idx,
                     const int32_t* refill_idx, int T, int K, int PD, int max_iter, float tol, float* C_out, float* wsum_out,
-                    int32_t* labels_out, int32_t* info_out, void* workspace, size_t workspace_bytes, fvs_stream_t stream_) {
-  FVS_REQUIRE(X && w && init_idx && refill_idx && C_out && wsum_out && labels_out && info_out && workspace,
-              "fvs_qwen_kmeans: null pointer");
-  FVS_REQUIRE(x_dtype == FVS_F16 || x_dtype == FVS_BF16 || x_dtype == FVS_F32, "fvs_qwen_kmeans: bad x dtype");
-  FVS_REQUIRE(T > 0 && K > 0 && K <= T, "fvs_qwen_kmeans: need 0 < K <= T (T=%d K=%d)", T, K);
-  FVS_REQUIRE(PD % SLICE == 0, "fvs_qwen_kmeans: PD (%d) must be a multiple of %d", PD, SLICE);
-  FVS_REQUIRE(max_iter >= 0 && max_iter <= 1000, "fvs_qwen_kmeans: bad max_iter");
-  FVS_REQUIRE(workspace_bytes >= fvs_qwen_kmeans_workspace_bytes(T, K, PD), "fvs_qwen_kmeans: workspace too small");
-  cudaStream_t stream = (cudaStream_t)stream_;
-  const int S = PD / SLICE;
-  const KO B = ko_carve(workspace, T, K, PD);
-  const size_t TK = size_t(T) * K + K;
-  static bool attr_done = false;
-  if (!attr_done) {
-    FVS_CUDA_OK(cudaFuncSetAttribute(ko_partial_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, KO_PARTIAL_SMEM));
-    attr_done = true;
-  }
-  ko_init_kernel<<<(K * S + 7) / 8, 256, 0, stream>>>(B, X, x_dtype, uniq_idx, init_idx, T, K, PD);
-  FVS_CHECK_LAUNCH("ko_init_kernel");
-  ko_xnorm_kernel<<<(T * S + 7) / 8, 256, 0, stream>>>(B, X, x_dtype, T, PD);
-  FVS_CHECK_LAUNCH("ko_xnorm_kernel");
-  seq_reduce_kernel<<<(T + 7) / 8, 256, 0, stream>>>(B.a2, B.a2t, T, S, nullptr);
-  FVS_CHECK_LAUNCH("seq_reduce_kernel");
-  // max_iter == 0: the degenerate path of the reference (fewer unique rows than clusters): one assignment, no update
-  const int iters = max_iter == 0 ? 1 : max_iter;
-  for (int it = 0; it < iters; ++it) {     // 6 launches per iteration, all early-exit once the device-side loop is over
-    ko_partial_kernel<<<((T + 7) / 8) * S, 256, KO_PARTIAL_SMEM, stream>>>(B, X, x_dtype, T, K, PD);
-    FVS_CHECK_LAUNCH("ko_partial_kernel");
-    seq_reduce_kernel<<<int((TK + 7) / 8), 256, 0, stream>>>(B.ab, B.abt, int(TK), S, B.state);
-    FVS_CHECK_LAUNCH("seq_reduce_kernel");
-    ko_assign_kernel<<<(T + 7) / 8, 256, 0, stream>>>(B, T, K, PD);
-    FVS_CHECK_LAUNCH("ko_assign_kernel");
-    if (max_iter == 0) break;
-    ko_update_kernel<<<(K * S + 7) / 8, 256, 0, stream>>>(B, X, x_dtype, w, refill_idx, T, K, PD, it);
-    FVS_CHECK_LAUNCH("ko_update_kernel");
-    ko_converge_kernel<<<1, 1024, 0, stream>>>(B, K, PD, it, max_iter, tol);
-    FVS_CHECK_LAUNCH("ko_converge_kernel");
-    ko_commit_kernel<<<(K * S + 7) / 8, 256, 0, stream>>>(B, K, PD, it, max_iter);
-    FVS_CHECK_LAUNCH("ko_commit_kernel");
-  }
-  ko_finish_kernel<<<device_sm_count() * 8, 256, 0, stream>>>(B, C_out, wsum_out, labels_out, info_out, T, K, PD);
-  FVS_CHECK_LAUNCH("ko_finish_kernel");
-  return FVS_OK;
+                    int32_t* labels_out, int32_t* info_out, void* workspace, size_t workspace_bytes, fvs_stream_t stream) {
+  MemJobDev J{};
+  J.X = X; J.dt = x_dtype; J.w = w; J.uniq_idx = const_cast<int32_t*>(uniq_idx); J.init_idx = init_idx;
+  J.refill_idx = refill_idx; J.T = T; J.K = K; J.PD = PD; J.max_iter = max_iter; J.tol = tol;
+  J.C = C_out; J.wsum = wsum_out; J.labels = labels_out; J.info = info_out; J.km_ws = workspace;
+  return mem_single("fvs_qwen_kmeans", J, workspace_bytes, kCallKmeans, stream);
 }
 
 int fvs_qwen_kmeans_finalize(const int32_t* labels, const float* wsum, int T, int K, const int64_t* order_in,
                              int64_t* sorted_idx_out, float* ts_out, float* w_out, int32_t* flags_out, fvs_stream_t stream) {
-  FVS_REQUIRE(labels && wsum && sorted_idx_out && ts_out && w_out && flags_out, "fvs_qwen_kmeans_finalize: null pointer");
-  FVS_REQUIRE(T > 0 && K > 0 && K <= kMaxFinalizeK, "fvs_qwen_kmeans_finalize: need T > 0, 0 < K <= %d (T=%d K=%d)", kMaxFinalizeK, T, K);
-  ko_finalize_kernel<<<1, 256, 0, (cudaStream_t)stream>>>(labels, wsum, T, K, (const long long*)order_in,
-                                                         (long long*)sorted_idx_out, ts_out, w_out, flags_out);
-  FVS_CHECK_LAUNCH("ko_finalize_kernel");
-  return FVS_OK;
+  MemJobDev J{};
+  J.labels = const_cast<int32_t*>(labels); J.wsum = const_cast<float*>(wsum); J.T = T; J.K = K;
+  J.order_in = (const long long*)order_in; J.sorted_idx = (long long*)sorted_idx_out; J.ts = ts_out; J.w_sorted = w_out;
+  J.flags = flags_out;
+  return mem_single("fvs_qwen_kmeans_finalize", J, 0, kCallFinalize, stream);
 }
 
 int fvs_gather_rows_cast(const float* src, const int64_t* idx, void* out, int n, int64_t row_elems, int out_dtype,
                          fvs_stream_t stream) {
-  FVS_REQUIRE(src && idx && out && n > 0 && row_elems > 0, "fvs_gather_rows_cast: bad argument");
-  FVS_REQUIRE(row_elems % 4 == 0, "fvs_gather_rows_cast: row_elems must be a multiple of 4");
-  int bx = int((row_elems / 4 + 255) / 256);
-  if (bx > 64) bx = 64;
-  gather_cast_kernel<<<dim3(bx, n), 256, 0, (cudaStream_t)stream>>>(src, (const long long*)idx, out, size_t(row_elems), out_dtype);
-  FVS_CHECK_LAUNCH("gather_cast_kernel");
-  return FVS_OK;
+  MemJobDev J{};
+  J.C = const_cast<float*>(src); J.sorted_idx = (long long*)const_cast<int64_t*>(idx); J.out = out; J.K = n;
+  J.row_elems = row_elems; J.out_dt = out_dtype;
+  return mem_single("fvs_gather_rows_cast", J, 0, kCallGather, stream);
 }
 
 size_t fvs_qwen_klarge_workspace_bytes(int k, int t_total, int PD) {
@@ -1507,57 +1426,45 @@ int fvs_qwen_mem_plan(const fvs_qwen_mem_job* jobs_h, int n_jobs, int budget, in
 }
 
 int fvs_qwen_unique_rows_multi(const fvs_qwen_mem_job* jobs_h, int n_jobs, int budget, fvs_stream_t stream) {
-  return run_mem_multi("fvs_qwen_unique_rows_multi", jobs_h, n_jobs, budget, stream, kCallUnique);
+  return mem_table("fvs_qwen_unique_rows_multi", jobs_h, n_jobs, budget, stream, kCallUnique);
 }
 int fvs_qwen_kmeans_multi(const fvs_qwen_mem_job* jobs_h, int n_jobs, int budget, fvs_stream_t stream) {
-  return run_mem_multi("fvs_qwen_kmeans_multi", jobs_h, n_jobs, budget, stream, kCallKmeans);
+  return mem_table("fvs_qwen_kmeans_multi", jobs_h, n_jobs, budget, stream, kCallKmeans);
 }
 int fvs_qwen_kmeans_finalize_multi(const fvs_qwen_mem_job* jobs_h, int n_jobs, int budget, fvs_stream_t stream) {
-  return run_mem_multi("fvs_qwen_kmeans_finalize_multi", jobs_h, n_jobs, budget, stream, kCallFinalize);
+  return mem_table("fvs_qwen_kmeans_finalize_multi", jobs_h, n_jobs, budget, stream, kCallFinalize);
 }
 int fvs_gather_rows_cast_multi(const fvs_qwen_mem_job* jobs_h, int n_jobs, int budget, fvs_stream_t stream) {
-  return run_mem_multi("fvs_gather_rows_cast_multi", jobs_h, n_jobs, budget, stream, kCallGather);
+  return mem_table("fvs_gather_rows_cast_multi", jobs_h, n_jobs, budget, stream, kCallGather);
 }
 
 int fvs_qwen_klarge_retrieve_multi(const fvs_qwen_retrieve_job* jobs_h, int n_jobs, int dtype, int metric,
                                    fvs_stream_t stream) {
   const char* api = "fvs_qwen_klarge_retrieve_multi";
   FVS_REQUIRE(jobs_h && n_jobs > 0, "%s: need a job table and n_jobs > 0", api);
-  FVS_REQUIRE(dtype == FVS_F16 || dtype == FVS_BF16, "%s: dtype must be f16 or bf16", api);
-  FVS_REQUIRE(metric == FVS_KLARGE_EUCLIDEAN || metric == FVS_KLARGE_COSINE, "%s: unknown metric %d", api, metric);
-  struct Range { uintptr_t lo, hi; int job; };
-  std::vector<Range> out;
-  for (int i = 0; i < n_jobs; ++i) {          // the checks of fvs_qwen_klarge_retrieve, per job
+  std::vector<KlJobDev> dev(n_jobs);
+  JobOutputs out;
+  int r;
+  for (int i = 0; i < n_jobs; ++i) {
     const fvs_qwen_retrieve_job& j = jobs_h[i];
-    FVS_REQUIRE(j.tem_x && j.klarge_idx && j.bank && j.idx_out && j.workspace, "%s: job %d: null pointer", api, i);
-    FVS_REQUIRE(j.k > 0 && j.k <= 64 && j.t_total > 0, "%s: job %d: need 0 < k <= 64, t > 0 (k=%d t=%d)", api, i, j.k,
-                j.t_total);
-    FVS_REQUIRE(j.PD > 0 && j.PD % SLICE == 0, "%s: job %d: PD (%d) must be a positive multiple of %d", api, i, j.PD, SLICE);
-    FVS_REQUIRE(j.n_dev == j.t_total, "%s: job %d: %d of its %d bank rows are in host memory: step it through "
-                "fvs_qwen_klarge_retrieve_tiered", api, i, j.t_total - j.n_dev, j.t_total);
-    const size_t ws = fvs_qwen_klarge_workspace_bytes(j.k, j.t_total, j.PD);
-    FVS_REQUIRE(j.workspace_bytes >= ws, "%s: job %d: workspace too small", api, i);
-    out.push_back({uintptr_t(j.idx_out), uintptr_t(j.idx_out) + size_t(j.k) * 8, i});
-    out.push_back({uintptr_t(j.workspace), uintptr_t(j.workspace) + ws, i});
-    if (j.dist_out) out.push_back({uintptr_t(j.dist_out), uintptr_t(j.dist_out) + size_t(j.k) * j.t_total * 4, i});
+    char who[96];
+    snprintf(who, sizeof who, "%s: job %d", api, i);
+    FVS_REQUIRE(j.n_dev == j.t_total, "%s: %d of its %d bank rows are in host memory: step it through "
+                "fvs_qwen_klarge_retrieve_tiered", who, j.t_total - j.n_dev, j.t_total);
+    const KlargeBank b{j.bank, j.n_dev, nullptr, 0, j.t_total};
+    if ((r = check_klarge(who, j.tem_x, j.klarge_idx, b, j.k, j.PD, dtype, metric, j.idx_out, j.workspace, j.workspace_bytes)))
+      return r;
+    dev[i] = kl_job_dev(j.tem_x, j.klarge_idx, j.bank, j.k, j.t_total, j.PD, j.idx_out, j.dist_out, j.workspace);
+    out.add(j.idx_out, size_t(j.k) * 8, i);
+    out.add(j.workspace, fvs_qwen_klarge_workspace_bytes(j.k, j.t_total, j.PD), i);
+    if (j.dist_out) out.add(j.dist_out, size_t(j.k) * j.t_total * 4, i);
   }
-  for (size_t a = 0; a < out.size(); ++a)
-    for (size_t b = a + 1; b < out.size(); ++b)
-      FVS_REQUIRE(out[a].job == out[b].job || out[a].hi <= out[b].lo || out[b].hi <= out[a].lo,
-                  "%s: jobs %d and %d share an output", api, out[a].job, out[b].job);
+  if ((r = out.check(api))) return r;
   for (int i0 = 0; i0 < n_jobs; i0 += kMemJobs) {
-    KlLaunch L;
-    L.n = std::min(kMemJobs, n_jobs - i0);
-    for (int q = 0; q < L.n; ++q) {
-      const fvs_qwen_retrieve_job& j = jobs_h[i0 + q];
-      const size_t units = size_t(j.t_total) * j.k + j.t_total + j.k;
-      float* part = (float*)j.workspace;
-      float* tot = (float*)((uint8_t*)j.workspace + al(units * (j.PD / SLICE) * 4));
-      L.job[q] = KlJobDev{(const uint16_t*)j.tem_x, (const long long*)j.klarge_idx, (const uint16_t*)j.bank, part, tot,
-                          (long long*)j.idx_out, j.dist_out, j.k, j.t_total, j.PD, (j.t_total + 31) / 32};
-    }
-    const int r = dtype == FVS_BF16 ? kl_group<true>(L, metric, (cudaStream_t)stream)
-                                    : kl_group<false>(L, metric, (cudaStream_t)stream);
+    const int n = std::min(kMemJobs, n_jobs - i0);
+    const bool bf = dtype == FVS_BF16;
+    r = n == 1 ? kl_run<1>(dev.data() + i0, 1, bf, metric, nullptr, (cudaStream_t)stream)
+               : kl_run<kMemJobs>(dev.data() + i0, n, bf, metric, nullptr, (cudaStream_t)stream);
     if (r) return r;
   }
   return FVS_OK;

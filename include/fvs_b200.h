@@ -434,19 +434,20 @@ int fvs_qwen_kmeans_finalize(const int32_t* labels, const float* wsum, int T, in
                              int64_t* sorted_idx_out, float* ts_out, float* w_out, int32_t* flags_out, fvs_stream_t stream);
 
 /* out[i, :] = cast<out_dtype>(src[idx[i], :]): the `reduced_feature[sorted_indices] ... .to(dtype)` of
- * compress_functions.py:283,297 in one pass.  src fp32, idx int64. */
+ * compress_functions.py:283,297 in one pass.  src fp32, idx int64, 0 < n <= 65535, row_elems % 4 == 0. */
 int fvs_gather_rows_cast(const float* src, const int64_t* idx, void* out, int n, int64_t row_elems, int out_dtype,
                          fvs_stream_t stream);
 
 /* ---- the CSM chain of many Qwen2-VL streams in one launch per kernel (DESIGN.md §3.17) -------------------------------
  * One fvs_qwen_mem_job per stream: its candidates X [T, PD] (x_dtype), draws and outputs, all device pointers.  Each
- * *_multi call below gives job i exactly the bits the single-stream call gives it, whatever the other jobs are: a job
- * always gets the blocks its single call launches, laid end to end with the other jobs' blocks in one flat grid (a block
- * finds its job in a block-offset table passed as a kernel parameter), so no reduction of a job depends on its
- * neighbours or on the budget.  Jobs go into launches in order, at most FVS_QWEN_MEM_JOBS_PER_LAUNCH per launch and, when
+ * single-stream call above runs as a table of one job, so each *_multi call below gives job i exactly the bits the
+ * single-stream call gives it, whatever the other jobs are: a job always gets the blocks of its one-job launch, laid end
+ * to end with the other jobs' blocks in one flat grid (a block finds its job in a block-offset table passed as a kernel
+ * parameter), so no reduction of a job depends on its neighbours or on the budget.  Jobs go into launches in order, at most FVS_QWEN_MEM_JOBS_PER_LAUNCH per launch and, when
  * budget > 0, at most `budget` Lloyd-sweep blocks per launch (a larger job goes alone); every kernel of a call is then
- * launched once per launch group.  Every job is validated before anything is enqueued: on FVS_EINVAL (a bad shape or
- * pointer, a workspace too small, an output range shared by two jobs) nothing was launched.  No allocation, no host sync.
+ * launched once per launch group.  Every job gets the checks of its single call plus the table's own (the shapes of
+ * fvs_qwen_mem_plan, known dtype codes, no output range shared by two jobs) before anything is enqueued: on FVS_EINVAL
+ * nothing was launched.  No allocation, no host sync.
  *   fvs_qwen_unique_rows_multi:     fvs_qwen_unique_rows(X, T, PD, x_dtype, uniq_idx, n_unique, uniq_workspace, ...)
  *   fvs_qwen_kmeans_multi:          fvs_qwen_kmeans(X, x_dtype, w, uniq_idx, init_idx, refill_idx, T, K, PD, max_iter, tol,
  *                                                   C, wsum, labels, info, km_workspace, ...); each job keeps its own
@@ -521,8 +522,8 @@ int fvs_qwen_klarge_retrieve_tiered(const void* tem_x, const int64_t* klarge_idx
 
 /* The klarge retrieval of many streams in one launch per kernel (DESIGN.md §3.17): job i gets exactly the bits of
  * fvs_qwen_klarge_retrieve(tem_x, klarge_idx, bank, k, t_total, PD, dtype, metric, idx_out, dist_out, workspace, ...)
- * whatever the other jobs are: its sweep keeps the single call's split-K partition (PD/1024 slices x ceil(t_total/32)
- * row splits), laid end to end with the other jobs' blocks.  dtype and metric are the call's; k, t_total, PD, the bank
+ * whatever the other jobs are (the single call is the one-job table): its sweep keeps the split-K partition (PD/1024
+ * slices x ceil(t_total/32) row splits), laid end to end with the other jobs' blocks.  dtype and metric are the call's; k, t_total, PD, the bank
  * and klarge_idx are each job's.  The bank must be wholly in HBM: a job with n_dev != t_total (host rows, which the
  * tiered sweep reads through fvs_qwen_klarge_retrieve_tiered) is refused.  At most FVS_QWEN_MEM_JOBS_PER_LAUNCH jobs per
  * launch; FVS_EINVAL with nothing launched on a bad job or an output shared by two jobs. */
@@ -561,8 +562,8 @@ int fvs_qwen_dam_gather(const int64_t* picks, int n, int64_t n_frames, const voi
                         int64_t n_dev, const void* const* host_chunks, int chunk_frames, const int64_t* prev_picks, int m,
                         const void* prev_x, const void* prev_merged, int64_t x_frame_elems, int64_t merged_frame_elems,
                         int dtype, void* spa_x_out, void* merged_out, uint64_t* host_fetches, fvs_stream_t stream);
-/* fvs_qwen_dam_gather of many streams in one launch: job i gets exactly the bits (and host_fetches count) of the single
- * call with its own arguments — its own two-tier bank, previous DAM and chunk table.  dtype is the call's.  At most
+/* fvs_qwen_dam_gather of many streams in one launch (the single call is the one-job launch): job i gets exactly the bits
+ * (and host_fetches count) of the single call with its own arguments — its own two-tier bank, previous DAM and chunk table.  dtype is the call's.  At most
  * FVS_QWEN_MEM_JOBS_PER_LAUNCH jobs per launch; every job gets the single call's checks, and no output (spa_x_out,
  * merged_out, host_fetches) may be shared by two jobs: FVS_EINVAL with nothing launched otherwise. */
 typedef struct fvs_qwen_gather_job {

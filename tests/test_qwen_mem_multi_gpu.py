@@ -139,6 +139,47 @@ def test_refused_table_launches_nothing(lib):
     assert lib.fvs_launch_count() == n0
 
 
+def launches(lib, fn):
+    n0 = lib.fvs_launch_count()
+    fn()
+    return lib.fvs_launch_count() - n0
+
+
+@pytest.mark.parametrize("call, max_iter, want", [("unique", 10, 2), ("kmeans", 10, 3 + 6 * 10 + 1),
+                                                  ("kmeans", 3, 3 + 6 * 3 + 1), ("kmeans", 0, 7), ("finalize", 10, 1),
+                                                  ("gather", 10, 1)])
+def test_single_call_launch_counts(lib, call, max_iter, want):
+    """a single call is the one-job table: the launches of its stage sequence, one per stage and iteration"""
+    from flash_vstream_b200.qwen import ops as Q
+    j = make_job(3, 33, 8, 2, torch.bfloat16, max_iter=max_iter)
+    uniq, _ = Q.unique_rows(j["X"])
+    kmeans = lambda: Q.kmeans_ordered(j["X"], j["w"], uniq, j["init"], j["refill"], j["K"], j["max_iter"], j["tol"])  # noqa: E731
+    C, wsum, labels, _ = kmeans()
+    sidx = Q.kmeans_finalize(labels, wsum)[0]
+    fns = dict(unique=lambda: Q.unique_rows(j["X"]), kmeans=kmeans, finalize=lambda: Q.kmeans_finalize(labels, wsum),
+               gather=lambda: Q.gather_rows_cast(C, sidx, torch.bfloat16))
+    assert launches(lib, fns[call]) == want
+
+
+@pytest.mark.parametrize("n_dev", [11, 5, 0])
+@pytest.mark.parametrize("metric, sweeps", [("euclidean", 1), ("cosine", 2)])
+def test_klarge_launch_counts(lib, metric, sweeps, n_dev):
+    """3 (Euclidean) or 6 (cosine) launches, plus one per extra tier of a bank with host rows in each sweep"""
+    from flash_vstream_b200.qwen import ops as Q
+    from tests.test_qwen_small_tier_gpu import _tiered
+    g = torch.Generator().manual_seed(5)
+    t, F = 11, 4
+    bank = torch.randn(t, 2048, generator=g).bfloat16().cuda()
+    tem_x = torch.randn(40, 2048, generator=g).bfloat16().cuda()
+    kidx = torch.randperm(40, generator=g)[:30].cuda()
+    tb, chunks = _tiered(bank, n_dev, F)
+    want = (3 if metric == "euclidean" else 6) + sweeps * (len(Q.klarge_plan(t, n_dev, F)) - 1)
+    assert launches(lib, lambda: Q.klarge_retrieve(tem_x, kidx, tb, metric=metric)) == want
+    if n_dev == t:
+        assert launches(lib, lambda: Q.klarge_retrieve(tem_x, kidx, bank, metric=metric)) == want
+    torch.cuda.synchronize()
+
+
 @pytest.mark.parametrize("metric", ["euclidean", "cosine"])
 @pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16])
 def test_klarge_retrieve_multi_equals_single_calls(lib, metric, dtype):

@@ -2,9 +2,9 @@
 
 csrc/qwen_kernels.cu is bit-exact against oracle/qwen_oracle.py, but most of its code only runs past the toy shapes of
 test_qwen_gpu_parity.py: the 2-stage cp.async ring of KO_KC = 8 centroid slices (K > 8), the 32-partial chains of
-seq_reduce_kernel / ko_converge_kernel (S >= 33 slices: two passes), the incremental Lloyd loop (dirty / refilled
+seq_reduce / ko_converge (S >= 33 slices: two passes), the incremental Lloyd loop (dirty / refilled
 clusters, a change list that shrinks, no commit on a tolerance stop), the klarge row groups and the f16 overflow to
-inf / NaN, and lex_compare_kernel's 1024-element chunks.  This file holds the case table that
+inf / NaN, and lex_compare's 1024-element chunks.  This file holds the case table that
 test_qwen_memory_shapes_gpu.py runs on the GPU, pins its seeded generators, and proves with the oracle's trace that each
 case reaches the branch it names — so an RNG or torch change that moves a case off its branch fails here, on any
 machine, instead of passing quietly on the GPU."""
@@ -17,7 +17,7 @@ from tests.golden_inputs import _gen, checksum
 from tests.qwen_inputs import DT
 
 SLICE = 1024
-KO_KC = 8          # centroid slices per cp.async stage of ko_partial_kernel
+KO_KC = 8          # centroid slices per cp.async stage of ko_partial
 PD_REAL = 184320   # 12x12 half-resolution tokens x 1280 (336 px)
 NEVER = 0.0        # tol that never stops the loop (diff < 0 is never true)
 
@@ -103,7 +103,7 @@ def kmeans_oracle(c):
 
 
 def dirty(trace, i):
-    """clusters that gained or lost a row between iterations i-1 and i (ko_assign_kernel's dirty flags)"""
+    """clusters that gained or lost a row between iterations i-1 and i (ko_assign's dirty flags)"""
     a, b = trace[i - 1]["labels"], trace[i]["labels"]
     m = a != b
     return set(a[m].tolist()) | set(b[m].tolist())
@@ -118,7 +118,7 @@ def reached(c, trace):
     if S >= 33:
         got.add("two_passes")                # seq_reduce / ko_converge chain over two 32-partial passes
     if T % 8:
-        got.add("t_ragged")                  # the last 8-row block of ko_partial_kernel is partial
+        got.add("t_ragged")                  # the last 8-row block of ko_partial is partial
     if c["max_iter"] == 0:
         got.add("degenerate")
         return got
@@ -138,14 +138,14 @@ def reached(c, trace):
     if sum(1 for r in trace[1:4] if r["moved"] > 0) == 3:
         got.add("moving")                    # labels still move in iterations 1, 2 and 3
     for i in range(1, len(trace)):
-        sweep = trace[i - 1]["changed"]      # the change list ko_partial_kernel sweeps in iteration i
+        sweep = trace[i - 1]["changed"]      # the change list ko_partial sweeps in iteration i
         if 0 < len(sweep) < K:
             got.add("subset")
         if not sweep:
-            got.add("idle")                  # nothing changed: ko_partial_kernel and ko_commit_kernel have nothing to do
+            got.add("idle")                  # nothing changed: ko_partial and ko_commit have nothing to do
         clean = set(range(K)) - dirty(trace, i) - set(trace[i - 1]["refilled"])
         if clean:
-            got.add("skip")                  # ko_update_kernel skips an unchanged cluster
+            got.add("skip")                  # ko_update skips an unchanged cluster
         if set(trace[i - 1]["refilled"]) - dirty(trace, i):
             got.add("re_refill")             # refilled, no row moved, and still re-drawn: only wprev says so
     if sum(1 for r in trace if r["refilled"]) >= 2:
