@@ -378,7 +378,8 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
 }  // namespace attn
 
 template <bool kBF16, bool kX>
-static int attention_launch_t(const AttnMaps& m, int tokens, int heads, int tiles, float scale_log2e, cudaStream_t stream) {
+static int attention_launch_t(const AttnMaps& m, int tokens, int heads, int tiles, float scale_log2e, cudaStream_t stream,
+                              bool pdl) {
   using namespace attn;
   static bool done = false;
   if (!done) {
@@ -386,13 +387,13 @@ static int attention_launch_t(const AttnMaps& m, int tokens, int heads, int tile
     done = true;
   }
   const int grid = tiles < device_sm_count() ? tiles : device_sm_count();
-  FVS_CUDA_OK(launch_ex(attention_kernel<kBF16, kX>, dim3(grid), dim3(kThreads), Lay<kX>::BYTES, stream, 1, /*pdl=*/true, m.q,
+  FVS_CUDA_OK(launch_ex(attention_kernel<kBF16, kX>, dim3(grid), dim3(kThreads), Lay<kX>::BYTES, stream, 1, pdl, m.q,
                         m.kv, m.ctx, m.qx, m.kvx, m.ctxx, tokens, heads, tiles, scale_log2e));
   return FVS_OK;
 }
 
 int attention_launch(const AttnMaps& m, int frames, int tokens, int heads, float scale, int dtype, cudaStream_t stream,
-                     int head_dim) {
+                     int head_dim, bool pdl) {
   using namespace attn;
   const float scale_log2e = scale * 1.4426950408889634f;
   const long long tiles_ll = (long long)((tokens + BQ - 1) / BQ) * heads * frames;
@@ -400,10 +401,10 @@ int attention_launch(const AttnMaps& m, int frames, int tokens, int heads, float
   const int tiles = int(tiles_ll);
   const bool bf = dtype == FVS_BF16, x80 = head_dim == 80;
   const int prof = prof_begin(FVS_PROF_ATTENTION, 4.0 * frames * double(heads) * tokens * double(tokens) * head_dim, stream);
-  const int r = x80 ? (bf ? attention_launch_t<true, true>(m, tokens, heads, tiles, scale_log2e, stream)
-                          : attention_launch_t<false, true>(m, tokens, heads, tiles, scale_log2e, stream))
-                    : (bf ? attention_launch_t<true, false>(m, tokens, heads, tiles, scale_log2e, stream)
-                          : attention_launch_t<false, false>(m, tokens, heads, tiles, scale_log2e, stream));
+  const int r = x80 ? (bf ? attention_launch_t<true, true>(m, tokens, heads, tiles, scale_log2e, stream, pdl)
+                          : attention_launch_t<false, true>(m, tokens, heads, tiles, scale_log2e, stream, pdl))
+                    : (bf ? attention_launch_t<true, false>(m, tokens, heads, tiles, scale_log2e, stream, pdl)
+                          : attention_launch_t<false, false>(m, tokens, heads, tiles, scale_log2e, stream, pdl));
   if (r) return r;
   prof_end(prof, stream);
   FVS_CHECK_LAUNCH("attention_kernel");

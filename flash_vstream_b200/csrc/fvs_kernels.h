@@ -4,12 +4,15 @@
 
 namespace fvs {
 
+// The ViT launchers take `pdl`: launch with the programmatic-dependent-launch attribute (the kernels trigger their
+// dependents on entry, so a dependent's CTAs take SMs as soon as any free up).
+
 // gemm_sm90.cu
 int linear_make_maps(CUtensorMap* ta, CUtensorMap* tb, CUtensorMap* to, const void* A, const void* W, void* out,
                      int M, int N, int K, int lda, int ldo, bool out_f32);
 int linear_launch(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& to, const void* bias,
                   const void* aux, int M, int N, int K, int ld_aux, int epilogue, int aux_period, int dtype,
-                  cudaStream_t stream);
+                  cudaStream_t stream, bool pdl = true);
 
 // attention_sm90.cu
 struct AttnMaps {
@@ -18,11 +21,11 @@ struct AttnMaps {
 };
 int attention_make_maps(AttnMaps* m, const void* qkv, void* ctx, int frames, int tokens, int heads, int head_dim = 64);
 int attention_launch(const AttnMaps& m, int frames, int tokens, int heads, float scale, int dtype, cudaStream_t stream,
-                     int head_dim = 64);
+                     int head_dim = 64, bool pdl = true);
 
 // vit_misc.cu
 int layernorm_launch(const void* x, const void* gamma, const void* beta, void* y, int rows, int dim, float eps,
-                     int dtype, bool x_f32, bool y_f32, const void* delta, cudaStream_t stream);
+                     int dtype, bool x_f32, bool y_f32, const void* delta, cudaStream_t stream, bool pdl = true);
 int im2col_launch(const void* pixels, void* patches, int B, int S, int P, int Kpad, cudaStream_t stream);
 int drop_cls_launch(const void* x, const void* delta, void* out, int B, int tokens, int D, int dtype, cudaStream_t stream,
                     bool keep_cls = false);

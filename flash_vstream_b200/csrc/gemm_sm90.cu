@@ -259,7 +259,7 @@ linear_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant_
 
 template <int kEpi, bool kBF16, int kBN>
 static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& to, const void* bias,
-                  const void* aux, int M, int N, int K, int ld_aux, int aux_period, cudaStream_t stream) {
+                  const void* aux, int M, int N, int K, int ld_aux, int aux_period, cudaStream_t stream, bool pdl) {
   auto kern = linear_kernel<kEpi, kBF16, kBN>;
   constexpr int smem = Cfg<kBN>::SMEM_BYTES;
   static bool attr_done = false;  // per instantiation
@@ -271,7 +271,7 @@ static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMa
   int grid = device_sm_count();
   if (grid > num_tiles) grid = num_tiles;
   const int prof = prof_begin(FVS_PROF_LINEAR, 2.0 * M * double(N) * K, stream);
-  cudaError_t e = launch_ex(kern, dim3(grid), dim3(kThreads), smem, stream, 1, /*pdl=*/true, ta, tb, to,
+  cudaError_t e = launch_ex(kern, dim3(grid), dim3(kThreads), smem, stream, 1, pdl, ta, tb, to,
                             reinterpret_cast<const uint16_t*>(bias), reinterpret_cast<const uint16_t*>(aux), M, N, K,
                             ld_aux, aux_period);
   prof_end(prof, stream);
@@ -282,16 +282,16 @@ static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMa
 
 template <int kEpi, int kBN>
 static int launch_dt(bool bf, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& to, const void* bias,
-                     const void* aux, int M, int N, int K, int ld_aux, int aux_period, cudaStream_t stream) {
-  return bf ? launch<kEpi, true, kBN>(ta, tb, to, bias, aux, M, N, K, ld_aux, aux_period, stream)
-            : launch<kEpi, false, kBN>(ta, tb, to, bias, aux, M, N, K, ld_aux, aux_period, stream);
+                     const void* aux, int M, int N, int K, int ld_aux, int aux_period, cudaStream_t stream, bool pdl) {
+  return bf ? launch<kEpi, true, kBN>(ta, tb, to, bias, aux, M, N, K, ld_aux, aux_period, stream, pdl)
+            : launch<kEpi, false, kBN>(ta, tb, to, bias, aux, M, N, K, ld_aux, aux_period, stream, pdl);
 }
 template <int kEpi>
 static int launch_epi(bool bf, int bn, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& to,
                       const void* bias, const void* aux, int M, int N, int K, int ld_aux, int aux_period,
-                      cudaStream_t stream) {
-  return bn == 128 ? launch_dt<kEpi, 128>(bf, ta, tb, to, bias, aux, M, N, K, ld_aux, aux_period, stream)
-                   : launch_dt<kEpi, 256>(bf, ta, tb, to, bias, aux, M, N, K, ld_aux, aux_period, stream);
+                      cudaStream_t stream, bool pdl) {
+  return bn == 128 ? launch_dt<kEpi, 128>(bf, ta, tb, to, bias, aux, M, N, K, ld_aux, aux_period, stream, pdl)
+                   : launch_dt<kEpi, 256>(bf, ta, tb, to, bias, aux, M, N, K, ld_aux, aux_period, stream, pdl);
 }
 
 }  // namespace gemm
@@ -314,21 +314,21 @@ int linear_tile_n(int M, int N) {
 // Internal entry used by the ViT engine as well (tensor maps can be cached by the caller).
 int linear_launch(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& to, const void* bias,
                   const void* aux, int M, int N, int K, int ld_aux, int epilogue, int aux_period, int dtype,
-                  cudaStream_t stream) {
+                  cudaStream_t stream, bool pdl) {
   using namespace gemm;
   const bool bf = dtype == FVS_BF16;
   const int bn = linear_tile_n(M, N);
   switch (epilogue) {
-    case FVS_EPI_BIAS: return launch_epi<FVS_EPI_BIAS>(bf, bn, ta, tb, to, bias, aux, M, N, K, ld_aux, aux_period, stream);
+    case FVS_EPI_BIAS: return launch_epi<FVS_EPI_BIAS>(bf, bn, ta, tb, to, bias, aux, M, N, K, ld_aux, aux_period, stream, pdl);
     case FVS_EPI_BIAS_QUICKGELU:
-      return launch_epi<FVS_EPI_BIAS_QUICKGELU>(bf, bn, ta, tb, to, bias, aux, M, N, K, ld_aux, aux_period, stream);
+      return launch_epi<FVS_EPI_BIAS_QUICKGELU>(bf, bn, ta, tb, to, bias, aux, M, N, K, ld_aux, aux_period, stream, pdl);
     case FVS_EPI_BIAS_RESIDUAL:
-      return launch_epi<FVS_EPI_BIAS_RESIDUAL>(bf, bn, ta, tb, to, bias, aux, M, N, K, ld_aux, aux_period, stream);
-    case FVS_EPI_ROWTABLE: return launch_epi<FVS_EPI_ROWTABLE>(bf, bn, ta, tb, to, bias, aux, M, N, K, ld_aux, aux_period, stream);
+      return launch_epi<FVS_EPI_BIAS_RESIDUAL>(bf, bn, ta, tb, to, bias, aux, M, N, K, ld_aux, aux_period, stream, pdl);
+    case FVS_EPI_ROWTABLE: return launch_epi<FVS_EPI_ROWTABLE>(bf, bn, ta, tb, to, bias, aux, M, N, K, ld_aux, aux_period, stream, pdl);
     case FVS_EPI_BIAS_RESIDUAL_F32:
-      return launch_epi<FVS_EPI_BIAS_RESIDUAL_F32>(bf, bn, ta, tb, to, bias, aux, M, N, K, ld_aux, aux_period, stream);
+      return launch_epi<FVS_EPI_BIAS_RESIDUAL_F32>(bf, bn, ta, tb, to, bias, aux, M, N, K, ld_aux, aux_period, stream, pdl);
     case FVS_EPI_BIAS_GELU:
-      return launch_epi<FVS_EPI_BIAS_GELU>(bf, bn, ta, tb, to, bias, aux, M, N, K, ld_aux, aux_period, stream);
+      return launch_epi<FVS_EPI_BIAS_GELU>(bf, bn, ta, tb, to, bias, aux, M, N, K, ld_aux, aux_period, stream, pdl);
   }
   return set_error(FVS_EINVAL, "fvs_linear: unknown epilogue %d", epilogue);
 }
@@ -371,5 +371,5 @@ extern "C" int fvs_linear(const void* A, const void* W, const void* bias, const 
     FVS_CUDA_OK(cudaMemcpy2DAsync(out, size_t(ldo) * 4, aux, size_t(ldo) * 4, size_t(N) * 4, size_t(M), cudaMemcpyDeviceToDevice,
                                   static_cast<cudaStream_t>(stream)));
   return linear_launch(ta, tb, to, bias, aux, M, N, K, ld_aux, epilogue, aux_period, dtype,
-                       static_cast<cudaStream_t>(stream));
+                       static_cast<cudaStream_t>(stream), /*pdl=*/true);
 }

@@ -14,6 +14,7 @@
 //   im2col -> linear(ROWTABLE: + pos/cls table) -> layernorm(pre) ->
 //   23 x [layernorm, linear(BIAS) qkv, attention, linear(BIAS_RESIDUAL_F32: x += out-proj),
 //         layernorm, linear(BIAS_QUICKGELU), linear(BIAS_RESIDUAL_F32: x += fc2)] -> drop_cls / pooled tail (x rounded once)
+// with everything between im2col and the tail run as two concurrent half-batches from kSplitMinRows rows on (stack_launches).
 // The residual adds live in the out-proj / fc2 epilogue as TMA reduce-add stores (the L2 performs x += acc + bias), so
 // the fp32 stream never enters an SM on that side and a LayerNorm only reads x and writes y: 6 B/element per LayerNorm
 // instead of 12.  Round 1's row-per-thread version of the epilogue (uncoalesced fp32 loads and stores) made out-proj
@@ -62,15 +63,16 @@ __global__ void vit_prepare_kernel(const uint16_t* __restrict__ patch_w, const u
 
 // Execution plan of one micro-batch shape on one workspace: every tensor map of the layer stack is encoded ONCE (279
 // cuTensorMapEncodeTiled calls per micro-batch otherwise), and from the second use on the whole layer stack — patch GEMM to
-// the last fc2, 209 launches for 23 layers — replays as ONE CUDA graph (captured from the very launches it replaces, PDL
-// edges included).  Only im2col (reads the caller's pixels) and the tail (writes the caller's output) stay outside, so the
-// graph depends on nothing but the workspace and the weights.  What this buys is host independence: a step is 3 driver
+// the last fc2, 209 launches for 23 layers, twice that as two half-batch branches — replays as ONE CUDA graph (captured from
+// the very launches it replaces, PDL edges and the branches' fork and join included).  Only im2col (reads the caller's
+// pixels) and the tail (writes the caller's output) stay outside, so the graph depends on nothing but the workspace and
+// the weights.  What this buys is host independence: a step is 3 driver
 // calls instead of ~500, which is what keeps 8 ranks on one host from starving their GPUs (SCALE_r01: 0.51 at N=8).
 struct VitPlan {
   const void* ws_base = nullptr;
   int nf = 0;
   std::vector<CUtensorMap> maps;      // in consumption order (see MapCursor)
-  fvs::AttnMaps attn;
+  fvs::AttnMaps attn[2];              // one per half-batch (only [0] without the split)
   bool maps_ready = false;
   cudaGraphExec_t exec = nullptr;
   cudaGraphExec_t exec_prof = nullptr;   // same launches with an external event-record node before and after every tensor-core kernel
@@ -90,6 +92,8 @@ struct fvs_vit {
   std::vector<VitPlan> plans;
   uint64_t clock = 0;
   cudaStream_t cap_stream = nullptr;   // capture happens here: the caller's stream may be the legacy default stream, which cannot capture
+  cudaStream_t side = nullptr;         // the second half-batch's stream (see stack_launches)
+  cudaEvent_t fork = nullptr, join = nullptr;
 };
 
 namespace {
@@ -172,37 +176,97 @@ struct MapCursor {
   }
 };
 
-// the layer stack of one micro-batch: patch GEMM (+pos/CLS table) -> pre_layrnorm -> layers_run x [...] (everything
-// between im2col and the tail); reads ws.patches, leaves the residual stream (fp32) in ws.x
-int stack_launches(fvs_vit* h, VitPlan& p, const Workspace& ws, int nf, cudaStream_t stream) {
+// Rows per micro-batch (frames x tokens) from which the layer stack runs as two concurrent half-batches
+// (stack_launches).  On an H100 the split is faster at every ViT-L/14-336 micro-batch measured, from 2 frames (2 x 577
+// rows) to 32 (DESIGN.md §4); smaller micro-batches (small towers) were not measured and stay whole.
+constexpr int kSplitMinRows = 2 * 577;
+
+// frames [f0, ..) of a micro-batch's workspace: the same buffers from the frame's first row on
+Workspace frames_from(const fvs_vit* h, const Workspace& ws, int f0) {
+  const size_t rows = size_t(f0) * h->tokens, H = h->cfg.hidden;
+  Workspace s = ws;
+  s.patches += rows * h->kpad * 2;
+  s.x += rows * H * 4;
+  s.y += rows * H * 2;
+  s.qkv += rows * 3 * H * 2;
+  s.ctx += rows * H * 2;
+  s.act += rows * size_t(h->cfg.mlp) * 2;
+  return s;
+}
+
+// one half-batch of the layer stack: its frames' rows of the workspace, its stream, its attention maps
+struct Branch {
+  Workspace ws;
+  int nf;
+  fvs::AttnMaps* attn;
+  cudaStream_t stream;
+};
+
+// stage -1: patch GEMM (+pos/CLS table) -> pre_layrnorm; stage l >= 0: layer l
+int stage_launches(fvs_vit* h, VitPlan& p, MapCursor& mc, const Branch& b, int l, bool pdl) {
   using namespace fvs;
   const fvs_vit_config& c = h->cfg;
-  const int H = c.hidden, T = h->tokens, dt = c.dtype, M = nf * T;
-  const float scale = 0.125f;  // head_dim^-0.5
-  MapCursor mc{p};
+  const int H = c.hidden, T = h->tokens, dt = c.dtype, M = b.nf * T;
+  const Workspace& ws = b.ws;
+  cudaStream_t stream = b.stream;
   const CUtensorMap *ta, *tb, *to;
   int r;
-  if ((r = mc.linear(ta, tb, to, ws.patches, h->patch_w_pad, ws.y, M, H, h->kpad))) return r;
-  if ((r = linear_launch(*ta, *tb, *to, nullptr, h->table, M, H, h->kpad, H, FVS_EPI_ROWTABLE, T, dt, stream))) return r;
-  if ((r = layernorm_launch(ws.y, h->w.pre_ln_w, h->w.pre_ln_b, ws.x, M, H, c.ln_eps, dt, false, true, nullptr, stream))) return r;
-  if (!p.maps_ready && (r = attention_make_maps(&p.attn, ws.qkv, ws.ctx, nf, T, c.heads))) return r;
-  for (int l = 0; l < c.layers_run; ++l) {
-    const fvs_vit_layer_weights& L = h->layers[l];
-    if ((r = layernorm_launch(ws.x, L.ln1_w, L.ln1_b, ws.y, M, H, c.ln_eps, dt, true, false, nullptr, stream))) return r;
-    if ((r = mc.linear(ta, tb, to, ws.y, L.qkv_w, ws.qkv, M, 3 * H, H))) return r;
-    if ((r = linear_launch(*ta, *tb, *to, L.qkv_b, nullptr, M, 3 * H, H, 3 * H, FVS_EPI_BIAS, 0, dt, stream))) return r;
-    if ((r = attention_launch(p.attn, nf, T, c.heads, scale, dt, stream))) return r;
-    // out-proj and fc2 add straight into the fp32 residual stream (TMA-staged in the GEMM epilogue), so a LayerNorm
-    // only reads x and writes y
-    if ((r = mc.linear(ta, tb, to, ws.ctx, L.o_w, ws.x, M, H, H, true))) return r;
-    if ((r = linear_launch(*ta, *tb, *to, L.o_b, ws.x, M, H, H, H, FVS_EPI_BIAS_RESIDUAL_F32, 0, dt, stream))) return r;
-    if ((r = layernorm_launch(ws.x, L.ln2_w, L.ln2_b, ws.y, M, H, c.ln_eps, dt, true, false, nullptr, stream))) return r;
-    if ((r = mc.linear(ta, tb, to, ws.y, L.fc1_w, ws.act, M, c.mlp, H))) return r;
-    if ((r = linear_launch(*ta, *tb, *to, L.fc1_b, nullptr, M, c.mlp, H, c.mlp, FVS_EPI_BIAS_QUICKGELU, 0, dt, stream)))
+  if (l < 0) {
+    if ((r = mc.linear(ta, tb, to, ws.patches, h->patch_w_pad, ws.y, M, H, h->kpad))) return r;
+    if ((r = linear_launch(*ta, *tb, *to, nullptr, h->table, M, H, h->kpad, H, FVS_EPI_ROWTABLE, T, dt, stream, pdl))) return r;
+    if ((r = layernorm_launch(ws.y, h->w.pre_ln_w, h->w.pre_ln_b, ws.x, M, H, c.ln_eps, dt, false, true, nullptr, stream, pdl)))
       return r;
-    if ((r = mc.linear(ta, tb, to, ws.act, L.fc2_w, ws.x, M, H, c.mlp, true))) return r;
-    if ((r = linear_launch(*ta, *tb, *to, L.fc2_b, ws.x, M, H, c.mlp, H, FVS_EPI_BIAS_RESIDUAL_F32, 0, dt, stream))) return r;
+    if (!p.maps_ready && (r = attention_make_maps(b.attn, ws.qkv, ws.ctx, b.nf, T, c.heads))) return r;
+    return FVS_OK;
   }
+  const float scale = 0.125f;  // head_dim^-0.5
+  const fvs_vit_layer_weights& L = h->layers[l];
+  if ((r = layernorm_launch(ws.x, L.ln1_w, L.ln1_b, ws.y, M, H, c.ln_eps, dt, true, false, nullptr, stream, pdl))) return r;
+  if ((r = mc.linear(ta, tb, to, ws.y, L.qkv_w, ws.qkv, M, 3 * H, H))) return r;
+  if ((r = linear_launch(*ta, *tb, *to, L.qkv_b, nullptr, M, 3 * H, H, 3 * H, FVS_EPI_BIAS, 0, dt, stream, pdl))) return r;
+  if ((r = attention_launch(*b.attn, b.nf, T, c.heads, scale, dt, stream, 64, pdl))) return r;
+  // out-proj and fc2 add straight into the fp32 residual stream (TMA-staged in the GEMM epilogue), so a LayerNorm
+  // only reads x and writes y
+  if ((r = mc.linear(ta, tb, to, ws.ctx, L.o_w, ws.x, M, H, H, true))) return r;
+  if ((r = linear_launch(*ta, *tb, *to, L.o_b, ws.x, M, H, H, H, FVS_EPI_BIAS_RESIDUAL_F32, 0, dt, stream, pdl))) return r;
+  if ((r = layernorm_launch(ws.x, L.ln2_w, L.ln2_b, ws.y, M, H, c.ln_eps, dt, true, false, nullptr, stream, pdl))) return r;
+  if ((r = mc.linear(ta, tb, to, ws.y, L.fc1_w, ws.act, M, c.mlp, H))) return r;
+  if ((r = linear_launch(*ta, *tb, *to, L.fc1_b, nullptr, M, c.mlp, H, c.mlp, FVS_EPI_BIAS_QUICKGELU, 0, dt, stream, pdl)))
+    return r;
+  if ((r = mc.linear(ta, tb, to, ws.act, L.fc2_w, ws.x, M, H, c.mlp, true))) return r;
+  if ((r = linear_launch(*ta, *tb, *to, L.fc2_b, ws.x, M, H, c.mlp, H, FVS_EPI_BIAS_RESIDUAL_F32, 0, dt, stream, pdl))) return r;
+  return FVS_OK;
+}
+
+// the layer stack of one micro-batch: patch GEMM (+pos/CLS table) -> pre_layrnorm -> layers_run x [...] (everything
+// between im2col and the tail); reads ws.patches, leaves the residual stream (fp32) in ws.x.
+// From kSplitMinRows rows on, frames [0, nf/2) and [nf/2, nf) run the whole stack as two independent chains, the second on
+// h->side, forked from and joined back into `stream` by events (captured, the graph has two parallel branches).  While
+// one half's GEMM drains its last wave or runs a LayerNorm, the other half's kernels take the idle SMs.  Every kernel is
+// row-wise or frame-wise and each output element's K sum runs in the same order whatever M is, so the split leaves every
+// bit as it was; the halves meet at a frame boundary, so the ROWTABLE row % tokens still holds, and each half's tensor
+// maps end at its last row, so neither half reads or writes the other's rows.
+int stack_launches(fvs_vit* h, VitPlan& p, const Workspace& ws, int nf, cudaStream_t stream) {
+  const bool split = nf >= 2 && nf * h->tokens >= kSplitMinRows;
+  const int n0 = split ? nf / 2 : nf;
+  Branch br[2] = {{ws, n0, &p.attn[0], stream}, {frames_from(h, ws, n0), nf - n0, &p.attn[1], h->side}};
+  const int nb = split ? 2 : 1;
+  // Split, the launches go without PDL: every kernel triggers its dependents on entry, so a same-half dependent would
+  // park its CTAs on exactly the SMs the other half should fill (measured slower at every micro-batch, DESIGN.md §4).
+  const bool pdl = !split;
+  if (split) {
+    FVS_CUDA_OK(cudaEventRecord(h->fork, stream));
+    FVS_CUDA_OK(cudaStreamWaitEvent(h->side, h->fork, 0));
+  }
+  MapCursor mc{p};
+  int r = FVS_OK;
+  for (int l = -1; l < h->cfg.layers_run && !r; ++l)   // issued layer by layer, alternating halves (matters eagerly only)
+    for (int b = 0; b < nb && !r; ++b) r = stage_launches(h, p, mc, br[b], l, pdl);
+  if (split) {   // joined even after a failed launch, so no work is left unordered behind the caller's stream
+    FVS_CUDA_OK(cudaEventRecord(h->join, h->side));
+    FVS_CUDA_OK(cudaStreamWaitEvent(stream, h->join, 0));
+  }
+  if (r) return r;
   p.maps_ready = true;
   return FVS_OK;
 }
@@ -267,9 +331,12 @@ int fvs_vit_create(fvs_vit_t* out, const fvs_vit_config* cfg, const fvs_vit_weig
   h->kpad = (h->kreal + 63) / 64 * 64;
   cudaError_t e = cudaMalloc(&h->patch_w_pad, size_t(cfg->hidden) * h->kpad * 2);
   if (e == cudaSuccess) e = cudaMalloc(&h->table, size_t(h->tokens) * cfg->hidden * 2);
+  if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&h->side, cudaStreamNonBlocking);
+  if (e == cudaSuccess) e = cudaEventCreateWithFlags(&h->fork, cudaEventDisableTiming);
+  if (e == cudaSuccess) e = cudaEventCreateWithFlags(&h->join, cudaEventDisableTiming);
   if (e != cudaSuccess) {
     fvs_vit_destroy(h);
-    return set_error(FVS_ECUDA, "fvs_vit_create: cudaMalloc: %s", cudaGetErrorString(e));
+    return set_error(FVS_ECUDA, "fvs_vit_create: %s", cudaGetErrorString(e));
   }
   vit_prepare_kernel<<<256, 256, 0, stream>>>((const uint16_t*)w->patch_w, (const uint16_t*)w->class_emb,
                                               (const uint16_t*)w->pos_emb, (uint16_t*)h->patch_w_pad,
@@ -291,6 +358,9 @@ int fvs_vit_destroy(fvs_vit_t h) {
   if (h->table) cudaFree(h->table);
   for (auto& p : h->plans) drop_plan(p);
   if (h->cap_stream) cudaStreamDestroy(h->cap_stream);
+  if (h->side) cudaStreamDestroy(h->side);
+  if (h->fork) cudaEventDestroy(h->fork);
+  if (h->join) cudaEventDestroy(h->join);
   delete h;
   return FVS_OK;
 }

@@ -154,7 +154,7 @@ __global__ void drop_cls_kernel(const float* __restrict__ x, const uint4* __rest
 }
 
 int layernorm_launch(const void* x, const void* gamma, const void* beta, void* y, int rows, int dim, float eps,
-                     int dtype, bool x_f32, bool y_f32, const void* delta, cudaStream_t stream) {
+                     int dtype, bool x_f32, bool y_f32, const void* delta, cudaStream_t stream, bool pdl) {
   if (delta != nullptr && !x_f32) return set_error(FVS_EINVAL, "layernorm: a residual delta needs an fp32 x");
   if (dim % 256 != 0 || dim > 2048) return set_error(FVS_EINVAL, "layernorm: dim %d must be a multiple of 256, <= 2048", dim);
   const int chunks = dim / 256;
@@ -163,7 +163,7 @@ int layernorm_launch(const void* x, const void* gamma, const void* beta, void* y
   const uint4* g = (const uint4*)gamma;
   const uint4* b = (const uint4*)beta;
 #define FVS_LN_LAUNCH(C, BF, XF, YF)                                                                                  \
-  FVS_CUDA_OK(launch_ex(layernorm_kernel<C, BF, XF, YF>, grid, block, 0, stream, 1, /*pdl=*/true, x, g, b, y, rows, eps, \
+  FVS_CUDA_OK(launch_ex(layernorm_kernel<C, BF, XF, YF>, grid, block, 0, stream, 1, pdl, x, g, b, y, rows, eps,          \
                         (const uint4*)delta))
 #define FVS_LN_CASE(C)                                             \
   case C:                                                          \
@@ -221,7 +221,7 @@ extern "C" int fvs_layernorm(const void* x, const void* gamma, const void* beta,
   FVS_REQUIRE((x_dtype == dtype || x_dtype == FVS_F32) && (y_dtype == dtype || y_dtype == FVS_F32),
               "fvs_layernorm: x/y dtype must be the parameter dtype or f32");
   return layernorm_launch(x, gamma, beta, y, rows, dim, eps, dtype, x_dtype == FVS_F32, y_dtype == FVS_F32, nullptr,
-                          static_cast<cudaStream_t>(stream));
+                          static_cast<cudaStream_t>(stream), /*pdl=*/true);
 }
 
 extern "C" int fvs_add_layernorm(void* x, const void* delta, const void* gamma, const void* beta, void* y, int rows,
@@ -230,5 +230,6 @@ extern "C" int fvs_add_layernorm(void* x, const void* delta, const void* gamma, 
   FVS_REQUIRE(x && delta && gamma && beta && y, "fvs_add_layernorm: null pointer");
   FVS_REQUIRE(rows > 0, "fvs_add_layernorm: rows must be > 0");
   FVS_REQUIRE(dtype == FVS_F16 || dtype == FVS_BF16, "fvs_add_layernorm: dtype must be f16 or bf16");
-  return layernorm_launch(x, gamma, beta, y, rows, dim, eps, dtype, true, false, delta, static_cast<cudaStream_t>(stream));
+  return layernorm_launch(x, gamma, beta, y, rows, dim, eps, dtype, true, false, delta, static_cast<cudaStream_t>(stream),
+                          /*pdl=*/true);
 }
