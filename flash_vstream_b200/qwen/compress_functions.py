@@ -118,28 +118,20 @@ class LazyMembers:
         return repr(self._get())
 
 
-def ordered_kmeans_enqueue(img_feature: torch.Tensor, video_max_frames: int, weights: torch.Tensor, init_idx: torch.Tensor,
-                           refill_idx: torch.Tensor, order: Optional[torch.Tensor] = None):
-    """The non-degenerate branch of weighted_kmeans_ordered_feature (:216-290: at least T0 distinct frames) enqueued without
-    a single host round trip: unique rows, the Lloyd loop, the timestamp / ordering bookkeeping (fvs_qwen_kmeans_finalize) and
-    the sorted gather all stay on the device.  init_idx int32 [T0] indexes the unique-row list like `unique_X[indices]`
-    (:219), refill_idx int32 [MAX_ITER * T0] are the candidate draws.  Returns a dict of device tensors:
-      feat [T0, P, D] (input dtype), weights / timestamps fp32 [T0], members (LazyMembers), and what the caller has to look
-      at ONCE, after everything it wants has been enqueued, to know the result is valid:
-      n_unique int32 [1] (must be >= T0, and == T when init_idx was drawn as randperm(T)), info int32 [4] ({last iteration,
-      refills consumed, converged, 0}), flags int32 [1] (empty clusters: ZeroDivisionError in the reference).
-    The one-request case of ordered_kmeans_enqueue_multi."""
-    outs, _ = ordered_kmeans_enqueue_multi([(img_feature, weights, init_idx, refill_idx, order)], video_max_frames)
-    return outs[0]
-
-
 def ordered_kmeans_enqueue_multi(reqs, video_max_frames: int, budget: int = 0):
-    """ordered_kmeans_enqueue for many streams at once (DESIGN.md §3.17): reqs = [(img_feature [T, P, D], weights [T],
-    init_idx, refill_idx, order or None)], each as ordered_kmeans_enqueue takes it.  The four kernels of the chain (unique
-    rows, Lloyd loop, finalize, ordered cast) run once per launch group for all streams; a stream's bits do not depend on
-    the other streams.  Returns (per stream the dict of ordered_kmeans_enqueue, readback) where readback is
-    a device int32 [n, 8] holding each stream's n_unique, info[4] and flags in columns 0, 1-4 and 5 (the dicts' n_unique,
-    info and flags are views of it), so the caller copies every stream's read-back at once."""
+    """The non-degenerate branch of weighted_kmeans_ordered_feature (:216-290: at least T0 distinct frames) for many
+    streams at once (DESIGN.md §3.17), enqueued without a single host round trip: unique rows, the Lloyd loop, the
+    timestamp / ordering bookkeeping (fvs_qwen_kmeans_finalize) and the sorted gather all stay on the device, and each of
+    those four kernels runs once per launch group for all streams; a stream's bits do not depend on the other streams.
+    reqs = [(img_feature [T, P, D], weights [T], init_idx, refill_idx, order or None)]: init_idx int32 [T0] indexes the
+    unique-row list like `unique_X[indices]` (:219), refill_idx int32 [MAX_ITER * T0] are the candidate draws.
+    Returns (outs, readback).  outs: per stream a dict of device tensors, feat [T0, P, D] (input dtype), weights /
+    timestamps fp32 [T0], members (LazyMembers), and what the caller has to look at ONCE, after everything it wants has
+    been enqueued, to know the result is valid: n_unique int32 [1] (must be >= T0, and == T when init_idx was drawn as
+    randperm(T)), info int32 [4] ({last iteration, refills consumed, converged, 0}), flags int32 [1] (empty clusters:
+    ZeroDivisionError in the reference).  readback: a device int32 [n, 8] holding each stream's n_unique, info[4] and
+    flags in columns 0, 1-4 and 5 (the dicts' n_unique, info and flags are views of it), so the caller copies every
+    stream's read-back at once."""
     n, K = len(reqs), int(video_max_frames)
     dev = reqs[0][0].device
     Ts = [r[0].shape[0] for r in reqs]

@@ -9,10 +9,11 @@ One `step` is one round over the listed streams, each with one clip:
      more than `TOWER_ROWS` rows is split into several calls (plan_tower_calls);
   4. ONE PatchMerger call merges every stream's new full-resolution frames;
   5. each stream's memory step is enqueued, the round waits ONCE for all their read-backs, and each stream is completed
-     (QwenStreamState.complete).  With batch_memory (the default), the CSM k-means of every stream past its CSM length
-     (unique rows, Lloyd loop, finalize, ordered cast) runs as ONE job table per kernel (fvs_qwen_*_multi, DESIGN.md
-     §3.17) between each stream's QwenStreamState.enqueue_input and enqueue_csm, and the round's read-backs land in one
-     pinned [S, 8] buffer with one copy; without it each stream runs QwenStreamState.enqueue on its own.
+     (QwenStreamState.complete).  Every stream runs QwenStreamState.enqueue_input; then ONE stream_state.enqueue_csm call
+     steps the CSM half of every stream past its CSM length (ordered k-means, klarge retrieval, DAM gather, PatchMerger
+     rows) as one job table per kernel (fvs_qwen_*_multi, DESIGN.md §3.17), and the round's read-backs land in one
+     pinned [S, 8] buffer with one copy.  A round of fewer than BATCH_MIN_JOBS such streams makes one one-item call per
+     stream instead, as a stream stepped alone does.
 
 Exact by construction: the tower is invariant to batch composition (§3.7) and the merger is row-wise (§3.5), so a pool
 stream gets the bits it gets alone through QwenStreamState with the same draws, however the round is composed or split.
@@ -28,10 +29,8 @@ from typing import Optional
 import torch
 
 from .. import _lib as L
-from . import compress_functions as CF
-from . import ops as Q
 from ..draws import DrawSource
-from .stream_state import _KMEANS_METHODS, QwenStreamState, check_device_frames
+from .stream_state import _KMEANS_METHODS, QwenStreamState, check_device_frames, enqueue_csm
 from .vision_tower import QwenVisionBlocksB200
 
 MAX_GRIDS = 16            # grid entries one fvs_qwen_vit_encode call takes
@@ -100,14 +99,13 @@ class QwenStreamPool:
     call (its workspace is about 30 KB per row at 1280 wide).  `preprocess` (a preprocess.Qwen2VLFramePreprocessor):
     `step` also takes decoded uint8 frames [T, H, W, 3] per stream (any mix of sizes, host or device); the round's clips
     go through ONE `preprocess.many` call, and each stream's rows and grid then make its (pixel_values_videos,
-    video_grid_thw).  `batch_memory=False` steps each stream's memory on its own (QwenStreamState.enqueue), the path
-    the batched one is measured and bisected against; both give the same bits."""
+    video_grid_thw)."""
 
     TOWER_ROWS = 65536
-    BATCH_MIN_JOBS = 4        # fewer k-means streams in a round take the single-stream memory calls
+    BATCH_MIN_JOBS = 4        # fewer k-means streams in a round take one enqueue_csm call each
 
     def __init__(self, model, device_frames: Optional[int] = None, max_streams: Optional[int] = None,
-                 small_device_frames: Optional[int] = None, preprocess=None, batch_memory: bool = True):
+                 small_device_frames: Optional[int] = None, preprocess=None):
         visual = model.visual
         flash, tower = visual.flash_memory, visual.encode_patches
         if not isinstance(tower, QwenVisionBlocksB200):
@@ -130,8 +128,7 @@ class QwenStreamPool:
         self.small_device_frames = check_device_frames(small_device_frames, "small_device_frames")
         self.max_streams = max_streams
         self.preprocess = preprocess
-        self.batch_memory = bool(batch_memory)
-        self._readbacks: Optional[torch.Tensor] = None     # pinned int32 [S, 8]: the batched round's read-backs
+        self._readbacks: Optional[torch.Tensor] = None     # pinned int32 [S, 8]: the round's read-backs
         self._streams: dict[int, _Stream] = {}
         self._next = 0
 
@@ -275,13 +272,13 @@ class QwenStreamPool:
         self._complete(sids)
 
     def _enqueue_memory(self, sids, items, feats, merged, draws) -> bool:
-        """every listed stream's memory step, enqueued; -> whether any stream reads back.  With batch_memory, the streams
-        whose clip needs the CSM k-means (past the CSM length) are collected and stepped together by _enqueue_csm; the
+        """every listed stream's memory step, enqueued; -> whether any stream reads back.  The streams whose clip needs
+        the CSM k-means (past the CSM length) are collected and stepped by one enqueue_csm call, or, in a round of fewer
+        than BATCH_MIN_JOBS of them, by one one-item call each (a job table does not pay off there, DESIGN.md §4); the
         others (memory still filling) run their pass-through inside enqueue_input.  Should a stream's enqueue_input
-        raise, the streams collected before it are enqueued first, so the round leaves every stream as the per-stream
-        mode would."""
-        pending = False
-        reqs = []                                      # (state, k-means request) of the batched round
+        raise, the streams collected before it are enqueued first, so the round leaves every stream as stepping each
+        stream alone would."""
+        reqs = []                                      # (state, k-means request) of the round
         try:
             for k, sid in enumerate(sids):
                 st = self._streams[sid]
@@ -289,70 +286,22 @@ class QwenStreamPool:
                 pub = st.__dict__.get("_qwen_publication")
                 if pub is not None and st.stream_state.n_frames == 0:
                     pub.new_stream()
-                args = (feats[k][0], feats[k][1], t, (h, w), (h // 2, w // 2), st.stream_state.n_frames)
-                if self.batch_memory:
-                    _, req = st.stream_state.enqueue_input(*args, draws=draws.get(sid), merged=merged[k])
-                    if req is not None:
-                        reqs.append((st.stream_state, req))
-                else:
-                    st.stream_state.enqueue(*args, draws=draws.get(sid), merged=merged[k])
-                pending = pending or bool(st.stream_state._pending)
+                _, req = st.stream_state.enqueue_input(feats[k][0], feats[k][1], t, (h, w), (h // 2, w // 2),
+                                                       st.stream_state.n_frames, draws=draws.get(sid), merged=merged[k])
+                if req is not None:
+                    reqs.append((st.stream_state, req))
         finally:
             if reqs:
-                self._enqueue_csm(reqs)
-        return pending or bool(reqs)
-
-    def _enqueue_csm(self, reqs):
-        """the rest of the memory step of the collected streams.  Fewer than BATCH_MIN_JOBS of them take the single-stream
-        calls (same bits; a job table does not pay off there, DESIGN.md §4); otherwise _enqueue_table"""
-        if len(reqs) < self.BATCH_MIN_JOBS:
-            for state, r in reqs:
-                state.enqueue_csm(r, CF.ordered_kmeans_enqueue(r["cand"], self.flash.temporal_length, r["cand_w"],
-                                                               r["init"], r["refill"], r["order"]))
-            return
-        self._enqueue_table(reqs)
-
-    def _enqueue_table(self, reqs):
-        """one job table per kernel for every listed stream: the CSM k-means, the klarge retrieval (streams whose
-        half-resolution bank is wholly in HBM; the others retrieve on their own), the DAM gather and ONE PatchMerger call
-        over every stream's CSM rows; then the one copy of all their read-backs"""
-        T0 = self.flash.temporal_length
-        kms, rb = CF.ordered_kmeans_enqueue_multi([(r["cand"], r["cand_w"], r["init"], r["refill"], r["order"])
-                                                   for _, r in reqs], T0)
-        n = len(reqs)
-        if self._readbacks is None or self._readbacks.shape[0] < n:
-            self._readbacks = torch.empty(max(n, 2 * (0 if self._readbacks is None else self._readbacks.shape[0])), 8,
-                                          dtype=torch.int32).pin_memory()
-        ctxs = []
-        for i, ((state, req), km) in enumerate(zip(reqs, kms)):
-            P, D = req["cand"].shape[1], req["cand"].shape[2]
-            ctxs.append((state, state._rest_retrieval(km["feat"].view(T0 * P, D), km["weights"], km["timestamps"], T0,
-                                                      km["members"], req["d"])))
-            state._set_pending(req, self._readbacks[i])
-        groups = {}                                    # one retrieval table per (metric, dtype)
-        for _, c in ctxs:
-            if c["retrieve"] is not None:
-                groups.setdefault((c["retrieve"][3], c["retrieve"][2].dtype), []).append(c)
-        for (metric, _), cs in groups.items():
-            for c, picks in zip(cs, Q.klarge_retrieve_multi([c["retrieve"][:3] for c in cs], metric)):
-                c["picks"] = picks
-        gathers, merges = {}, []
-        for state, c in ctxs:
-            g, m = state._rest_outputs(c)
-            if g is not None:
-                out = g["spa_x_out"] if g["spa_x_out"] is not None else g["merged_out"]
-                gathers.setdefault(out.dtype, []).append(g)
-            if m is not None:
-                merges.append(m)
-        for calls in gathers.values():
-            Q.dam_gather_multi(calls)
-        if merges:                                     # the merger is row-wise (§3.5): one call, the same bits per row
-            y = self.merger(torch.cat([x for x, _ in merges]) if len(merges) > 1 else merges[0][0])
-            r = 0
-            for x, out in merges:
-                out.copy_(y[r: r + out.shape[0]])
-                r += out.shape[0]
-        self._readbacks[:n].copy_(rb, non_blocking=True)
+                n = len(reqs)
+                if self._readbacks is None or self._readbacks.shape[0] < n:
+                    self._readbacks = torch.empty(max(n, 2 * (0 if self._readbacks is None else self._readbacks.shape[0])),
+                                                  8, dtype=torch.int32).pin_memory()
+                if n >= self.BATCH_MIN_JOBS:
+                    enqueue_csm(reqs, self._readbacks)
+                else:
+                    for i, item in enumerate(reqs):
+                        enqueue_csm([item], self._readbacks[i: i + 1])
+        return bool(reqs)
 
     def _complete(self, sids):
         """complete every enqueued stream of the round and publish it; then raise one error for those that raised"""

@@ -176,7 +176,7 @@ def klarge_retrieve_multi(items, metric: str = "euclidean", want_dist: bool = Fa
         keep.append((tem_x, klarge_idx, bank))
         sizes.append(_al(lib.fvs_qwen_klarge_workspace_bytes(klarge_idx.numel(), bank.shape[0], bank.shape[1])))
     dev = keep[0][0].device
-    ws = _workspace(sum(sizes), dev, "klarge_multi")
+    ws = _workspace(sum(sizes), dev, "klarge")         # klarge_retrieve's: a stream's bank may move between the two
     jobs, outs, o = [], [], 0
     for (tem_x, klarge_idx, bank), nb in zip(keep, sizes):
         k, t = klarge_idx.numel(), bank.shape[0]

@@ -124,12 +124,13 @@ class QwenStreamState:
                 draws: Optional[dict] = None, merged: Optional[torch.Tensor] = None):
         """The first half of step(): the clip's work up to and including the copy of its 32-byte read-back, enqueued on
         the current stream.  The caller waits until that copy has landed (an event recorded after it), then calls
-        complete().  Several states may be enqueued before one wait (QwenStreamPool).  = enqueue_input(), the CSM
-        k-means of its request (ordered_kmeans_enqueue), enqueue_csm()."""
+        complete().  = enqueue_input(), then enqueue_csm() of its request alone (QwenStreamPool enqueues the inputs of
+        many states and then one enqueue_csm() for all of them, before one wait)."""
         banks, req = self.enqueue_input(x_new, small_new, t, grid, small_grid, start_idx, draws, merged)
         if req is not None:
-            self.enqueue_csm(req, CF.ordered_kmeans_enqueue(req["cand"], self.flash.temporal_length, req["cand_w"],
-                                                            req["init"], req["refill"], req["order"]))
+            if self._readback is None:
+                self._readback = torch.empty(8, dtype=torch.int32).pin_memory()
+            enqueue_csm([(self, req)], self._readback.view(1, 8))
         return banks
 
     def enqueue_input(self, x_new: torch.Tensor, small_new: torch.Tensor, t: int, grid, small_grid, start_idx: int,
@@ -137,7 +138,7 @@ class QwenStreamState:
         """The clip up to the CSM k-means: banks, candidates and the k-means draws, taken from this state's draw source
         in the order step() takes them.  -> ((bank, small_bank), req): req is None when the clip needs no fast-path
         k-means (memory still filling, or a branch the synchronous path runs, which is then already enqueued); otherwise
-        the k-means to run (cand [T, P, D], cand_w, init, refill, order) before enqueue_csm(req, result)."""
+        the k-means to run (cand [T, P, D], cand_w, init, refill, order), which enqueue_csm() takes."""
         flash = self.flash
         dev, dt, D = x_new.device, x_new.dtype, x_new.shape[-1]
         h, w = grid
@@ -195,23 +196,6 @@ class QwenStreamState:
                    init=init_dev, refill=refill_dev, order=order_dev)
         return (bank, small_bank), req
 
-    def enqueue_csm(self, req: dict, km: dict, readback: Optional[torch.Tensor] = None):
-        """The rest of the clip once the CSM k-means of enqueue_input's `req` is enqueued (km: the dict of
-        ordered_kmeans_enqueue): DAM retrieval, merged memory and the read-back.  readback: a pinned int32 [8] row the
-        caller fills itself with km's n_unique, info and flags after its last kernel (QwenStreamPool copies every
-        stream's at once); None: this state copies its own."""
-        T0, P = self.flash.temporal_length, req["cand"].shape[1]
-        D = req["cand"].shape[2]
-        tem_x, tem_w, tem_ts = km["feat"].view(T0 * P, D), km["weights"], km["timestamps"]
-        self._enqueue_rest(tem_x, tem_w, tem_ts, T0, km["members"], req["d"])
-        # ---- the one read-back of the step
-        if readback is None:
-            if self._readback is None:
-                self._readback = torch.empty(8, dtype=torch.int32).pin_memory()
-            self._readback[:6].copy_(torch.cat([km["n_unique"], km["info"], km["flags"]]), non_blocking=True)
-            readback = self._readback
-        self._set_pending(req, readback)
-
     def _set_pending(self, req: dict, readback: torch.Tensor):
         """what complete() needs of the enqueued fast-path clip; readback: the row it reads"""
         keep = ("cand", "cand_w", "T", "d", "start_idx", "t", "snap", "own_refills")
@@ -246,24 +230,10 @@ class QwenStreamState:
         g = self.small_grid if small else self.grid
         return torch.tensor([n, g[0], g[1]])                    # host tensor: what the reference's list holds at rest
 
-    def _enqueue_rest(self, tem_x, tem_w, tem_ts, n_tem, members, d):
-        """DAM retrieval and the merged memory for a CSM that is already (being) computed; no host round trip for the
-        default spatial methods.  = _rest_retrieval, the retrieval it asks for, _rest_outputs, the gather and the merger
-        (QwenStreamPool runs the middle three as one job table each for all its streams)."""
-        ctx = self._rest_retrieval(tem_x, tem_w, tem_ts, n_tem, members, d)
-        if ctx["retrieve"] is not None:
-            centroids, heaviest, bank, metric = ctx["retrieve"]
-            ctx["picks"] = Q.klarge_retrieve(centroids, heaviest, bank, metric=metric)
-        gather, merge = self._rest_outputs(ctx)
-        if gather is not None:
-            Q.dam_gather(**gather)
-        if merge is not None:
-            self.merger(merge[0], out=merge[1])
-
     def _rest_retrieval(self, tem_x, tem_w, tem_ts, n_tem, members, d):
         """the CSM fields, and the DAM picks or, for a klarge retrieval over a bank wholly in HBM (k <= 64), what it
         needs: ctx["retrieve"] = (centroids [st, PD], heaviest int64 [k], bank [n, PD], metric); picks are then set by
-        the caller"""
+        _rest_stage"""
         flash = self.flash
         D = tem_x.shape[-1]
         n = self.n_frames
@@ -433,7 +403,7 @@ class QwenStreamState:
         ts_in = torch.arange(T, device=cand.device, dtype=torch.float32)      # accepted and ignored by the reference (:279)
         tem_x, tem_thw, tem_w, tem_ts, members = flash.temporal_compress(
             cand.reshape(T * P, D), self._thw(T, small=True), flash.temporal_length, cand_w, ts_in, draws={**d, "source": self.rng})
-        self._enqueue_rest(tem_x, tem_w, tem_ts, int(tem_thw[0]), members, d)
+        _rest_stage([(self, self._rest_retrieval(tem_x, tem_w, tem_ts, int(tem_thw[0]), members, d))])
 
     # ------------------------------------------------------------------------------------------------ checkpoint / restore
     # What a step reads: the three banks, the CSM (tem_x, weights; n_tem), n_frames and the grids; what as_list() and a
@@ -538,6 +508,58 @@ class QwenStreamState:
         return [self.tem_x, self._thw(self.n_tem, small=True), self.tem_weights, self.tem_timestamp,
                 self.spa_x, self._thw(n_spa), self.spa_positions,
                 x, self._thw(n), small, self._thw(n, small=True), ve, None if ve is None else ve.shape]
+
+
+def enqueue_csm(items, readbacks: torch.Tensor):
+    """The CSM half of the memory step of every (state, req) in `items`, req as QwenStreamState.enqueue_input returns
+    it, enqueued on the current stream: the ordered k-means as one job table per kernel, the DAM retrieval and the merged
+    memory (_rest_stage), then ONE copy of every read-back into rows [0, n) of `readbacks` (pinned int32 [>= n, 8]); the
+    complete() of items[i] reads row i.  The states share one FlashMemory config and one merger.  A stream stepped alone
+    is the one-item call (DESIGN.md §3.17)."""
+    T0 = items[0][0].flash.temporal_length
+    kms, rb = CF.ordered_kmeans_enqueue_multi([(r["cand"], r["cand_w"], r["init"], r["refill"], r["order"])
+                                               for _, r in items], T0)
+    ctxs = []
+    for i, ((state, req), km) in enumerate(zip(items, kms)):
+        P, D = req["cand"].shape[1], req["cand"].shape[2]
+        ctxs.append((state, state._rest_retrieval(km["feat"].view(T0 * P, D), km["weights"], km["timestamps"], T0,
+                                                  km["members"], req["d"])))
+        state._set_pending(req, readbacks[i])
+    _rest_stage(ctxs)
+    readbacks[: len(items)].copy_(rb, non_blocking=True)
+
+
+def _rest_stage(ctxs):
+    """DAM retrieval and merged memory of every (state, ctx of its _rest_retrieval) in `ctxs`, for CSMs already (being)
+    computed; no host round trip for the default spatial methods.  One klarge retrieval table per (metric, dtype) for
+    the contexts that ask for one (a bank with host rows has retrieved on its own), _rest_outputs, one DAM gather table
+    per dtype, and one PatchMerger call over every CSM slice: the merger is row-wise (§3.5), so each row gets its bits."""
+    groups = {}
+    for _, c in ctxs:
+        if c["retrieve"] is not None:
+            groups.setdefault((c["retrieve"][3], c["retrieve"][2].dtype), []).append(c)
+    for (metric, _), cs in groups.items():
+        for c, picks in zip(cs, Q.klarge_retrieve_multi([c["retrieve"][:3] for c in cs], metric)):
+            c["picks"] = picks
+    gathers, merges = {}, []
+    for state, c in ctxs:
+        g, m = state._rest_outputs(c)
+        if g is not None:
+            out = g["spa_x_out"] if g["spa_x_out"] is not None else g["merged_out"]
+            gathers.setdefault(out.dtype, []).append(g)
+        if m is not None:
+            merges.append(m)
+    for calls in gathers.values():
+        Q.dam_gather_multi(calls)
+    merger = ctxs[0][0].merger
+    if len(merges) == 1:
+        merger(merges[0][0], out=merges[0][1])
+    elif merges:
+        y = merger(torch.cat([x for x, _ in merges]))
+        r = 0
+        for x, out in merges:
+            out.copy_(y[r: r + out.shape[0]])
+            r += out.shape[0]
 
 
 def _on_host(rb: RowBank, chunks, n: int, row_shape, dt) -> torch.Tensor:

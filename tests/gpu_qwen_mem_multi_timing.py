@@ -1,6 +1,6 @@
-"""Timing script (not a pytest file): the memory part of a QwenStreamPool round with the CSM chain batched over the
-streams (batch_memory=True: one job table per kernel, DESIGN.md §3.17) against each stream's own memory step
-(batch_memory=False), same tower, same clips.
+"""Timing script (not a pytest file): the memory part of a QwenStreamPool round with the CSM half batched over the
+streams (the default BATCH_MIN_JOBS: one job table per kernel, DESIGN.md §3.17) against a pool whose BATCH_MIN_JOBS is
+above S, so each stream steps its memory in a one-item call, as it does alone; same tower, same clips.
 
 Setup and windows of gpu_qwen_multistream_timing.py: 336 px, the 32-layer tower (seeded weights, bf16), the default
 Flash Memory (CSM 60 frames, DAM 30), single-patch clips, memory full (64 warm-up rounds).  Both modes alternate window
@@ -62,7 +62,9 @@ def main():
             return out
 
     def make(S, batch):
-        pool = QwenStreamPool(host, batch_memory=batch)
+        pool = QwenStreamPool(host)
+        if not batch:
+            pool.BATCH_MIN_JOBS = S + 1
         pool.tower = Timed(tower)
         sids = [pool.open(seed=100 + i) for i in range(S)]
 
@@ -92,7 +94,8 @@ def main():
                 tot[name][1] += sum(x.elapsed_time(y) for x, y in spans)
                 tot[name][2] += 4
             r += 4
-        row = {"S": S}
+        row = {"S": S, "batched_batch_min_jobs": made["batched"][0].BATCH_MIN_JOBS,
+               "per_stream_batch_min_jobs": made["per_stream"][0].BATCH_MIN_JOBS}
         for name, (ms, tower_ms, n) in tot.items():
             row[f"{name}_ms_per_round"] = ms / n
             row[f"{name}_tower_ms_per_round"] = tower_ms / n

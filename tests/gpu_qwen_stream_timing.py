@@ -91,7 +91,7 @@ def measure(depth=None, t_clip=None, steps=None, breakdown=True, prefill_patches
         return r
     host.visual.forward_simple_not_merge = timed_fsm
     from flash_vstream_b200.qwen import compress_functions as CF
-    orig_km, orig_se, orig_mg = CF.ordered_kmeans_enqueue, host.visual.flash_memory.spatial_enhance, host.visual.merger.forward
+    orig_km, orig_se, orig_mg = CF.ordered_kmeans_enqueue_multi, host.visual.flash_memory.spatial_enhance, host.visual.merger.forward
 
     def wrap(fn, key):
         def f(*a, **k):
@@ -100,7 +100,7 @@ def measure(depth=None, t_clip=None, steps=None, breakdown=True, prefill_patches
             torch.cuda.synchronize(); marks[key] = marks.get(key, 0.0) + (time.perf_counter() - t0) * 1e3
             return r
         return f
-    CF.ordered_kmeans_enqueue = wrap(orig_km, "temporal_compress")        # the k-means of the CSM (stream_state.py)
+    CF.ordered_kmeans_enqueue_multi = wrap(orig_km, "temporal_compress")  # the k-means of the CSM (stream_state.py)
     host.visual.flash_memory.spatial_enhance = wrap(orig_se, "spatial_enhance")
     host.visual.merger.forward = wrap(orig_mg, "merger")
     acc = {}
@@ -109,7 +109,7 @@ def measure(depth=None, t_clip=None, steps=None, breakdown=True, prefill_patches
         host.embed_new_video_clip(clips[s], thw, s * t_clip)
         for k, v in marks.items():
             acc.setdefault(k, []).append(v)
-    CF.ordered_kmeans_enqueue = orig_km
+    CF.ordered_kmeans_enqueue_multi = orig_km
     out["breakdown_ms_synchronised"] = {k: float(np.median(v)) for k, v in acc.items()}   # merger = new frames + CSM rows
     return out
 

@@ -110,4 +110,4 @@ def run(pool, alone, rounds, tag, others=()):
             alone[sid].step(c)
         for p in (pool, *others):
             for sid in alone:
-                Alone.compare(p.state(sid), alone[sid].st, (tag, r, sid, p.batch_memory))
+                Alone.compare(p.state(sid), alone[sid].st, (tag, r, sid, p.BATCH_MIN_JOBS))

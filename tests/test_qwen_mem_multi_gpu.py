@@ -2,8 +2,9 @@
 
 ABI level: random jobs of different T, K, PD, dtypes, draws, iteration caps and tolerances go once through each
 fvs_qwen_*_multi entry point and once through the single-stream calls; every output must be torch.equal, whatever the
-budget (down to one job per launch group).  Pool level: QwenStreamPool(batch_memory=True) against the same streams
-stepped alone through QwenStreamState, and against batch_memory=False, bit for bit after every round."""
+budget (down to one job per launch group).  Pool level: QwenStreamPool against the same streams stepped alone through
+QwenStreamState, and against a pool whose BATCH_MIN_JOBS is above its stream count (every k-means stream steps its
+memory in a one-item call), bit for bit after every round."""
 import random
 
 import pytest
@@ -248,13 +249,15 @@ def test_dam_gather_multi_equals_single_calls(lib):
 def pool_run(rt, tower, merger, S, rounds_n=8, method="klarge_retrieve", ts=(1, 2, 8), caps=None, grids=None, seed=0,  # noqa: F811
              temporal_method=None, **kw):
     """S streams opened over the first rounds (half at round 0, the rest at round 3) in a batched and a per-stream
-    pool, random clip lengths, some streams sitting rounds out; caps: small_device_frames per stream (cycled)"""
+    pool (BATCH_MIN_JOBS above S: one-item calls only), random clip lengths, some streams sitting rounds out; caps:
+    small_device_frames per stream (cycled)"""
     from flash_vstream_b200.qwen import QwenStreamPool
     host = host_for(rt, tower, merger, method=method)
     if temporal_method is not None:
         host.visual.flash_memory.temporal_method = temporal_method
-    pool, per_stream = QwenStreamPool(host, **kw), QwenStreamPool(host, batch_memory=False, **kw)
+    pool, per_stream = QwenStreamPool(host, **kw), QwenStreamPool(host, **kw)
     pool.BATCH_MIN_JOBS = 2                                       # job tables from two k-means streams on
+    per_stream.BATCH_MIN_JOBS = S + 1                             # every k-means stream alone
     r = random.Random(seed)
     alone = {}
     for k in range(rounds_n):
@@ -272,40 +275,40 @@ def pool_run(rt, tower, merger, S, rounds_n=8, method="klarge_retrieve", ts=(1, 
 
 
 @pytest.mark.parametrize("S", [1, 2, 5, 16, 32])
-def test_pool_batched_memory_equals_streams_alone(rt, tower, merger, S):  # noqa: F811
-    from flash_vstream_b200.qwen import multistream as MS
-    calls = {"kmeans": 0, "retrieve": 0, "gather": 0}
-    orig = (MS.CF.ordered_kmeans_enqueue_multi, MS.Q.klarge_retrieve_multi, MS.Q.dam_gather_multi)
+def test_pool_memory_equals_streams_alone(rt, tower, merger, S):  # noqa: F811
+    from flash_vstream_b200.qwen import stream_state as SS
+    calls = {"kmeans": 0, "retrieve": 0, "gather": 0}               # calls with more than one job
+    orig = (SS.CF.ordered_kmeans_enqueue_multi, SS.Q.klarge_retrieve_multi, SS.Q.dam_gather_multi)
 
     def spy(name, fn):
-        def f(*a, **k):
-            calls[name] += 1
-            return fn(*a, **k)
+        def f(jobs, *a, **k):
+            calls[name] += len(jobs) > 1
+            return fn(jobs, *a, **k)
         return f
-    MS.CF.ordered_kmeans_enqueue_multi = spy("kmeans", orig[0])
-    MS.Q.klarge_retrieve_multi = spy("retrieve", orig[1])
-    MS.Q.dam_gather_multi = spy("gather", orig[2])
+    SS.CF.ordered_kmeans_enqueue_multi = spy("kmeans", orig[0])
+    SS.Q.klarge_retrieve_multi = spy("retrieve", orig[1])
+    SS.Q.dam_gather_multi = spy("gather", orig[2])
     try:
         pool, sids = pool_run(rt, tower, merger, S, rounds_n=9 if S < 32 else 7)
     finally:
-        MS.CF.ordered_kmeans_enqueue_multi, MS.Q.klarge_retrieve_multi, MS.Q.dam_gather_multi = orig
+        SS.CF.ordered_kmeans_enqueue_multi, SS.Q.klarge_retrieve_multi, SS.Q.dam_gather_multi = orig
     assert any(pool.state(s).fast_steps for s in sids)
-    if S >= 5:                                                    # the job tables ran, not only the lone-stream calls
+    if S >= 5:                                                    # the job tables ran, not only the one-item calls
         assert min(calls.values()) > 0, calls
 
 
 @pytest.mark.parametrize("method", ["klarge_retrieve", "klarge_retrieve_cos"])
-def test_pool_methods_grids_and_clip_lengths(rt, tower, merger, method):  # noqa: F811
+def test_pool_memory_methods_grids_and_clip_lengths(rt, tower, merger, method):  # noqa: F811
     pool_run(rt, tower, merger, 5, method=method, ts=(1, 8), grids=[(8, 8), (8, 16)], seed=3)
 
 
-def test_pool_fast_kmeans_and_capped_banks(rt, tower, merger):  # noqa: F811
+def test_pool_memory_fast_kmeans_and_capped_banks(rt, tower, merger):  # noqa: F811
     pool, sids = pool_run(rt, tower, merger, 4, rounds_n=8, seed=5, temporal_method="fast_kmeans_ordered", device_frames=0,
                           caps=[None, 2])
     assert any(pool.state(s).n_small_host for s in sids) and not all(pool.state(s).n_small_host for s in sids)
 
 
-def test_pool_duplicate_rows_redo(rt, tower, merger):  # noqa: F811
+def test_pool_memory_duplicate_rows_redo(rt, tower, merger):  # noqa: F811
     from flash_vstream_b200.qwen import QwenStreamPool
     host = host_for(rt, tower, merger)
     pool = QwenStreamPool(host)
@@ -318,7 +321,7 @@ def test_pool_duplicate_rows_redo(rt, tower, merger):  # noqa: F811
     assert pool.state(1).redone_steps == 1 and pool.state(0).redone_steps == 0
 
 
-def test_pool_real_tower_336(rt, merger):  # noqa: F811
+def test_pool_memory_real_tower_336(rt, merger):  # noqa: F811
     """the 32-layer tower at 336 px and the default memory (CSM 60, DAM 30): 3 streams past the CSM length"""
     from flash_vstream_b200.qwen import QwenStreamPool
     from flash_vstream_b200.qwen.vision_tower import QwenVisionBlocksB200

@@ -205,7 +205,7 @@ class FakeState:
     """a stream whose enqueue_input asks for the k-means when `full` (else runs its pass-through), or raises"""
 
     def __init__(self, full, fail=False):
-        self.full, self.fail, self._pending, self.n_frames, self.enqueued = full, fail, None, 5, []
+        self.full, self.fail, self._pending, self.n_frames = full, fail, None, 5
 
     def enqueue_input(self, *a, draws=None, merged=None):
         if self.fail:
@@ -213,17 +213,16 @@ class FakeState:
         self._pending = {}
         return (None, None), (dict(me=self) if self.full else None)
 
-    def enqueue_csm(self, req, km):
-        self.enqueued.append(km)
 
-
-def fake_pool(states, min_jobs=4):
-    from flash_vstream_b200.qwen.multistream import QwenStreamPool, _Stream
-    pool = QwenStreamPool.__new__(QwenStreamPool)
-    pool.batch_memory, pool.BATCH_MIN_JOBS = True, min_jobs
-    pool._streams = {i: _Stream(None, st) for i, st in enumerate(states)}
-    pool.tables = []
-    pool._enqueue_table = lambda reqs: pool.tables.append([r["me"] for _, r in reqs])
+def fake_pool(monkeypatch, states, min_jobs=4):
+    """a pool of FakeStates whose enqueue_csm calls are recorded as ([state, ...], readbacks)"""
+    from flash_vstream_b200.qwen import multistream as MS
+    pool = MS.QwenStreamPool.__new__(MS.QwenStreamPool)
+    pool.BATCH_MIN_JOBS = min_jobs
+    pool._streams = {i: MS._Stream(None, st) for i, st in enumerate(states)}
+    pool._readbacks = torch.zeros(8, 8, dtype=torch.int32)     # pinned in a real pool; large enough not to grow here
+    pool.calls = []
+    monkeypatch.setattr(MS, "enqueue_csm", lambda items, rb: pool.calls.append(([r["me"] for _, r in items], rb)))
     return pool
 
 
@@ -231,34 +230,27 @@ def args(n):
     return list(range(n)), [(None, 1, 8, 8)] * n, [(None, None)] * n, [None] * n, {}
 
 
-def test_pool_collects_only_streams_past_the_csm_length():
+def test_pool_enqueues_only_streams_past_the_csm_length(monkeypatch):
     states = [FakeState(full=f) for f in (True, False, True, True, False, True)]
-    pool = fake_pool(states)
+    pool = fake_pool(monkeypatch, states)
     assert pool._enqueue_memory(*args(6))
-    assert pool.tables == [[states[0], states[2], states[3], states[5]]]
+    assert len(pool.calls) == 1 and pool.calls[0][0] == [states[0], states[2], states[3], states[5]]
+    assert pool.calls[0][1] is pool._readbacks
 
 
-def test_small_rounds_take_the_single_stream_calls(monkeypatch):
-    from flash_vstream_b200.qwen import multistream as MS
-    monkeypatch.setattr(MS.CF, "ordered_kmeans_enqueue", lambda *a: "km")
-    monkeypatch.setattr(MS.QwenStreamPool, "flash", type("F", (), {"temporal_length": 4})(), raising=False)
+def test_small_rounds_make_one_item_calls(monkeypatch):
+    """under BATCH_MIN_JOBS k-means streams: one one-item call per stream, the call a stream stepped alone makes"""
     states = [FakeState(full=f) for f in (True, False, True)]
-    pool = fake_pool(states)
-    orig = FakeState.enqueue_input
-
-    def with_fields(self, *a, **k):
-        banks, req = orig(self, *a, **k)
-        if req is not None:
-            req.update(cand=None, cand_w=None, init=None, refill=None, order=None)
-        return banks, req
-    monkeypatch.setattr(FakeState, "enqueue_input", with_fields)
+    pool = fake_pool(monkeypatch, states)
     pool._enqueue_memory(*args(3))
-    assert pool.tables == [] and states[0].enqueued == ["km"] and states[2].enqueued == ["km"] and not states[1].enqueued
+    assert [c[0] for c in pool.calls] == [[states[0]], [states[2]]]
+    for i, (_, rb) in enumerate(pool.calls):                     # each stream its own row of the round's read-backs
+        assert rb.shape == (1, 8) and rb.data_ptr() == pool._readbacks[i].data_ptr()
 
 
-def test_a_failing_stream_leaves_the_collected_ones_enqueued():
+def test_a_failing_stream_still_enqueues_the_collected_ones(monkeypatch):
     states = [FakeState(full=True), FakeState(full=True), FakeState(full=True, fail=True), FakeState(full=True)]
-    pool = fake_pool(states, min_jobs=1)
+    pool = fake_pool(monkeypatch, states, min_jobs=1)
     with pytest.raises(RuntimeError, match="enqueue_input failed"):
         pool._enqueue_memory(*args(4))
-    assert pool.tables == [[states[0], states[1]]]   # the streams before the failing one, as the per-stream mode leaves them
+    assert [c[0] for c in pool.calls] == [[states[0], states[1]]]   # the streams before the failing one
