@@ -93,6 +93,23 @@ class QwenGatherJob(C.Structure):  # fvs_qwen_gather_job
                 ("merged_out", C.c_void_p), ("host_fetches", C.c_void_p)]
 
 
+class QwenPickPlanJob(C.Structure):  # fvs_qwen_pick_plan_job
+    _fields_ = [("picks", C.c_void_p), ("n", C.c_int), ("n_frames", C.c_int64), ("encoded", C.c_void_p),
+                ("plan", C.c_void_p), ("count", C.c_void_p)]
+
+
+class QwenPixelJob(C.Structure):  # fvs_qwen_pixel_job
+    _fields_ = [("plan", C.c_void_p), ("n", C.c_int), ("n_frames", C.c_int64), ("base", C.c_int64),
+                ("host_chunks", C.c_void_p), ("chunk_frames", C.c_int), ("frame_elems", C.c_int64), ("out", C.c_void_p)]
+
+
+class QwenScatterJob(C.Structure):  # fvs_qwen_scatter_job
+    _fields_ = [("plan", C.c_void_p), ("n", C.c_int), ("n_frames", C.c_int64), ("x_rows", C.c_void_p),
+                ("merged_rows", C.c_void_p), ("dev_x", C.c_void_p), ("dev_merged", C.c_void_p), ("n_dev", C.c_int64),
+                ("host_chunks", C.c_void_p), ("chunk_frames", C.c_int), ("x_frame_elems", C.c_int64),
+                ("merged_frame_elems", C.c_int64)]
+
+
 QWEN_MEM_JOBS_PER_LAUNCH = 16
 PRE_CLIP, PRE_QWEN = 0, 1
 KLARGE_EUCLIDEAN, KLARGE_COSINE = 0, 1
@@ -173,6 +190,10 @@ SIGNATURES = {
     "fvs_qwen_dam_gather": (_i, [_vp, _i, C.c_int64, _vp, _vp, C.c_int64, _vp, _i, _vp, _i, _vp, _vp, C.c_int64, C.c_int64,
                                  _i, _vp, _vp, _vp, _vp]),
     "fvs_host_device_ptr": (_i, [_vp, C.POINTER(_vp)]),
+    # lazy full-resolution bank
+    "fvs_qwen_pick_plan_multi": (_i, [C.POINTER(QwenPickPlanJob), _i, _vp]),
+    "fvs_qwen_pixel_gather_multi": (_i, [C.POINTER(QwenPixelJob), _i, _i, _vp]),
+    "fvs_qwen_bank_scatter_multi": (_i, [C.POINTER(QwenScatterJob), _i, _i, _vp]),
     # publication of the Qwen2-VL streaming memory (seqlock)
     "fvs_qwen_pub_layout": (_i, [_i, _i, _i, _i, _i, _i, _i, _i64p]),
     "fvs_qwen_publish": (_i, [_vp, _sz, _i, _i, C.c_int64, _i, _vp, C.c_int64, _vp, _i, _vp, _i, _i, _i, _i, _i, C.c_uint64,

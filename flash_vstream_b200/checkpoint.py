@@ -115,6 +115,9 @@ class StreamCheckpoint:
             out["bank_merged"] = ((n["n_frames"], h * w // 4, md), dt)
         if md is not None:
             out["video_embeds"] = ((n["n_spa"] * h * w // 4 + n["n_tem"] * hs * ws // 4, md), dt)
+        if "pix_frames" in n:                         # a lazy_full_res stream: its mask, the pixel rows of its frames not yet encoded
+            out["encoded"] = ((n["n_frames"],), torch.uint8)
+            out["pixels"] = ((n["pix_frames"], h * w, 3 * 2 * 14 * 14), dt)
         return out
 
     def _check(self):

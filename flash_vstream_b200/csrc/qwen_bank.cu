@@ -28,7 +28,7 @@ __device__ __forceinline__ void dam_gather_body(
     const uint4 *sx = nullptr, *sm = nullptr;
     if (p >= 0 && p < n_frames) {
       if (p < n_dev) {
-        sx = dev_x + p * fx;
+        sx = dev_x ? dev_x + p * fx : nullptr;      // no device tier (the pixel store): zeros
         sm = dev_m ? dev_m + p * fm : nullptr;
       } else {
         int j = 0;
@@ -187,6 +187,134 @@ int dam_gather_jobs(const char* api, const fvs_qwen_gather_job* jobs, int n_jobs
   }
   return FVS_OK;
 }
+
+// ---- lazy full-resolution bank (DESIGN.md §3.18) --------------------------------------------------------------------
+// Pick plan: one warp per job walks the picks in order, 32 at a time.  A pick is planned when it is in range, its frame's
+// mask bit is clear and no earlier pick names the same frame; the warp's ballot compacts the planned frames in pick order.
+// The mask bit of a planned frame is set by the lane that planned it; a later pick of that frame is never planned again,
+// whether or not it sees the bit, because it is not the first pick of its frame.
+struct PlanJobDev {
+  const long long* picks;
+  unsigned char* encoded;
+  long long* plan;
+  int* count;
+  long long n_frames;
+  int n;
+};
+template <int kJobs>
+struct PlanLaunch {
+  PlanJobDev job[kJobs];
+};
+template <int kJobs>
+__global__ void __launch_bounds__(32) pick_plan_kernel(const __grid_constant__ PlanLaunch<kJobs> L) {
+  const PlanJobDev& J = L.job[blockIdx.x];
+  const unsigned lane = threadIdx.x;
+  int base = 0;
+  for (int i0 = 0; i0 < J.n; i0 += 32) {
+    const int i = i0 + int(lane);
+    long long p = -1;
+    bool first = false;
+    if (i < J.n) {
+      p = J.picks ? J.picks[i] : i;
+      first = p >= 0 && p < J.n_frames && !J.encoded[p];
+      if (first && J.picks)
+        for (int j = 0; j < i; ++j)
+          if (J.picks[j] == p) { first = false; break; }
+    }
+    const unsigned ball = __ballot_sync(0xffffffffu, first);
+    if (first) {
+      J.plan[base + __popc(ball & ((1u << lane) - 1u))] = p;
+      J.encoded[p] = 1;
+    }
+    base += __popc(ball);
+  }
+  if (lane == 0) *J.count = base;
+}
+
+template <int kJobs>
+int pick_plan_launch(const fvs_qwen_pick_plan_job* jobs, int n, cudaStream_t stream) {
+  PlanLaunch<kJobs> L;
+  for (int q = 0; q < n; ++q)
+    L.job[q] = PlanJobDev{(const long long*)jobs[q].picks, jobs[q].encoded, (long long*)jobs[q].plan, (int*)jobs[q].count,
+                          (long long)jobs[q].n_frames, jobs[q].n};
+  pick_plan_kernel<kJobs><<<n, 32, 0, stream>>>(L);
+  FVS_CHECK_LAUNCH("pick_plan_kernel");
+  return FVS_OK;
+}
+
+// Bank scatter: the reverse of the DAM gather without its previous-DAM source.  Job j's block b writes share b % bx of
+// planned frame b / bx: x words first, then merged words, to the device tier or the frame's host chunk.
+struct ScatterJobDev {
+  const long long* plan;
+  const uint4* src_x;
+  const uint4* src_m;
+  uint4* dev_x;
+  uint4* dev_m;
+  uint4* const* chunks;
+  long long n_frames, n_dev, chunk_frames, fx, fm;
+  int bx;
+};
+template <int kJobs>
+struct ScatterLaunch {
+  ScatterJobDev job[kJobs];
+  int first[kJobs + 1];
+  int n;
+};
+template <int kJobs>
+__global__ void __launch_bounds__(256) bank_scatter_kernel(const __grid_constant__ ScatterLaunch<kJobs> L) {
+  int j = 0;
+  if constexpr (kJobs > 1)
+    while (j + 1 < L.n && blockIdx.x >= unsigned(L.first[j + 1])) ++j;
+  const ScatterJobDev& J = L.job[j];
+  const unsigned b = blockIdx.x - unsigned(L.first[j]), bx = b % unsigned(J.bx);
+  const long long i = b / unsigned(J.bx);
+  __shared__ uint4* dst[2];
+  if (threadIdx.x == 0) {
+    const long long p = J.plan[i];
+    uint4 *dx = nullptr, *dm = nullptr;
+    if (p >= 0 && p < J.n_frames) {
+      if (p < J.n_dev) {
+        dx = J.dev_x + p * J.fx;
+        dm = J.dev_m ? J.dev_m + p * J.fm : nullptr;
+      } else {
+        const long long q = p - J.n_dev, off = q % J.chunk_frames;
+        uint4* c = J.chunks[q / J.chunk_frames];
+        dx = c + off * J.fx;
+        dm = c + J.chunk_frames * J.fx + off * J.fm;
+      }
+    }
+    dst[0] = dx;
+    dst[1] = J.src_m ? dm : nullptr;
+  }
+  __syncthreads();
+  uint4 *dx = dst[0], *dm = dst[1];
+  if (!dx) return;
+  const long long total = J.fx + (dm ? J.fm : 0), stride = (long long)J.bx * blockDim.x;
+  for (long long w = (long long)bx * blockDim.x + threadIdx.x; w < total; w += stride) {
+    if (w < J.fx) dx[w] = J.src_x[i * J.fx + w];
+    else dm[w - J.fx] = J.src_m[i * J.fm + (w - J.fx)];
+  }
+}
+
+template <int kJobs>
+int bank_scatter_launch(const fvs_qwen_scatter_job* jobs, int n, cudaStream_t stream) {
+  ScatterLaunch<kJobs> L;
+  L.n = n;
+  L.first[0] = 0;
+  for (int q = 0; q < n; ++q) {
+    const fvs_qwen_scatter_job& s = jobs[q];
+    const long long fx = s.x_frame_elems * 2 / 16, fm = s.merged_frame_elems * 2 / 16;
+    long long bx = (fx + (s.merged_rows ? fm : 0) + 4 * 256 - 1) / (4 * 256);
+    bx = bx > 64 ? 64 : bx < 1 ? 1 : bx;
+    L.job[q] = ScatterJobDev{(const long long*)s.plan, (const uint4*)s.x_rows, (const uint4*)s.merged_rows, (uint4*)s.dev_x,
+                             (uint4*)s.dev_merged, (uint4* const*)s.host_chunks, (long long)s.n_frames, (long long)s.n_dev,
+                             (long long)s.chunk_frames, fx, fm, int(bx)};
+    L.first[q + 1] = L.first[q] + int(bx) * s.n;
+  }
+  bank_scatter_kernel<kJobs><<<L.first[n], 256, 0, stream>>>(L);
+  FVS_CHECK_LAUNCH("bank_scatter_kernel");
+  return FVS_OK;
+}
 }  // namespace
 
 extern "C" {
@@ -213,6 +341,89 @@ int fvs_qwen_dam_gather(const int64_t* picks, int n, int64_t n_frames, const voi
 
 int fvs_qwen_dam_gather_multi(const fvs_qwen_gather_job* jobs_h, int n_jobs, int dtype, fvs_stream_t stream) {
   return dam_gather_jobs("fvs_qwen_dam_gather_multi", jobs_h, n_jobs, dtype, (cudaStream_t)stream, true);
+}
+
+int fvs_qwen_pick_plan_multi(const fvs_qwen_pick_plan_job* jobs, int n_jobs, fvs_stream_t stream) {
+  const char* api = "fvs_qwen_pick_plan_multi";
+  FVS_REQUIRE(jobs && n_jobs > 0, "%s: need a job table and n_jobs > 0", api);
+  for (int i = 0; i < n_jobs; ++i) {
+    const fvs_qwen_pick_plan_job& j = jobs[i];
+    FVS_REQUIRE(j.n >= 0 && j.n_frames >= 0 && (j.picks || j.n <= j.n_frames), "%s: job %d: bad sizes (n=%d, n_frames=%lld)",
+                api, i, j.n, (long long)j.n_frames);
+    FVS_REQUIRE(j.encoded && j.count && (j.plan || j.n == 0), "%s: job %d: null mask, plan or count", api, i);
+    FVS_REQUIRE(((uintptr_t)j.picks & 7) == 0 && ((uintptr_t)j.plan & 7) == 0 && ((uintptr_t)j.count & 3) == 0,
+                "%s: job %d: misaligned picks, plan or count", api, i);
+    for (int k = 0; k < i; ++k)
+      FVS_REQUIRE(jobs[k].encoded != j.encoded && jobs[k].count != j.count && (j.n == 0 || jobs[k].plan != j.plan),
+                  "%s: jobs %d and %d share an output", api, k, i);
+  }
+  for (int i0 = 0; i0 < n_jobs; i0 += kGatherJobs) {
+    const int n = std::min(kGatherJobs, n_jobs - i0);
+    const int r = n == 1 ? pick_plan_launch<1>(jobs + i0, 1, (cudaStream_t)stream)
+                         : pick_plan_launch<kGatherJobs>(jobs + i0, n, (cudaStream_t)stream);
+    if (r) return r;
+  }
+  return FVS_OK;
+}
+
+int fvs_qwen_pixel_gather_multi(const fvs_qwen_pixel_job* jobs, int n_jobs, int dtype, fvs_stream_t stream) {
+  const char* api = "fvs_qwen_pixel_gather_multi";
+  FVS_REQUIRE(jobs && n_jobs > 0, "%s: need a job table and n_jobs > 0", api);
+  FVS_REQUIRE(dtype == FVS_F16 || dtype == FVS_BF16, "%s: dtype must be f16 or bf16", api);
+  std::vector<fvs_qwen_gather_job> g(n_jobs);
+  for (int i = 0; i < n_jobs; ++i) {
+    const fvs_qwen_pixel_job& j = jobs[i];
+    FVS_REQUIRE(j.plan && j.out && j.n > 0 && j.n <= 65535, "%s: job %d: need a plan, an output and 0 < n <= 65535", api, i);
+    FVS_REQUIRE(j.base >= 0 && j.base < j.n_frames && j.host_chunks && j.chunk_frames > 0,
+                "%s: job %d: need 0 <= base < n_frames and a chunk table", api, i);
+    FVS_REQUIRE(j.frame_elems > 0 && (j.frame_elems * 2) % 16 == 0, "%s: job %d: frame size must be a multiple of 16 bytes",
+                api, i);
+    FVS_REQUIRE(aligned16(j.out) && ((uintptr_t)j.plan & 7) == 0 && ((uintptr_t)j.host_chunks & 7) == 0,
+                "%s: job %d: misaligned output or table", api, i);
+    // the DAM gather with no device tier: frames below `base` have no pixel rows and read as zeros
+    g[i] = fvs_qwen_gather_job{j.plan, j.n, j.n_frames, nullptr, nullptr, j.base, j.host_chunks, j.chunk_frames, nullptr,
+                               0, nullptr, nullptr, j.frame_elems, 0, j.out, nullptr, nullptr};
+    for (int k = 0; k < i; ++k) {
+      const uintptr_t a = uintptr_t(jobs[k].out), ae = a + size_t(jobs[k].n) * jobs[k].frame_elems * 2;
+      const uintptr_t b = uintptr_t(j.out), be = b + size_t(j.n) * j.frame_elems * 2;
+      FVS_REQUIRE(ae <= b || be <= a, "%s: jobs %d and %d share an output", api, k, i);
+    }
+  }
+  for (int i0 = 0; i0 < n_jobs; i0 += kGatherJobs) {
+    const int n = std::min(kGatherJobs, n_jobs - i0);
+    const int r = n == 1 ? dam_gather_launch<1>(g.data() + i0, 1, (cudaStream_t)stream)
+                         : dam_gather_launch<kGatherJobs>(g.data() + i0, n, (cudaStream_t)stream);
+    if (r) return r;
+  }
+  return FVS_OK;
+}
+
+int fvs_qwen_bank_scatter_multi(const fvs_qwen_scatter_job* jobs, int n_jobs, int dtype, fvs_stream_t stream) {
+  const char* api = "fvs_qwen_bank_scatter_multi";
+  FVS_REQUIRE(jobs && n_jobs > 0, "%s: need a job table and n_jobs > 0", api);
+  FVS_REQUIRE(dtype == FVS_F16 || dtype == FVS_BF16, "%s: dtype must be f16 or bf16", api);
+  for (int i = 0; i < n_jobs; ++i) {
+    const fvs_qwen_scatter_job& j = jobs[i];
+    FVS_REQUIRE(j.plan && j.x_rows && j.n > 0 && j.n <= 65535, "%s: job %d: need a plan, x rows and 0 < n <= 65535", api, i);
+    FVS_REQUIRE(j.n_frames > 0 && j.n_dev >= 0 && j.n_dev <= j.n_frames, "%s: job %d: need 0 <= n_dev <= n_frames", api, i);
+    FVS_REQUIRE(j.x_frame_elems > 0 && j.merged_frame_elems >= 0 && (j.x_frame_elems * 2) % 16 == 0 &&
+                    (j.merged_frame_elems * 2) % 16 == 0,
+                "%s: job %d: frame sizes must be multiples of 16 bytes", api, i);
+    FVS_REQUIRE(!j.merged_rows || j.merged_frame_elems > 0, "%s: job %d: merged rows without a merged bank", api, i);
+    FVS_REQUIRE(j.n_dev == 0 || (j.dev_x && (!j.merged_rows || j.dev_merged)), "%s: job %d: null device tier", api, i);
+    FVS_REQUIRE(j.n_dev == j.n_frames || (j.host_chunks && j.chunk_frames > 0), "%s: job %d: host frames without a chunk "
+                "table", api, i);
+    for (const void* p : {j.x_rows, j.merged_rows, (const void*)j.dev_x, (const void*)j.dev_merged})
+      FVS_REQUIRE(aligned16(p), "%s: job %d: row tensors must be 16-byte aligned", api, i);
+    FVS_REQUIRE(((uintptr_t)j.plan & 7) == 0 && ((uintptr_t)j.host_chunks & 7) == 0, "%s: job %d: misaligned tables", api, i);
+  }
+  for (int i0 = 0; i0 < n_jobs; i0 += kGatherJobs) {
+    const int n = std::min(kGatherJobs, n_jobs - i0);
+    const int r = n == 1 ? bank_scatter_launch<1>(jobs + i0, 1, (cudaStream_t)stream)
+                         : bank_scatter_launch<kGatherJobs>(jobs + i0, n, (cudaStream_t)stream);
+    if (r) return r;
+  }
+  return FVS_OK;
 }
 
 }  // extern "C"

@@ -30,11 +30,13 @@ import torch
 
 from .. import _lib as L
 from ..draws import DrawSource
-from .stream_state import _KMEANS_METHODS, QwenStreamState, check_device_frames, enqueue_csm
+from . import ops as Q
+from .stream_state import (_KMEANS_METHODS, PATCH_DIM, QwenStreamState, _rest_finish, check_device_frames,
+                           check_lazy_full_res, enqueue_csm)
 from .vision_tower import QwenVisionBlocksB200
 
 MAX_GRIDS = 16            # grid entries one fvs_qwen_vit_encode call takes
-PATCH_DIM = 3 * 2 * 14 * 14
+TOWER_ROWS = 65536        # rows of one tower call (its workspace is about 30 KB per row at 1280 wide)
 
 
 def plan_tower_calls(clips, max_rows: int, max_grids: int = MAX_GRIDS):
@@ -77,6 +79,69 @@ def _call_layout(clips, members):
     return [(t, h, w) for (h, w), t in tsum.items()], places
 
 
+def encode_picked(states, readbacks: torch.Tensor, max_rows: int = TOWER_ROWS):
+    """The full-resolution half of a lazy_full_res round (DESIGN.md §3.18), for states whose retrieval is enqueued
+    (state._lazy_ctx): ONE fvs_qwen_pick_plan_multi call plans every state's first-time frames (count of states[k] to
+    slot 7 of readbacks[k], pinned int32 [>= len(states), 8]); the round's ONE host wait, when a count or a k-means
+    read-back is still on its way (a DAM that is the whole bank plans the frames not yet encoded, and an empty DAM,
+    spatial_length 0, nothing: counts the host knows); then the planned frames' pixel rows go through one fvs_qwen_pixel_gather_multi, the tower and the
+    PatchMerger per tower call (plan_tower_calls), and fvs_qwen_bank_scatter_multi writes them into the banks.  Last,
+    the DAM gathers and the CSM merger of every state (stream_state._rest_finish).  The tower, the first state's, is
+    invariant to batch composition (§3.7) and the merger row-wise (§3.5), so each frame gets the bits of the eager
+    path."""
+    if any(st._lazy_ctx["n_spa"] and st.tower is None for st in states):     # refused before any mask byte is set
+        raise NotImplementedError("lazy_full_res: no full-resolution tower was given to the stream state")
+    addr = Q.host_device_ptr(readbacks)
+    jobs, counts = [], []
+    for k, st in enumerate(states):
+        c = st._lazy_ctx
+        n_spa, n = c["n_spa"], st.n_frames
+        st._plan = torch.empty(max(1, n_spa), dtype=torch.int64, device=st.encoded.buf.device)
+        if n_spa == 0:                     # spatial_length 0: nothing is ever retrieved, so nothing is encoded
+            counts.append(0)
+            continue
+        whole = n_spa == n
+        jobs.append((None if whole else c["picks"], n_spa, st.encoded.buf, n, st._plan,
+                     addr + (k * 8 + 7) * readbacks.element_size()))
+        counts.append(n - st.n_encoded if whole else None)
+    if jobs:
+        Q.pick_plan_multi(jobs)
+    if any(v is None for v in counts) or any(st._pending for st in states):
+        done = torch.cuda.Event()
+        done.record()
+        done.synchronize()
+    counts = [int(readbacks[k, 7]) if v is None else v for k, v in enumerate(counts)]
+    todo = [(st, n) for st, n in zip(states, counts) if n]
+    for st, n in todo:
+        st.n_encoded += n
+    if todo:
+        tower, merger = todo[0][0].tower, todo[0][0].merger
+        for grids, places in plan_tower_calls([[(n, *st.grid)] for st, n in todo], max_rows):
+            rows = sum(t * h * w for t, h, w in grids)
+            inp = torch.empty(rows, PATCH_DIM, dtype=todo[0][0].pixels.dtype, device=todo[0][0].encoded.buf.device)
+            gathers = []
+            for i, (off,) in places:
+                st, n = todo[i]
+                px = st.pixels
+                gathers.append((st._plan, n, st.n_frames, px.base, px.table, px.chunk_frames,
+                                inp[off: off + n * st.grid[0] * st.grid[1]], px.frame_elems))
+            Q.pixel_gather_multi(gathers)
+            feats = tower(inp, grids)
+            merged = merger(feats) if todo[0][0]._layout[2] is not None else None
+            scatters = []
+            for i, (off,) in places:
+                st, n = todo[i]
+                r = n * st.grid[0] * st.grid[1]
+                scatters.append(st._scatter_args(n, feats[off: off + r],
+                                                 None if merged is None else merged[off // 4: (off + r) // 4]))
+            Q.bank_scatter_multi(scatters)
+    ctxs = []
+    for st in states:
+        ctxs.append((st, st._lazy_ctx))
+        st._lazy_ctx, st._in_round = None, False
+    _rest_finish(ctxs)
+
+
 class _Stream:
     """one pool stream; it has what qwen.serve.export_qwen_memory reads of a host (visual, stream_state), so it can be
     exported like one"""
@@ -99,13 +164,14 @@ class QwenStreamPool:
     call (its workspace is about 30 KB per row at 1280 wide).  `preprocess` (a preprocess.Qwen2VLFramePreprocessor):
     `step` also takes decoded uint8 frames [T, H, W, 3] per stream (any mix of sizes, host or device); the round's clips
     go through ONE `preprocess.many` call, and each stream's rows and grid then make its (pixel_values_videos,
-    video_grid_thw)."""
+    video_grid_thw).  `lazy_full_res` (QwenStreamState's): the round runs the full-resolution tower once, after its one
+    host wait, on only the frames some stream's DAM picks for the first time (encode_picked, DESIGN.md §3.18)."""
 
-    TOWER_ROWS = 65536
+    TOWER_ROWS = TOWER_ROWS
     BATCH_MIN_JOBS = 4        # fewer k-means streams in a round take one enqueue_csm call each
 
     def __init__(self, model, device_frames: Optional[int] = None, max_streams: Optional[int] = None,
-                 small_device_frames: Optional[int] = None, preprocess=None):
+                 small_device_frames: Optional[int] = None, preprocess=None, lazy_full_res: bool = False):
         visual = model.visual
         flash, tower = visual.flash_memory, visual.encode_patches
         if not isinstance(tower, QwenVisionBlocksB200):
@@ -126,6 +192,7 @@ class QwenStreamPool:
         self.visual, self.flash, self.merger, self.tower = visual, flash, visual.merger, tower
         self.device_frames = check_device_frames(device_frames, "device_frames")
         self.small_device_frames = check_device_frames(small_device_frames, "small_device_frames")
+        self.lazy_full_res = check_lazy_full_res(lazy_full_res, flash)
         self.max_streams = max_streams
         self.preprocess = preprocess
         self._readbacks: Optional[torch.Tensor] = None     # pinned int32 [S, 8]: the round's read-backs
@@ -144,10 +211,12 @@ class QwenStreamPool:
             raise ValueError("QwenStreamPool.open: this checkpoint carries no draw source (single-stream host): pass seed=")
         if checkpoint is None:
             state = QwenStreamState(self.flash, self.merger, device_frames=self.device_frames,
-                                    small_device_frames=self.small_device_frames)
+                                    small_device_frames=self.small_device_frames, lazy_full_res=self.lazy_full_res)
         else:
             state = QwenStreamState.restore(checkpoint, self.flash, self.merger, self.device, device_frames=self.device_frames,
-                                            small_device_frames=self.small_device_frames)
+                                            small_device_frames=self.small_device_frames,
+                                            lazy_full_res=self.lazy_full_res)
+        state.tower = self.tower
         if seed is None and checkpoint is None:
             seed = int.from_bytes(os.urandom(8), "little") >> 1
         rng = DrawSource(int(seed) if seed is not None else 0, self.device)
@@ -216,19 +285,27 @@ class QwenStreamPool:
 
     def _encode(self, items):
         """items: [(pixels, t, h, w)] -> per item (x_new [t*h*w, D], small_new [t*h*w/4, D]) through as few tower calls
-        as plan_tower_calls allows"""
-        rows, segs = [], []
+        as plan_tower_calls allows; with lazy_full_res, (the pixel rows [t*h*w, 1176] on the device, small_new): only the
+        half-resolution rows go through the tower here"""
+        rows, segs, fulls = [], [], []
         for pix, t, h, w in items:
             full = pix.type(self.visual.get_dtype()).to(self.device, non_blocking=True).view(-1, PATCH_DIM)
             small, _ = self.flash.temporal_pool(full, [t, h, w])
-            rows.append((full, small))
-            segs.append([(t, h, w), (t, h // 2, w // 2)])
+            fulls.append(full)
+            if self.lazy_full_res:
+                rows.append((small,))
+                segs.append([(t, h // 2, w // 2)])
+            else:
+                rows.append((full, small))
+                segs.append([(t, h, w), (t, h // 2, w // 2)])
         out = [None] * len(items)
         for grids, places in plan_tower_calls(segs, self.TOWER_ROWS):
             pieces = sorted(((off, rows[i][k]) for i, offs in places for k, off in enumerate(offs)), key=lambda p: p[0])
             feats = self.tower(torch.cat([p for _, p in pieces]) if len(pieces) > 1 else pieces[0][1], grids)
             for i, offs in places:
                 out[i] = tuple(feats[off: off + r.shape[0]] for off, r in zip(offs, rows[i]))
+        if self.lazy_full_res:
+            out = [(full, o[0]) for full, o in zip(fulls, out)]
         return out
 
     def step(self, clips: dict, draws: Optional[dict] = None):
@@ -257,6 +334,21 @@ class QwenStreamPool:
         items = [self._validate(sid, clips[sid]) for sid in sids]
         feats = self._encode(items)
         merged = [None] * len(sids)
+        if self.lazy_full_res:
+            self._readback_rows(len(sids))
+            states = [self._streams[sid].stream_state for sid in sids]
+            for st in states:
+                st._in_round = True
+            try:
+                self._enqueue_memory(sids, items, feats, merged, draws)
+            finally:
+                started = [st for st in states if st._lazy_ctx is not None]
+                for st in states:
+                    st._in_round = False
+                if started:                            # the round's one host wait is in there
+                    encode_picked(started, self._readbacks, self.TOWER_ROWS)
+            self._complete(sids)
+            return
         if self.flash.spatial_length > 0 and self.merger is not None:
             xs = [x for x, _ in feats]
             m = self.merger(torch.cat(xs) if len(xs) > 1 else xs[0])
@@ -293,15 +385,18 @@ class QwenStreamPool:
         finally:
             if reqs:
                 n = len(reqs)
-                if self._readbacks is None or self._readbacks.shape[0] < n:
-                    self._readbacks = torch.empty(max(n, 2 * (0 if self._readbacks is None else self._readbacks.shape[0])),
-                                                  8, dtype=torch.int32).pin_memory()
+                self._readback_rows(n)
                 if n >= self.BATCH_MIN_JOBS:
                     enqueue_csm(reqs, self._readbacks)
                 else:
                     for i, item in enumerate(reqs):
                         enqueue_csm([item], self._readbacks[i: i + 1])
         return bool(reqs)
+
+    def _readback_rows(self, n: int):
+        if self._readbacks is None or self._readbacks.shape[0] < n:
+            self._readbacks = torch.empty(max(n, 2 * (0 if self._readbacks is None else self._readbacks.shape[0])), 8,
+                                          dtype=torch.int32).pin_memory()
 
     def _complete(self, sids):
         """complete every enqueued stream of the round and publish it; then raise one error for those that raised"""

@@ -218,6 +218,53 @@ def dam_gather_multi(calls):
             "fvs_qwen_dam_gather_multi")
 
 
+def pick_plan_multi(jobs):
+    """fvs_qwen_pick_plan_multi: jobs = [(picks int64 [n] or None for frames 0..n-1, n, encoded uint8 [>= n_frames],
+    n_frames, plan int64 [>= n], count address)], count address = an int: the mapped address of an int32 slot of pinned
+    memory (host_device_ptr) or of a device int32.  Sets the planned frames' mask bytes."""
+    arr = []
+    for picks, n, encoded, n_frames, plan, count in jobs:
+        _chk_cuda(picks, encoded, plan)
+        assert (picks is None or (picks.dtype == torch.int64 and picks.is_contiguous() and picks.numel() >= n))
+        assert encoded.dtype == torch.uint8 and plan.dtype == torch.int64 and plan.numel() >= n
+        arr.append(L.QwenPickPlanJob(picks=L.ptr(picks), n=int(n), n_frames=int(n_frames), encoded=encoded.data_ptr(),
+                                     plan=plan.data_ptr(), count=int(count)))
+    L.check(L.load().fvs_qwen_pick_plan_multi((L.QwenPickPlanJob * len(arr))(*arr), len(arr), L.cur_stream()),
+            "fvs_qwen_pick_plan_multi")
+
+
+def pixel_gather_multi(jobs):
+    """fvs_qwen_pixel_gather_multi: jobs = [(plan int64, n, n_frames, base, chunk table (device int64), chunk_frames,
+    out [n, ...] of 16-bit rows, frame_elems)], all outputs of one dtype"""
+    arr = []
+    for plan, n, n_frames, base, table, cf, out, fe in jobs:
+        _chk_cuda(plan, table, out)
+        assert plan.dtype == torch.int64 and table.dtype == torch.int64 and out.is_contiguous() and out.numel() == n * fe
+        arr.append(L.QwenPixelJob(plan=plan.data_ptr(), n=int(n), n_frames=int(n_frames), base=int(base),
+                                  host_chunks=table.data_ptr(), chunk_frames=int(cf), frame_elems=int(fe),
+                                  out=out.data_ptr()))
+    L.check(L.load().fvs_qwen_pixel_gather_multi((L.QwenPixelJob * len(arr))(*arr), len(arr), L.dtype_code(jobs[0][6].dtype),
+                                                 L.cur_stream()), "fvs_qwen_pixel_gather_multi")
+
+
+def bank_scatter_multi(jobs):
+    """fvs_qwen_bank_scatter_multi: jobs = [dict(plan, n, n_frames, x_rows, merged_rows, dev_x, dev_merged, n_dev, chunks,
+    chunk_frames, x_frame_elems, merged_frame_elems)], every row tensor of one 16-bit dtype"""
+    arr = []
+    for a in jobs:
+        _chk_cuda(a["plan"], a["x_rows"], a["merged_rows"], a["dev_x"], a["dev_merged"], a["chunks"])
+        assert a["plan"].dtype == torch.int64 and a["x_rows"].is_contiguous()
+        assert a["merged_rows"] is None or a["merged_rows"].is_contiguous()
+        arr.append(L.QwenScatterJob(
+            plan=a["plan"].data_ptr(), n=int(a["n"]), n_frames=int(a["n_frames"]), x_rows=a["x_rows"].data_ptr(),
+            merged_rows=L.ptr(a["merged_rows"]), dev_x=L.ptr(a["dev_x"]), dev_merged=L.ptr(a["dev_merged"]),
+            n_dev=int(a["n_dev"]), host_chunks=L.ptr(a["chunks"]), chunk_frames=int(a["chunk_frames"]),
+            x_frame_elems=int(a["x_frame_elems"]), merged_frame_elems=int(a["merged_frame_elems"])))
+    L.check(L.load().fvs_qwen_bank_scatter_multi((L.QwenScatterJob * len(arr))(*arr), len(arr),
+                                                 L.dtype_code(jobs[0]["x_rows"].dtype), L.cur_stream()),
+            "fvs_qwen_bank_scatter_multi")
+
+
 def mem_workspace_bytes(T: int, K: int, PD: int) -> int:
     """bytes one job of the CSM chain needs besides its outputs: fp32 centroids, unique-rows and k-means workspaces"""
     lib = L.load()

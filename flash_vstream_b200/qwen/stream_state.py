@@ -38,6 +38,7 @@ from ..draws import GLOBAL, to_device
 from ..host_tier import CHUNK_BYTES, check_device_frames, chunk_frames, placement  # noqa: F401
 
 _KMEANS_METHODS = ("kmeans_ordered", "fast_kmeans_ordered")
+PATCH_DIM = 3 * 2 * 14 * 14           # elements of one full-resolution pixel row (what the tower reads)
 
 
 class RowBank:
@@ -70,14 +71,18 @@ class QwenStreamState:
     them (fvs_qwen_dam_gather).
     small_device_frames: how many frames of the half-resolution bank stay in HBM (None: all of them).  Later frames go to
     pinned host chunks of their own; the klarge retrieval sweeps them in place over PCIe (fvs_qwen_klarge_retrieve_tiered),
-    once per step, twice with the cosine metric.  The two caps are independent; results are bit-identical either way."""
+    once per step, twice with the cosine metric.  The two caps are independent; results are bit-identical either way.
+    lazy_full_res: keep each clip's full-resolution pixel rows in pinned host chunks instead of its tower features, and
+    run the full-resolution tower on a frame only the first time the DAM picks it (DESIGN.md §3.18); step() then takes
+    the pixel rows in place of x_new, and the tower.  The published bits are the eager state's."""
 
     CHUNK_BYTES = CHUNK_BYTES
 
-    def __init__(self, flash, merger, device_frames=None, small_device_frames=None):
+    def __init__(self, flash, merger, device_frames=None, small_device_frames=None, lazy_full_res=False):
         self.flash, self.merger = flash, merger
         self.device_frames = check_device_frames(device_frames)
         self.small_device_frames = check_device_frames(small_device_frames, "small_device_frames")
+        self.lazy_full_res = check_lazy_full_res(lazy_full_res, flash)
         self.rng = GLOBAL                     # the draws.DrawSource of every k-means draw (a QwenStreamPool stream owns one)
         self.reset()
 
@@ -105,13 +110,38 @@ class QwenStreamState:
         self._pending = None                  # what complete() needs of an enqueued clip ({} when nothing is read back)
         self.fast_steps = self.redone_steps = 0
         self.steps = 0                        # clips whose step completed (a clip that raises is not counted)
+        self.encoded = RowBank()              # lazy_full_res: device uint8 [n_frames], 1 once a frame's bank slots are filled
+        self.pixels: Optional[PixelStore] = None   # lazy_full_res: the frames' full-resolution pixel rows
+        self.n_encoded = 0                    # lazy_full_res: frames the full-resolution tower has encoded
+        self.tower = None                     # lazy_full_res: callable(pixel rows, grids) -> full-resolution features
+        self._in_round = False                # lazy_full_res: the outputs of this step wait for multistream.encode_picked
+        self._lazy_ctx = None                 # lazy_full_res: the retrieval context those outputs are made from
+        self._plan = None                     # lazy_full_res: device int64, the last pick plan
 
     # ------------------------------------------------------------------------------------------------ one clip
     def step(self, x_new: torch.Tensor, small_new: torch.Tensor, t: int, grid, small_grid, start_idx: int,
-             draws: Optional[dict] = None, merged: Optional[torch.Tensor] = None):
+             draws: Optional[dict] = None, merged: Optional[torch.Tensor] = None, tower=None):
         """x_new [t * h * w, D] / small_new [t * hs * ws, D]: the tower's two-resolution features of the clip (device);
         grid = (h, w), small_grid = (hs, ws) host integers; merged: the PatchMerger rows of x_new, when the caller has
-        merged them already (None: merged here).  Updates the state.  enqueue(), one host wait, complete()."""
+        merged them already (None: merged here).  Updates the state.  enqueue(), one host wait, complete().
+        With lazy_full_res, x_new is the clip's full-resolution pixel rows [t * h * w, 1176] (device) and `tower`
+        (callable(rows, grids)) encodes the frames the DAM picks for the first time: the one-stream round of
+        multistream.encode_picked, still one host wait."""
+        if self.lazy_full_res:
+            from .multistream import encode_picked
+            if tower is not None:
+                self.tower = tower
+            if self._readback is None:
+                self._readback = torch.empty(8, dtype=torch.int32).pin_memory()
+            self._in_round = True
+            try:
+                banks = self.enqueue(x_new, small_new, t, grid, small_grid, start_idx, draws, merged)
+            finally:
+                if self._lazy_ctx is not None:
+                    encode_picked([self], self._readback.view(1, 8))
+                self._in_round = False
+            self.complete()
+            return banks
         banks = self.enqueue(x_new, small_new, t, grid, small_grid, start_idx, draws, merged)
         if self._pending:
             done = torch.cuda.Event()
@@ -140,7 +170,7 @@ class QwenStreamState:
         k-means (memory still filling, or a branch the synchronous path runs, which is then already enqueued); otherwise
         the k-means to run (cand [T, P, D], cand_w, init, refill, order), which enqueue_csm() takes."""
         flash = self.flash
-        dev, dt, D = x_new.device, x_new.dtype, x_new.shape[-1]
+        dev, dt, D = small_new.device, small_new.dtype, small_new.shape[-1]
         h, w = grid
         hs, ws = small_grid
         if self.grid is None:
@@ -151,11 +181,14 @@ class QwenStreamState:
         self._prev_dam = self._dam()
         self._append_small(small_new.view(t, hs * ws, D), dev)
         small_bank = self.bank_small.rows() if self.bank_small.n else None
-        if S0 > 0 and self.merger is not None:
-            merged = (self.merger(x_new) if merged is None else merged).view(t, h * w // 4, -1)
+        if self.lazy_full_res:
+            self._append_lazy(x_new.view(t, h * w, PATCH_DIM), dt, D, dev)
         else:
-            merged = None
-        self._append_frames(x_new.view(t, h * w, D), merged, dev)
+            if S0 > 0 and self.merger is not None:
+                merged = (self.merger(x_new) if merged is None else merged).view(t, h * w // 4, -1)
+            else:
+                merged = None
+            self._append_frames(x_new.view(t, h * w, D), merged, dev)
         bank = self.bank_x.rows() if self.bank_x.n else None
         self.n_frames += t
         # ---- CSM input: carried centroids followed by the clip's half-resolution frames
@@ -333,6 +366,39 @@ class QwenStreamState:
                 cm[dst: dst + cnt].copy_(m3[s: s + cnt], non_blocking=True)
             self.n_host += cnt
 
+    def _append_lazy(self, pix3, dt, D, dev):
+        """lazy_full_res: the clip's pixel rows pix3 [t, h*w, 1176] appended to the pixel store (asynchronous copies to its
+        pinned chunks), and t bank slots (zero rows in HBM, chunk rows on the host) with clear mask bytes"""
+        t, hw = pix3.shape[0], pix3.shape[1]
+        if self._layout is None:
+            ms = None
+            if self.flash.spatial_length > 0 and self.merger is not None:
+                ms = torch.Size([hw // 4, int(self.merger.dim)])
+            self._layout = (dt, torch.Size([hw, D]), ms)
+        if self.pixels is None:
+            self.pixels = PixelStore(pix3.dtype, hw * PATCH_DIM, self.n_frames, self.CHUNK_BYTES)
+        self.pixels.append(pix3.reshape(t, -1), dev)
+        dt, xs, ms = self._layout
+        for c, _, _, cnt in placement(self.bank_x.n + self.n_host, t, self.device_frames, self._per_chunk()):
+            if c < 0:
+                self.bank_x.append(torch.zeros((cnt,) + tuple(xs), dtype=dt, device=dev))
+                if ms is not None:
+                    self.bank_merged.append(torch.zeros((cnt,) + tuple(ms), dtype=dt, device=dev))
+                continue
+            self._chunk(c, dev)
+            self.n_host += cnt
+        self.encoded.append(torch.zeros(t, dtype=torch.uint8, device=dev))
+
+    def _scatter_args(self, n: int, x_rows, merged_rows) -> dict:
+        """the job of Q.bank_scatter_multi that writes the n frames of this state's last pick plan into its banks"""
+        dt, xs, ms = self._layout
+        return dict(plan=self._plan, n=n, n_frames=self.bank_x.n + self.n_host, x_rows=x_rows,
+                    merged_rows=merged_rows if ms is not None else None,
+                    dev_x=self.bank_x.buf if self.bank_x.n else None,
+                    dev_merged=self.bank_merged.buf if self.bank_merged.n and ms is not None else None,
+                    n_dev=self.bank_x.n, chunks=self._chunk_table, chunk_frames=self._per_chunk(),
+                    x_frame_elems=xs.numel(), merged_frame_elems=0 if ms is None else ms.numel())
+
     def _small_per_chunk(self) -> int:
         dt, ps = self._small_layout
         return chunk_frames(ps.numel() * dt.itemsize, self.CHUNK_BYTES)
@@ -426,6 +492,9 @@ class QwenStreamState:
                     "merged": int(n > 0 and self._layout[2] is not None),
                     "tem_weights_dtype": None if self.tem_weights is None else CK.dtype_name(self.tem_weights.dtype),
                     "tem_timestamp_dtype": "float32" if n == 0 else CK.dtype_name(self.tem_timestamp.dtype)}
+        if self.lazy_full_res and n:          # eager checkpoints carry neither the counter nor the tensors below
+            todo = torch.nonzero(self.encoded.rows().cpu() == 0).flatten().tolist()   # frames not yet encoded
+            counters["pix_frames"] = len(todo)
         if n == 0:
             return CK.qwen(self._config(0, "float16"), counters, {})
         dt, ps = self._small_layout
@@ -436,6 +505,9 @@ class QwenStreamState:
             tensors["video_embeds"] = self.video_embeds
         with torch.cuda.device(self.tem_x.device):
             owned = {}                            # spilled banks: assembled in pinned memory here, taken as they are
+            if self.lazy_full_res:                # the mask, and the pixel rows of the frames not yet encoded, in order
+                tensors["encoded"] = self.encoded.rows()
+                owned["pixels"] = self.pixels.rows_of(todo).view(len(todo), self._layout[1][0], PATCH_DIM)
             if self.n_small_host:
                 owned["bank_small"] = self._small_on_host()
             else:
@@ -452,10 +524,13 @@ class QwenStreamState:
         return ck
 
     @classmethod
-    def restore(cls, ckpt, flash, merger, device, device_frames=None, small_device_frames=None) -> "QwenStreamState":
+    def restore(cls, ckpt, flash, merger, device, device_frames=None, small_device_frames=None,
+                lazy_full_res=False) -> "QwenStreamState":
         """A state on `device` that continues `ckpt` bit for bit; `flash` / `merger` must have the configuration the
         checkpoint was taken with (ValueError naming the field otherwise).  The banks' frames are placed by this state's
-        `device_frames` and `small_device_frames`, whatever the caps of the state that took the checkpoint."""
+        `device_frames` and `small_device_frames`, whatever the caps of the state that took the checkpoint.  An eager
+        checkpoint (every frame encoded) restores into a lazy_full_res state; a lazy one restores into an eager state
+        only once every frame is encoded (NotImplementedError naming the knob otherwise)."""
         from .. import checkpoint as CK
         if ckpt.family != CK.QWEN:
             raise ValueError(f"QwenStreamState.restore: a {ckpt.family!r} checkpoint is not a Qwen2-VL stream's")
@@ -468,14 +543,37 @@ class QwenStreamState:
         if n["n_frames"] and c["merger_dim"] != md:
             raise ValueError(f"QwenStreamState.restore: config.merger_dim of the checkpoint ({c['merger_dim']}) differs "
                              f"from the merger's ({md})")
-        st = cls(flash, merger, device_frames, small_device_frames)
+        st = cls(flash, merger, device_frames, small_device_frames, lazy_full_res=lazy_full_res)
         if n["n_frames"] == 0:
             return st
+        lazy_ck = "pix_frames" in n
+        if lazy_ck:                               # the frames not yet encoded, whose pixel rows the checkpoint holds
+            todo = torch.nonzero(ckpt.tensor("encoded") == 0).flatten().tolist()
+            if len(todo) != n["pix_frames"]:
+                raise ValueError(f"QwenStreamState.restore: counters.pix_frames ({n['pix_frames']}) is not the number of "
+                                 f"frames the mask leaves unencoded ({len(todo)})")
+        if lazy_ck and not lazy_full_res and todo:
+            raise NotImplementedError("QwenStreamState.restore: the checkpoint is of a lazy_full_res stream with frames "
+                                      "not yet encoded at full resolution: restore it with lazy_full_res=True")
         dev = torch.device(device)
         with torch.cuda.device(dev):
             get = lambda k: ckpt.tensor(k).to(dev, non_blocking=True)
             st._append_frames(ckpt.tensor("bank_x"), ckpt.tensor("bank_merged") if n["merged"] else None, dev)
             st._append_small(ckpt.tensor("bank_small"), dev)
+            if lazy_full_res:
+                hw = int(c["grid"][0]) * int(c["grid"][1])
+                if lazy_ck:                       # the store starts at the first frame not yet encoded
+                    st.encoded.append(get("encoded"))
+                    st.n_encoded = n["n_frames"] - len(todo)
+                    base = todo[0] if todo else n["n_frames"]
+                    st.pixels = PixelStore(st._layout[0], hw * PATCH_DIM, base, st.CHUNK_BYTES)
+                    if todo:
+                        st.pixels.append(None, dev, t=n["n_frames"] - base)
+                        st.pixels.put(todo, ckpt.tensor("pixels").view(len(todo), -1))
+                else:                             # an eager stream: every frame is encoded, no frame has pixel rows
+                    st.encoded.append(torch.ones(n["n_frames"], dtype=torch.uint8, device=dev))
+                    st.n_encoded = n["n_frames"]
+                    st.pixels = PixelStore(st._layout[0], hw * PATCH_DIM, n["n_frames"], st.CHUNK_BYTES)
             st.n_frames, st.steps = n["n_frames"], n["steps"]
             st.fast_steps, st.redone_steps = n["fast_steps"], n["redone_steps"]
             st.grid, st.small_grid = tuple(c["grid"]), tuple(c["small_grid"])
@@ -494,8 +592,8 @@ class QwenStreamState:
     # ------------------------------------------------------------------------------------------------ the reference's list
     def as_list(self):
         """the 13 items of `video_embedding_memory` (:620-624); the thw entries are host tensors, everything else lives in HBM.
-        Once frames have spilled to the host chunks, item 7 (the full-resolution bank, which no reader of the list uses) is
-        the zero-row stand-in x[:0]; its thw (item 8) stays exact.  Likewise item 9 (the half-resolution bank) once its
+        Once frames have spilled to the host chunks, or with lazy_full_res, item 7 (the full-resolution bank, which no
+        reader of the list uses) is the zero-row stand-in x[:0]; its thw (item 8) stays exact.  Likewise item 9 (the half-resolution bank) once its
         frames have spilled; item 10 stays exact."""
         n, h, w = self.n_frames, *self.grid
         n_spa = 0 if self.spa_positions is None else int(self.spa_positions.numel())
@@ -504,7 +602,7 @@ class QwenStreamState:
         # the stand-ins are zero-row device views of the banks' dtype (tem_x's when no half-resolution frame is in HBM)
         rows = self.bank_small.rows().view(-1, D) if self.bank_small.n else self.tem_x.reshape(-1, D)
         small = rows if self.n_small_host == 0 else rows[:0]
-        x = self.bank_x.rows().view(n * h * w, -1) if self.n_host == 0 else rows[:0]
+        x = self.bank_x.rows().view(n * h * w, -1) if self.n_host == 0 and not self.lazy_full_res else rows[:0]
         return [self.tem_x, self._thw(self.n_tem, small=True), self.tem_weights, self.tem_timestamp,
                 self.spa_x, self._thw(n_spa), self.spa_positions,
                 x, self._thw(n), small, self._thw(n, small=True), ve, None if ve is None else ve.shape]
@@ -541,6 +639,26 @@ def _rest_stage(ctxs):
     for (metric, _), cs in groups.items():
         for c, picks in zip(cs, Q.klarge_retrieve_multi([c["retrieve"][:3] for c in cs], metric)):
             c["picks"] = picks
+    lazy = []                        # lazy_full_res: the outputs wait until the picked frames are encoded
+    for state, c in ctxs:
+        if state.lazy_full_res:
+            state._lazy_ctx = c
+            if not state._in_round:   # a clip redone by complete(), outside its round: encoded here, synchronously
+                lazy.append(state)
+    if lazy:
+        from .multistream import encode_picked
+        for state in lazy:
+            if state._readback is None:
+                state._readback = torch.empty(8, dtype=torch.int32).pin_memory()
+            encode_picked([state], state._readback.view(1, 8))
+    _rest_finish([(s, c) for s, c in ctxs if not s.lazy_full_res])
+
+
+def _rest_finish(ctxs):
+    """the second half of _rest_stage, once the retrieved frames are in the banks: _rest_outputs, one DAM gather table
+    per dtype, and one PatchMerger call over every CSM slice"""
+    if not ctxs:
+        return
     gathers, merges = {}, []
     for state, c in ctxs:
         g, m = state._rest_outputs(c)
@@ -560,6 +678,66 @@ def _rest_stage(ctxs):
         for x, out in merges:
             out.copy_(y[r: r + out.shape[0]])
             r += out.shape[0]
+
+
+def check_lazy_full_res(v, flash, who: str = "lazy_full_res") -> bool:
+    """a bool; NotImplementedError when on with a temporal pool size other than 2 (with pool size 1 the half-resolution
+    bank is the full-resolution one, so there is nothing to defer)"""
+    if not isinstance(v, bool):
+        raise ValueError(f"{who} must be True or False, got {v!r}")
+    if v and flash.temporal_poolsize != 2:
+        raise NotImplementedError(f"{who}=True needs flash_memory_temporal_poolsize=2 (got {flash.temporal_poolsize}): "
+                                  f"with pool size 1 the full-resolution bank is the half-resolution one")
+    return v
+
+
+class PixelStore:
+    """lazy_full_res: the full-resolution pixel rows of frames [base, n) of a stream in pinned host chunks of
+    chunk_frames frames each (host_tier's chunk arithmetic with no device tier), with a device table of the chunks'
+    mapped pointers that fvs_qwen_pixel_gather_multi reads them through.  Frames below `base` (encoded before the stream
+    came here from a checkpoint) have no pixel rows; a restored stream's encoded frames above it have unwritten slots."""
+
+    def __init__(self, dtype, frame_elems: int, base: int, chunk_bytes: int = CHUNK_BYTES):
+        self.dtype, self.frame_elems, self.base, self.n = dtype, int(frame_elems), int(base), int(base)
+        self.chunk_frames = chunk_frames(self.frame_elems * dtype.itemsize, chunk_bytes)
+        self.chunks, self.table = [], None
+
+    def append(self, rows: Optional[torch.Tensor], dev, t: Optional[int] = None):
+        """rows [t, frame_elems] (device or host): asynchronous copies on the current stream; rows None: t slots left
+        unwritten (frames whose rows are put() later or never read)"""
+        t = rows.shape[0] if rows is not None else int(t)
+        for c, dst, s, cnt in placement(self.n - self.base, t, 0, self.chunk_frames):
+            while len(self.chunks) <= c:
+                k = len(self.chunks)
+                buf = torch.empty(self.chunk_frames, self.frame_elems, dtype=self.dtype, pin_memory=True)
+                if self.table is None or self.table.numel() <= k:
+                    tab = torch.zeros(max(16, 2 * k), dtype=torch.int64, device=dev)
+                    if k:
+                        tab[:k].copy_(self.table[:k])
+                    self.table = tab
+                self.table[k].fill_(Q.host_device_ptr(buf))
+                self.chunks.append(buf)
+            if rows is not None:
+                self.chunks[c][dst: dst + cnt].copy_(rows[s: s + cnt], non_blocking=True)
+        self.n += t
+
+    def _row(self, f: int) -> torch.Tensor:
+        c, r = divmod(f - self.base, self.chunk_frames)
+        return self.chunks[c][r]
+
+    def rows_of(self, frames) -> torch.Tensor:
+        """the rows of `frames` (each in [base, n)) as one pinned tensor [len(frames), frame_elems], once the pending
+        copies have landed"""
+        out = torch.empty(len(frames), self.frame_elems, dtype=self.dtype, pin_memory=True)
+        torch.cuda.current_stream().synchronize()
+        for i, f in enumerate(frames):
+            out[i].copy_(self._row(int(f)))
+        return out
+
+    def put(self, frames, rows: torch.Tensor):
+        """rows [len(frames), frame_elems] (host) into the slots of `frames`"""
+        for i, f in enumerate(frames):
+            self._row(int(f)).copy_(rows[i])
 
 
 def _on_host(rb: RowBank, chunks, n: int, row_shape, dt) -> torch.Tensor:

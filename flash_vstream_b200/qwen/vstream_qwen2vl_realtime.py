@@ -29,7 +29,7 @@ from . import offline as _offline_pass
 from . import vstream_qwen2vl_model as _offline
 from .compress_functions import weighted_kmeans_ordered_feature
 from .patch_merger import PatchMerger
-from .stream_state import QwenStreamState, check_device_frames
+from .stream_state import QwenStreamState, check_device_frames, check_lazy_full_res
 
 
 class FlashMemory(_offline.FlashMemory):
@@ -149,10 +149,16 @@ class RealtimeStreamingMixin:
     (and to load_video_stream); changing it in the middle of a stream raises ValueError.
 
     fvs_bank_small_device_frames: the same for the half-resolution bank, whose later frames the retrieval sweeps in place
-    over PCIe every step (DESIGN.md §3.13).  With both caps set, a stream's HBM no longer grows with its length."""
+    over PCIe every step (DESIGN.md §3.13).  With both caps set, a stream's HBM no longer grows with its length.
+
+    fvs_lazy_full_res: False (default) or True — keep each clip's full-resolution pixel rows and run the full-resolution
+    tower on a frame only the first time the DAM picks it (DESIGN.md §3.18); item 7 of the list is then the zero-row
+    stand-in.  Needs flash_memory_temporal_poolsize=2.  Like the caps, it applies from the next stream (and to
+    load_video_stream); changing it in the middle of a stream raises ValueError."""
 
     fvs_bank_device_frames = None
     fvs_bank_small_device_frames = None
+    fvs_lazy_full_res = False
 
     def _bank_device_frames(self):
         return self._cap("fvs_bank_device_frames", "device_frames")
@@ -160,9 +166,13 @@ class RealtimeStreamingMixin:
     def _bank_small_device_frames(self):
         return self._cap("fvs_bank_small_device_frames", "small_device_frames")
 
-    def _cap(self, knob, attr):
+    def _lazy_full_res(self):
+        return self._cap("fvs_lazy_full_res", "lazy_full_res",
+                         lambda v, k: check_lazy_full_res(v, self.visual.flash_memory, k))
+
+    def _cap(self, knob, attr, check=check_device_frames):
         """the validated value of the cap attribute `knob`, which the stream in progress (its state's `attr`) must share"""
-        cap = check_device_frames(getattr(self, knob), knob)
+        cap = check(getattr(self, knob), knob)
         st = self.__dict__.get("stream_state")
         if st is not None and st.n_frames > 0 and self.video_embedding_memory and getattr(st, attr) != cap:
             raise ValueError(f"{knob} changed from {getattr(st, attr)} to {cap} in the middle of a stream: "
@@ -199,14 +209,24 @@ class RealtimeStreamingMixin:
         with the read-back ("temporal_compress" .. "merger" of the reference's meter are one bucket here: time_3..time_6)."""
         time_0 = time.perf_counter()
         assert self.use_video_streaming_mode
-        cap, small_cap = self._bank_device_frames(), self._bank_small_device_frames()
+        cap, small_cap, lazy = self._bank_device_frames(), self._bank_small_device_frames(), self._lazy_full_res()
         grid_host = video_grid_thw.cpu()          # the grid stays on the host: every shape below comes from it (a CUDA grid
         t, h, w = (int(v) for v in grid_host.reshape(-1, 3)[0].tolist())   # costs one sync here, a host grid none)
         pixel_values_videos = pixel_values_videos.type(self.visual.get_dtype()).to(self.visual.get_device(), non_blocking=True)
         time_1 = time.perf_counter()
-        feats, _, small_grid_thw = self.visual.forward_simple_not_merge(pixel_values_videos, grid_host)
+        if lazy:                                  # only the half-resolution rows now; the picked frames' full rows later
+            small, small_grid = self.visual.flash_memory.temporal_pool(pixel_values_videos.view(-1, 3 * 2 * 14 * 14),
+                                                                       grid_host.reshape(-1, 3)[0])
+            if self.visual.encode_patches is None:
+                raise NotImplementedError("fvs_lazy_full_res: no vision tower attached (visual.encode_patches)")
+            feats = self.visual.encode_patches(small, small_grid.view(1, 3))
+        else:
+            feats, _, small_grid_thw = self.visual.forward_simple_not_merge(pixel_values_videos, grid_host)
         time_2 = time.perf_counter()
-        if small_grid_thw is not None:
+        if lazy:
+            hs, ws = h // 2, w // 2
+            x_new, small_new = pixel_values_videos.view(-1, 3 * 2 * 14 * 14), feats
+        elif small_grid_thw is not None:
             hs, ws = h // 2, w // 2
             x_new, small_new = feats[: t * h * w], feats[t * h * w: t * h * w + t * hs * ws]
         else:
@@ -215,11 +235,12 @@ class RealtimeStreamingMixin:
         pub = self.__dict__.get("_qwen_publication")              # set by qwen.serve.export_qwen_memory (opt-in)
         if self.stream_state is None or not self.video_embedding_memory:
             self.stream_state = QwenStreamState(self.visual.flash_memory, self.visual.merger, device_frames=cap,
-                                                small_device_frames=small_cap)
+                                                small_device_frames=small_cap, lazy_full_res=lazy)
             if pub is not None:
                 pub.new_stream()
         time_3 = time.perf_counter()
-        self.stream_state.step(x_new, small_new, t, (h, w), (hs, ws), start_idx, draws=draws)
+        self.stream_state.step(x_new, small_new, t, (h, w), (hs, ws), start_idx, draws=draws,
+                               tower=self.visual.encode_patches if lazy else None)
         time_6 = time.perf_counter()
         if pub is not None:
             pub.publish(self.stream_state)                         # the clip is final: one launch, under the seqlock
@@ -253,8 +274,10 @@ class RealtimeStreamingMixin:
                              f"the exported grid {pub.grid} / {pub.small_grid}")
         cap = check_device_frames(self.fvs_bank_device_frames, "fvs_bank_device_frames")
         small_cap = check_device_frames(self.fvs_bank_small_device_frames, "fvs_bank_small_device_frames")
+        lazy = check_lazy_full_res(self.fvs_lazy_full_res, self.visual.flash_memory, "fvs_lazy_full_res")
         state = QwenStreamState.restore(ckpt, self.visual.flash_memory, self.visual.merger, self.visual.get_device(),
-                                        device_frames=cap, small_device_frames=small_cap)
+                                        device_frames=cap, small_device_frames=small_cap, lazy_full_res=lazy)
+        state.tower = self.visual.encode_patches if lazy else None
         if state.n_frames == 0:
             self.stream_state = None
             self._publish([])

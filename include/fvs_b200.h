@@ -585,6 +585,59 @@ typedef struct fvs_qwen_gather_job {
   uint64_t* host_fetches;
 } fvs_qwen_gather_job;
 int fvs_qwen_dam_gather_multi(const fvs_qwen_gather_job* jobs_h, int n_jobs, int dtype, fvs_stream_t stream);
+
+/* Lazy full-resolution bank (DESIGN.md §3.18): a stream keeps each frame's full-resolution pixel rows in pinned host
+ * chunks and encodes a frame the first time the DAM picks it.  Each call is a job table (one stream = the one-job
+ * table); every job is checked before anything is enqueued (FVS_EINVAL otherwise), at most
+ * FVS_QWEN_MEM_JOBS_PER_LAUNCH jobs per launch, and no two jobs may share an output.
+ *
+ * fvs_qwen_pick_plan_multi: per job, walks picks (device int64 [n]; NULL = frames 0..n-1, the DAM while it is the whole
+ * bank) in order and writes to plan (device int64 [n]) every pick that is in [0, n_frames), whose byte in `encoded`
+ * (device uint8 [n_frames]) is 0 and that no earlier pick names: the stream's first-time frames, unique, in pick order.
+ * Their mask bytes are set to 1 and their number is stored to *count (int32; device memory or the mapped address of
+ * pinned host memory, e.g. a slot of the stream's read-back row). */
+typedef struct fvs_qwen_pick_plan_job {
+  const int64_t* picks;
+  int n;
+  int64_t n_frames;
+  uint8_t* encoded;
+  int64_t* plan;
+  int32_t* count;
+} fvs_qwen_pick_plan_job;
+int fvs_qwen_pick_plan_multi(const fvs_qwen_pick_plan_job* jobs, int n_jobs, fvs_stream_t stream);
+/* fvs_qwen_pixel_gather_multi: per job, out[i] = pixel rows of frame plan[i] (i < n): frame f >= base is frame f - base
+ * of the pinned pixel chunks, chunk c holding chunk_frames frames of frame_elems 16-bit elements each; host_chunks is a
+ * DEVICE table of the chunks' mapped device pointers.  The chunks are read in place, as fvs_qwen_dam_gather reads its
+ * host tier (the same kernel, with no device tier); a frame outside [base, n_frames) yields zeros. */
+typedef struct fvs_qwen_pixel_job {
+  const int64_t* plan;
+  int n;
+  int64_t n_frames;
+  int64_t base;
+  const void* const* host_chunks;
+  int chunk_frames;
+  int64_t frame_elems;
+  void* out;
+} fvs_qwen_pixel_job;
+int fvs_qwen_pixel_gather_multi(const fvs_qwen_pixel_job* jobs, int n_jobs, int dtype, fvs_stream_t stream);
+/* fvs_qwen_bank_scatter_multi: per job, the reverse of fvs_qwen_dam_gather: x[plan[i]] = x_rows[i] and, when merged_rows
+ * is given, merged[plan[i]] = merged_rows[i], into the two-tier bank (device tier frames [0, n_dev), host chunks laid
+ * out as fvs_qwen_dam_gather reads them).  A plan entry outside [0, n_frames) writes nothing. */
+typedef struct fvs_qwen_scatter_job {
+  const int64_t* plan;
+  int n;
+  int64_t n_frames;
+  const void* x_rows;
+  const void* merged_rows;
+  void* dev_x;
+  void* dev_merged;
+  int64_t n_dev;
+  void* const* host_chunks;  /* DEVICE table */
+  int chunk_frames;
+  int64_t x_frame_elems;
+  int64_t merged_frame_elems;
+} fvs_qwen_scatter_job;
+int fvs_qwen_bank_scatter_multi(const fvs_qwen_scatter_job* jobs, int n_jobs, int dtype, fvs_stream_t stream);
 /* *dev_out = the device address of pinned host memory `host` (cudaHostGetDevicePointer); FVS_EINVAL if it is not pinned */
 int fvs_host_device_ptr(const void* host, void** dev_out);
 
