@@ -110,6 +110,21 @@ class QwenScatterJob(C.Structure):  # fvs_qwen_scatter_job
                 ("merged_frame_elems", C.c_int64)]
 
 
+class QwenPickPlanPrevJob(C.Structure):  # fvs_qwen_pick_plan_prev_job
+    _fields_ = [("picks", C.c_void_p), ("n", C.c_int), ("n_frames", C.c_int64), ("frames", C.c_void_p),
+                ("prev_picks", C.c_void_p), ("m", C.c_int), ("plan", C.c_void_p), ("count", C.c_void_p),
+                ("re_encodes", C.c_void_p)]
+
+
+class QwenFreshGatherJob(C.Structure):  # fvs_qwen_fresh_gather_job
+    _fields_ = [("picks", C.c_void_p), ("n", C.c_int), ("n_frames", C.c_int64), ("prev_picks", C.c_void_p),
+                ("m", C.c_int), ("prev_x", C.c_void_p), ("prev_merged", C.c_void_p), ("fresh_frames", C.c_void_p),
+                ("n_fresh", C.c_int), ("fresh_x", C.c_void_p), ("fresh_merged", C.c_void_p), ("n_base", C.c_int64),
+                ("dev_x", C.c_void_p), ("dev_merged", C.c_void_p), ("n_dev", C.c_int64), ("host_chunks", C.c_void_p),
+                ("chunk_frames", C.c_int), ("x_frame_elems", C.c_int64), ("merged_frame_elems", C.c_int64),
+                ("spa_x_out", C.c_void_p), ("merged_out", C.c_void_p), ("host_fetches", C.c_void_p)]
+
+
 QWEN_MEM_JOBS_PER_LAUNCH = 16
 PRE_CLIP, PRE_QWEN = 0, 1
 KLARGE_EUCLIDEAN, KLARGE_COSINE = 0, 1
@@ -194,6 +209,9 @@ SIGNATURES = {
     "fvs_qwen_pick_plan_multi": (_i, [C.POINTER(QwenPickPlanJob), _i, _vp]),
     "fvs_qwen_pixel_gather_multi": (_i, [C.POINTER(QwenPixelJob), _i, _i, _vp]),
     "fvs_qwen_bank_scatter_multi": (_i, [C.POINTER(QwenScatterJob), _i, _i, _vp]),
+    # no full-resolution bank
+    "fvs_qwen_pick_plan_prev_multi": (_i, [C.POINTER(QwenPickPlanPrevJob), _i, _vp]),
+    "fvs_qwen_dam_gather_fresh_multi": (_i, [C.POINTER(QwenFreshGatherJob), _i, _i, _vp]),
     # publication of the Qwen2-VL streaming memory (seqlock)
     "fvs_qwen_pub_layout": (_i, [_i, _i, _i, _i, _i, _i, _i, _i64p]),
     "fvs_qwen_publish": (_i, [_vp, _sz, _i, _i, C.c_int64, _i, _vp, C.c_int64, _vp, _i, _vp, _i, _i, _i, _i, _i, C.c_uint64,

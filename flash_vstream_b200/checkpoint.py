@@ -17,6 +17,10 @@ continue bit for bit as if it had never stopped (DESIGN.md §3.12):
       video_embeds [n_spa*h*w/4 + n_tem*hs*ws/4, merger_dim] (with a merger);
     counters n_frames, steps, n_tem, n_spa, fast_steps, redone_steps and the dtypes of the two CSM vectors; config = the
     FlashMemory config, grid, small_grid, dtype, dim, merger_dim.
+    A lazy_full_res state adds counters.pix_frames, encoded uint8 [n_frames] and pixels [pix_frames, h*w, 1176] (the
+    frames with pixel rows only).  A state without a full-resolution bank also adds counters.bank_frames: bank_x and
+    bank_merged then hold its base bank [bank_frames, ...], its mask bytes are 2 for a stored frame, and spa_x
+    [n_spa, h*w, D] carries the DAM's rows.
   * `rng`: the draw source a StreamPool stream owns (draws.DrawSource): torch CPU and CUDA generator states (uint8 tensors
     "rng.cpu" / "rng.cuda") and the `random.Random` state.  Streams that draw from the global generators carry none.
 
@@ -105,19 +109,24 @@ class StreamCheckpoint:
             return {}
         (h, w), (hs, ws) = c["grid"], c["small_grid"]
         D, md, dt = int(c["dim"]), c["merger_dim"], _dtype(c["dtype"], "config.dtype")
-        out = {"bank_x": ((n["n_frames"], h * w, D), dt), "bank_small": ((n["n_frames"], hs * ws, D), dt),
+        nb = n.get("bank_frames", n["n_frames"])      # frames with stored full-resolution rows (a stream without a bank: its base)
+        if not 0 <= nb <= n["n_frames"]:
+            raise ValueError(f"stream checkpoint: counters.bank_frames ({nb}) is outside [0, n_frames]")
+        out = {"bank_x": ((nb, h * w, D), dt), "bank_small": ((n["n_frames"], hs * ws, D), dt),
                "tem_x": ((n["n_tem"] * hs * ws, D), dt),
                "tem_timestamp": ((n["n_tem"],), _dtype(n["tem_timestamp_dtype"], "counters.tem_timestamp_dtype")),
                "spa_positions": ((n["n_spa"],), torch.int64)}
         if n["tem_weights_dtype"] is not None:       # temporal_method 'sample' keeps no weights
             out["tem_weights"] = ((n["n_tem"],), _dtype(n["tem_weights_dtype"], "counters.tem_weights_dtype"))
         if n["merged"]:
-            out["bank_merged"] = ((n["n_frames"], h * w // 4, md), dt)
+            out["bank_merged"] = ((nb, h * w // 4, md), dt)
         if md is not None:
             out["video_embeds"] = ((n["n_spa"] * h * w // 4 + n["n_tem"] * hs * ws // 4, md), dt)
         if "pix_frames" in n:                         # a lazy_full_res stream: its mask, the pixel rows of its frames not yet encoded
             out["encoded"] = ((n["n_frames"],), torch.uint8)
             out["pixels"] = ((n["pix_frames"], h * w, 3 * 2 * 14 * 14), dt)
+        if "bank_frames" in n:                        # no full-resolution bank: the DAM's rows, which no bank can rebuild
+            out["spa_x"] = ((n["n_spa"], h * w, D), dt)
         return out
 
     def _check(self):

@@ -12,6 +12,32 @@
 namespace fvs {
 namespace qwen {
 
+// The block's strided share (bx of nbx) of pick i's 16-byte words, from sources sx / sm (null: zeros): x words first,
+// then merged words.
+__device__ __forceinline__ void gather_copy(unsigned bx, unsigned nbx, int i, const uint4* sx, const uint4* sm,
+                                            long long fx, long long fm, uint4* out_x, uint4* out_m) {
+  const long long nx = out_x ? fx : 0, total = nx + (out_m ? fm : 0);
+  const long long stride = (long long)nbx * blockDim.x;
+  const uint4 zero = make_uint4(0, 0, 0, 0);
+  // four independent loads in flight per thread before the stores: a zero-copy read over PCIe has microseconds of latency
+  for (long long w0 = (long long)bx * blockDim.x + threadIdx.x; w0 < total; w0 += 4 * stride) {
+    uint4 v[4];
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+      const long long w = w0 + u * stride;
+      v[u] = zero;
+      if (w < nx) { if (sx) v[u] = sx[w]; }
+      else if (w < total && sm) v[u] = sm[w - nx];
+    }
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+      const long long w = w0 + u * stride;
+      if (w < nx) out_x[i * fx + w] = v[u];
+      else if (w < total) out_m[i * fm + (w - nx)] = v[u];
+    }
+  }
+}
+
 // Every block copies a strided share of one pick's 16-byte words: x words first, then merged words.
 // Sources, in order: the device tier, the same frame in the previous step's DAM (prev_x / prev_m), the host chunk.
 // A pick outside [0, n_frames) writes zeros (the host validates nothing on the device's behalf).
@@ -49,27 +75,7 @@ __device__ __forceinline__ void dam_gather_body(
     src[1] = sm;
   }
   __syncthreads();
-  const uint4 *sx = src[0], *sm = src[1];
-  const long long nx = out_x ? fx : 0, total = nx + (out_m ? fm : 0);
-  const long long stride = (long long)nbx * blockDim.x;
-  const uint4 zero = make_uint4(0, 0, 0, 0);
-  // four independent loads in flight per thread before the stores: a zero-copy read over PCIe has microseconds of latency
-  for (long long w0 = (long long)bx * blockDim.x + threadIdx.x; w0 < total; w0 += 4 * stride) {
-    uint4 v[4];
-#pragma unroll
-    for (int u = 0; u < 4; ++u) {
-      const long long w = w0 + u * stride;
-      v[u] = zero;
-      if (w < nx) { if (sx) v[u] = sx[w]; }
-      else if (w < total && sm) v[u] = sm[w - nx];
-    }
-#pragma unroll
-    for (int u = 0; u < 4; ++u) {
-      const long long w = w0 + u * stride;
-      if (w < nx) out_x[i * fx + w] = v[u];
-      else if (w < total) out_m[i * fm + (w - nx)] = v[u];
-    }
-  }
+  gather_copy(bx, nbx, i, src[0], src[1], fx, fm, out_x, out_m);
 }
 }  // namespace qwen
 }  // namespace fvs
@@ -315,6 +321,164 @@ int bank_scatter_launch(const fvs_qwen_scatter_job* jobs, int n, cudaStream_t st
   FVS_CHECK_LAUNCH("bank_scatter_kernel");
   return FVS_OK;
 }
+
+// ---- no full-resolution bank (DESIGN.md §3.19) ------------------------------------------------------------------------
+// Pick plan against the previous DAM: the pick_plan_kernel walk, with "held" meaning "in prev_picks, or byte 2 (stored
+// in the base bank)".  The plan reads prev_picks instead of a per-frame "in the previous DAM" mask, so nothing has to
+// move a mask from the old picks to the new ones after the gather, and a clip that complete() redoes plans against the
+// same previous DAM with nothing to undo.  The frame bytes only count re-encodes (0 -> 1 on a first encode), and only
+// the lane that plans a frame (its first pick) writes its byte, so the walk stays race-free.
+struct PlanPrevJobDev {
+  const long long* picks;
+  unsigned char* frames;
+  const long long* prev;
+  long long* plan;
+  int* count;
+  unsigned long long* re_encodes;
+  long long n_frames;
+  int n, m;
+};
+template <int kJobs>
+struct PlanPrevLaunch {
+  PlanPrevJobDev job[kJobs];
+};
+template <int kJobs>
+__global__ void __launch_bounds__(32) pick_plan_prev_kernel(const __grid_constant__ PlanPrevLaunch<kJobs> L) {
+  const PlanPrevJobDev& J = L.job[blockIdx.x];
+  const unsigned lane = threadIdx.x;
+  int base = 0, again = 0;
+  for (int i0 = 0; i0 < J.n; i0 += 32) {
+    const int i = i0 + int(lane);
+    long long p = -1;
+    bool first = false;
+    if (i < J.n) {
+      p = J.picks[i];
+      first = p >= 0 && p < J.n_frames && J.frames[p] != 2;
+      for (int j = 0; first && j < J.m; ++j)
+        if (J.prev[j] == p) first = false;
+      for (int j = 0; first && j < i; ++j)
+        if (J.picks[j] == p) first = false;
+    }
+    const unsigned ball = __ballot_sync(0xffffffffu, first);
+    if (first) {
+      J.plan[base + __popc(ball & ((1u << lane) - 1u))] = p;
+      again += J.frames[p] == 1;
+      J.frames[p] = 1;
+    }
+    base += __popc(ball);
+  }
+#pragma unroll
+  for (int o = 16; o; o >>= 1) again += __shfl_xor_sync(0xffffffffu, again, o);
+  if (lane == 0) {
+    *J.count = base;
+    if (J.re_encodes && again) atomicAdd(J.re_encodes, (unsigned long long)again);
+  }
+}
+
+template <int kJobs>
+int pick_plan_prev_launch(const fvs_qwen_pick_plan_prev_job* jobs, int n, cudaStream_t stream) {
+  PlanPrevLaunch<kJobs> L;
+  for (int q = 0; q < n; ++q) {
+    const fvs_qwen_pick_plan_prev_job& j = jobs[q];
+    L.job[q] = PlanPrevJobDev{(const long long*)j.picks, j.frames, (const long long*)j.prev_picks, (long long*)j.plan,
+                              (int*)j.count, (unsigned long long*)j.re_encodes, (long long)j.n_frames, j.n, j.m};
+  }
+  pick_plan_prev_kernel<kJobs><<<n, 32, 0, stream>>>(L);
+  FVS_CHECK_LAUNCH("pick_plan_prev_kernel");
+  return FVS_OK;
+}
+
+// Gather without a bank: dam_gather_body with the sources in the order previous DAM, fresh rows, stored base bank.  The
+// base comes last because a frame a lazy stream had not yet encoded when its checkpoint was taken has a zero slot there
+// (frame byte 0): such a frame is always planned, so it is found among the fresh rows first.
+struct FreshJobDev {
+  const long long* picks;
+  const long long* prev_picks;
+  const uint4* prev_x;
+  const uint4* prev_m;
+  const long long* fresh;
+  const uint4* fresh_x;
+  const uint4* fresh_m;
+  const uint4* dev_x;
+  const uint4* dev_m;
+  const uint4* const* chunks;
+  uint4* out_x;
+  uint4* out_m;
+  unsigned long long* host_fetches;
+  long long n_frames, n_base, n_dev, chunk_frames, fx, fm;
+  int m, n_fresh, bx;
+};
+template <int kJobs>
+struct FreshLaunch {
+  FreshJobDev job[kJobs];
+  int first[kJobs + 1];
+  int n;
+};
+template <int kJobs>
+__global__ void __launch_bounds__(256) fresh_gather_kernel(const __grid_constant__ FreshLaunch<kJobs> L) {
+  int j = 0;
+  if constexpr (kJobs > 1)
+    while (j + 1 < L.n && blockIdx.x >= unsigned(L.first[j + 1])) ++j;
+  const FreshJobDev& J = L.job[j];
+  const unsigned b = blockIdx.x - unsigned(L.first[j]), bx = b % unsigned(J.bx);
+  const int i = int(b / unsigned(J.bx));
+  __shared__ const uint4* src[2];
+  if (threadIdx.x == 0) {
+    const long long p = J.picks[i];
+    const uint4 *sx = nullptr, *sm = nullptr;
+    if (p >= 0 && p < J.n_frames) {
+      int k = 0;
+      while (k < J.m && J.prev_picks[k] != p) ++k;
+      if (k < J.m) {
+        sx = J.prev_x + k * J.fx;
+        sm = J.prev_m ? J.prev_m + k * J.fm : nullptr;
+      } else {
+        k = 0;
+        while (k < J.n_fresh && J.fresh[k] != p) ++k;
+        if (k < J.n_fresh) {
+          sx = J.fresh_x + k * J.fx;
+          sm = J.fresh_m ? J.fresh_m + k * J.fm : nullptr;
+        } else if (p < J.n_dev) {
+          sx = J.dev_x + p * J.fx;
+          sm = J.dev_m ? J.dev_m + p * J.fm : nullptr;
+        } else if (p < J.n_base) {
+          const long long q = p - J.n_dev, off = q % J.chunk_frames;
+          const uint4* c = J.chunks[q / J.chunk_frames];
+          sx = c + off * J.fx;
+          sm = c + J.chunk_frames * J.fx + off * J.fm;
+          if (bx == 0 && J.host_fetches) atomicAdd(J.host_fetches, 1ull);
+        }
+      }
+    }
+    src[0] = sx;
+    src[1] = sm;
+  }
+  __syncthreads();
+  gather_copy(bx, J.bx, i, src[0], src[1], J.fx, J.fm, J.out_x, J.out_m);
+}
+
+template <int kJobs>
+int fresh_gather_launch(const fvs_qwen_fresh_gather_job* jobs, int n, cudaStream_t stream) {
+  FreshLaunch<kJobs> L;
+  L.n = n;
+  L.first[0] = 0;
+  for (int q = 0; q < n; ++q) {
+    const fvs_qwen_fresh_gather_job& g = jobs[q];
+    const long long fx = g.x_frame_elems * 2 / 16, fm = g.merged_frame_elems * 2 / 16;
+    long long bx = ((g.spa_x_out ? fx : 0) + (g.merged_out ? fm : 0) + 4 * 256 - 1) / (4 * 256);
+    bx = bx > 64 ? 64 : bx < 1 ? 1 : bx;
+    L.job[q] = FreshJobDev{(const long long*)g.picks, (const long long*)g.prev_picks, (const uint4*)g.prev_x,
+                           (const uint4*)g.prev_merged, (const long long*)g.fresh_frames, (const uint4*)g.fresh_x,
+                           (const uint4*)g.fresh_merged, (const uint4*)g.dev_x, (const uint4*)g.dev_merged,
+                           (const uint4* const*)g.host_chunks, (uint4*)g.spa_x_out, (uint4*)g.merged_out,
+                           (unsigned long long*)g.host_fetches, (long long)g.n_frames, (long long)g.n_base,
+                           (long long)g.n_dev, (long long)g.chunk_frames, fx, fm, g.m, g.n_fresh, int(bx)};
+    L.first[q + 1] = L.first[q] + int(bx) * g.n;
+  }
+  fresh_gather_kernel<kJobs><<<L.first[n], 256, 0, stream>>>(L);
+  FVS_CHECK_LAUNCH("fresh_gather_kernel");
+  return FVS_OK;
+}
 }  // namespace
 
 extern "C" {
@@ -421,6 +585,80 @@ int fvs_qwen_bank_scatter_multi(const fvs_qwen_scatter_job* jobs, int n_jobs, in
     const int n = std::min(kGatherJobs, n_jobs - i0);
     const int r = n == 1 ? bank_scatter_launch<1>(jobs + i0, 1, (cudaStream_t)stream)
                          : bank_scatter_launch<kGatherJobs>(jobs + i0, n, (cudaStream_t)stream);
+    if (r) return r;
+  }
+  return FVS_OK;
+}
+
+int fvs_qwen_pick_plan_prev_multi(const fvs_qwen_pick_plan_prev_job* jobs, int n_jobs, fvs_stream_t stream) {
+  const char* api = "fvs_qwen_pick_plan_prev_multi";
+  FVS_REQUIRE(jobs && n_jobs > 0, "%s: need a job table and n_jobs > 0", api);
+  for (int i = 0; i < n_jobs; ++i) {
+    const fvs_qwen_pick_plan_prev_job& j = jobs[i];
+    FVS_REQUIRE(j.n >= 0 && j.n <= 65535 && j.m >= 0 && j.m <= 65535 && j.n_frames >= 0,
+                "%s: job %d: bad sizes (n=%d, m=%d, n_frames=%lld)", api, i, j.n, j.m, (long long)j.n_frames);
+    FVS_REQUIRE((j.picks || j.n == 0) && (j.prev_picks || j.m == 0), "%s: job %d: null picks or previous picks", api, i);
+    FVS_REQUIRE(j.frames && j.count && (j.plan || j.n == 0), "%s: job %d: null frame bytes, plan or count", api, i);
+    FVS_REQUIRE(((uintptr_t)j.picks & 7) == 0 && ((uintptr_t)j.prev_picks & 7) == 0 && ((uintptr_t)j.plan & 7) == 0 &&
+                    ((uintptr_t)j.count & 3) == 0 && ((uintptr_t)j.re_encodes & 7) == 0,
+                "%s: job %d: misaligned picks, plan, count or counter", api, i);
+    for (int k = 0; k < i; ++k)
+      FVS_REQUIRE(jobs[k].frames != j.frames && jobs[k].count != j.count && (j.n == 0 || jobs[k].plan != j.plan) &&
+                      (!j.re_encodes || jobs[k].re_encodes != j.re_encodes),
+                  "%s: jobs %d and %d share an output", api, k, i);
+  }
+  for (int i0 = 0; i0 < n_jobs; i0 += kGatherJobs) {
+    const int n = std::min(kGatherJobs, n_jobs - i0);
+    const int r = n == 1 ? pick_plan_prev_launch<1>(jobs + i0, 1, (cudaStream_t)stream)
+                         : pick_plan_prev_launch<kGatherJobs>(jobs + i0, n, (cudaStream_t)stream);
+    if (r) return r;
+  }
+  return FVS_OK;
+}
+
+int fvs_qwen_dam_gather_fresh_multi(const fvs_qwen_fresh_gather_job* jobs, int n_jobs, int dtype, fvs_stream_t stream) {
+  const char* api = "fvs_qwen_dam_gather_fresh_multi";
+  FVS_REQUIRE(jobs && n_jobs > 0, "%s: need a job table and n_jobs > 0", api);
+  FVS_REQUIRE(dtype == FVS_F16 || dtype == FVS_BF16, "%s: dtype must be f16 or bf16", api);
+  struct Range { uintptr_t lo, hi; int job; };
+  std::vector<Range> out;
+  for (int i = 0; i < n_jobs; ++i) {
+    const fvs_qwen_fresh_gather_job& j = jobs[i];
+    const int64_t fx = j.x_frame_elems, fm = j.merged_frame_elems;
+    FVS_REQUIRE(j.picks && j.n > 0 && j.n <= 65535, "%s: job %d: need picks and 0 < n <= 65535", api, i);
+    FVS_REQUIRE(j.spa_x_out || j.merged_out, "%s: job %d: no output", api, i);
+    FVS_REQUIRE(j.n_frames > 0 && j.n_dev >= 0 && j.n_dev <= j.n_base && j.n_base <= j.n_frames,
+                "%s: job %d: need 0 <= n_dev <= n_base <= n_frames, n_frames > 0", api, i);
+    FVS_REQUIRE(fx > 0 && fm >= 0 && (fx * 2) % 16 == 0 && (fm * 2) % 16 == 0,
+                "%s: job %d: frame sizes must be multiples of 16 bytes", api, i);
+    FVS_REQUIRE(!j.merged_out || fm > 0, "%s: job %d: merged_out without merged rows", api, i);
+    FVS_REQUIRE(j.m >= 0 && j.m <= 65535 && (j.m == 0 || (j.prev_picks && j.prev_x && (!j.merged_out || j.prev_merged))),
+                "%s: job %d: bad previous DAM", api, i);
+    FVS_REQUIRE(j.n_fresh >= 0 && j.n_fresh <= 65535 &&
+                    (j.n_fresh == 0 || (j.fresh_frames && j.fresh_x && (!j.merged_out || j.fresh_merged))),
+                "%s: job %d: bad fresh rows", api, i);
+    FVS_REQUIRE(j.n_dev == 0 || (j.dev_x && (!j.merged_out || j.dev_merged)), "%s: job %d: null device tier", api, i);
+    FVS_REQUIRE(j.n_dev == j.n_base || (j.host_chunks && j.chunk_frames > 0), "%s: job %d: host frames without a chunk table",
+                api, i);
+    for (const void* p : {j.prev_x, j.prev_merged, j.fresh_x, j.fresh_merged, j.dev_x, j.dev_merged,
+                          (const void*)j.spa_x_out, (const void*)j.merged_out})
+      FVS_REQUIRE(aligned16(p), "%s: job %d: row tensors must be 16-byte aligned", api, i);
+    FVS_REQUIRE(((uintptr_t)j.picks & 7) == 0 && ((uintptr_t)j.prev_picks & 7) == 0 &&
+                    ((uintptr_t)j.fresh_frames & 7) == 0 && ((uintptr_t)j.host_chunks & 7) == 0 &&
+                    ((uintptr_t)j.host_fetches & 7) == 0,
+                "%s: job %d: index tables must be 8-byte aligned", api, i);
+    if (j.spa_x_out) out.push_back({uintptr_t(j.spa_x_out), uintptr_t(j.spa_x_out) + size_t(j.n) * fx * 2, i});
+    if (j.merged_out) out.push_back({uintptr_t(j.merged_out), uintptr_t(j.merged_out) + size_t(j.n) * fm * 2, i});
+    if (j.host_fetches) out.push_back({uintptr_t(j.host_fetches), uintptr_t(j.host_fetches) + 8, i});
+  }
+  for (size_t a = 0; a < out.size(); ++a)
+    for (size_t b = a + 1; b < out.size(); ++b)
+      FVS_REQUIRE(out[a].job == out[b].job || out[a].hi <= out[b].lo || out[b].hi <= out[a].lo,
+                  "%s: jobs %d and %d share an output", api, out[a].job, out[b].job);
+  for (int i0 = 0; i0 < n_jobs; i0 += kGatherJobs) {
+    const int n = std::min(kGatherJobs, n_jobs - i0);
+    const int r = n == 1 ? fresh_gather_launch<1>(jobs + i0, 1, (cudaStream_t)stream)
+                         : fresh_gather_launch<kGatherJobs>(jobs + i0, n, (cudaStream_t)stream);
     if (r) return r;
   }
   return FVS_OK;

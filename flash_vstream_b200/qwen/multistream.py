@@ -32,7 +32,7 @@ from .. import _lib as L
 from ..draws import DrawSource
 from . import ops as Q
 from .stream_state import (_KMEANS_METHODS, PATCH_DIM, QwenStreamState, _rest_finish, check_device_frames,
-                           check_lazy_full_res, enqueue_csm)
+                           check_full_res_bank, check_lazy_full_res, enqueue_csm)
 from .vision_tower import QwenVisionBlocksB200
 
 MAX_GRIDS = 16            # grid entries one fvs_qwen_vit_encode call takes
@@ -88,11 +88,15 @@ def encode_picked(states, readbacks: torch.Tensor, max_rows: int = TOWER_ROWS):
     PatchMerger per tower call (plan_tower_calls), and fvs_qwen_bank_scatter_multi writes them into the banks.  Last,
     the DAM gathers and the CSM merger of every state (stream_state._rest_finish).  The tower, the first state's, is
     invariant to batch composition (§3.7) and the merger row-wise (§3.5), so each frame gets the bits of the eager
-    path."""
+    path.
+    A state without full_res_bank (§3.19) plans through fvs_qwen_pick_plan_prev_multi instead: the picks its previous
+    DAM does not hold (a DAM that is the whole bank plans the frames the previous one did not have, a count the host
+    knows).  Its tower and merger rows are not scattered anywhere: they stay as the state's fresh rows, which the DAM
+    gather (fvs_qwen_dam_gather_fresh_multi) reads beside the previous DAM, and are dropped after it."""
     if any(st._lazy_ctx["n_spa"] and st.tower is None for st in states):     # refused before any mask byte is set
         raise NotImplementedError("lazy_full_res: no full-resolution tower was given to the stream state")
     addr = Q.host_device_ptr(readbacks)
-    jobs, counts = [], []
+    jobs, prev_jobs, counts = [], [], []
     for k, st in enumerate(states):
         c = st._lazy_ctx
         n_spa, n = c["n_spa"], st.n_frames
@@ -101,11 +105,22 @@ def encode_picked(states, readbacks: torch.Tensor, max_rows: int = TOWER_ROWS):
             counts.append(0)
             continue
         whole = n_spa == n
-        jobs.append((None if whole else c["picks"], n_spa, st.encoded.buf, n, st._plan,
-                     addr + (k * 8 + 7) * readbacks.element_size()))
-        counts.append(n - st.n_encoded if whole else None)
+        count = addr + (k * 8 + 7) * readbacks.element_size()
+        if st.full_res_bank:
+            jobs.append((None if whole else c["picks"], n_spa, st.encoded.buf, n, st._plan, count))
+            counts.append(n - st.n_encoded if whole else None)
+            continue
+        # the previous DAM of a whole-bank DAM is frames [0, m) (spatial_picks returns arange while n <= spatial_length)
+        prev = st._prev_dam
+        if st.re_encodes is None:
+            st.re_encodes = torch.zeros(1, dtype=torch.int64, device=st._plan.device)
+        prev_jobs.append((c["picks"], st.encoded.buf, n, None if prev is None else prev[0], st._plan, count,
+                          st.re_encodes))
+        counts.append(n - (0 if prev is None else prev[0].numel()) if whole else None)
     if jobs:
         Q.pick_plan_multi(jobs)
+    if prev_jobs:
+        Q.pick_plan_prev_multi(prev_jobs)
     if any(v is None for v in counts) or any(st._pending for st in states):
         done = torch.cuda.Event()
         done.record()
@@ -132,14 +147,20 @@ def encode_picked(states, readbacks: torch.Tensor, max_rows: int = TOWER_ROWS):
             for i, (off,) in places:
                 st, n = todo[i]
                 r = n * st.grid[0] * st.grid[1]
-                scatters.append(st._scatter_args(n, feats[off: off + r],
-                                                 None if merged is None else merged[off // 4: (off + r) // 4]))
-            Q.bank_scatter_multi(scatters)
+                rows = (feats[off: off + r], None if merged is None else merged[off // 4: (off + r) // 4])
+                if st.full_res_bank:
+                    scatters.append(st._scatter_args(n, *rows))
+                else:
+                    st._fresh = (st._plan, n) + rows
+            if scatters:
+                Q.bank_scatter_multi(scatters)
     ctxs = []
     for st in states:
         ctxs.append((st, st._lazy_ctx))
         st._lazy_ctx, st._in_round = None, False
     _rest_finish(ctxs)
+    for st in states:
+        st._fresh = None                   # the DAM holds the fresh rows it picked now
 
 
 class _Stream:
@@ -165,13 +186,17 @@ class QwenStreamPool:
     `step` also takes decoded uint8 frames [T, H, W, 3] per stream (any mix of sizes, host or device); the round's clips
     go through ONE `preprocess.many` call, and each stream's rows and grid then make its (pixel_values_videos,
     video_grid_thw).  `lazy_full_res` (QwenStreamState's): the round runs the full-resolution tower once, after its one
-    host wait, on only the frames some stream's DAM picks for the first time (encode_picked, DESIGN.md §3.18)."""
+    host wait, on only the frames some stream's DAM picks for the first time (encode_picked, DESIGN.md §3.18).
+    `full_res_bank=False` (with lazy_full_res): every stream keeps no full-resolution or merged rows beyond its DAM, and
+    the round's one tower pass also re-encodes the picks a stream's previous DAM does not hold (§3.19).  The knobs are the
+    pool's: eager, lazy and bank-less streams do not share a pool."""
 
     TOWER_ROWS = TOWER_ROWS
     BATCH_MIN_JOBS = 4        # fewer k-means streams in a round take one enqueue_csm call each
 
     def __init__(self, model, device_frames: Optional[int] = None, max_streams: Optional[int] = None,
-                 small_device_frames: Optional[int] = None, preprocess=None, lazy_full_res: bool = False):
+                 small_device_frames: Optional[int] = None, preprocess=None, lazy_full_res: bool = False,
+                 full_res_bank: bool = True):
         visual = model.visual
         flash, tower = visual.flash_memory, visual.encode_patches
         if not isinstance(tower, QwenVisionBlocksB200):
@@ -193,6 +218,7 @@ class QwenStreamPool:
         self.device_frames = check_device_frames(device_frames, "device_frames")
         self.small_device_frames = check_device_frames(small_device_frames, "small_device_frames")
         self.lazy_full_res = check_lazy_full_res(lazy_full_res, flash)
+        self.full_res_bank = check_full_res_bank(full_res_bank, self.lazy_full_res)
         self.max_streams = max_streams
         self.preprocess = preprocess
         self._readbacks: Optional[torch.Tensor] = None     # pinned int32 [S, 8]: the round's read-backs
@@ -211,11 +237,12 @@ class QwenStreamPool:
             raise ValueError("QwenStreamPool.open: this checkpoint carries no draw source (single-stream host): pass seed=")
         if checkpoint is None:
             state = QwenStreamState(self.flash, self.merger, device_frames=self.device_frames,
-                                    small_device_frames=self.small_device_frames, lazy_full_res=self.lazy_full_res)
+                                    small_device_frames=self.small_device_frames, lazy_full_res=self.lazy_full_res,
+                                    full_res_bank=self.full_res_bank)
         else:
             state = QwenStreamState.restore(checkpoint, self.flash, self.merger, self.device, device_frames=self.device_frames,
                                             small_device_frames=self.small_device_frames,
-                                            lazy_full_res=self.lazy_full_res)
+                                            lazy_full_res=self.lazy_full_res, full_res_bank=self.full_res_bank)
         state.tower = self.tower
         if seed is None and checkpoint is None:
             seed = int.from_bytes(os.urandom(8), "little") >> 1

@@ -265,6 +265,59 @@ def bank_scatter_multi(jobs):
             "fvs_qwen_bank_scatter_multi")
 
 
+def pick_plan_prev_multi(jobs):
+    """fvs_qwen_pick_plan_prev_multi: jobs = [(picks int64 [n], frames uint8 [>= n_frames], n_frames, prev_picks int64
+    [m] or None, plan int64 [>= n], count address, re_encodes int64 [1] or None)], count address as for
+    pick_plan_multi.  Plans the picks the previous DAM does not hold (frame byte 2: stored in the base bank) and sets the
+    planned frames' bytes to 1."""
+    arr, keep = [], []
+    for picks, frames, n_frames, prev, plan, count, re_enc in jobs:
+        _chk_cuda(picks, frames, prev, plan, re_enc)
+        picks, prev = _c(picks), None if prev is None or prev.numel() == 0 else _c(prev)
+        assert picks.dtype == torch.int64 and frames.dtype == torch.uint8 and plan.dtype == torch.int64
+        assert plan.numel() >= picks.numel() and (prev is None or prev.dtype == torch.int64)
+        keep.append((picks, prev))
+        arr.append(L.QwenPickPlanPrevJob(picks=picks.data_ptr(), n=picks.numel(), n_frames=int(n_frames),
+                                         frames=frames.data_ptr(), prev_picks=L.ptr(prev),
+                                         m=0 if prev is None else prev.numel(), plan=plan.data_ptr(), count=int(count),
+                                         re_encodes=L.ptr(re_enc)))
+    L.check(L.load().fvs_qwen_pick_plan_prev_multi((L.QwenPickPlanPrevJob * len(arr))(*arr), len(arr), L.cur_stream()),
+            "fvs_qwen_pick_plan_prev_multi")
+
+
+def dam_gather_fresh_multi(calls):
+    """fvs_qwen_dam_gather_fresh_multi: calls = [dict(picks, n_frames, prev (picks, x rows, merged rows or None) or None,
+    fresh (plan int64, n_fresh, x rows, merged rows or None) or None, n_base, dev_x, dev_merged, n_dev, chunks,
+    chunk_frames, x_frame_elems, merged_frame_elems, spa_x_out, merged_out, host_fetches)], one per stream, all outputs of
+    one dtype"""
+    jobs, keep = [], []
+    for a in calls:
+        picks, prev, fresh, sx, mo = _c(a["picks"]), a.get("prev"), a.get("fresh"), a.get("spa_x_out"), a.get("merged_out")
+        _chk_cuda(picks, a["dev_x"], a["dev_merged"], a["chunks"], sx, mo, a.get("host_fetches"))
+        m, pp, px, pm = 0, None, None, None
+        if prev is not None and prev[0] is not None and prev[0].numel():
+            pp, px, pm = prev
+            pp = _c(pp)
+            m = pp.numel()
+        nf, fp, fx, fm = 0, None, None, None
+        if fresh is not None and fresh[1]:
+            fp, nf, fx, fm = fresh
+            _chk_cuda(fp, fx, fm)
+            assert fp.dtype == torch.int64 and fx.is_contiguous() and (fm is None or fm.is_contiguous())
+        keep.append((picks, pp))
+        jobs.append(L.QwenFreshGatherJob(
+            picks=picks.data_ptr(), n=picks.numel(), n_frames=int(a["n_frames"]), prev_picks=L.ptr(pp), m=m,
+            prev_x=L.ptr(px), prev_merged=L.ptr(pm), fresh_frames=L.ptr(fp), n_fresh=int(nf), fresh_x=L.ptr(fx),
+            fresh_merged=L.ptr(fm), n_base=int(a["n_base"]), dev_x=L.ptr(a["dev_x"]), dev_merged=L.ptr(a["dev_merged"]),
+            n_dev=int(a["n_dev"]), host_chunks=L.ptr(a["chunks"]), chunk_frames=int(a["chunk_frames"]),
+            x_frame_elems=int(a["x_frame_elems"]), merged_frame_elems=int(a["merged_frame_elems"]), spa_x_out=L.ptr(sx),
+            merged_out=L.ptr(mo), host_fetches=L.ptr(a.get("host_fetches"))))
+    out0 = calls[0].get("spa_x_out") if calls[0].get("spa_x_out") is not None else calls[0].get("merged_out")
+    arr = (L.QwenFreshGatherJob * len(jobs))(*jobs)
+    L.check(L.load().fvs_qwen_dam_gather_fresh_multi(arr, len(jobs), L.dtype_code(out0.dtype), L.cur_stream()),
+            "fvs_qwen_dam_gather_fresh_multi")
+
+
 def mem_workspace_bytes(T: int, K: int, PD: int) -> int:
     """bytes one job of the CSM chain needs besides its outputs: fp32 centroids, unique-rows and k-means workspaces"""
     lib = L.load()

@@ -74,15 +74,20 @@ class QwenStreamState:
     once per step, twice with the cosine metric.  The two caps are independent; results are bit-identical either way.
     lazy_full_res: keep each clip's full-resolution pixel rows in pinned host chunks instead of its tower features, and
     run the full-resolution tower on a frame only the first time the DAM picks it (DESIGN.md §3.18); step() then takes
-    the pixel rows in place of x_new, and the tower.  The published bits are the eager state's."""
+    the pixel rows in place of x_new, and the tower.  The published bits are the eager state's.
+    full_res_bank: False (with lazy_full_res only) keeps no full-resolution or merged row of the frames the stream
+    encodes: the step gathers its DAM from the previous DAM and from this step's tower output, and re-encodes a pick the
+    previous DAM does not hold from its pixel rows (DESIGN.md §3.19).  Same bits again."""
 
     CHUNK_BYTES = CHUNK_BYTES
 
-    def __init__(self, flash, merger, device_frames=None, small_device_frames=None, lazy_full_res=False):
+    def __init__(self, flash, merger, device_frames=None, small_device_frames=None, lazy_full_res=False,
+                 full_res_bank=True):
         self.flash, self.merger = flash, merger
         self.device_frames = check_device_frames(device_frames)
         self.small_device_frames = check_device_frames(small_device_frames, "small_device_frames")
         self.lazy_full_res = check_lazy_full_res(lazy_full_res, flash)
+        self.full_res_bank = check_full_res_bank(full_res_bank, self.lazy_full_res)
         self.rng = GLOBAL                     # the draws.DrawSource of every k-means draw (a QwenStreamPool stream owns one)
         self.reset()
 
@@ -111,8 +116,12 @@ class QwenStreamState:
         self.fast_steps = self.redone_steps = 0
         self.steps = 0                        # clips whose step completed (a clip that raises is not counted)
         self.encoded = RowBank()              # lazy_full_res: device uint8 [n_frames], 1 once a frame's bank slots are filled
+        #                                       (no full_res_bank: 1 once encoded, 2 when its rows are in the base bank)
         self.pixels: Optional[PixelStore] = None   # lazy_full_res: the frames' full-resolution pixel rows
-        self.n_encoded = 0                    # lazy_full_res: frames the full-resolution tower has encoded
+        self.n_encoded = 0                    # lazy_full_res: frames the full-resolution tower has encoded (no
+        #                                       full_res_bank: every encode, re-encodes included)
+        self.re_encodes = None                # no full_res_bank: device int64 [1], encodes of frames encoded before
+        self._fresh = None                    # no full_res_bank: (plan, n, x rows, merged rows) of this step's encodes
         self.tower = None                     # lazy_full_res: callable(pixel rows, grids) -> full-resolution features
         self._in_round = False                # lazy_full_res: the outputs of this step wait for multistream.encode_picked
         self._lazy_ctx = None                 # lazy_full_res: the retrieval context those outputs are made from
@@ -297,7 +306,8 @@ class QwenStreamState:
         tem_x, picks, n_spa = ctx["tem_x"], ctx["picks"], ctx["n_spa"]
         D = tem_x.shape[-1]
         dt, dev = self._small_layout[0], tem_x.device
-        whole = n_spa == self.n_frames and self.n_host == 0   # memory still filling: the DAM is the whole bank, a view of it
+        # memory still filling: the DAM is the whole bank, a view of it (a state without a bank gathers it)
+        whole = n_spa == self.n_frames and self.n_host == 0 and self.full_res_bank
         spa_x = self.bank_x.rows() if whole else torch.empty(n_spa, h * w, D, dtype=dt, device=dev)
         self.spa_x, self.spa_positions = spa_x, picks
         pm = h * w // 4                                               # merged tokens of a retrieved frame
@@ -368,7 +378,8 @@ class QwenStreamState:
 
     def _append_lazy(self, pix3, dt, D, dev):
         """lazy_full_res: the clip's pixel rows pix3 [t, h*w, 1176] appended to the pixel store (asynchronous copies to its
-        pinned chunks), and t bank slots (zero rows in HBM, chunk rows on the host) with clear mask bytes"""
+        pinned chunks), and t bank slots (zero rows in HBM, chunk rows on the host; none without full_res_bank) with clear
+        mask bytes"""
         t, hw = pix3.shape[0], pix3.shape[1]
         if self._layout is None:
             ms = None
@@ -378,6 +389,12 @@ class QwenStreamState:
         if self.pixels is None:
             self.pixels = PixelStore(pix3.dtype, hw * PATCH_DIM, self.n_frames, self.CHUNK_BYTES)
         self.pixels.append(pix3.reshape(t, -1), dev)
+        if self.full_res_bank:
+            self._append_slots(t, dev)
+        self.encoded.append(torch.zeros(t, dtype=torch.uint8, device=dev))
+
+    def _append_slots(self, t: int, dev):
+        """t zero bank slots (rows in HBM, chunk rows on the host) at the end of the two-tier bank"""
         dt, xs, ms = self._layout
         for c, _, _, cnt in placement(self.bank_x.n + self.n_host, t, self.device_frames, self._per_chunk()):
             if c < 0:
@@ -387,7 +404,6 @@ class QwenStreamState:
                 continue
             self._chunk(c, dev)
             self.n_host += cnt
-        self.encoded.append(torch.zeros(t, dtype=torch.uint8, device=dev))
 
     def _scatter_args(self, n: int, x_rows, merged_rows) -> dict:
         """the job of Q.bank_scatter_multi that writes the n frames of this state's last pick plan into its banks"""
@@ -432,13 +448,26 @@ class QwenStreamState:
                             self._small_per_chunk(), rb.n + self.n_small_host, self._small_layout[0], dev)
 
     def _gather(self, picks, spa_x, merged, prev):
-        Q.dam_gather(**self._gather_args(picks, spa_x, merged, prev))
+        args = self._gather_args(picks, spa_x, merged, prev)
+        if self.full_res_bank:
+            Q.dam_gather(**args)
+        else:
+            Q.dam_gather_fresh_multi([args])
 
     def _gather_args(self, picks, spa_x, merged, prev) -> dict:
-        """the keyword arguments of the Q.dam_gather that writes spa_x / merged for `picks` from this state's banks"""
+        """the keyword arguments of the Q.dam_gather that writes spa_x / merged for `picks` from this state's banks;
+        without full_res_bank, of the Q.dam_gather_fresh_multi job that reads the previous DAM `prev`, this step's fresh
+        rows and the base bank"""
         dt, xs, ms = self._layout
         if self.host_fetches is None:
             self.host_fetches = torch.zeros(1, dtype=torch.int64, device=picks.device)
+        if not self.full_res_bank:
+            return dict(picks=picks, n_frames=self.n_frames, prev=prev, fresh=self._fresh,
+                        n_base=self.bank_x.n + self.n_host, dev_x=self.bank_x.buf if self.bank_x.n else None,
+                        dev_merged=self.bank_merged.buf if self.bank_merged.n else None, n_dev=self.bank_x.n,
+                        chunks=self._chunk_table, chunk_frames=self._per_chunk(), x_frame_elems=xs.numel(),
+                        merged_frame_elems=0 if ms is None else ms.numel(), spa_x_out=spa_x, merged_out=merged,
+                        host_fetches=self.host_fetches)
         return dict(picks=picks, n_frames=self.bank_x.n + self.n_host, dev_x=self.bank_x.buf if self.bank_x.n else None,
                     dev_merged=self.bank_merged.buf if self.bank_merged.n else None, n_dev=self.bank_x.n,
                     chunks=self._chunk_table, chunk_frames=self._per_chunk(), x_frame_elems=xs.numel(),
@@ -449,12 +478,22 @@ class QwenStreamState:
         """retrieved frames read from the host chunks since the stream started here (synchronises; tests and timing)"""
         return 0 if self.host_fetches is None else int(self.host_fetches.item())
 
+    def re_encode_count(self) -> int:
+        """without full_res_bank: full-resolution encodes of frames the tower had encoded before, since the stream
+        started here (a clip redone by complete() counts its encodes again; synchronises; tests and timing)"""
+        return 0 if self.re_encodes is None else int(self.re_encodes.item())
+
     def _bank_on_host(self, merged: bool) -> torch.Tensor:
         """the whole full-resolution (or merged) bank as one pinned host tensor: device rows D2H, chunk rows H2H"""
         dt, xs, ms = self._layout
         rb = self.bank_merged if merged else self.bank_x
         chunks = [self._chunk(c, None)[int(merged)] for c in range(len(self.host_chunks))]
-        return _on_host(rb, chunks, self.n_frames, ms if merged else xs, dt)
+        return _on_host(rb, chunks, self.bank_x.n + self.n_host, ms if merged else xs, dt)
+
+    def pinned_bytes(self) -> int:
+        """bytes of pinned host memory the state holds: bank chunks, half-resolution chunks and pixel chunks"""
+        bufs = self.host_chunks + self.small_chunks + ([] if self.pixels is None else self.pixels.chunks)
+        return sum(b.numel() * b.element_size() for b in bufs)
 
     def _small_on_host(self) -> torch.Tensor:
         """the whole half-resolution bank as one pinned host tensor: device rows D2H, chunk rows H2H"""
@@ -493,8 +532,11 @@ class QwenStreamState:
                     "tem_weights_dtype": None if self.tem_weights is None else CK.dtype_name(self.tem_weights.dtype),
                     "tem_timestamp_dtype": "float32" if n == 0 else CK.dtype_name(self.tem_timestamp.dtype)}
         if self.lazy_full_res and n:          # eager checkpoints carry neither the counter nor the tensors below
-            todo = torch.nonzero(self.encoded.rows().cpu() == 0).flatten().tolist()   # frames not yet encoded
+            stored = 2 if not self.full_res_bank else 1           # the mask byte of a frame whose rows are stored
+            todo = torch.nonzero(self.encoded.rows().cpu() != stored).flatten().tolist()   # frames with pixel rows only
             counters["pix_frames"] = len(todo)
+            if not self.full_res_bank:        # the stored (base) bank's frames; the DAM's rows travel as spa_x
+                counters["bank_frames"] = self.bank_x.n + self.n_host
         if n == 0:
             return CK.qwen(self._config(0, "float16"), counters, {})
         dt, ps = self._small_layout
@@ -508,6 +550,8 @@ class QwenStreamState:
             if self.lazy_full_res:                # the mask, and the pixel rows of the frames not yet encoded, in order
                 tensors["encoded"] = self.encoded.rows()
                 owned["pixels"] = self.pixels.rows_of(todo).view(len(todo), self._layout[1][0], PATCH_DIM)
+            if not self.full_res_bank:
+                tensors["spa_x"] = self.spa_x
             if self.n_small_host:
                 owned["bank_small"] = self._small_on_host()
             else:
@@ -515,22 +559,29 @@ class QwenStreamState:
             for name, merged in (("bank_x", False), ("bank_merged", True)):
                 if merged and not counters["merged"]:
                     continue
+                rb = self.bank_merged if merged else self.bank_x
                 if self.n_host:
                     owned[name] = self._bank_on_host(merged)
-                else:
-                    tensors[name] = (self.bank_merged if merged else self.bank_x).rows()
+                elif rb.n:
+                    tensors[name] = rb.rows()
+                else:                             # no full_res_bank and no base bank: zero frames
+                    dt_, xs, ms = self._layout
+                    tensors[name] = torch.empty((0,) + tuple(ms if merged else xs), dtype=dt_)
             ck = CK.qwen(self._config(int(ps[-1]), CK.dtype_name(dt)), counters, tensors, owned=owned)
             torch.cuda.current_stream().synchronize()
         return ck
 
     @classmethod
     def restore(cls, ckpt, flash, merger, device, device_frames=None, small_device_frames=None,
-                lazy_full_res=False) -> "QwenStreamState":
+                lazy_full_res=False, full_res_bank=True) -> "QwenStreamState":
         """A state on `device` that continues `ckpt` bit for bit; `flash` / `merger` must have the configuration the
         checkpoint was taken with (ValueError naming the field otherwise).  The banks' frames are placed by this state's
         `device_frames` and `small_device_frames`, whatever the caps of the state that took the checkpoint.  An eager
         checkpoint (every frame encoded) restores into a lazy_full_res state; a lazy one restores into an eager state
-        only once every frame is encoded (NotImplementedError naming the knob otherwise)."""
+        only once every frame is encoded (NotImplementedError naming the knob otherwise).  Into a state without
+        full_res_bank, an eager or lazy checkpoint's stored rows become a frozen base bank (placed by `device_frames`)
+        and later frames keep pixel rows only; a checkpoint of such a state restores into a lazy_full_res state (its
+        frames without stored rows "not yet encoded"), and into an eager one only when it has no such frame."""
         from .. import checkpoint as CK
         if ckpt.family != CK.QWEN:
             raise ValueError(f"QwenStreamState.restore: a {ckpt.family!r} checkpoint is not a Qwen2-VL stream's")
@@ -543,16 +594,28 @@ class QwenStreamState:
         if n["n_frames"] and c["merger_dim"] != md:
             raise ValueError(f"QwenStreamState.restore: config.merger_dim of the checkpoint ({c['merger_dim']}) differs "
                              f"from the merger's ({md})")
-        st = cls(flash, merger, device_frames, small_device_frames, lazy_full_res=lazy_full_res)
+        st = cls(flash, merger, device_frames, small_device_frames, lazy_full_res=lazy_full_res,
+                 full_res_bank=full_res_bank)
         if n["n_frames"] == 0:
             return st
-        lazy_ck = "pix_frames" in n
-        if lazy_ck:                               # the frames not yet encoded, whose pixel rows the checkpoint holds
-            todo = torch.nonzero(ckpt.tensor("encoded") == 0).flatten().tolist()
+        N = n["n_frames"]
+        lazy_ck, bankless_ck = "pix_frames" in n, "bank_frames" in n
+        stored = torch.ones(N, dtype=torch.bool)  # frames whose rows the checkpoint's bank holds (an eager one: all)
+        todo = []
+        if lazy_ck:                               # the frames with pixel rows only, which the checkpoint holds
+            enc = ckpt.tensor("encoded")
+            stored = enc == (2 if bankless_ck else 1)
+            if bankless_ck and bool(stored[n["bank_frames"]:].any()):
+                raise ValueError(f"QwenStreamState.restore: the mask marks frames past counters.bank_frames "
+                                 f"({n['bank_frames']}) as stored")
+            todo = torch.nonzero(~stored).flatten().tolist()
             if len(todo) != n["pix_frames"]:
                 raise ValueError(f"QwenStreamState.restore: counters.pix_frames ({n['pix_frames']}) is not the number of "
                                  f"frames the mask leaves unencoded ({len(todo)})")
-        if lazy_ck and not lazy_full_res and todo:
+        if todo and not lazy_full_res:
+            if bankless_ck:
+                raise NotImplementedError("QwenStreamState.restore: the checkpoint is of a stream without a "
+                                          "full-resolution bank (full_res_bank=False): restore it with lazy_full_res=True")
             raise NotImplementedError("QwenStreamState.restore: the checkpoint is of a lazy_full_res stream with frames "
                                       "not yet encoded at full resolution: restore it with lazy_full_res=True")
         dev = torch.device(device)
@@ -562,18 +625,20 @@ class QwenStreamState:
             st._append_small(ckpt.tensor("bank_small"), dev)
             if lazy_full_res:
                 hw = int(c["grid"][0]) * int(c["grid"][1])
-                if lazy_ck:                       # the store starts at the first frame not yet encoded
+                # the pixel store starts at the first frame with pixel rows only; frames without a stored row get them
+                base = todo[0] if todo else N
+                st.pixels = PixelStore(st._layout[0], hw * PATCH_DIM, base, st.CHUNK_BYTES)
+                if todo:
+                    st.pixels.append(None, dev, t=N - base)
+                    st.pixels.put(todo, ckpt.tensor("pixels").view(len(todo), -1))
+                st.n_encoded = N - len(todo)
+                if full_res_bank:                 # frames past the checkpoint's bank get zero slots, "not yet encoded"
+                    st._append_slots(N - (st.bank_x.n + st.n_host), dev)
+                    st.encoded.append(stored.to(torch.uint8).to(dev))
+                elif bankless_ck:                 # the base bank and the "encoded before" bytes carry over as they are
                     st.encoded.append(get("encoded"))
-                    st.n_encoded = n["n_frames"] - len(todo)
-                    base = todo[0] if todo else n["n_frames"]
-                    st.pixels = PixelStore(st._layout[0], hw * PATCH_DIM, base, st.CHUNK_BYTES)
-                    if todo:
-                        st.pixels.append(None, dev, t=n["n_frames"] - base)
-                        st.pixels.put(todo, ckpt.tensor("pixels").view(len(todo), -1))
-                else:                             # an eager stream: every frame is encoded, no frame has pixel rows
-                    st.encoded.append(torch.ones(n["n_frames"], dtype=torch.uint8, device=dev))
-                    st.n_encoded = n["n_frames"]
-                    st.pixels = PixelStore(st._layout[0], hw * PATCH_DIM, n["n_frames"], st.CHUNK_BYTES)
+                else:                             # the checkpoint's stored rows become the frozen base bank
+                    st.encoded.append((stored.to(torch.uint8) * 2).to(dev))
             st.n_frames, st.steps = n["n_frames"], n["steps"]
             st.fast_steps, st.redone_steps = n["fast_steps"], n["redone_steps"]
             st.grid, st.small_grid = tuple(c["grid"]), tuple(c["small_grid"])
@@ -582,9 +647,12 @@ class QwenStreamState:
             st.n_tem = n["n_tem"]
             st.spa_positions = get("spa_positions")
             h, w = st.grid
-            st.spa_x = torch.empty(n["n_spa"], h * w, int(c["dim"]), dtype=st._layout[0], device=dev)
-            if n["n_spa"]:
-                st._gather(st.spa_positions, st.spa_x, None, None)
+            if "spa_x" in ckpt.tensors:           # a stream without a bank: the DAM's rows as they were
+                st.spa_x = get("spa_x")
+            else:
+                st.spa_x = torch.empty(n["n_spa"], h * w, int(c["dim"]), dtype=st._layout[0], device=dev)
+                if n["n_spa"]:
+                    st._gather(st.spa_positions, st.spa_x, None, None)
             st.video_embeds = get("video_embeds") if "video_embeds" in ckpt.tensors else None
             torch.cuda.current_stream().synchronize()     # the pinned sources may be freed as soon as this returns
         return st
@@ -655,8 +723,8 @@ def _rest_stage(ctxs):
 
 
 def _rest_finish(ctxs):
-    """the second half of _rest_stage, once the retrieved frames are in the banks: _rest_outputs, one DAM gather table
-    per dtype, and one PatchMerger call over every CSM slice"""
+    """the second half of _rest_stage, once the retrieved frames are in the banks (or, without full_res_bank, in the
+    fresh rows): _rest_outputs, one DAM gather table per dtype and kind, and one PatchMerger call over every CSM slice"""
     if not ctxs:
         return
     gathers, merges = {}, []
@@ -664,11 +732,11 @@ def _rest_finish(ctxs):
         g, m = state._rest_outputs(c)
         if g is not None:
             out = g["spa_x_out"] if g["spa_x_out"] is not None else g["merged_out"]
-            gathers.setdefault(out.dtype, []).append(g)
+            gathers.setdefault((out.dtype, state.full_res_bank), []).append(g)
         if m is not None:
             merges.append(m)
-    for calls in gathers.values():
-        Q.dam_gather_multi(calls)
+    for (_, bank), calls in gathers.items():
+        (Q.dam_gather_multi if bank else Q.dam_gather_fresh_multi)(calls)
     merger = ctxs[0][0].merger
     if len(merges) == 1:
         merger(merges[0][0], out=merges[0][1])
@@ -688,6 +756,16 @@ def check_lazy_full_res(v, flash, who: str = "lazy_full_res") -> bool:
     if v and flash.temporal_poolsize != 2:
         raise NotImplementedError(f"{who}=True needs flash_memory_temporal_poolsize=2 (got {flash.temporal_poolsize}): "
                                   f"with pool size 1 the full-resolution bank is the half-resolution one")
+    return v
+
+
+def check_full_res_bank(v, lazy: bool, who: str = "full_res_bank", lazy_who: str = "lazy_full_res") -> bool:
+    """a bool; False needs lazy_full_res (ValueError otherwise: an eager stream's bank is where its features go)"""
+    if not isinstance(v, bool):
+        raise ValueError(f"{who} must be True or False, got {v!r}")
+    if not v and not lazy:
+        raise ValueError(f"{who}=False needs {lazy_who}=True: a stream without a full-resolution bank re-encodes its "
+                         f"frames from their pixel rows, which only a lazy_full_res stream keeps")
     return v
 
 

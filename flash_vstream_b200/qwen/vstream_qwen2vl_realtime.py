@@ -29,7 +29,7 @@ from . import offline as _offline_pass
 from . import vstream_qwen2vl_model as _offline
 from .compress_functions import weighted_kmeans_ordered_feature
 from .patch_merger import PatchMerger
-from .stream_state import QwenStreamState, check_device_frames, check_lazy_full_res
+from .stream_state import QwenStreamState, check_device_frames, check_full_res_bank, check_lazy_full_res
 
 
 class FlashMemory(_offline.FlashMemory):
@@ -154,11 +154,16 @@ class RealtimeStreamingMixin:
     fvs_lazy_full_res: False (default) or True — keep each clip's full-resolution pixel rows and run the full-resolution
     tower on a frame only the first time the DAM picks it (DESIGN.md §3.18); item 7 of the list is then the zero-row
     stand-in.  Needs flash_memory_temporal_poolsize=2.  Like the caps, it applies from the next stream (and to
-    load_video_stream); changing it in the middle of a stream raises ValueError."""
+    load_video_stream); changing it in the middle of a stream raises ValueError.
+
+    fvs_full_res_bank: True (default) or False — with fvs_lazy_full_res, keep no full-resolution or merged row beyond
+    the DAM, and re-encode from its pixel rows a pick the previous DAM does not hold (DESIGN.md §3.19).  False without
+    fvs_lazy_full_res raises ValueError; it applies, and refuses a change mid-stream, like the knobs above."""
 
     fvs_bank_device_frames = None
     fvs_bank_small_device_frames = None
     fvs_lazy_full_res = False
+    fvs_full_res_bank = True
 
     def _bank_device_frames(self):
         return self._cap("fvs_bank_device_frames", "device_frames")
@@ -169,6 +174,10 @@ class RealtimeStreamingMixin:
     def _lazy_full_res(self):
         return self._cap("fvs_lazy_full_res", "lazy_full_res",
                          lambda v, k: check_lazy_full_res(v, self.visual.flash_memory, k))
+
+    def _full_res_bank(self, lazy: bool):
+        return self._cap("fvs_full_res_bank", "full_res_bank",
+                         lambda v, k: check_full_res_bank(v, lazy, k, "fvs_lazy_full_res"))
 
     def _cap(self, knob, attr, check=check_device_frames):
         """the validated value of the cap attribute `knob`, which the stream in progress (its state's `attr`) must share"""
@@ -210,6 +219,7 @@ class RealtimeStreamingMixin:
         time_0 = time.perf_counter()
         assert self.use_video_streaming_mode
         cap, small_cap, lazy = self._bank_device_frames(), self._bank_small_device_frames(), self._lazy_full_res()
+        bank = self._full_res_bank(lazy)
         grid_host = video_grid_thw.cpu()          # the grid stays on the host: every shape below comes from it (a CUDA grid
         t, h, w = (int(v) for v in grid_host.reshape(-1, 3)[0].tolist())   # costs one sync here, a host grid none)
         pixel_values_videos = pixel_values_videos.type(self.visual.get_dtype()).to(self.visual.get_device(), non_blocking=True)
@@ -235,7 +245,7 @@ class RealtimeStreamingMixin:
         pub = self.__dict__.get("_qwen_publication")              # set by qwen.serve.export_qwen_memory (opt-in)
         if self.stream_state is None or not self.video_embedding_memory:
             self.stream_state = QwenStreamState(self.visual.flash_memory, self.visual.merger, device_frames=cap,
-                                                small_device_frames=small_cap, lazy_full_res=lazy)
+                                                small_device_frames=small_cap, lazy_full_res=lazy, full_res_bank=bank)
             if pub is not None:
                 pub.new_stream()
         time_3 = time.perf_counter()
@@ -275,8 +285,10 @@ class RealtimeStreamingMixin:
         cap = check_device_frames(self.fvs_bank_device_frames, "fvs_bank_device_frames")
         small_cap = check_device_frames(self.fvs_bank_small_device_frames, "fvs_bank_small_device_frames")
         lazy = check_lazy_full_res(self.fvs_lazy_full_res, self.visual.flash_memory, "fvs_lazy_full_res")
+        bank = check_full_res_bank(self.fvs_full_res_bank, lazy, "fvs_full_res_bank", "fvs_lazy_full_res")
         state = QwenStreamState.restore(ckpt, self.visual.flash_memory, self.visual.merger, self.visual.get_device(),
-                                        device_frames=cap, small_device_frames=small_cap, lazy_full_res=lazy)
+                                        device_frames=cap, small_device_frames=small_cap, lazy_full_res=lazy,
+                                        full_res_bank=bank)
         state.tower = self.visual.encode_patches if lazy else None
         if state.n_frames == 0:
             self.stream_state = None

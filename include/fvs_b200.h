@@ -638,6 +638,63 @@ typedef struct fvs_qwen_scatter_job {
   int64_t merged_frame_elems;
 } fvs_qwen_scatter_job;
 int fvs_qwen_bank_scatter_multi(const fvs_qwen_scatter_job* jobs, int n_jobs, int dtype, fvs_stream_t stream);
+
+/* No full-resolution bank (DESIGN.md §3.19): a lazy stream that stores no x or merged row for the frames it encodes.
+ * It keeps every frame's pixel rows and the previous step's DAM rows, and re-encodes a pick the previous DAM does not
+ * hold.  A stream restored from a checkpoint may also hold a frozen base bank of stored rows (frames [0, n_base), laid
+ * out as fvs_qwen_dam_gather reads its two tiers).  Job tables as above.
+ *
+ * fvs_qwen_pick_plan_prev_multi: the plan compares the picks against prev_picks itself, so the stream keeps no mask that
+ * a redone clip would have to roll back.  Per job, walks picks (device int64 [n]) in order and writes to plan (device
+ * int64 [n]) every pick p that is in [0, n_frames), that no earlier pick names, that is not in prev_picks (device int64
+ * [m], the previous step's DAM; NULL when m = 0) and whose byte in `frames` (device uint8 [n_frames]) is not 2 (2: the
+ * frame's rows are in the stored base bank).  A planned frame whose byte is 1 (encoded before) adds 1 to *re_encodes
+ * (device uint64, optional); every planned frame's byte is then set to 1.  The plan's length goes to *count (int32;
+ * device memory or the mapped address of pinned host memory), as fvs_qwen_pick_plan_multi stores it. */
+typedef struct fvs_qwen_pick_plan_prev_job {
+  const int64_t* picks;
+  int n;
+  int64_t n_frames;
+  uint8_t* frames;
+  const int64_t* prev_picks;
+  int m;
+  int64_t* plan;
+  int32_t* count;
+  uint64_t* re_encodes;
+} fvs_qwen_pick_plan_prev_job;
+int fvs_qwen_pick_plan_prev_multi(const fvs_qwen_pick_plan_prev_job* jobs, int n_jobs, fvs_stream_t stream);
+/* fvs_qwen_dam_gather_fresh_multi: the DAM gather of a stream without a full-resolution bank.  Per job, for every pick i,
+ * spa_x_out[i] = x[picks[i]] and merged_out[i] = merged[picks[i]] (either output may be NULL; not both), each read from
+ * the first source that has the frame: the previous DAM (prev_picks [m], prev_x, prev_merged); this step's fresh rows
+ * (fresh_frames [n_fresh], fresh_x [n_fresh, x_frame_elems], fresh_merged [n_fresh, merged_frame_elems]: the tower and
+ * PatchMerger output of the planned frames, in plan order); the stored base bank, frames [0, n_base): device tier
+ * [0, n_dev) and host chunks as for fvs_qwen_dam_gather.  *host_fetches (optional) grows by the picks read from the host
+ * chunks.  A pick outside [0, n_frames), or in no source, yields zero rows.  n_fresh is a host integer (the count of the
+ * plan, read back).  The outputs must not alias any source; no output may be shared by two jobs. */
+typedef struct fvs_qwen_fresh_gather_job {
+  const int64_t* picks;
+  int n;
+  int64_t n_frames;
+  const int64_t* prev_picks;
+  int m;
+  const void* prev_x;
+  const void* prev_merged;
+  const int64_t* fresh_frames;
+  int n_fresh;
+  const void* fresh_x;
+  const void* fresh_merged;
+  int64_t n_base;
+  const void* dev_x;
+  const void* dev_merged;
+  int64_t n_dev;
+  const void* const* host_chunks;  /* DEVICE table */
+  int chunk_frames;
+  int64_t x_frame_elems, merged_frame_elems;
+  void* spa_x_out;
+  void* merged_out;
+  uint64_t* host_fetches;
+} fvs_qwen_fresh_gather_job;
+int fvs_qwen_dam_gather_fresh_multi(const fvs_qwen_fresh_gather_job* jobs, int n_jobs, int dtype, fvs_stream_t stream);
 /* *dev_out = the device address of pinned host memory `host` (cudaHostGetDevicePointer); FVS_EINVAL if it is not pinned */
 int fvs_host_device_ptr(const void* host, void** dev_out);
 
