@@ -103,6 +103,12 @@ class QwenPixelJob(C.Structure):  # fvs_qwen_pixel_job
                 ("host_chunks", C.c_void_p), ("chunk_frames", C.c_int), ("frame_elems", C.c_int64), ("out", C.c_void_p)]
 
 
+class QwenPixelCodesJob(C.Structure):  # fvs_qwen_pixel_codes_job
+    _fields_ = [("plan", C.c_void_p), ("n", C.c_int), ("n_frames", C.c_int64), ("base", C.c_int64),
+                ("host_chunks", C.c_void_p), ("chunk_frames", C.c_int), ("frame_elems", C.c_int64), ("table", C.c_void_p),
+                ("out", C.c_void_p)]
+
+
 class QwenScatterJob(C.Structure):  # fvs_qwen_scatter_job
     _fields_ = [("plan", C.c_void_p), ("n", C.c_int), ("n_frames", C.c_int64), ("x_rows", C.c_void_p),
                 ("merged_rows", C.c_void_p), ("dev_x", C.c_void_p), ("dev_merged", C.c_void_p), ("n_dev", C.c_int64),
@@ -126,7 +132,7 @@ class QwenFreshGatherJob(C.Structure):  # fvs_qwen_fresh_gather_job
 
 
 QWEN_MEM_JOBS_PER_LAUNCH = 16
-PRE_CLIP, PRE_QWEN = 0, 1
+PRE_CLIP, PRE_QWEN, PRE_QWEN_CODES = 0, 1, 2
 KLARGE_EUCLIDEAN, KLARGE_COSINE = 0, 1
 INPUT_PIXELS, INPUT_FEATURES = 0, 1
 
@@ -212,6 +218,9 @@ SIGNATURES = {
     # no full-resolution bank
     "fvs_qwen_pick_plan_prev_multi": (_i, [C.POINTER(QwenPickPlanPrevJob), _i, _vp]),
     "fvs_qwen_dam_gather_fresh_multi": (_i, [C.POINTER(QwenFreshGatherJob), _i, _i, _vp]),
+    # 8-bit pixel codes
+    "fvs_qwen_pixel_decode": (_i, [_vp, C.c_int64, _vp, _i, _vp, _vp]),
+    "fvs_qwen_pixel_gather_codes_multi": (_i, [C.POINTER(QwenPixelCodesJob), _i, _i, _vp]),
     # publication of the Qwen2-VL streaming memory (seqlock)
     "fvs_qwen_pub_layout": (_i, [_i, _i, _i, _i, _i, _i, _i, _i64p]),
     "fvs_qwen_publish": (_i, [_vp, _sz, _i, _i, C.c_int64, _i, _vp, C.c_int64, _vp, _i, _vp, _i, _i, _i, _i, _i, C.c_uint64,

@@ -20,7 +20,8 @@ continue bit for bit as if it had never stopped (DESIGN.md §3.12):
     A lazy_full_res state adds counters.pix_frames, encoded uint8 [n_frames] and pixels [pix_frames, h*w, 1176] (the
     frames with pixel rows only).  A state without a full-resolution bank also adds counters.bank_frames: bank_x and
     bank_merged then hold its base bank [bank_frames, ...], its mask bytes are 2 for a stored frame, and spa_x
-    [n_spa, h*w, D] carries the DAM's rows.
+    [n_spa, h*w, D] carries the DAM's rows.  A compact_pixels state (config.compact_pixels true) carries its pixel rows
+    as pix_codes uint8 [pix_frames, h*w*1176] and their value table pixel_table float32 [3, 256] in place of pixels.
   * `rng`: the draw source a StreamPool stream owns (draws.DrawSource): torch CPU and CUDA generator states (uint8 tensors
     "rng.cpu" / "rng.cuda") and the `random.Random` state.  Streams that draw from the global generators carry none.
 
@@ -124,7 +125,11 @@ class StreamCheckpoint:
             out["video_embeds"] = ((n["n_spa"] * h * w // 4 + n["n_tem"] * hs * ws // 4, md), dt)
         if "pix_frames" in n:                         # a lazy_full_res stream: its mask, the pixel rows of its frames not yet encoded
             out["encoded"] = ((n["n_frames"],), torch.uint8)
-            out["pixels"] = ((n["pix_frames"], h * w, 3 * 2 * 14 * 14), dt)
+            if c.get("compact_pixels"):               # 8-bit codes and the table they decode through
+                out["pix_codes"] = ((n["pix_frames"], h * w * 3 * 2 * 14 * 14), torch.uint8)
+                out["pixel_table"] = ((3, 256), torch.float32)
+            else:
+                out["pixels"] = ((n["pix_frames"], h * w, 3 * 2 * 14 * 14), dt)
         if "bank_frames" in n:                        # no full-resolution bank: the DAM's rows, which no bank can rebuild
             out["spa_x"] = ((n["n_spa"], h * w, D), dt)
         return out

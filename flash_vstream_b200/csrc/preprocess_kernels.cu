@@ -19,6 +19,7 @@
 #include <algorithm>
 #include <cmath>
 #include <cstdio>
+#include <type_traits>
 #include <vector>
 
 #include "fvs_common.h"
@@ -184,7 +185,8 @@ __device__ __forceinline__ void resample_row(const Job& a, int r, int t, uint8_t
 // Vertical pass over output row y of frame t, then the table lookup and the layout write:
 //   FVS_PRE_CLIP  f16 [T, 3, out_rows, cols];
 //   FVS_PRE_QWEN  fp32 [T/2 * gh * gw, 1176], row ((ti*gh/2 + bh)*gw/2 + bw)*4 + mh*2 + mw, column ((c*2 + tp)*14 + py)*14
-//                 + px; a one-frame clip fills both temporal slots.
+//                 + px; a one-frame clip fills both temporal slots;
+//   FVS_PRE_QWEN_CODES  the same rows and columns as uint8: the resampled byte itself, before the table lookup.
 template <int kLayout>
 __device__ __forceinline__ void resample_col(const Job& a, int y, int t, const float* lut) {
   const int2 b = a.yb[y];
@@ -202,10 +204,12 @@ __device__ __forceinline__ void resample_col(const Job& a, int y, int t, const f
       const int gh2 = a.out_rows / (kPatch * kMerge), gw2 = a.cols / (kPatch * kMerge);
       const size_t orow = ((size_t(t / kTemporal) * gh2 + hy / kMerge) * gw2 + hx / kMerge) * (kMerge * kMerge) +
                           (hy % kMerge) * kMerge + (hx % kMerge);
-      float* o = static_cast<float*>(a.out) + orow * kQwenCols + (c * kTemporal * kPatch + py) * kPatch + px;
+      using E = std::conditional_t<kLayout == FVS_PRE_QWEN, float, uint8_t>;
+      const E e = kLayout == FVS_PRE_QWEN ? E(v) : E(clip8(acc));
+      E* o = static_cast<E*>(a.out) + orow * kQwenCols + (c * kTemporal * kPatch + py) * kPatch + px;
       const int tp = t % kTemporal;
-      o[tp * kPatch * kPatch] = v;
-      if (a.T == 1) o[(1 - tp) * kPatch * kPatch] = v;
+      o[tp * kPatch * kPatch] = e;
+      if (a.T == 1) o[(1 - tp) * kPatch * kPatch] = e;
     }
   }
 }
@@ -222,8 +226,10 @@ __global__ void __launch_bounds__(kThreads) resample_rows_kernel(const __grid_co
 template <int kLayout>
 __global__ void __launch_bounds__(kThreads) resample_cols_kernel(const __grid_constant__ MultiArgs m) {
   __shared__ float lut[3 * 256];
-  for (int i = threadIdx.x; i < 3 * 256; i += blockDim.x) lut[i] = m.table[i];
-  __syncthreads();
+  if (kLayout != FVS_PRE_QWEN_CODES) {     // codes are the bytes before the lookup
+    for (int i = threadIdx.x; i < 3 * 256; i += blockDim.x) lut[i] = m.table[i];
+    __syncthreads();
+  }
   const int j = find_job(m.col_block0, m.n, blockIdx.x);
   const Job& a = m.job[j];
   const int b = blockIdx.x - m.col_block0[j], t = b / a.out_rows;
@@ -246,8 +252,9 @@ int check_job(const fvs_preprocess_job& jb, int layout, int pool, const char* ap
   if ((r = check_axis(&jb.x, jb.W, "x", api)) || (r = check_axis(&jb.y, jb.H, "y", api))) return r;
   FVS_REQUIRE(size_t(jb.x.span_count) * 3 <= kRowSmemMax, "%s: a window reading %d source columns is wider than the %zu "
               "supported", api, jb.x.span_count, kRowSmemMax / 3);
-  FVS_REQUIRE(layout == FVS_PRE_CLIP || layout == FVS_PRE_QWEN, "%s: unknown layout %d", api, layout);
-  if (layout == FVS_PRE_QWEN) {
+  FVS_REQUIRE(layout == FVS_PRE_CLIP || layout == FVS_PRE_QWEN || layout == FVS_PRE_QWEN_CODES, "%s: unknown layout %d",
+              api, layout);
+  if (layout != FVS_PRE_CLIP) {
     FVS_REQUIRE(jb.T == 1 || jb.T % kTemporal == 0, "%s: Qwen2-VL clips hold 1 or an even number of frames, not %d", api,
                 jb.T);
     FVS_REQUIRE(pool >= 1, "%s: pool %d < 1", api, pool);
@@ -304,7 +311,7 @@ int preprocess_jobs(const fvs_preprocess_job* jobs, int n, const float* table, i
   if (launches < 0) return launches;
   FVS_REQUIRE(workspace_bytes_ >= size_t(ws_total), "%s: workspace of %zu bytes < %zu", api, workspace_bytes_,
               size_t(ws_total));
-  const size_t esize = layout == FVS_PRE_CLIP ? sizeof(__half) : sizeof(float);
+  const size_t esize = layout == FVS_PRE_CLIP ? sizeof(__half) : layout == FVS_PRE_QWEN ? sizeof(float) : 1;
   for (int g = 0; g < launches; ++g) {
     MultiArgs m = {};
     m.table = table;
@@ -342,8 +349,10 @@ int preprocess_jobs(const fvs_preprocess_job* jobs, int n, const float* table, i
     FVS_CHECK_LAUNCH("resample_rows_kernel");
     if (layout == FVS_PRE_CLIP) {
       resample_cols_kernel<FVS_PRE_CLIP><<<m.col_block0[m.n], kThreads, 0, st>>>(m);
-    } else {
+    } else if (layout == FVS_PRE_QWEN) {
       resample_cols_kernel<FVS_PRE_QWEN><<<m.col_block0[m.n], kThreads, 0, st>>>(m);
+    } else {
+      resample_cols_kernel<FVS_PRE_QWEN_CODES><<<m.col_block0[m.n], kThreads, 0, st>>>(m);
     }
     FVS_CHECK_LAUNCH("resample_cols_kernel");
   }

@@ -4,6 +4,9 @@
 // [n_dev, n_frames) live in pinned host chunks of chunk_frames frames each, laid out [x rows of the chunk | merged rows of
 // the chunk] and read through their mapped device pointers.  The picks come from the retrieval kernels and stay on the
 // device: the kernel resolves every pick itself, so the step needs no host round trip to know where its frames are.
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
+
 #include <algorithm>
 #include <vector>
 
@@ -479,6 +482,132 @@ int fresh_gather_launch(const fvs_qwen_fresh_gather_job* jobs, int n, cudaStream
   FVS_CHECK_LAUNCH("fresh_gather_kernel");
   return FVS_OK;
 }
+
+// ---- 8-bit pixel codes (DESIGN.md §3.20) -------------------------------------------------------------------------------
+// A code row holds the resampled bytes u of one full-resolution pixel row, columns ((c*2 + tp)*14 + py)*14 + px; the
+// tower reads dtype(table[c][u]).  392 = 2*14*14 columns per channel is a multiple of 8, so the 8 codes of one 8-byte
+// word share a channel: word w of a row (147 words) is channel (w % 147) / 49.
+constexpr long long kCodeWordsPerRow = 1176 / 8, kCodeWordsPerChannel = 392 / 8;
+constexpr int kCodeJobs = FVS_QWEN_MEM_JOBS_PER_LAUNCH;
+
+template <int kDtype>
+__device__ __forceinline__ unsigned decode_pair(float a, float b) {
+  if constexpr (kDtype == FVS_BF16) {
+    const __nv_bfloat162 v = __floats2bfloat162_rn(a, b);    // round to nearest even, as torch's fp32 -> bf16 cast
+    return *reinterpret_cast<const unsigned*>(&v);
+  } else {
+    const __half2 v = __floats2half2_rn(a, b);
+    return *reinterpret_cast<const unsigned*>(&v);
+  }
+}
+
+// 8 codes of channel-table `lut` -> 8 tower values (16 bytes)
+template <int kDtype>
+__device__ __forceinline__ uint4 decode_word(uint2 c, const float* lut) {
+  uint4 o;
+  o.x = decode_pair<kDtype>(lut[c.x & 255], lut[(c.x >> 8) & 255]);
+  o.y = decode_pair<kDtype>(lut[(c.x >> 16) & 255], lut[c.x >> 24]);
+  o.z = decode_pair<kDtype>(lut[c.y & 255], lut[(c.y >> 8) & 255]);
+  o.w = decode_pair<kDtype>(lut[(c.y >> 16) & 255], lut[c.y >> 24]);
+  return o;
+}
+
+// the [3, 256] table into shared memory, for every thread of the block
+__device__ __forceinline__ void load_lut(float* lut, const float* table) {
+  for (int i = threadIdx.x; i < 3 * 256; i += blockDim.x) lut[i] = table[i];
+  __syncthreads();
+}
+
+// words [first, total) of whole code rows, `stride` apart: out[w] = decode(src[w]) (src null: zeros).  Four loads in
+// flight per thread before the stores, as gather_copy: a zero-copy read over PCIe has microseconds of latency.
+template <int kDtype>
+__device__ __forceinline__ void decode_words(const uint2* src, uint4* out, long long first, long long total,
+                                             long long stride, const float* lut) {
+  for (long long w0 = first; w0 < total; w0 += 4 * stride) {
+    uint2 v[4];
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+      const long long w = w0 + u * stride;
+      v[u] = make_uint2(0, 0);
+      if (w < total && src) v[u] = src[w];
+    }
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+      const long long w = w0 + u * stride;
+      if (w < total)
+        out[w] = src ? decode_word<kDtype>(v[u], lut + (w % kCodeWordsPerRow) / kCodeWordsPerChannel * 256)
+                     : make_uint4(0, 0, 0, 0);
+    }
+  }
+}
+
+template <int kDtype>
+__global__ void __launch_bounds__(256) pixel_decode_kernel(const uint2* __restrict__ codes, const float* __restrict__ table,
+                                                           long long words, uint4* __restrict__ out) {
+  __shared__ float lut[3 * 256];
+  load_lut(lut, table);
+  decode_words<kDtype>(codes, out, (long long)blockIdx.x * blockDim.x + threadIdx.x, words,
+                       (long long)gridDim.x * blockDim.x, lut);
+}
+
+// The job table of the pixel gather over code chunks: job j's block b decodes share b % bx of planned frame b / bx,
+// read in place from its pinned chunk; a frame outside [base, n_frames) yields zeros.
+struct CodesJobDev {
+  const long long* plan;
+  const uint8_t* const* chunks;
+  const float* table;
+  uint4* out;
+  long long n_frames, base, chunk_frames, words;    // words: 8-byte code words per frame
+  int bx;
+};
+template <int kJobs>
+struct CodesLaunch {
+  CodesJobDev job[kJobs];
+  int first[kJobs + 1];
+  int n;
+};
+template <int kJobs, int kDtype>
+__global__ void __launch_bounds__(256) pixel_codes_gather_kernel(const __grid_constant__ CodesLaunch<kJobs> L) {
+  int j = 0;
+  if constexpr (kJobs > 1)
+    while (j + 1 < L.n && blockIdx.x >= unsigned(L.first[j + 1])) ++j;
+  const CodesJobDev& J = L.job[j];
+  const unsigned b = blockIdx.x - unsigned(L.first[j]), bx = b % unsigned(J.bx);
+  const long long i = b / unsigned(J.bx);
+  __shared__ float lut[3 * 256];
+  __shared__ const uint2* src;
+  if (threadIdx.x == 0) {
+    const long long p = J.plan[i];
+    const uint2* s = nullptr;
+    if (p >= J.base && p < J.n_frames) {
+      const long long q = p - J.base;
+      s = reinterpret_cast<const uint2*>(J.chunks[q / J.chunk_frames]) + (q % J.chunk_frames) * J.words;
+    }
+    src = s;
+  }
+  load_lut(lut, J.table);
+  decode_words<kDtype>(src, J.out + i * J.words, (long long)bx * blockDim.x + threadIdx.x, J.words,
+                       (long long)J.bx * blockDim.x, lut);
+}
+
+template <int kJobs, int kDtype>
+int codes_gather_launch(const fvs_qwen_pixel_codes_job* jobs, int n, cudaStream_t stream) {
+  CodesLaunch<kJobs> L;
+  L.n = n;
+  L.first[0] = 0;
+  for (int q = 0; q < n; ++q) {
+    const fvs_qwen_pixel_codes_job& g = jobs[q];
+    const long long words = g.frame_elems / 8;
+    long long bx = (words + 4 * 256 - 1) / (4 * 256);
+    bx = bx > 64 ? 64 : bx < 1 ? 1 : bx;
+    L.job[q] = CodesJobDev{(const long long*)g.plan, (const uint8_t* const*)g.host_chunks, g.table, (uint4*)g.out,
+                           (long long)g.n_frames, (long long)g.base, (long long)g.chunk_frames, words, int(bx)};
+    L.first[q + 1] = L.first[q] + int(bx) * g.n;
+  }
+  pixel_codes_gather_kernel<kJobs, kDtype><<<L.first[n], 256, 0, stream>>>(L);
+  FVS_CHECK_LAUNCH("pixel_codes_gather_kernel");
+  return FVS_OK;
+}
 }  // namespace
 
 extern "C" {
@@ -659,6 +788,62 @@ int fvs_qwen_dam_gather_fresh_multi(const fvs_qwen_fresh_gather_job* jobs, int n
     const int n = std::min(kGatherJobs, n_jobs - i0);
     const int r = n == 1 ? fresh_gather_launch<1>(jobs + i0, 1, (cudaStream_t)stream)
                          : fresh_gather_launch<kGatherJobs>(jobs + i0, n, (cudaStream_t)stream);
+    if (r) return r;
+  }
+  return FVS_OK;
+}
+
+int fvs_qwen_pixel_decode(const uint8_t* codes, int64_t rows, const float* table, int dtype, void* out,
+                          fvs_stream_t stream) {
+  const char* api = "fvs_qwen_pixel_decode";
+  FVS_REQUIRE(codes && table && out, "%s: null pointer", api);
+  FVS_REQUIRE(dtype == FVS_F16 || dtype == FVS_BF16, "%s: dtype must be f16 or bf16", api);
+  FVS_REQUIRE(rows > 0, "%s: need rows > 0 (rows=%lld)", api, (long long)rows);
+  FVS_REQUIRE(((uintptr_t)codes & 7) == 0 && aligned16(out) && ((uintptr_t)table & 3) == 0,
+              "%s: codes must be 8-byte and out 16-byte aligned", api);
+  const long long words = (long long)rows * kCodeWordsPerRow;
+  long long blocks = (words + 4 * 256 - 1) / (4 * 256);
+  if (blocks > 4096) blocks = 4096;
+  if (dtype == FVS_BF16) {
+    pixel_decode_kernel<FVS_BF16><<<int(blocks), 256, 0, (cudaStream_t)stream>>>((const uint2*)codes, table, words,
+                                                                                   (uint4*)out);
+  } else {
+    pixel_decode_kernel<FVS_F16><<<int(blocks), 256, 0, (cudaStream_t)stream>>>((const uint2*)codes, table, words,
+                                                                                  (uint4*)out);
+  }
+  FVS_CHECK_LAUNCH("pixel_decode_kernel");
+  return FVS_OK;
+}
+
+int fvs_qwen_pixel_gather_codes_multi(const fvs_qwen_pixel_codes_job* jobs, int n_jobs, int dtype, fvs_stream_t stream) {
+  const char* api = "fvs_qwen_pixel_gather_codes_multi";
+  FVS_REQUIRE(jobs && n_jobs > 0, "%s: need a job table and n_jobs > 0", api);
+  FVS_REQUIRE(dtype == FVS_F16 || dtype == FVS_BF16, "%s: dtype must be f16 or bf16", api);
+  for (int i = 0; i < n_jobs; ++i) {
+    const fvs_qwen_pixel_codes_job& j = jobs[i];
+    FVS_REQUIRE(j.plan && j.out && j.table && j.n > 0 && j.n <= 65535,
+                "%s: job %d: need a plan, a table, an output and 0 < n <= 65535", api, i);
+    FVS_REQUIRE(j.base >= 0 && j.base < j.n_frames && j.host_chunks && j.chunk_frames > 0,
+                "%s: job %d: need 0 <= base < n_frames and a chunk table", api, i);
+    FVS_REQUIRE(j.frame_elems > 0 && j.frame_elems % 1176 == 0, "%s: job %d: frame size %lld is not whole rows of 1176 "
+                "codes", api, i, (long long)j.frame_elems);
+    FVS_REQUIRE(aligned16(j.out) && ((uintptr_t)j.plan & 7) == 0 && ((uintptr_t)j.host_chunks & 7) == 0 &&
+                    ((uintptr_t)j.table & 3) == 0,
+                "%s: job %d: misaligned output or table", api, i);
+    for (int k = 0; k < i; ++k) {
+      const uintptr_t a = uintptr_t(jobs[k].out), ae = a + size_t(jobs[k].n) * jobs[k].frame_elems * 2;
+      const uintptr_t b = uintptr_t(j.out), be = b + size_t(j.n) * j.frame_elems * 2;
+      FVS_REQUIRE(ae <= b || be <= a, "%s: jobs %d and %d share an output", api, k, i);
+    }
+  }
+  for (int i0 = 0; i0 < n_jobs; i0 += kCodeJobs) {
+    const int n = std::min(kCodeJobs, n_jobs - i0);
+    const cudaStream_t st = (cudaStream_t)stream;
+    int r;
+    if (dtype == FVS_BF16)
+      r = n == 1 ? codes_gather_launch<1, FVS_BF16>(jobs + i0, 1, st) : codes_gather_launch<kCodeJobs, FVS_BF16>(jobs + i0, n, st);
+    else
+      r = n == 1 ? codes_gather_launch<1, FVS_F16>(jobs + i0, 1, st) : codes_gather_launch<kCodeJobs, FVS_F16>(jobs + i0, n, st);
     if (r) return r;
   }
   return FVS_OK;

@@ -132,6 +132,9 @@ class _FramePreprocessor:
 
     def _table(self, device):
         import torch
+        device = torch.device(device)
+        if device.type == "cuda" and device.index is None:
+            device = torch.device("cuda", torch.cuda.current_device())
         t = self._tables.get(device)
         if t is None:
             t = self._tables[device] = torch.from_numpy(self.table).to(device)
@@ -164,12 +167,18 @@ class _FramePreprocessor:
         x, y, _, _ = self._plan(torch.device(device) if device is not None else self._device(), height, width)
         return int(_lib.load().fvs_preprocess_workspace_bytes(C.byref(x), C.byref(y), frames))
 
-    def _run(self, frames, out=None, workspace=None):
+    @staticmethod
+    def _out_dtype(layout):
+        import torch
+        return {_lib.PRE_CLIP: torch.float16, _lib.PRE_QWEN: torch.float32, _lib.PRE_QWEN_CODES: torch.uint8}[layout]
+
+    def _run(self, frames, out=None, workspace=None, layout=None):
         import torch
         frames, device = self._frames(frames)
+        layout = self._layout if layout is None else layout
         T, H, W, ch = frames.shape
         x, y, pool, _ = self._plan(device, H, W)
-        shape, dtype = self.output_shape(T, H, W), (torch.float16 if self._layout == _lib.PRE_CLIP else torch.float32)
+        shape, dtype = self.output_shape(T, H, W), self._out_dtype(layout)
         if out is None:
             out = torch.empty(shape, dtype=dtype, device=device)
         elif tuple(out.shape) != shape or out.dtype != dtype or out.device != device or not out.is_contiguous():
@@ -181,14 +190,15 @@ class _FramePreprocessor:
             raise ValueError(f"workspace must be on {device}")
         with torch.cuda.device(device):
             _lib.check(_lib.load().fvs_preprocess(frames.data_ptr(), T, H, W, ch, C.byref(x), C.byref(y),
-                                                  self._table(device).data_ptr(), self._layout, pool, out.data_ptr(),
+                                                  self._table(device).data_ptr(), layout, pool, out.data_ptr(),
                                                   workspace.data_ptr(), workspace.numel() * workspace.element_size(),
                                                   _lib.cur_stream()), "fvs_preprocess")
         return out
 
-    def _many(self, clips, out=None, workspace=None):
+    def _many(self, clips, out=None, workspace=None, layout=None):
         """-> (out, one view of `out` per clip): every clip through one fvs_preprocess_multi call"""
         import torch
+        layout = self._layout if layout is None else layout
         if not isinstance(clips, (list, tuple)):
             raise TypeError(f"clips must be a list of uint8 [T, H, W, 3] clips, got {type(clips).__name__}")
         if not clips:
@@ -206,7 +216,7 @@ class _FramePreprocessor:
             jobs[i] = _lib.PreprocessJob(f.data_ptr(), T, H, W, ch, x, y)
         lib = _lib.load()
         plan, totals = (C.c_int64 * (4 * n))(), (C.c_int64 * 2)()
-        launches = lib.fvs_preprocess_plan(jobs, n, self._layout, pool, plan, totals)
+        launches = lib.fvs_preprocess_plan(jobs, n, layout, pool, plan, totals)
         if launches < 0:
             _lib.check(launches, "fvs_preprocess_plan")
         frames = [(f if f.is_cuda else f.to(device, non_blocking=True)).contiguous() for f in clips]
@@ -217,7 +227,7 @@ class _FramePreprocessor:
             shape = (sum(s[0] for s in shapes),) + shapes[0][1:]
         else:
             shape = (int(totals[0]),)
-        dtype = torch.float16 if self._layout == _lib.PRE_CLIP else torch.float32
+        dtype = self._out_dtype(layout)
         if out is None:
             out = torch.empty(shape, dtype=dtype, device=device)
         elif tuple(out.shape) != shape or out.dtype != dtype or out.device != device or not out.is_contiguous():
@@ -227,7 +237,7 @@ class _FramePreprocessor:
         elif workspace.device != device:
             raise ValueError(f"workspace must be on {device}")
         with torch.cuda.device(device):
-            _lib.check(lib.fvs_preprocess_multi(jobs, n, self._table(device).data_ptr(), self._layout, pool, out.data_ptr(),
+            _lib.check(lib.fvs_preprocess_multi(jobs, n, self._table(device).data_ptr(), layout, pool, out.data_ptr(),
                                                 workspace.data_ptr(), workspace.numel() * workspace.element_size(),
                                                 _lib.cur_stream()), "fvs_preprocess_multi")
         flat = out.view(-1)
@@ -294,7 +304,10 @@ class Qwen2VLFramePreprocessor(_FramePreprocessor):
     [[t, gh, gw]] on the host}, the dict embed_new_video_clip(**video_inputs) takes, equal to what
     FlashVStreamQwen2VLImageProcessor makes of the clip (smart_resize to a multiple of 28 * additional_pool_size, bicubic
     resize, rescale, normalize, patchify).  A one-frame clip fills both temporal slots; an odd frame count > 1 is refused,
-    as the reference's reshape fails there.  The defaults are Qwen2VLImageProcessor's."""
+    as the reference's reshape fails there.  The defaults are Qwen2VLImageProcessor's.
+    codes=True returns uint8 rows instead (FVS_PRE_QWEN_CODES, DESIGN.md §3.20): the same rows and columns holding the
+    resampled byte u, which the fp32 row element table[column // 392][u] is a function of; `device_table` is that
+    table, which qwen.ops.pixel_decode decodes them through."""
     _layout = _lib.PRE_QWEN
 
     def __init__(self, min_pixels: int = 56 * 56, max_pixels: int = 28 * 28 * 1280, additional_pool_size: int = 1,
@@ -317,18 +330,22 @@ class Qwen2VLFramePreprocessor(_FramePreprocessor):
         t, gh, gw = self.grid_thw(frames, height, width)
         return (t * gh * gw, 3 * QWEN_TEMPORAL * QWEN_PATCH * QWEN_PATCH)
 
-    def __call__(self, frames, out=None, workspace=None):
+    def device_table(self, device=None):
+        """the float32 [3, 256] value table on `device` (default: this preprocessor's), the one a call reads"""
+        return self._table(device if device is not None else self._device())
+
+    def __call__(self, frames, out=None, workspace=None, codes: bool = False):
         import torch
-        pixels = self._run(frames, out, workspace)
+        pixels = self._run(frames, out, workspace, _lib.PRE_QWEN_CODES if codes else None)
         T, H, W = (int(v) for v in frames.shape[:3])
         return {"pixel_values_videos": pixels, "video_grid_thw": torch.tensor([self.grid_thw(T, H, W)], dtype=torch.int64)}
 
-    def many(self, clips, out=None, workspace=None):
+    def many(self, clips, out=None, workspace=None, codes: bool = False):
         """Many clips (a list of uint8 [T, H, W, 3], host or device, any mix of sizes) in one launch pair per 32 clips ->
-        (out, views, grids): out fp32 [sum t*gh*gw, 1176], views[i] clip i's rows and grids[i] its int64 [[t, gh, gw]]
-        (host), bit-identical to self(clips[i]).  out and workspace (the sum of workspace_bytes
+        (out, views, grids): out fp32 [sum t*gh*gw, 1176] (uint8 with codes=True), views[i] clip i's rows and grids[i]
+        its int64 [[t, gh, gw]] (host), bit-identical to self(clips[i]).  out and workspace (the sum of workspace_bytes
         over the clips) may be given."""
         import torch
-        out, views = self._many(clips, out, workspace)
+        out, views = self._many(clips, out, workspace, _lib.PRE_QWEN_CODES if codes else None)
         grids = [torch.tensor([self.grid_thw(*(int(v) for v in f.shape[:3]))], dtype=torch.int64) for f in clips]
         return out, views, grids

@@ -31,8 +31,8 @@ import torch
 from .. import _lib as L
 from ..draws import DrawSource
 from . import ops as Q
-from .stream_state import (_KMEANS_METHODS, PATCH_DIM, QwenStreamState, _rest_finish, check_device_frames,
-                           check_full_res_bank, check_lazy_full_res, enqueue_csm)
+from .stream_state import (_KMEANS_METHODS, PATCH_DIM, QwenStreamState, _rest_finish, check_compact_pixels,
+                           check_device_frames, check_full_res_bank, check_lazy_full_res, enqueue_csm)
 from .vision_tower import QwenVisionBlocksB200
 
 MAX_GRIDS = 16            # grid entries one fvs_qwen_vit_encode call takes
@@ -92,7 +92,9 @@ def encode_picked(states, readbacks: torch.Tensor, max_rows: int = TOWER_ROWS):
     A state without full_res_bank (§3.19) plans through fvs_qwen_pick_plan_prev_multi instead: the picks its previous
     DAM does not hold (a DAM that is the whole bank plans the frames the previous one did not have, a count the host
     knows).  Its tower and merger rows are not scattered anywhere: they stay as the state's fresh rows, which the DAM
-    gather (fvs_qwen_dam_gather_fresh_multi) reads beside the previous DAM, and are dropped after it."""
+    gather (fvs_qwen_dam_gather_fresh_multi) reads beside the previous DAM, and are dropped after it.
+    A state with compact_pixels (§3.20) gathers through fvs_qwen_pixel_gather_codes_multi, which decodes its codes into
+    the rows fvs_qwen_pixel_gather_multi would have read."""
     if any(st._lazy_ctx["n_spa"] and st.tower is None for st in states):     # refused before any mask byte is set
         raise NotImplementedError("lazy_full_res: no full-resolution tower was given to the stream state")
     addr = Q.host_device_ptr(readbacks)
@@ -133,14 +135,21 @@ def encode_picked(states, readbacks: torch.Tensor, max_rows: int = TOWER_ROWS):
         tower, merger = todo[0][0].tower, todo[0][0].merger
         for grids, places in plan_tower_calls([[(n, *st.grid)] for st, n in todo], max_rows):
             rows = sum(t * h * w for t, h, w in grids)
-            inp = torch.empty(rows, PATCH_DIM, dtype=todo[0][0].pixels.dtype, device=todo[0][0].encoded.buf.device)
-            gathers = []
+            inp = torch.empty(rows, PATCH_DIM, dtype=todo[0][0].pixels.out_dtype, device=todo[0][0].encoded.buf.device)
+            gathers, code_gathers = [], []
             for i, (off,) in places:
                 st, n = todo[i]
                 px = st.pixels
-                gathers.append((st._plan, n, st.n_frames, px.base, px.table, px.chunk_frames,
-                                inp[off: off + n * st.grid[0] * st.grid[1]], px.frame_elems))
-            Q.pixel_gather_multi(gathers)
+                job = (st._plan, n, st.n_frames, px.base, px.table, px.chunk_frames,
+                       inp[off: off + n * st.grid[0] * st.grid[1]], px.frame_elems)
+                if px.values is None:
+                    gathers.append(job)
+                else:
+                    code_gathers.append(job + (px.values,))
+            if gathers:
+                Q.pixel_gather_multi(gathers)
+            if code_gathers:
+                Q.pixel_gather_codes_multi(code_gathers)
             feats = tower(inp, grids)
             merged = merger(feats) if todo[0][0]._layout[2] is not None else None
             scatters = []
@@ -188,15 +197,19 @@ class QwenStreamPool:
     video_grid_thw).  `lazy_full_res` (QwenStreamState's): the round runs the full-resolution tower once, after its one
     host wait, on only the frames some stream's DAM picks for the first time (encode_picked, DESIGN.md §3.18).
     `full_res_bank=False` (with lazy_full_res): every stream keeps no full-resolution or merged rows beyond its DAM, and
-    the round's one tower pass also re-encodes the picks a stream's previous DAM does not hold (§3.19).  The knobs are the
-    pool's: eager, lazy and bank-less streams do not share a pool."""
+    the round's one tower pass also re-encodes the picks a stream's previous DAM does not hold (§3.19).
+    `compact_pixels=True` (with lazy_full_res and a Qwen2VLFramePreprocessor): the round's frames come out of
+    `preprocess.many` as uint8 codes, ONE fvs_qwen_pixel_decode call makes the tower's rows of the whole round from
+    them, and each stream keeps the codes, half the pinned bytes of tower-dtype rows; its re-encodes decode as they
+    gather (§3.20).  Rounds of (pixels, grid) clips are refused.  The knobs are the pool's: eager, lazy and bank-less
+    streams do not share a pool."""
 
     TOWER_ROWS = TOWER_ROWS
     BATCH_MIN_JOBS = 4        # fewer k-means streams in a round take one enqueue_csm call each
 
     def __init__(self, model, device_frames: Optional[int] = None, max_streams: Optional[int] = None,
                  small_device_frames: Optional[int] = None, preprocess=None, lazy_full_res: bool = False,
-                 full_res_bank: bool = True):
+                 full_res_bank: bool = True, compact_pixels: bool = False):
         visual = model.visual
         flash, tower = visual.flash_memory, visual.encode_patches
         if not isinstance(tower, QwenVisionBlocksB200):
@@ -219,6 +232,12 @@ class QwenStreamPool:
         self.small_device_frames = check_device_frames(small_device_frames, "small_device_frames")
         self.lazy_full_res = check_lazy_full_res(lazy_full_res, flash)
         self.full_res_bank = check_full_res_bank(full_res_bank, self.lazy_full_res)
+        self.compact_pixels = check_compact_pixels(compact_pixels, self.lazy_full_res)
+        if self.compact_pixels:
+            from ..preprocess import Qwen2VLFramePreprocessor
+            if not isinstance(preprocess, Qwen2VLFramePreprocessor):
+                raise ValueError("QwenStreamPool: compact_pixels=True needs preprocess=Qwen2VLFramePreprocessor(...): the "
+                                 "codes are what it makes of uint8 frames")
         self.max_streams = max_streams
         self.preprocess = preprocess
         self._readbacks: Optional[torch.Tensor] = None     # pinned int32 [S, 8]: the round's read-backs
@@ -238,12 +257,14 @@ class QwenStreamPool:
         if checkpoint is None:
             state = QwenStreamState(self.flash, self.merger, device_frames=self.device_frames,
                                     small_device_frames=self.small_device_frames, lazy_full_res=self.lazy_full_res,
-                                    full_res_bank=self.full_res_bank)
+                                    full_res_bank=self.full_res_bank, compact_pixels=self.compact_pixels)
         else:
             state = QwenStreamState.restore(checkpoint, self.flash, self.merger, self.device, device_frames=self.device_frames,
                                             small_device_frames=self.small_device_frames,
-                                            lazy_full_res=self.lazy_full_res, full_res_bank=self.full_res_bank)
+                                            lazy_full_res=self.lazy_full_res, full_res_bank=self.full_res_bank,
+                                            compact_pixels=self.compact_pixels, pixel_table=self._pixel_table())
         state.tower = self.tower
+        state.pixel_table = self._pixel_table()
         if seed is None and checkpoint is None:
             seed = int.from_bytes(os.urandom(8), "little") >> 1
         rng = DrawSource(int(seed) if seed is not None else 0, self.device)
@@ -285,6 +306,10 @@ class QwenStreamPool:
         """the stream's 13-item `video_embedding_memory` list (QwenStreamState.as_list)"""
         return self._streams[sid].stream_state.as_list()
 
+    def _pixel_table(self):
+        """compact_pixels: the preprocessor's value table on the pool's device (None otherwise)"""
+        return self.preprocess.device_table(self.device) if self.compact_pixels else None
+
     # ---- one round -----------------------------------------------------------------------------------------------------
     def _validate(self, sid, clip):
         """-> (pixel rows on the device in the tower's dtype, t, h, w); raises before anything is enqueued"""
@@ -310,10 +335,10 @@ class QwenStreamPool:
             raise ValueError(f"QwenStreamPool.step: stream {sid}: grid {(h, w)} differs from the stream's grid {grid}")
         return pix, t, h, w
 
-    def _encode(self, items):
+    def _encode(self, items, codes=None):
         """items: [(pixels, t, h, w)] -> per item (x_new [t*h*w, D], small_new [t*h*w/4, D]) through as few tower calls
         as plan_tower_calls allows; with lazy_full_res, (the pixel rows [t*h*w, 1176] on the device, small_new): only the
-        half-resolution rows go through the tower here"""
+        half-resolution rows go through the tower here; with compact_pixels, (the item's codes, small_new)"""
         rows, segs, fulls = [], [], []
         for pix, t, h, w in items:
             full = pix.type(self.visual.get_dtype()).to(self.device, non_blocking=True).view(-1, PATCH_DIM)
@@ -332,7 +357,7 @@ class QwenStreamPool:
             for i, offs in places:
                 out[i] = tuple(feats[off: off + r.shape[0]] for off, r in zip(offs, rows[i]))
         if self.lazy_full_res:
-            out = [(full, o[0]) for full, o in zip(fulls, out)]
+            out = [(full, o[0]) for full, o in zip(fulls if codes is None else codes, out)]
         return out
 
     def step(self, clips: dict, draws: Optional[dict] = None):
@@ -342,13 +367,15 @@ class QwenStreamPool:
         while being completed (ZeroDivisionError on an empty cluster, as the reference) is left as the single-stream
         path leaves it; every other stream completes, and then the round raises one error naming the failing sids
         (`.errors`: sid -> exception).  With `preprocess`, a round of uint8 frames ({sid: [T, H, W, 3]}) is pre-processed
-        in one call first; a round mixing them with (pixels, grid) clips is refused."""
+        in one call first; a round mixing them with (pixels, grid) clips is refused, and so is a round of (pixels, grid)
+        clips in a compact_pixels pool."""
         draws = draws or {}
         sids = list(clips)
         frames = {not isinstance(clips[sid], (tuple, list)) for sid in sids}
         if len(frames) > 1:
             raise ValueError("QwenStreamPool.step: one round takes uint8 frames or (pixels, grid) clips for every stream, "
                              "not a mix")
+        codes = None
         if frames == {True}:
             if self.preprocess is None:
                 raise ValueError("QwenStreamPool.step: uint8 frames need a pool made with "
@@ -356,10 +383,21 @@ class QwenStreamPool:
             for sid in sids:
                 if sid not in self._streams:
                     raise KeyError(f"QwenStreamPool.step: no stream {sid}")
-            _, rows, grids = self.preprocess.many([clips[sid] for sid in sids])
+            out, rows, grids = self.preprocess.many([clips[sid] for sid in sids], codes=self.compact_pixels)
+            if self.compact_pixels:              # one decode of the round's codes into the rows the tower reads
+                out = out.to(self.device, non_blocking=True)
+                full, r, codes, rows = Q.pixel_decode(out, self._pixel_table(), self.visual.get_dtype()), 0, [], []
+                for g in grids:
+                    n = int(torch.prod(g))
+                    codes.append(out[r: r + n])
+                    rows.append(full[r: r + n])
+                    r += n
             clips = dict(zip(sids, zip(rows, grids)))
         items = [self._validate(sid, clips[sid]) for sid in sids]
-        feats = self._encode(items)
+        if codes is None and self.compact_pixels:
+            raise ValueError("QwenStreamPool.step: a compact_pixels pool keeps uint8 codes, which only uint8 frames give: "
+                             "(pixels, grid) clips are refused")
+        feats = self._encode(items, codes)
         merged = [None] * len(sids)
         if self.lazy_full_res:
             self._readback_rows(len(sids))

@@ -247,6 +247,39 @@ def pixel_gather_multi(jobs):
                                                  L.cur_stream()), "fvs_qwen_pixel_gather_multi")
 
 
+def pixel_decode(codes: torch.Tensor, table: torch.Tensor, dtype: torch.dtype,
+                 out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """fvs_qwen_pixel_decode: codes uint8 [rows, 1176] -> dtype(table[column // 392][code]) [rows, 1176] (f16 / bf16),
+    the bits of casting the fp32 rows the codes stand for (DESIGN.md §3.20)"""
+    _chk_cuda(codes, table, out)
+    codes, table = _c(codes), _c(table)
+    assert codes.dtype == torch.uint8 and codes.dim() == 2 and codes.shape[1] == 1176, f"codes {codes.dtype} {tuple(codes.shape)}"
+    assert table.dtype == torch.float32 and table.numel() == 3 * 256
+    if out is None:
+        out = torch.empty(codes.shape, dtype=dtype, device=codes.device)
+    assert out.dtype == dtype and out.is_contiguous() and out.shape == codes.shape
+    L.check(L.load().fvs_qwen_pixel_decode(codes.data_ptr(), codes.shape[0], table.data_ptr(), L.dtype_code(dtype),
+                                           out.data_ptr(), L.cur_stream()), "fvs_qwen_pixel_decode")
+    return out
+
+
+def pixel_gather_codes_multi(jobs):
+    """fvs_qwen_pixel_gather_codes_multi: jobs = [(plan int64, n, n_frames, base, chunk table (device int64),
+    chunk_frames, out [n, ...] of 16-bit rows, frame_elems (codes per frame), value table fp32 [3, 256])], all outputs
+    of one dtype: pixel_gather_multi over code chunks, decoded in the same pass"""
+    arr = []
+    for plan, n, n_frames, base, chunks, cf, out, fe, table in jobs:
+        _chk_cuda(plan, chunks, out, table)
+        assert plan.dtype == torch.int64 and chunks.dtype == torch.int64 and out.is_contiguous() and out.numel() == n * fe
+        assert table.dtype == torch.float32 and table.is_contiguous() and table.numel() == 3 * 256
+        arr.append(L.QwenPixelCodesJob(plan=plan.data_ptr(), n=int(n), n_frames=int(n_frames), base=int(base),
+                                       host_chunks=chunks.data_ptr(), chunk_frames=int(cf), frame_elems=int(fe),
+                                       table=table.data_ptr(), out=out.data_ptr()))
+    L.check(L.load().fvs_qwen_pixel_gather_codes_multi((L.QwenPixelCodesJob * len(arr))(*arr), len(arr),
+                                                       L.dtype_code(jobs[0][6].dtype), L.cur_stream()),
+            "fvs_qwen_pixel_gather_codes_multi")
+
+
 def bank_scatter_multi(jobs):
     """fvs_qwen_bank_scatter_multi: jobs = [dict(plan, n, n_frames, x_rows, merged_rows, dev_x, dev_merged, n_dev, chunks,
     chunk_frames, x_frame_elems, merged_frame_elems)], every row tensor of one 16-bit dtype"""

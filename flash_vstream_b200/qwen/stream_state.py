@@ -77,17 +77,23 @@ class QwenStreamState:
     the pixel rows in place of x_new, and the tower.  The published bits are the eager state's.
     full_res_bank: False (with lazy_full_res only) keeps no full-resolution or merged row of the frames the stream
     encodes: the step gathers its DAM from the previous DAM and from this step's tower output, and re-encodes a pick the
-    previous DAM does not hold from its pixel rows (DESIGN.md §3.19).  Same bits again."""
+    previous DAM does not hold from its pixel rows (DESIGN.md §3.19).  Same bits again.
+    compact_pixels: True (with lazy_full_res only) keeps each pixel row as the uint8 codes of FVS_PRE_QWEN_CODES, half
+    the bytes of the tower dtype: step() then takes the codes [t * h * w, 1176] in place of the pixel rows, and
+    `pixel_table` (the pre-processor's float32 [3, 256] device table) is what they decode through, on each re-encode,
+    into the rows the tower would have read (DESIGN.md §3.20).  Same bits again."""
 
     CHUNK_BYTES = CHUNK_BYTES
 
     def __init__(self, flash, merger, device_frames=None, small_device_frames=None, lazy_full_res=False,
-                 full_res_bank=True):
+                 full_res_bank=True, compact_pixels=False):
         self.flash, self.merger = flash, merger
         self.device_frames = check_device_frames(device_frames)
         self.small_device_frames = check_device_frames(small_device_frames, "small_device_frames")
         self.lazy_full_res = check_lazy_full_res(lazy_full_res, flash)
         self.full_res_bank = check_full_res_bank(full_res_bank, self.lazy_full_res)
+        self.compact_pixels = check_compact_pixels(compact_pixels, self.lazy_full_res)
+        self.pixel_table = None               # compact_pixels: device float32 [3, 256], what the codes decode through
         self.rng = GLOBAL                     # the draws.DrawSource of every k-means draw (a QwenStreamPool stream owns one)
         self.reset()
 
@@ -129,17 +135,20 @@ class QwenStreamState:
 
     # ------------------------------------------------------------------------------------------------ one clip
     def step(self, x_new: torch.Tensor, small_new: torch.Tensor, t: int, grid, small_grid, start_idx: int,
-             draws: Optional[dict] = None, merged: Optional[torch.Tensor] = None, tower=None):
+             draws: Optional[dict] = None, merged: Optional[torch.Tensor] = None, tower=None, pixel_table=None):
         """x_new [t * h * w, D] / small_new [t * hs * ws, D]: the tower's two-resolution features of the clip (device);
         grid = (h, w), small_grid = (hs, ws) host integers; merged: the PatchMerger rows of x_new, when the caller has
         merged them already (None: merged here).  Updates the state.  enqueue(), one host wait, complete().
         With lazy_full_res, x_new is the clip's full-resolution pixel rows [t * h * w, 1176] (device) and `tower`
         (callable(rows, grids)) encodes the frames the DAM picks for the first time: the one-stream round of
-        multistream.encode_picked, still one host wait."""
+        multistream.encode_picked, still one host wait.  With compact_pixels, x_new is the clip's codes and
+        `pixel_table` their value table (kept for later steps)."""
         if self.lazy_full_res:
             from .multistream import encode_picked
             if tower is not None:
                 self.tower = tower
+            if pixel_table is not None:
+                self.pixel_table = pixel_table
             if self._readback is None:
                 self._readback = torch.empty(8, dtype=torch.int32).pin_memory()
             self._in_round = True
@@ -191,6 +200,9 @@ class QwenStreamState:
         self._append_small(small_new.view(t, hs * ws, D), dev)
         small_bank = self.bank_small.rows() if self.bank_small.n else None
         if self.lazy_full_res:
+            if self.compact_pixels and (x_new.dtype != torch.uint8 or self.pixel_table is None):
+                raise ValueError(f"compact_pixels: the stream takes uint8 codes and their pixel_table (got {x_new.dtype} "
+                                 f"rows, table {'set' if self.pixel_table is not None else 'missing'})")
             self._append_lazy(x_new.view(t, h * w, PATCH_DIM), dt, D, dev)
         else:
             if S0 > 0 and self.merger is not None:
@@ -387,11 +399,19 @@ class QwenStreamState:
                 ms = torch.Size([hw // 4, int(self.merger.dim)])
             self._layout = (dt, torch.Size([hw, D]), ms)
         if self.pixels is None:
-            self.pixels = PixelStore(pix3.dtype, hw * PATCH_DIM, self.n_frames, self.CHUNK_BYTES)
+            self.pixels = self._pixel_store(hw, self.n_frames, pix3.dtype)
         self.pixels.append(pix3.reshape(t, -1), dev)
         if self.full_res_bank:
             self._append_slots(t, dev)
         self.encoded.append(torch.zeros(t, dtype=torch.uint8, device=dev))
+
+    def _pixel_store(self, hw: int, base: int, dtype) -> "PixelStore":
+        """an empty pixel store from frame `base` on: uint8 codes with their table that decode to the bank dtype
+        (compact_pixels), or rows of `dtype`"""
+        if self.compact_pixels:
+            return PixelStore(torch.uint8, hw * PATCH_DIM, base, self.CHUNK_BYTES, values=self.pixel_table,
+                              out_dtype=self._layout[0])
+        return PixelStore(dtype, hw * PATCH_DIM, base, self.CHUNK_BYTES)
 
     def _append_slots(self, t: int, dev):
         """t zero bank slots (rows in HBM, chunk rows on the host) at the end of the two-tier bank"""
@@ -516,9 +536,12 @@ class QwenStreamState:
     # is rebuilt by a bit-exact gather; the member lists are read by no step (only by spatial_enhance of the step that
     # made them), so a restored state has none, like a reset one.
     def _config(self, dim, dtype):
-        return {"flash": dict(self.flash.config), "grid": None if self.grid is None else list(self.grid),
-                "small_grid": None if self.small_grid is None else list(self.small_grid), "dtype": dtype, "dim": dim,
-                "merger_dim": None if self.merger is None else int(self.merger.dim)}
+        cfg = {"flash": dict(self.flash.config), "grid": None if self.grid is None else list(self.grid),
+               "small_grid": None if self.small_grid is None else list(self.small_grid), "dtype": dtype, "dim": dim,
+               "merger_dim": None if self.merger is None else int(self.merger.dim)}
+        if self.compact_pixels:
+            cfg["compact_pixels"] = True
+        return cfg
 
     def checkpoint(self):
         """The state as a checkpoint.StreamCheckpoint in pinned host memory (filled rows only; returns once the copies
@@ -549,7 +572,11 @@ class QwenStreamState:
             owned = {}                            # spilled banks: assembled in pinned memory here, taken as they are
             if self.lazy_full_res:                # the mask, and the pixel rows of the frames not yet encoded, in order
                 tensors["encoded"] = self.encoded.rows()
-                owned["pixels"] = self.pixels.rows_of(todo).view(len(todo), self._layout[1][0], PATCH_DIM)
+                if self.compact_pixels:           # as codes, with the table they decode through
+                    owned["pix_codes"] = self.pixels.rows_of(todo)
+                    tensors["pixel_table"] = self.pixels.values
+                else:
+                    owned["pixels"] = self.pixels.rows_of(todo).view(len(todo), self._layout[1][0], PATCH_DIM)
             if not self.full_res_bank:
                 tensors["spa_x"] = self.spa_x
             if self.n_small_host:
@@ -573,7 +600,7 @@ class QwenStreamState:
 
     @classmethod
     def restore(cls, ckpt, flash, merger, device, device_frames=None, small_device_frames=None,
-                lazy_full_res=False, full_res_bank=True) -> "QwenStreamState":
+                lazy_full_res=False, full_res_bank=True, compact_pixels=False, pixel_table=None) -> "QwenStreamState":
         """A state on `device` that continues `ckpt` bit for bit; `flash` / `merger` must have the configuration the
         checkpoint was taken with (ValueError naming the field otherwise).  The banks' frames are placed by this state's
         `device_frames` and `small_device_frames`, whatever the caps of the state that took the checkpoint.  An eager
@@ -581,7 +608,12 @@ class QwenStreamState:
         only once every frame is encoded (NotImplementedError naming the knob otherwise).  Into a state without
         full_res_bank, an eager or lazy checkpoint's stored rows become a frozen base bank (placed by `device_frames`)
         and later frames keep pixel rows only; a checkpoint of such a state restores into a lazy_full_res state (its
-        frames without stored rows "not yet encoded"), and into an eager one only when it has no such frame."""
+        frames without stored rows "not yet encoded"), and into an eager one only when it has no such frame.
+        A compact_pixels checkpoint (codes and their table) restores into a compact_pixels state whose `pixel_table`
+        (None: the checkpoint's) equals its table (ValueError naming pixel_table otherwise), and into a lazy_full_res
+        state without compact_pixels with its codes decoded, bit for bit.  A lazy_full_res checkpoint without codes
+        does not restore into a compact_pixels state (NotImplementedError naming compact_pixels): its rows need not
+        be codes of any table."""
         from .. import checkpoint as CK
         if ckpt.family != CK.QWEN:
             raise ValueError(f"QwenStreamState.restore: a {ckpt.family!r} checkpoint is not a Qwen2-VL stream's")
@@ -595,7 +627,22 @@ class QwenStreamState:
             raise ValueError(f"QwenStreamState.restore: config.merger_dim of the checkpoint ({c['merger_dim']}) differs "
                              f"from the merger's ({md})")
         st = cls(flash, merger, device_frames, small_device_frames, lazy_full_res=lazy_full_res,
-                 full_res_bank=full_res_bank)
+                 full_res_bank=full_res_bank, compact_pixels=compact_pixels)
+        compact_ck = bool(c.get("compact_pixels")) and "pix_frames" in n
+        if compact_pixels and "pix_frames" in n and not compact_ck:
+            raise NotImplementedError("QwenStreamState.restore: the checkpoint keeps its pixel rows in the tower dtype, "
+                                      "which need not be codes of any table: restore it with compact_pixels=False")
+        if compact_pixels and compact_ck and pixel_table is not None and not torch.equal(
+                ckpt.tensor("pixel_table"), pixel_table.detach().cpu().float()):
+            raise ValueError("QwenStreamState.restore: the checkpoint's pixel_table differs from the stream's: its codes "
+                             "would decode to other rows")
+        if compact_pixels:
+            st.pixel_table = pixel_table if pixel_table is not None or not compact_ck else ckpt.tensor("pixel_table")
+            if st.pixel_table is None and n["n_frames"] and lazy_full_res:
+                raise ValueError("QwenStreamState.restore: compact_pixels=True needs pixel_table=, the table the "
+                                 "stream's codes decode through")
+            if st.pixel_table is not None:
+                st.pixel_table = st.pixel_table.to(device).float().contiguous()
         if n["n_frames"] == 0:
             return st
         N = n["n_frames"]
@@ -627,10 +674,14 @@ class QwenStreamState:
                 hw = int(c["grid"][0]) * int(c["grid"][1])
                 # the pixel store starts at the first frame with pixel rows only; frames without a stored row get them
                 base = todo[0] if todo else N
-                st.pixels = PixelStore(st._layout[0], hw * PATCH_DIM, base, st.CHUNK_BYTES)
+                st.pixels = st._pixel_store(hw, base, st._layout[0])
                 if todo:
                     st.pixels.append(None, dev, t=N - base)
-                    st.pixels.put(todo, ckpt.tensor("pixels").view(len(todo), -1))
+                    if compact_ck and not compact_pixels:     # decoded here into the rows the tower reads
+                        rows = Q.pixel_decode(get("pix_codes").view(-1, PATCH_DIM), get("pixel_table"), st._layout[0])
+                        st.pixels.put(todo, rows.view(len(todo), -1).cpu())
+                    else:
+                        st.pixels.put(todo, ckpt.tensor("pix_codes" if compact_ck else "pixels").view(len(todo), -1))
                 st.n_encoded = N - len(todo)
                 if full_res_bank:                 # frames past the checkpoint's bank get zero slots, "not yet encoded"
                     st._append_slots(N - (st.bank_x.n + st.n_host), dev)
@@ -759,6 +810,16 @@ def check_lazy_full_res(v, flash, who: str = "lazy_full_res") -> bool:
     return v
 
 
+def check_compact_pixels(v, lazy: bool, who: str = "compact_pixels", lazy_who: str = "lazy_full_res") -> bool:
+    """a bool; True needs lazy_full_res (ValueError otherwise: only a lazy_full_res stream keeps pixel rows)"""
+    if not isinstance(v, bool):
+        raise ValueError(f"{who} must be True or False, got {v!r}")
+    if v and not lazy:
+        raise ValueError(f"{who}=True needs {lazy_who}=True: the codes stand in for the pixel rows only a "
+                         f"lazy_full_res stream keeps")
+    return v
+
+
 def check_full_res_bank(v, lazy: bool, who: str = "full_res_bank", lazy_who: str = "lazy_full_res") -> bool:
     """a bool; False needs lazy_full_res (ValueError otherwise: an eager stream's bank is where its features go)"""
     if not isinstance(v, bool):
@@ -773,10 +834,15 @@ class PixelStore:
     """lazy_full_res: the full-resolution pixel rows of frames [base, n) of a stream in pinned host chunks of
     chunk_frames frames each (host_tier's chunk arithmetic with no device tier), with a device table of the chunks'
     mapped pointers that fvs_qwen_pixel_gather_multi reads them through.  Frames below `base` (encoded before the stream
-    came here from a checkpoint) have no pixel rows; a restored stream's encoded frames above it have unwritten slots."""
+    came here from a checkpoint) have no pixel rows; a restored stream's encoded frames above it have unwritten slots.
+    dtype: the rows' element type, the tower dtype or uint8 codes (compact_pixels); a store of codes holds `values`,
+    the float32 [3, 256] device table they decode through, and gathers (gather_jobs) decode into `out_dtype`."""
 
-    def __init__(self, dtype, frame_elems: int, base: int, chunk_bytes: int = CHUNK_BYTES):
+    def __init__(self, dtype, frame_elems: int, base: int, chunk_bytes: int = CHUNK_BYTES, values=None, out_dtype=None):
         self.dtype, self.frame_elems, self.base, self.n = dtype, int(frame_elems), int(base), int(base)
+        if (dtype == torch.uint8) != (values is not None and out_dtype is not None):
+            raise ValueError("PixelStore: uint8 codes go with their value table and the dtype they decode to")
+        self.values, self.out_dtype = values, dtype if out_dtype is None else out_dtype
         self.chunk_frames = chunk_frames(self.frame_elems * dtype.itemsize, chunk_bytes)
         self.chunks, self.table = [], None
 
@@ -813,7 +879,9 @@ class PixelStore:
         return out
 
     def put(self, frames, rows: torch.Tensor):
-        """rows [len(frames), frame_elems] (host) into the slots of `frames`"""
+        """rows [len(frames), frame_elems] (host, the store's dtype) into the slots of `frames`"""
+        if rows.dtype != self.dtype:
+            raise ValueError(f"PixelStore.put: {rows.dtype} rows into a store of {self.dtype}")
         for i, f in enumerate(frames):
             self._row(int(f)).copy_(rows[i])
 

@@ -695,6 +695,33 @@ typedef struct fvs_qwen_fresh_gather_job {
   uint64_t* host_fetches;
 } fvs_qwen_fresh_gather_job;
 int fvs_qwen_dam_gather_fresh_multi(const fvs_qwen_fresh_gather_job* jobs, int n_jobs, int dtype, fvs_stream_t stream);
+
+/* 8-bit pixel codes (DESIGN.md §3.20): a stream fed uint8 frames keeps each full-resolution pixel row as the bytes u of
+ * FVS_PRE_QWEN_CODES, which the tower's input row dtype(table[c][u]) is a function of (c = column / 392, table the
+ * pre-processor's float32 [3, 256]).  Decode rounds to nearest even, as torch's fp32 -> bf16 / f16 cast does, so a
+ * decoded row equals the cast of the FVS_PRE_QWEN row bit for bit.
+ *
+ * fvs_qwen_pixel_decode: out[r, k] = dtype(table[k / 392][codes[r, k]]) for codes uint8 [rows, 1176] (8-byte aligned),
+ * table device float32 [3, 256], out f16 / bf16 [rows, 1176] (16-byte aligned).  One launch, no synchronisation. */
+int fvs_qwen_pixel_decode(const uint8_t* codes, int64_t rows, const float* table, int dtype, void* out,
+                          fvs_stream_t stream);
+/* fvs_qwen_pixel_gather_codes_multi: fvs_qwen_pixel_gather_multi over code chunks: per job, out[i] = the decoded rows of
+ * frame plan[i] (i < n), frame f >= base being frame f - base of the pinned chunks, chunk c holding chunk_frames frames
+ * of frame_elems bytes each (whole rows: frame_elems % 1176 == 0), read in place through host_chunks (a DEVICE table of
+ * mapped pointers) and decoded through `table` in the same pass; out [n, frame_elems] of `dtype`.  A frame outside
+ * [base, n_frames) yields zeros.  Job tables as above (FVS_EINVAL naming the job, nothing launched). */
+typedef struct fvs_qwen_pixel_codes_job {
+  const int64_t* plan;
+  int n;
+  int64_t n_frames;
+  int64_t base;
+  const void* const* host_chunks;
+  int chunk_frames;
+  int64_t frame_elems;
+  const float* table;
+  void* out;
+} fvs_qwen_pixel_codes_job;
+int fvs_qwen_pixel_gather_codes_multi(const fvs_qwen_pixel_codes_job* jobs, int n_jobs, int dtype, fvs_stream_t stream);
 /* *dev_out = the device address of pinned host memory `host` (cudaHostGetDevicePointer); FVS_EINVAL if it is not pinned */
 int fvs_host_device_ptr(const void* host, void** dev_out);
 
@@ -740,7 +767,7 @@ typedef struct fvs_resample_axis {
   const int32_t* bounds;        /* device int32 [count, 2] = {first source index, taps used}, 8-byte aligned */
   const int32_t* coeffs;        /* device int32 [count, taps], 22 fractional bits */
 } fvs_resample_axis;
-enum { FVS_PRE_CLIP = 0, FVS_PRE_QWEN = 1 };
+enum { FVS_PRE_CLIP = 0, FVS_PRE_QWEN = 1, FVS_PRE_QWEN_CODES = 2 };
 
 /* Host: PIL's per-axis plan (precompute_coeffs + normalize_coeffs_8bpc, in double, in PIL's order, no FMA contraction)
  * for the window [first, first + count) of in_size -> out_size.  Fills every field of *axis_h but bounds / coeffs, which
@@ -756,6 +783,8 @@ size_t fvs_preprocess_workspace_bytes(const fvs_resample_axis* x_h, const fvs_re
  *   FVS_PRE_QWEN: out fp32 pixel_values_videos [max(T, 2) / 2 * gh * gw, 1176] with gh = y.out_size / 14,
  *                 gw = x.out_size / 14 — the patchify of vstream_qwen2vl_processor.py:141-155; a one-frame clip fills both
  *                 temporal slots (:136-137).  The windows must be whole, T 1 or even, and both sizes multiples of 28 * pool.
+ *   FVS_PRE_QWEN_CODES: out uint8 [max(T, 2) / 2 * gh * gw, 1176], FVS_PRE_QWEN's rows and columns holding the resampled
+ *                 byte u itself instead of table[c][u], c = column / 392 (DESIGN.md §3.20); the same rules, the same plan.
  * FVS_EINVAL, with nothing launched, on null pointers, C != 3, an empty input, a plan that does not match the frames or
  * fvs_resample_plan, a window outside the resized image, a workspace below fvs_preprocess_workspace_bytes, or a Qwen2-VL
  * call breaking the rules above. */
@@ -776,6 +805,7 @@ typedef struct fvs_preprocess_job {
 } fvs_preprocess_job;
 /* Host plan of a job table (pure host arithmetic, validates like fvs_preprocess_multi, no CUDA call): plan_h [n_jobs, 4] =
  * {first block of the job in its rows launch, in its cols launch, output elements before it, workspace bytes before it};
+ * an element is 2 bytes (CLIP), 4 (Qwen2-VL) or 1 (Qwen2-VL codes), and the codes layout plans as FVS_PRE_QWEN does;
  * totals_h [2] = {output elements, workspace bytes}.  Returns the number of launch pairs (>= 1) or a negative error. */
 int fvs_preprocess_plan(const fvs_preprocess_job* jobs_h, int n_jobs, int layout, int pool, int64_t* plan_h,
                         int64_t* totals_h);
