@@ -90,23 +90,20 @@ class QwenGatherJob(C.Structure):  # fvs_qwen_gather_job
                 ("dev_merged", C.c_void_p), ("n_dev", C.c_int64), ("host_chunks", C.c_void_p), ("chunk_frames", C.c_int),
                 ("prev_picks", C.c_void_p), ("m", C.c_int), ("prev_x", C.c_void_p), ("prev_merged", C.c_void_p),
                 ("x_frame_elems", C.c_int64), ("merged_frame_elems", C.c_int64), ("spa_x_out", C.c_void_p),
-                ("merged_out", C.c_void_p), ("host_fetches", C.c_void_p)]
+                ("merged_out", C.c_void_p), ("host_fetches", C.c_void_p), ("fresh_frames", C.c_void_p),
+                ("n_fresh", C.c_int), ("fresh_x", C.c_void_p), ("fresh_merged", C.c_void_p), ("n_base", C.c_int64)]
 
 
 class QwenPickPlanJob(C.Structure):  # fvs_qwen_pick_plan_job
-    _fields_ = [("picks", C.c_void_p), ("n", C.c_int), ("n_frames", C.c_int64), ("encoded", C.c_void_p),
-                ("plan", C.c_void_p), ("count", C.c_void_p)]
+    _fields_ = [("picks", C.c_void_p), ("n", C.c_int), ("n_frames", C.c_int64), ("frames", C.c_void_p),
+                ("plan", C.c_void_p), ("count", C.c_void_p), ("prev_picks", C.c_void_p), ("m", C.c_int),
+                ("re_encodes", C.c_void_p), ("stored", C.c_uint8)]
 
 
 class QwenPixelJob(C.Structure):  # fvs_qwen_pixel_job
     _fields_ = [("plan", C.c_void_p), ("n", C.c_int), ("n_frames", C.c_int64), ("base", C.c_int64),
-                ("host_chunks", C.c_void_p), ("chunk_frames", C.c_int), ("frame_elems", C.c_int64), ("out", C.c_void_p)]
-
-
-class QwenPixelCodesJob(C.Structure):  # fvs_qwen_pixel_codes_job
-    _fields_ = [("plan", C.c_void_p), ("n", C.c_int), ("n_frames", C.c_int64), ("base", C.c_int64),
-                ("host_chunks", C.c_void_p), ("chunk_frames", C.c_int), ("frame_elems", C.c_int64), ("table", C.c_void_p),
-                ("out", C.c_void_p)]
+                ("host_chunks", C.c_void_p), ("chunk_frames", C.c_int), ("frame_elems", C.c_int64), ("out", C.c_void_p),
+                ("table", C.c_void_p)]
 
 
 class QwenScatterJob(C.Structure):  # fvs_qwen_scatter_job
@@ -114,21 +111,6 @@ class QwenScatterJob(C.Structure):  # fvs_qwen_scatter_job
                 ("merged_rows", C.c_void_p), ("dev_x", C.c_void_p), ("dev_merged", C.c_void_p), ("n_dev", C.c_int64),
                 ("host_chunks", C.c_void_p), ("chunk_frames", C.c_int), ("x_frame_elems", C.c_int64),
                 ("merged_frame_elems", C.c_int64)]
-
-
-class QwenPickPlanPrevJob(C.Structure):  # fvs_qwen_pick_plan_prev_job
-    _fields_ = [("picks", C.c_void_p), ("n", C.c_int), ("n_frames", C.c_int64), ("frames", C.c_void_p),
-                ("prev_picks", C.c_void_p), ("m", C.c_int), ("plan", C.c_void_p), ("count", C.c_void_p),
-                ("re_encodes", C.c_void_p)]
-
-
-class QwenFreshGatherJob(C.Structure):  # fvs_qwen_fresh_gather_job
-    _fields_ = [("picks", C.c_void_p), ("n", C.c_int), ("n_frames", C.c_int64), ("prev_picks", C.c_void_p),
-                ("m", C.c_int), ("prev_x", C.c_void_p), ("prev_merged", C.c_void_p), ("fresh_frames", C.c_void_p),
-                ("n_fresh", C.c_int), ("fresh_x", C.c_void_p), ("fresh_merged", C.c_void_p), ("n_base", C.c_int64),
-                ("dev_x", C.c_void_p), ("dev_merged", C.c_void_p), ("n_dev", C.c_int64), ("host_chunks", C.c_void_p),
-                ("chunk_frames", C.c_int), ("x_frame_elems", C.c_int64), ("merged_frame_elems", C.c_int64),
-                ("spa_x_out", C.c_void_p), ("merged_out", C.c_void_p), ("host_fetches", C.c_void_p)]
 
 
 QWEN_MEM_JOBS_PER_LAUNCH = 16
@@ -207,20 +189,13 @@ SIGNATURES = {
     "fvs_qwen_klarge_retrieve_tiered": (_i, [_vp, _vp, _vp, _i, C.POINTER(_vp), _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _sz,
                                              _vp]),
     "fvs_qwen_am_rope": (_i, [_vp, _i, _i, _i, _vp, _i, _i, _i, C.c_int64, _vp, _vp]),
-    # two-tier feature bank of the Qwen2-VL streaming state
-    "fvs_qwen_dam_gather": (_i, [_vp, _i, C.c_int64, _vp, _vp, C.c_int64, _vp, _i, _vp, _i, _vp, _vp, C.c_int64, C.c_int64,
-                                 _i, _vp, _vp, _vp, _vp]),
+    # feature bank of the Qwen2-VL streaming state
     "fvs_host_device_ptr": (_i, [_vp, C.POINTER(_vp)]),
-    # lazy full-resolution bank
     "fvs_qwen_pick_plan_multi": (_i, [C.POINTER(QwenPickPlanJob), _i, _vp]),
     "fvs_qwen_pixel_gather_multi": (_i, [C.POINTER(QwenPixelJob), _i, _i, _vp]),
     "fvs_qwen_bank_scatter_multi": (_i, [C.POINTER(QwenScatterJob), _i, _i, _vp]),
-    # no full-resolution bank
-    "fvs_qwen_pick_plan_prev_multi": (_i, [C.POINTER(QwenPickPlanPrevJob), _i, _vp]),
-    "fvs_qwen_dam_gather_fresh_multi": (_i, [C.POINTER(QwenFreshGatherJob), _i, _i, _vp]),
     # 8-bit pixel codes
     "fvs_qwen_pixel_decode": (_i, [_vp, C.c_int64, _vp, _i, _vp, _vp]),
-    "fvs_qwen_pixel_gather_codes_multi": (_i, [C.POINTER(QwenPixelCodesJob), _i, _i, _vp]),
     # publication of the Qwen2-VL streaming memory (seqlock)
     "fvs_qwen_pub_layout": (_i, [_i, _i, _i, _i, _i, _i, _i, _i64p]),
     "fvs_qwen_publish": (_i, [_vp, _sz, _i, _i, C.c_int64, _i, _vp, C.c_int64, _vp, _i, _vp, _i, _i, _i, _i, _i, C.c_uint64,

@@ -89,16 +89,15 @@ def encode_picked(states, readbacks: torch.Tensor, max_rows: int = TOWER_ROWS):
     the DAM gathers and the CSM merger of every state (stream_state._rest_finish).  The tower, the first state's, is
     invariant to batch composition (§3.7) and the merger row-wise (§3.5), so each frame gets the bits of the eager
     path.
-    A state without full_res_bank (§3.19) plans through fvs_qwen_pick_plan_prev_multi instead: the picks its previous
-    DAM does not hold (a DAM that is the whole bank plans the frames the previous one did not have, a count the host
-    knows).  Its tower and merger rows are not scattered anywhere: they stay as the state's fresh rows, which the DAM
-    gather (fvs_qwen_dam_gather_fresh_multi) reads beside the previous DAM, and are dropped after it.
-    A state with compact_pixels (§3.20) gathers through fvs_qwen_pixel_gather_codes_multi, which decodes its codes into
-    the rows fvs_qwen_pixel_gather_multi would have read."""
+    A state without full_res_bank (§3.19) plans the picks its previous DAM does not hold (a DAM that is the whole bank
+    plans the frames the previous one did not have, a count the host knows).  Its tower and merger rows are not
+    scattered anywhere: they stay as the state's fresh rows, which the DAM gather reads beside the previous DAM, and are
+    dropped after it.  A state with compact_pixels (§3.20) gathers its codes with their table, decoded into the rows a
+    store of tower-dtype rows would give."""
     if any(st._lazy_ctx["n_spa"] and st.tower is None for st in states):     # refused before any mask byte is set
         raise NotImplementedError("lazy_full_res: no full-resolution tower was given to the stream state")
     addr = Q.host_device_ptr(readbacks)
-    jobs, prev_jobs, counts = [], [], []
+    jobs, counts = [], []
     for k, st in enumerate(states):
         c = st._lazy_ctx
         n_spa, n = c["n_spa"], st.n_frames
@@ -106,23 +105,20 @@ def encode_picked(states, readbacks: torch.Tensor, max_rows: int = TOWER_ROWS):
         if n_spa == 0:                     # spatial_length 0: nothing is ever retrieved, so nothing is encoded
             counts.append(0)
             continue
+        # a DAM that is the whole bank is frames [0, n) (spatial_picks returns arange while n <= spatial_length)
         whole = n_spa == n
         count = addr + (k * 8 + 7) * readbacks.element_size()
-        if st.full_res_bank:
-            jobs.append((None if whole else c["picks"], n_spa, st.encoded.buf, n, st._plan, count))
-            counts.append(n - st.n_encoded if whole else None)
-            continue
-        # the previous DAM of a whole-bank DAM is frames [0, m) (spatial_picks returns arange while n <= spatial_length)
-        prev = st._prev_dam
-        if st.re_encodes is None:
+        prev = None if st.full_res_bank else st._prev_dam          # a bank holds every encoded frame: the mask says it
+        if not st.full_res_bank and st.re_encodes is None:
             st.re_encodes = torch.zeros(1, dtype=torch.int64, device=st._plan.device)
-        prev_jobs.append((c["picks"], st.encoded.buf, n, None if prev is None else prev[0], st._plan, count,
-                          st.re_encodes))
-        counts.append(n - (0 if prev is None else prev[0].numel()) if whole else None)
+        jobs.append((None if whole else c["picks"], n_spa, st.encoded.buf, n, st._plan, count,
+                     1 if st.full_res_bank else 2, None if prev is None else prev[0], st.re_encodes))
+        if not whole:
+            counts.append(None)
+        else:                              # the frames not yet encoded; without a bank, those the previous DAM lacks
+            counts.append(n - (st.n_encoded if st.full_res_bank else 0 if prev is None else prev[0].numel()))
     if jobs:
         Q.pick_plan_multi(jobs)
-    if prev_jobs:
-        Q.pick_plan_prev_multi(prev_jobs)
     if any(v is None for v in counts) or any(st._pending for st in states):
         done = torch.cuda.Event()
         done.record()
@@ -136,20 +132,13 @@ def encode_picked(states, readbacks: torch.Tensor, max_rows: int = TOWER_ROWS):
         for grids, places in plan_tower_calls([[(n, *st.grid)] for st, n in todo], max_rows):
             rows = sum(t * h * w for t, h, w in grids)
             inp = torch.empty(rows, PATCH_DIM, dtype=todo[0][0].pixels.out_dtype, device=todo[0][0].encoded.buf.device)
-            gathers, code_gathers = [], []
+            gathers = []                   # one kind: the states of a round share compact_pixels
             for i, (off,) in places:
                 st, n = todo[i]
                 px = st.pixels
-                job = (st._plan, n, st.n_frames, px.base, px.table, px.chunk_frames,
-                       inp[off: off + n * st.grid[0] * st.grid[1]], px.frame_elems)
-                if px.values is None:
-                    gathers.append(job)
-                else:
-                    code_gathers.append(job + (px.values,))
-            if gathers:
-                Q.pixel_gather_multi(gathers)
-            if code_gathers:
-                Q.pixel_gather_codes_multi(code_gathers)
+                gathers.append((st._plan, n, st.n_frames, px.base, px.table, px.chunk_frames,
+                                inp[off: off + n * st.grid[0] * st.grid[1]], px.frame_elems, px.values))
+            Q.pixel_gather_multi(gathers)
             feats = tower(inp, grids)
             merged = merger(feats) if todo[0][0]._layout[2] is not None else None
             scatters = []

@@ -194,24 +194,36 @@ def klarge_retrieve_multi(items, metric: str = "euclidean", want_dist: bool = Fa
 
 
 def dam_gather_multi(calls):
-    """fvs_qwen_dam_gather_multi: calls = [dict of dam_gather's keyword arguments], one per stream, all outputs of one
-    dtype; each stream gets the bits (and host_fetches count) of its own dam_gather call"""
+    """fvs_qwen_dam_gather_multi: calls = [dict(picks, n_frames, prev (picks, x rows, merged rows or None) or None,
+    fresh (plan int64, n_fresh, x rows, merged rows or None) or None, n_base (default: n_frames), dev_x, dev_merged,
+    n_dev, chunks (device int64 table of the host chunks' mapped pointers), chunk_frames, x_frame_elems,
+    merged_frame_elems, spa_x_out, merged_out, host_fetches (device int64 [1] counter or None))], one per stream, all
+    outputs of one 16-bit dtype: spa_x_out[i] = x[picks[i]], merged_out[i] = merged[picks[i]], each read from the first
+    of the previous DAM, the fresh rows, the device tier and the host chunks that holds the frame"""
     jobs, keep = [], []
     for a in calls:
-        picks, prev, sx, mo = _c(a["picks"]), a.get("prev"), a.get("spa_x_out"), a.get("merged_out")
+        picks, prev, fresh, sx, mo = _c(a["picks"]), a.get("prev"), a.get("fresh"), a.get("spa_x_out"), a.get("merged_out")
         _chk_cuda(picks, a["dev_x"], a["dev_merged"], a["chunks"], sx, mo, a.get("host_fetches"))
+        assert picks.dtype == torch.int64 and all(t is None or t.is_contiguous() for t in (sx, mo))
         m, pp, px, pm = 0, None, None, None
         if prev is not None and prev[0] is not None and prev[0].numel():
             pp, px, pm = prev
+            _chk_cuda(pp, px, pm)
             pp = _c(pp)
             m = pp.numel()
+        nf, fp, fx, fm = 0, None, None, None
+        if fresh is not None and fresh[1]:
+            fp, nf, fx, fm = fresh
+            _chk_cuda(fp, fx, fm)
+            assert fp.dtype == torch.int64 and fx.is_contiguous() and (fm is None or fm.is_contiguous())
         keep.append((picks, pp))
         jobs.append(L.QwenGatherJob(
             picks=picks.data_ptr(), n=picks.numel(), n_frames=int(a["n_frames"]), dev_x=L.ptr(a["dev_x"]),
             dev_merged=L.ptr(a["dev_merged"]), n_dev=int(a["n_dev"]), host_chunks=L.ptr(a["chunks"]),
             chunk_frames=int(a["chunk_frames"]), prev_picks=L.ptr(pp), m=m, prev_x=L.ptr(px), prev_merged=L.ptr(pm),
             x_frame_elems=int(a["x_frame_elems"]), merged_frame_elems=int(a["merged_frame_elems"]), spa_x_out=L.ptr(sx),
-            merged_out=L.ptr(mo), host_fetches=L.ptr(a.get("host_fetches"))))
+            merged_out=L.ptr(mo), host_fetches=L.ptr(a.get("host_fetches")), fresh_frames=L.ptr(fp), n_fresh=int(nf),
+            fresh_x=L.ptr(fx), fresh_merged=L.ptr(fm), n_base=int(a.get("n_base", a["n_frames"]))))
     out0 = calls[0].get("spa_x_out") if calls[0].get("spa_x_out") is not None else calls[0].get("merged_out")
     arr = (L.QwenGatherJob * len(jobs))(*jobs)
     L.check(L.load().fvs_qwen_dam_gather_multi(arr, len(jobs), L.dtype_code(out0.dtype), L.cur_stream()),
@@ -219,30 +231,40 @@ def dam_gather_multi(calls):
 
 
 def pick_plan_multi(jobs):
-    """fvs_qwen_pick_plan_multi: jobs = [(picks int64 [n] or None for frames 0..n-1, n, encoded uint8 [>= n_frames],
-    n_frames, plan int64 [>= n], count address)], count address = an int: the mapped address of an int32 slot of pinned
-    memory (host_device_ptr) or of a device int32.  Sets the planned frames' mask bytes."""
-    arr = []
-    for picks, n, encoded, n_frames, plan, count in jobs:
-        _chk_cuda(picks, encoded, plan)
-        assert (picks is None or (picks.dtype == torch.int64 and picks.is_contiguous() and picks.numel() >= n))
-        assert encoded.dtype == torch.uint8 and plan.dtype == torch.int64 and plan.numel() >= n
-        arr.append(L.QwenPickPlanJob(picks=L.ptr(picks), n=int(n), n_frames=int(n_frames), encoded=encoded.data_ptr(),
-                                     plan=plan.data_ptr(), count=int(count)))
+    """fvs_qwen_pick_plan_multi: jobs = [(picks int64 [n] or None for frames 0..n-1, n, frames uint8 [>= n_frames],
+    n_frames, plan int64 [>= n], count address[, stored, prev_picks int64 [m] or None, re_encodes int64 [1] or None])],
+    count address = an int: the mapped address of an int32 slot of pinned memory (host_device_ptr) or of a device int32.
+    Plans the picks whose frame byte is below `stored` (1, the default: a bank's "not yet encoded"; 2 without a bank:
+    not in the base bank) and that prev_picks does not hold, and sets the planned frames' bytes to 1.  A job of a
+    stream with a bank gives the first six items only."""
+    arr, keep = [], []
+    for picks, n, frames, n_frames, plan, count, *rest in jobs:
+        stored, prev, re_enc = rest or (1, None, None)
+        _chk_cuda(picks, frames, prev, plan, re_enc)
+        picks, prev = None if picks is None else _c(picks), None if prev is None or prev.numel() == 0 else _c(prev)
+        assert picks is None or (picks.dtype == torch.int64 and picks.numel() >= n)
+        assert frames.dtype == torch.uint8 and plan.dtype == torch.int64 and plan.numel() >= n
+        assert prev is None or prev.dtype == torch.int64
+        keep.append((picks, prev))
+        arr.append(L.QwenPickPlanJob(picks=L.ptr(picks), n=int(n), n_frames=int(n_frames), frames=frames.data_ptr(),
+                                     plan=plan.data_ptr(), count=int(count), prev_picks=L.ptr(prev),
+                                     m=0 if prev is None else prev.numel(), re_encodes=L.ptr(re_enc), stored=int(stored)))
     L.check(L.load().fvs_qwen_pick_plan_multi((L.QwenPickPlanJob * len(arr))(*arr), len(arr), L.cur_stream()),
             "fvs_qwen_pick_plan_multi")
 
 
 def pixel_gather_multi(jobs):
     """fvs_qwen_pixel_gather_multi: jobs = [(plan int64, n, n_frames, base, chunk table (device int64), chunk_frames,
-    out [n, ...] of 16-bit rows, frame_elems)], all outputs of one dtype"""
+    out [n, ...] of 16-bit rows, frame_elems, value table fp32 [3, 256] or None)], all outputs of one dtype and all jobs
+    of one kind: chunks of rows of out's dtype (no table), or of uint8 codes decoded through the table in the same pass"""
     arr = []
-    for plan, n, n_frames, base, table, cf, out, fe in jobs:
-        _chk_cuda(plan, table, out)
-        assert plan.dtype == torch.int64 and table.dtype == torch.int64 and out.is_contiguous() and out.numel() == n * fe
+    for plan, n, n_frames, base, chunks, cf, out, fe, table in jobs:
+        _chk_cuda(plan, chunks, out, table)
+        assert plan.dtype == torch.int64 and chunks.dtype == torch.int64 and out.is_contiguous() and out.numel() == n * fe
+        assert table is None or (table.dtype == torch.float32 and table.is_contiguous() and table.numel() == 3 * 256)
         arr.append(L.QwenPixelJob(plan=plan.data_ptr(), n=int(n), n_frames=int(n_frames), base=int(base),
-                                  host_chunks=table.data_ptr(), chunk_frames=int(cf), frame_elems=int(fe),
-                                  out=out.data_ptr()))
+                                  host_chunks=chunks.data_ptr(), chunk_frames=int(cf), frame_elems=int(fe),
+                                  out=out.data_ptr(), table=L.ptr(table)))
     L.check(L.load().fvs_qwen_pixel_gather_multi((L.QwenPixelJob * len(arr))(*arr), len(arr), L.dtype_code(jobs[0][6].dtype),
                                                  L.cur_stream()), "fvs_qwen_pixel_gather_multi")
 
@@ -263,23 +285,6 @@ def pixel_decode(codes: torch.Tensor, table: torch.Tensor, dtype: torch.dtype,
     return out
 
 
-def pixel_gather_codes_multi(jobs):
-    """fvs_qwen_pixel_gather_codes_multi: jobs = [(plan int64, n, n_frames, base, chunk table (device int64),
-    chunk_frames, out [n, ...] of 16-bit rows, frame_elems (codes per frame), value table fp32 [3, 256])], all outputs
-    of one dtype: pixel_gather_multi over code chunks, decoded in the same pass"""
-    arr = []
-    for plan, n, n_frames, base, chunks, cf, out, fe, table in jobs:
-        _chk_cuda(plan, chunks, out, table)
-        assert plan.dtype == torch.int64 and chunks.dtype == torch.int64 and out.is_contiguous() and out.numel() == n * fe
-        assert table.dtype == torch.float32 and table.is_contiguous() and table.numel() == 3 * 256
-        arr.append(L.QwenPixelCodesJob(plan=plan.data_ptr(), n=int(n), n_frames=int(n_frames), base=int(base),
-                                       host_chunks=chunks.data_ptr(), chunk_frames=int(cf), frame_elems=int(fe),
-                                       table=table.data_ptr(), out=out.data_ptr()))
-    L.check(L.load().fvs_qwen_pixel_gather_codes_multi((L.QwenPixelCodesJob * len(arr))(*arr), len(arr),
-                                                       L.dtype_code(jobs[0][6].dtype), L.cur_stream()),
-            "fvs_qwen_pixel_gather_codes_multi")
-
-
 def bank_scatter_multi(jobs):
     """fvs_qwen_bank_scatter_multi: jobs = [dict(plan, n, n_frames, x_rows, merged_rows, dev_x, dev_merged, n_dev, chunks,
     chunk_frames, x_frame_elems, merged_frame_elems)], every row tensor of one 16-bit dtype"""
@@ -296,59 +301,6 @@ def bank_scatter_multi(jobs):
     L.check(L.load().fvs_qwen_bank_scatter_multi((L.QwenScatterJob * len(arr))(*arr), len(arr),
                                                  L.dtype_code(jobs[0]["x_rows"].dtype), L.cur_stream()),
             "fvs_qwen_bank_scatter_multi")
-
-
-def pick_plan_prev_multi(jobs):
-    """fvs_qwen_pick_plan_prev_multi: jobs = [(picks int64 [n], frames uint8 [>= n_frames], n_frames, prev_picks int64
-    [m] or None, plan int64 [>= n], count address, re_encodes int64 [1] or None)], count address as for
-    pick_plan_multi.  Plans the picks the previous DAM does not hold (frame byte 2: stored in the base bank) and sets the
-    planned frames' bytes to 1."""
-    arr, keep = [], []
-    for picks, frames, n_frames, prev, plan, count, re_enc in jobs:
-        _chk_cuda(picks, frames, prev, plan, re_enc)
-        picks, prev = _c(picks), None if prev is None or prev.numel() == 0 else _c(prev)
-        assert picks.dtype == torch.int64 and frames.dtype == torch.uint8 and plan.dtype == torch.int64
-        assert plan.numel() >= picks.numel() and (prev is None or prev.dtype == torch.int64)
-        keep.append((picks, prev))
-        arr.append(L.QwenPickPlanPrevJob(picks=picks.data_ptr(), n=picks.numel(), n_frames=int(n_frames),
-                                         frames=frames.data_ptr(), prev_picks=L.ptr(prev),
-                                         m=0 if prev is None else prev.numel(), plan=plan.data_ptr(), count=int(count),
-                                         re_encodes=L.ptr(re_enc)))
-    L.check(L.load().fvs_qwen_pick_plan_prev_multi((L.QwenPickPlanPrevJob * len(arr))(*arr), len(arr), L.cur_stream()),
-            "fvs_qwen_pick_plan_prev_multi")
-
-
-def dam_gather_fresh_multi(calls):
-    """fvs_qwen_dam_gather_fresh_multi: calls = [dict(picks, n_frames, prev (picks, x rows, merged rows or None) or None,
-    fresh (plan int64, n_fresh, x rows, merged rows or None) or None, n_base, dev_x, dev_merged, n_dev, chunks,
-    chunk_frames, x_frame_elems, merged_frame_elems, spa_x_out, merged_out, host_fetches)], one per stream, all outputs of
-    one dtype"""
-    jobs, keep = [], []
-    for a in calls:
-        picks, prev, fresh, sx, mo = _c(a["picks"]), a.get("prev"), a.get("fresh"), a.get("spa_x_out"), a.get("merged_out")
-        _chk_cuda(picks, a["dev_x"], a["dev_merged"], a["chunks"], sx, mo, a.get("host_fetches"))
-        m, pp, px, pm = 0, None, None, None
-        if prev is not None and prev[0] is not None and prev[0].numel():
-            pp, px, pm = prev
-            pp = _c(pp)
-            m = pp.numel()
-        nf, fp, fx, fm = 0, None, None, None
-        if fresh is not None and fresh[1]:
-            fp, nf, fx, fm = fresh
-            _chk_cuda(fp, fx, fm)
-            assert fp.dtype == torch.int64 and fx.is_contiguous() and (fm is None or fm.is_contiguous())
-        keep.append((picks, pp))
-        jobs.append(L.QwenFreshGatherJob(
-            picks=picks.data_ptr(), n=picks.numel(), n_frames=int(a["n_frames"]), prev_picks=L.ptr(pp), m=m,
-            prev_x=L.ptr(px), prev_merged=L.ptr(pm), fresh_frames=L.ptr(fp), n_fresh=int(nf), fresh_x=L.ptr(fx),
-            fresh_merged=L.ptr(fm), n_base=int(a["n_base"]), dev_x=L.ptr(a["dev_x"]), dev_merged=L.ptr(a["dev_merged"]),
-            n_dev=int(a["n_dev"]), host_chunks=L.ptr(a["chunks"]), chunk_frames=int(a["chunk_frames"]),
-            x_frame_elems=int(a["x_frame_elems"]), merged_frame_elems=int(a["merged_frame_elems"]), spa_x_out=L.ptr(sx),
-            merged_out=L.ptr(mo), host_fetches=L.ptr(a.get("host_fetches"))))
-    out0 = calls[0].get("spa_x_out") if calls[0].get("spa_x_out") is not None else calls[0].get("merged_out")
-    arr = (L.QwenFreshGatherJob * len(jobs))(*jobs)
-    L.check(L.load().fvs_qwen_dam_gather_fresh_multi(arr, len(jobs), L.dtype_code(out0.dtype), L.cur_stream()),
-            "fvs_qwen_dam_gather_fresh_multi")
 
 
 def mem_workspace_bytes(T: int, K: int, PD: int) -> int:
@@ -423,32 +375,6 @@ def host_device_ptr(t: torch.Tensor) -> int:
     out = C.c_void_p()
     L.check(L.load().fvs_host_device_ptr(t.data_ptr(), C.byref(out)), "fvs_host_device_ptr")
     return out.value
-
-
-def dam_gather(picks: torch.Tensor, n_frames: int, dev_x: Optional[torch.Tensor], dev_merged: Optional[torch.Tensor],
-               n_dev: int, chunks: Optional[torch.Tensor], chunk_frames: int, x_frame_elems: int, merged_frame_elems: int,
-               prev=None, spa_x_out: Optional[torch.Tensor] = None, merged_out: Optional[torch.Tensor] = None,
-               host_fetches: Optional[torch.Tensor] = None):
-    """fvs_qwen_dam_gather: spa_x_out[i] = x[picks[i]], merged_out[i] = merged[picks[i]] over the two-tier bank.
-    dev_x / dev_merged: the device tier (frames [0, n_dev)); chunks: device int64 table of the host chunks' mapped
-    pointers; prev = (picks [m], x [m, ...], merged [m, ...] or None) of the previous step's DAM, or None; host_fetches:
-    device int64 [1] counter.  The outputs are the caller's fresh tensors of the bank's dtype."""
-    _chk_cuda(picks, dev_x, dev_merged, chunks, spa_x_out, merged_out, host_fetches)
-    assert picks.dtype == torch.int64 and (chunks is None or chunks.dtype == torch.int64)
-    out = spa_x_out if spa_x_out is not None else merged_out
-    for t in (spa_x_out, merged_out):
-        assert t is None or (t.is_contiguous() and t.dtype == out.dtype)
-    m, px, pm = 0, None, None
-    if prev is not None and prev[0] is not None and prev[0].numel():
-        pp, px, pm = prev
-        _chk_cuda(pp, px, pm)
-        m = pp.numel()
-    L.check(L.load().fvs_qwen_dam_gather(
-        L.ptr(_c(picks)), picks.numel(), int(n_frames), L.ptr(dev_x), L.ptr(dev_merged), int(n_dev), L.ptr(chunks),
-        int(chunk_frames), L.ptr(None if m == 0 else _c(pp)), m, L.ptr(px), L.ptr(pm), int(x_frame_elems),
-        int(merged_frame_elems), L.dtype_code(out.dtype), L.ptr(spa_x_out), L.ptr(merged_out), L.ptr(host_fetches),
-        L.cur_stream()), "fvs_qwen_dam_gather")
-    return spa_x_out, merged_out
 
 
 def am_rope(spa_positions: torch.Tensor, spa_grid, tem_positions: torch.Tensor, tem_grid, visual_start_id: int,

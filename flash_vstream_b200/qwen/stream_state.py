@@ -68,7 +68,7 @@ class QwenStreamState:
     """flash: the streaming FlashMemory (temporal_length / spatial_length in frames, methods); merger: PatchMerger.
     device_frames: how many frames of the full-resolution and merged banks stay in HBM (None: all of them).  Later frames
     are copied to pinned host chunks as they arrive and never move again; a step reads only its retrieved frames from
-    them (fvs_qwen_dam_gather).
+    them (fvs_qwen_dam_gather_multi).
     small_device_frames: how many frames of the half-resolution bank stay in HBM (None: all of them).  Later frames go to
     pinned host chunks of their own; the klarge retrieval sweeps them in place over PCIe (fvs_qwen_klarge_retrieve_tiered),
     once per step, twice with the cosine metric.  The two caps are independent; results are bit-identical either way.
@@ -339,7 +339,8 @@ class QwenStreamState:
 
     # ------------------------------------------------------------------------------------------------ two-tier bank
     def _dam(self):
-        """the current DAM as a previous-step source for fvs_qwen_dam_gather: (picks, spa_x, DAM rows of video_embeds)"""
+        """the current DAM as a previous-step source for fvs_qwen_dam_gather_multi: (picks, spa_x, DAM rows of
+        video_embeds)"""
         if self.spa_positions is None or self.spa_positions.numel() == 0 or not self.spa_x.is_cuda:
             return None
         m = self.spa_positions.numel()
@@ -355,17 +356,7 @@ class QwenStreamState:
         use"""
         dt, xs, ms = self._layout
         F, fx, fm = self._per_chunk(), xs.numel(), 0 if ms is None else ms.numel()
-        while len(self.host_chunks) <= c:
-            k = len(self.host_chunks)
-            buf = torch.empty(F * (fx + fm), dtype=dt, pin_memory=True)
-            tab = self._chunk_table
-            if tab is None or tab.numel() <= k:
-                tab = torch.zeros(max(16, 2 * k), dtype=torch.int64, device=dev)
-                if k:
-                    tab[:k].copy_(self._chunk_table[:k])
-                self._chunk_table = tab
-            tab[k].fill_(Q.host_device_ptr(buf))                  # stream-ordered: no host wait
-            self.host_chunks.append(buf)
+        self._chunk_table = grow_pinned(self.host_chunks, self._chunk_table, c, (F * (fx + fm),), dt, dev)
         buf = self.host_chunks[c]
         return buf[: F * fx].view(F, *xs), None if ms is None else buf[F * fx:].view(F, *ms)
 
@@ -425,15 +416,20 @@ class QwenStreamState:
             self._chunk(c, dev)
             self.n_host += cnt
 
+    def _bank_args(self) -> dict:
+        """this state's two-tier bank as the gather and scatter jobs read it; n_base: its frames (without
+        full_res_bank, those of the base bank, which may be fewer than the stream's)"""
+        dt, xs, ms = self._layout
+        return dict(n_base=self.bank_x.n + self.n_host, dev_x=self.bank_x.buf if self.bank_x.n else None,
+                    dev_merged=self.bank_merged.buf if self.bank_merged.n else None, n_dev=self.bank_x.n,
+                    chunks=self._chunk_table, chunk_frames=self._per_chunk(), x_frame_elems=xs.numel(),
+                    merged_frame_elems=0 if ms is None else ms.numel())
+
     def _scatter_args(self, n: int, x_rows, merged_rows) -> dict:
         """the job of Q.bank_scatter_multi that writes the n frames of this state's last pick plan into its banks"""
-        dt, xs, ms = self._layout
-        return dict(plan=self._plan, n=n, n_frames=self.bank_x.n + self.n_host, x_rows=x_rows,
-                    merged_rows=merged_rows if ms is not None else None,
-                    dev_x=self.bank_x.buf if self.bank_x.n else None,
-                    dev_merged=self.bank_merged.buf if self.bank_merged.n and ms is not None else None,
-                    n_dev=self.bank_x.n, chunks=self._chunk_table, chunk_frames=self._per_chunk(),
-                    x_frame_elems=xs.numel(), merged_frame_elems=0 if ms is None else ms.numel())
+        bank = self._bank_args()
+        return dict(bank, plan=self._plan, n=n, n_frames=bank["n_base"], x_rows=x_rows,
+                    merged_rows=merged_rows if bank["merged_frame_elems"] else None)
 
     def _small_per_chunk(self) -> int:
         dt, ps = self._small_layout
@@ -467,32 +463,13 @@ class QwenStreamState:
         return Q.TieredBank(rb.rows().view(rb.n, -1) if rb.n else None, rb.n, tuple(self._small_ptrs),
                             self._small_per_chunk(), rb.n + self.n_small_host, self._small_layout[0], dev)
 
-    def _gather(self, picks, spa_x, merged, prev):
-        args = self._gather_args(picks, spa_x, merged, prev)
-        if self.full_res_bank:
-            Q.dam_gather(**args)
-        else:
-            Q.dam_gather_fresh_multi([args])
-
     def _gather_args(self, picks, spa_x, merged, prev) -> dict:
-        """the keyword arguments of the Q.dam_gather that writes spa_x / merged for `picks` from this state's banks;
-        without full_res_bank, of the Q.dam_gather_fresh_multi job that reads the previous DAM `prev`, this step's fresh
-        rows and the base bank"""
-        dt, xs, ms = self._layout
+        """the Q.dam_gather_multi job that writes spa_x / merged for `picks` from the previous DAM `prev`, this step's
+        fresh rows (without full_res_bank) and this state's bank"""
         if self.host_fetches is None:
             self.host_fetches = torch.zeros(1, dtype=torch.int64, device=picks.device)
-        if not self.full_res_bank:
-            return dict(picks=picks, n_frames=self.n_frames, prev=prev, fresh=self._fresh,
-                        n_base=self.bank_x.n + self.n_host, dev_x=self.bank_x.buf if self.bank_x.n else None,
-                        dev_merged=self.bank_merged.buf if self.bank_merged.n else None, n_dev=self.bank_x.n,
-                        chunks=self._chunk_table, chunk_frames=self._per_chunk(), x_frame_elems=xs.numel(),
-                        merged_frame_elems=0 if ms is None else ms.numel(), spa_x_out=spa_x, merged_out=merged,
-                        host_fetches=self.host_fetches)
-        return dict(picks=picks, n_frames=self.bank_x.n + self.n_host, dev_x=self.bank_x.buf if self.bank_x.n else None,
-                    dev_merged=self.bank_merged.buf if self.bank_merged.n else None, n_dev=self.bank_x.n,
-                    chunks=self._chunk_table, chunk_frames=self._per_chunk(), x_frame_elems=xs.numel(),
-                    merged_frame_elems=0 if ms is None else ms.numel(), prev=prev, spa_x_out=spa_x, merged_out=merged,
-                    host_fetches=self.host_fetches)
+        return dict(self._bank_args(), picks=picks, n_frames=self.n_frames, prev=prev, fresh=self._fresh,
+                    spa_x_out=spa_x, merged_out=merged, host_fetches=self.host_fetches)
 
     def host_fetch_count(self) -> int:
         """retrieved frames read from the host chunks since the stream started here (synchronises; tests and timing)"""
@@ -703,7 +680,7 @@ class QwenStreamState:
             else:
                 st.spa_x = torch.empty(n["n_spa"], h * w, int(c["dim"]), dtype=st._layout[0], device=dev)
                 if n["n_spa"]:
-                    st._gather(st.spa_positions, st.spa_x, None, None)
+                    Q.dam_gather_multi([st._gather_args(st.spa_positions, st.spa_x, None, None)])
             st.video_embeds = get("video_embeds") if "video_embeds" in ckpt.tensors else None
             torch.cuda.current_stream().synchronize()     # the pinned sources may be freed as soon as this returns
         return st
@@ -775,7 +752,7 @@ def _rest_stage(ctxs):
 
 def _rest_finish(ctxs):
     """the second half of _rest_stage, once the retrieved frames are in the banks (or, without full_res_bank, in the
-    fresh rows): _rest_outputs, one DAM gather table per dtype and kind, and one PatchMerger call over every CSM slice"""
+    fresh rows): _rest_outputs, one DAM gather table per dtype, and one PatchMerger call over every CSM slice"""
     if not ctxs:
         return
     gathers, merges = {}, []
@@ -783,11 +760,11 @@ def _rest_finish(ctxs):
         g, m = state._rest_outputs(c)
         if g is not None:
             out = g["spa_x_out"] if g["spa_x_out"] is not None else g["merged_out"]
-            gathers.setdefault((out.dtype, state.full_res_bank), []).append(g)
+            gathers.setdefault(out.dtype, []).append(g)
         if m is not None:
             merges.append(m)
-    for (_, bank), calls in gathers.items():
-        (Q.dam_gather_multi if bank else Q.dam_gather_fresh_multi)(calls)
+    for calls in gathers.values():
+        Q.dam_gather_multi(calls)
     merger = ctxs[0][0].merger
     if len(merges) == 1:
         merger(merges[0][0], out=merges[0][1])
@@ -836,7 +813,7 @@ class PixelStore:
     mapped pointers that fvs_qwen_pixel_gather_multi reads them through.  Frames below `base` (encoded before the stream
     came here from a checkpoint) have no pixel rows; a restored stream's encoded frames above it have unwritten slots.
     dtype: the rows' element type, the tower dtype or uint8 codes (compact_pixels); a store of codes holds `values`,
-    the float32 [3, 256] device table they decode through, and gathers (gather_jobs) decode into `out_dtype`."""
+    the float32 [3, 256] device table the gather decodes them through into `out_dtype`."""
 
     def __init__(self, dtype, frame_elems: int, base: int, chunk_bytes: int = CHUNK_BYTES, values=None, out_dtype=None):
         self.dtype, self.frame_elems, self.base, self.n = dtype, int(frame_elems), int(base), int(base)
@@ -851,16 +828,7 @@ class PixelStore:
         unwritten (frames whose rows are put() later or never read)"""
         t = rows.shape[0] if rows is not None else int(t)
         for c, dst, s, cnt in placement(self.n - self.base, t, 0, self.chunk_frames):
-            while len(self.chunks) <= c:
-                k = len(self.chunks)
-                buf = torch.empty(self.chunk_frames, self.frame_elems, dtype=self.dtype, pin_memory=True)
-                if self.table is None or self.table.numel() <= k:
-                    tab = torch.zeros(max(16, 2 * k), dtype=torch.int64, device=dev)
-                    if k:
-                        tab[:k].copy_(self.table[:k])
-                    self.table = tab
-                self.table[k].fill_(Q.host_device_ptr(buf))
-                self.chunks.append(buf)
+            self.table = grow_pinned(self.chunks, self.table, c, (self.chunk_frames, self.frame_elems), self.dtype, dev)
             if rows is not None:
                 self.chunks[c][dst: dst + cnt].copy_(rows[s: s + cnt], non_blocking=True)
         self.n += t
@@ -884,6 +852,23 @@ class PixelStore:
             raise ValueError(f"PixelStore.put: {rows.dtype} rows into a store of {self.dtype}")
         for i, f in enumerate(frames):
             self._row(int(f)).copy_(rows[i])
+
+
+def grow_pinned(chunks: list, table: Optional[torch.Tensor], c: int, shape, dtype, dev) -> torch.Tensor:
+    """pinned host chunks of `shape` appended to `chunks` until chunk c exists, each one's mapped device pointer stored
+    to its slot of `table` (device int64, grown by doubling; None: none yet), which kernels read the chunks through in
+    place -> the table"""
+    while len(chunks) <= c:
+        k = len(chunks)
+        buf = torch.empty(shape, dtype=dtype, pin_memory=True)
+        if table is None or table.numel() <= k:
+            tab = torch.zeros(max(16, 2 * k), dtype=torch.int64, device=dev)
+            if k:
+                tab[:k].copy_(table[:k])
+            table = tab
+        table[k].fill_(Q.host_device_ptr(buf))                  # stream-ordered: no host wait
+        chunks.append(buf)
+    return table
 
 
 def _on_host(rb: RowBank, chunks, n: int, row_shape, dt) -> torch.Tensor:

@@ -545,27 +545,28 @@ int fvs_qwen_klarge_retrieve_multi(const fvs_qwen_retrieve_job* jobs_h, int n_jo
 int fvs_qwen_am_rope(const int64_t* spa_positions, int spa_t, int spa_h, int spa_w, const int64_t* tem_positions, int tem_t,
                      int tem_h, int tem_w, int64_t visual_start_id, int64_t* out, fvs_stream_t stream);
 
-/* ---- two-tier feature bank of the Qwen2-VL streaming state (DESIGN.md §3.13) --------------------------------------------
+/* ---- feature bank of the Qwen2-VL streaming state (DESIGN.md §3.13, §3.18-§3.20) ------------------------------------------
  * Frames [0, n_dev) of the full-resolution bank (x, x_frame_elems 16-bit elements per frame) and of the PatchMerger bank
- * (merged, merged_frame_elems per frame) are contiguous device rows dev_x / dev_merged.  Frames [n_dev, n_frames) live in
- * pinned host chunks: chunk c holds frames n_dev + c*chunk_frames + [0, chunk_frames) as [chunk_frames x rows |
- * chunk_frames merged rows]; host_chunks is a DEVICE table of the chunks' mapped device pointers (fvs_host_device_ptr).
+ * (merged, merged_frame_elems per frame) are contiguous device rows dev_x / dev_merged.  Later frames live in pinned host
+ * chunks: chunk c holds frames n_dev + c*chunk_frames + [0, chunk_frames) as [chunk_frames x rows | chunk_frames merged
+ * rows]; host_chunks is a DEVICE table of the chunks' mapped device pointers (fvs_host_device_ptr).
+ * Every call below is a job table (one stream = the one-job table): every job is checked before anything is enqueued
+ * (FVS_EINVAL naming the job otherwise), at most FVS_QWEN_MEM_JOBS_PER_LAUNCH jobs go into one launch, and no two jobs
+ * may share an output.
  *
- * fvs_qwen_dam_gather: one launch writes, for every pick i (picks: device int64 [n], e.g. fvs_qwen_klarge_retrieve's
- * output), spa_x_out[i] = x[picks[i]] and merged_out[i] = merged[picks[i]] (either output may be NULL; not both).  Each
- * pick is read from the first source that has it: the device tier; the previous step's DAM (prev_picks [m], prev_x
- * [m, x_frame_elems], prev_merged [m, merged_frame_elems] — HBM rows that already hold those frames); the host chunk, as
- * zero-copy 16-byte loads.  *host_fetches (device, optional) grows by the number of picks read from the host.  A pick
- * outside [0, n_frames) yields zero rows.  The outputs must not alias any source.  Row tensors 16-byte aligned, frame
- * sizes multiples of 16 bytes, n <= 65535.  FVS_EINVAL with nothing launched on a bad argument. */
-int fvs_qwen_dam_gather(const int64_t* picks, int n, int64_t n_frames, const void* dev_x, const void* dev_merged,
-                        int64_t n_dev, const void* const* host_chunks, int chunk_frames, const int64_t* prev_picks, int m,
-                        const void* prev_x, const void* prev_merged, int64_t x_frame_elems, int64_t merged_frame_elems,
-                        int dtype, void* spa_x_out, void* merged_out, uint64_t* host_fetches, fvs_stream_t stream);
-/* fvs_qwen_dam_gather of many streams in one launch (the single call is the one-job launch): job i gets exactly the bits
- * (and host_fetches count) of the single call with its own arguments — its own two-tier bank, previous DAM and chunk table.  dtype is the call's.  At most
- * FVS_QWEN_MEM_JOBS_PER_LAUNCH jobs per launch; every job gets the single call's checks, and no output (spa_x_out,
- * merged_out, host_fetches) may be shared by two jobs: FVS_EINVAL with nothing launched otherwise. */
+ * fvs_qwen_dam_gather_multi: per job, for every pick i (picks: device int64 [n], e.g. fvs_qwen_klarge_retrieve's
+ * output), spa_x_out[i] = x[picks[i]] and merged_out[i] = merged[picks[i]] (either output may be NULL; not both), each
+ * read from the first source that holds the frame:
+ *   1. the previous step's DAM: prev_picks [m], prev_x [m, x_frame_elems], prev_merged [m, merged_frame_elems];
+ *   2. this step's fresh rows: fresh_frames [n_fresh], fresh_x [n_fresh, x_frame_elems], fresh_merged [n_fresh,
+ *      merged_frame_elems] (a stream without a full-resolution bank: the tower and PatchMerger output of its planned
+ *      frames, in plan order; n_fresh is a host integer);
+ *   3. the device tier, frames [0, n_dev);
+ *   4. the host chunks, frames [n_dev, n_base), as zero-copy 16-byte loads; *host_fetches (device, optional) grows by
+ *      the number of picks read there.
+ * A pick outside [0, n_frames), or in no source, yields zero rows.  A stream with a bank passes n_fresh = 0 and
+ * n_base = n_frames.  The outputs must not alias any source.  Row tensors 16-byte aligned, frame sizes multiples of
+ * 16 bytes, n, m, n_fresh <= 65535.  dtype is the call's. */
 typedef struct fvs_qwen_gather_job {
   const int64_t* picks;
   int n;
@@ -573,7 +574,7 @@ typedef struct fvs_qwen_gather_job {
   const void* dev_x;
   const void* dev_merged;
   int64_t n_dev;
-  const void* const* host_chunks;  /* DEVICE table, as for fvs_qwen_dam_gather */
+  const void* const* host_chunks;  /* DEVICE table */
   int chunk_frames;
   const int64_t* prev_picks;
   int m;
@@ -583,32 +584,48 @@ typedef struct fvs_qwen_gather_job {
   void* spa_x_out;
   void* merged_out;
   uint64_t* host_fetches;
+  const int64_t* fresh_frames;
+  int n_fresh;
+  const void* fresh_x;
+  const void* fresh_merged;
+  int64_t n_base;
 } fvs_qwen_gather_job;
 int fvs_qwen_dam_gather_multi(const fvs_qwen_gather_job* jobs_h, int n_jobs, int dtype, fvs_stream_t stream);
 
 /* Lazy full-resolution bank (DESIGN.md §3.18): a stream keeps each frame's full-resolution pixel rows in pinned host
- * chunks and encodes a frame the first time the DAM picks it.  Each call is a job table (one stream = the one-job
- * table); every job is checked before anything is enqueued (FVS_EINVAL otherwise), at most
- * FVS_QWEN_MEM_JOBS_PER_LAUNCH jobs per launch, and no two jobs may share an output.
+ * chunks and encodes a frame the first time the DAM picks it.  Without a full-resolution bank (§3.19) it stores no x or
+ * merged row of the frames it encodes and re-encodes a pick the previous DAM does not hold; a stream restored from a
+ * checkpoint may then still hold a frozen base bank of stored rows (frames [0, n_base) of fvs_qwen_dam_gather_multi).
  *
  * fvs_qwen_pick_plan_multi: per job, walks picks (device int64 [n]; NULL = frames 0..n-1, the DAM while it is the whole
- * bank) in order and writes to plan (device int64 [n]) every pick that is in [0, n_frames), whose byte in `encoded`
- * (device uint8 [n_frames]) is 0 and that no earlier pick names: the stream's first-time frames, unique, in pick order.
- * Their mask bytes are set to 1 and their number is stored to *count (int32; device memory or the mapped address of
- * pinned host memory, e.g. a slot of the stream's read-back row). */
+ * bank) in order and writes to plan (device int64 [n]) every pick p that is in [0, n_frames), that no earlier pick
+ * names, that is not in prev_picks (device int64 [m], the previous step's DAM; NULL when m = 0) and whose byte in
+ * `frames` (device uint8 [n_frames]) is below `stored`: a byte >= stored means the frame's rows are held.  A stream with
+ * a bank passes stored = 1 and m = 0 (byte 0: not yet encoded); a stream without one passes stored = 2 (2: the frame's
+ * rows are in the base bank) and its previous DAM, so it keeps no mask that a redone clip would have to roll back.  A
+ * planned frame whose byte is 1 (encoded before) adds 1 to *re_encodes (device uint64, optional); every planned frame's
+ * byte is then set to 1.  The plan's length goes to *count (int32; device memory or the mapped address of pinned host
+ * memory, e.g. a slot of the stream's read-back row). */
 typedef struct fvs_qwen_pick_plan_job {
   const int64_t* picks;
   int n;
   int64_t n_frames;
-  uint8_t* encoded;
+  uint8_t* frames;
   int64_t* plan;
   int32_t* count;
+  const int64_t* prev_picks;
+  int m;
+  uint64_t* re_encodes;
+  uint8_t stored;
 } fvs_qwen_pick_plan_job;
 int fvs_qwen_pick_plan_multi(const fvs_qwen_pick_plan_job* jobs, int n_jobs, fvs_stream_t stream);
-/* fvs_qwen_pixel_gather_multi: per job, out[i] = pixel rows of frame plan[i] (i < n): frame f >= base is frame f - base
- * of the pinned pixel chunks, chunk c holding chunk_frames frames of frame_elems 16-bit elements each; host_chunks is a
- * DEVICE table of the chunks' mapped device pointers.  The chunks are read in place, as fvs_qwen_dam_gather reads its
- * host tier (the same kernel, with no device tier); a frame outside [base, n_frames) yields zeros. */
+/* fvs_qwen_pixel_gather_multi: per job, out[i] = the pixel rows of frame plan[i] (i < n), out [n, frame_elems] of
+ * `dtype`: frame f >= base is frame f - base of the pinned pixel chunks, chunk c holding chunk_frames frames, read in
+ * place through host_chunks (a DEVICE table of the chunks' mapped device pointers); a frame outside [base, n_frames)
+ * yields zeros.  table NULL: the chunks hold frame_elems 16-bit elements per frame, gathered as fvs_qwen_dam_gather_multi
+ * reads its host tier.  table non-null: the chunks hold frame_elems uint8 codes per frame (whole rows: frame_elems % 1176
+ * == 0), decoded through `table` (device float32 [3, 256]) in the same pass as fvs_qwen_pixel_decode decodes them.
+ * One call takes jobs of one kind: a table in every job or in none. */
 typedef struct fvs_qwen_pixel_job {
   const int64_t* plan;
   int n;
@@ -618,11 +635,12 @@ typedef struct fvs_qwen_pixel_job {
   int chunk_frames;
   int64_t frame_elems;
   void* out;
+  const float* table;
 } fvs_qwen_pixel_job;
 int fvs_qwen_pixel_gather_multi(const fvs_qwen_pixel_job* jobs, int n_jobs, int dtype, fvs_stream_t stream);
-/* fvs_qwen_bank_scatter_multi: per job, the reverse of fvs_qwen_dam_gather: x[plan[i]] = x_rows[i] and, when merged_rows
- * is given, merged[plan[i]] = merged_rows[i], into the two-tier bank (device tier frames [0, n_dev), host chunks laid
- * out as fvs_qwen_dam_gather reads them).  A plan entry outside [0, n_frames) writes nothing. */
+/* fvs_qwen_bank_scatter_multi: per job, the reverse of fvs_qwen_dam_gather_multi's bank tiers: x[plan[i]] = x_rows[i]
+ * and, when merged_rows is given, merged[plan[i]] = merged_rows[i], into the two-tier bank (device tier frames [0, n_dev),
+ * host chunks laid out as above).  A plan entry outside [0, n_frames) writes nothing. */
 typedef struct fvs_qwen_scatter_job {
   const int64_t* plan;
   int n;
@@ -639,63 +657,6 @@ typedef struct fvs_qwen_scatter_job {
 } fvs_qwen_scatter_job;
 int fvs_qwen_bank_scatter_multi(const fvs_qwen_scatter_job* jobs, int n_jobs, int dtype, fvs_stream_t stream);
 
-/* No full-resolution bank (DESIGN.md §3.19): a lazy stream that stores no x or merged row for the frames it encodes.
- * It keeps every frame's pixel rows and the previous step's DAM rows, and re-encodes a pick the previous DAM does not
- * hold.  A stream restored from a checkpoint may also hold a frozen base bank of stored rows (frames [0, n_base), laid
- * out as fvs_qwen_dam_gather reads its two tiers).  Job tables as above.
- *
- * fvs_qwen_pick_plan_prev_multi: the plan compares the picks against prev_picks itself, so the stream keeps no mask that
- * a redone clip would have to roll back.  Per job, walks picks (device int64 [n]) in order and writes to plan (device
- * int64 [n]) every pick p that is in [0, n_frames), that no earlier pick names, that is not in prev_picks (device int64
- * [m], the previous step's DAM; NULL when m = 0) and whose byte in `frames` (device uint8 [n_frames]) is not 2 (2: the
- * frame's rows are in the stored base bank).  A planned frame whose byte is 1 (encoded before) adds 1 to *re_encodes
- * (device uint64, optional); every planned frame's byte is then set to 1.  The plan's length goes to *count (int32;
- * device memory or the mapped address of pinned host memory), as fvs_qwen_pick_plan_multi stores it. */
-typedef struct fvs_qwen_pick_plan_prev_job {
-  const int64_t* picks;
-  int n;
-  int64_t n_frames;
-  uint8_t* frames;
-  const int64_t* prev_picks;
-  int m;
-  int64_t* plan;
-  int32_t* count;
-  uint64_t* re_encodes;
-} fvs_qwen_pick_plan_prev_job;
-int fvs_qwen_pick_plan_prev_multi(const fvs_qwen_pick_plan_prev_job* jobs, int n_jobs, fvs_stream_t stream);
-/* fvs_qwen_dam_gather_fresh_multi: the DAM gather of a stream without a full-resolution bank.  Per job, for every pick i,
- * spa_x_out[i] = x[picks[i]] and merged_out[i] = merged[picks[i]] (either output may be NULL; not both), each read from
- * the first source that has the frame: the previous DAM (prev_picks [m], prev_x, prev_merged); this step's fresh rows
- * (fresh_frames [n_fresh], fresh_x [n_fresh, x_frame_elems], fresh_merged [n_fresh, merged_frame_elems]: the tower and
- * PatchMerger output of the planned frames, in plan order); the stored base bank, frames [0, n_base): device tier
- * [0, n_dev) and host chunks as for fvs_qwen_dam_gather.  *host_fetches (optional) grows by the picks read from the host
- * chunks.  A pick outside [0, n_frames), or in no source, yields zero rows.  n_fresh is a host integer (the count of the
- * plan, read back).  The outputs must not alias any source; no output may be shared by two jobs. */
-typedef struct fvs_qwen_fresh_gather_job {
-  const int64_t* picks;
-  int n;
-  int64_t n_frames;
-  const int64_t* prev_picks;
-  int m;
-  const void* prev_x;
-  const void* prev_merged;
-  const int64_t* fresh_frames;
-  int n_fresh;
-  const void* fresh_x;
-  const void* fresh_merged;
-  int64_t n_base;
-  const void* dev_x;
-  const void* dev_merged;
-  int64_t n_dev;
-  const void* const* host_chunks;  /* DEVICE table */
-  int chunk_frames;
-  int64_t x_frame_elems, merged_frame_elems;
-  void* spa_x_out;
-  void* merged_out;
-  uint64_t* host_fetches;
-} fvs_qwen_fresh_gather_job;
-int fvs_qwen_dam_gather_fresh_multi(const fvs_qwen_fresh_gather_job* jobs, int n_jobs, int dtype, fvs_stream_t stream);
-
 /* 8-bit pixel codes (DESIGN.md §3.20): a stream fed uint8 frames keeps each full-resolution pixel row as the bytes u of
  * FVS_PRE_QWEN_CODES, which the tower's input row dtype(table[c][u]) is a function of (c = column / 392, table the
  * pre-processor's float32 [3, 256]).  Decode rounds to nearest even, as torch's fp32 -> bf16 / f16 cast does, so a
@@ -705,23 +666,6 @@ int fvs_qwen_dam_gather_fresh_multi(const fvs_qwen_fresh_gather_job* jobs, int n
  * table device float32 [3, 256], out f16 / bf16 [rows, 1176] (16-byte aligned).  One launch, no synchronisation. */
 int fvs_qwen_pixel_decode(const uint8_t* codes, int64_t rows, const float* table, int dtype, void* out,
                           fvs_stream_t stream);
-/* fvs_qwen_pixel_gather_codes_multi: fvs_qwen_pixel_gather_multi over code chunks: per job, out[i] = the decoded rows of
- * frame plan[i] (i < n), frame f >= base being frame f - base of the pinned chunks, chunk c holding chunk_frames frames
- * of frame_elems bytes each (whole rows: frame_elems % 1176 == 0), read in place through host_chunks (a DEVICE table of
- * mapped pointers) and decoded through `table` in the same pass; out [n, frame_elems] of `dtype`.  A frame outside
- * [base, n_frames) yields zeros.  Job tables as above (FVS_EINVAL naming the job, nothing launched). */
-typedef struct fvs_qwen_pixel_codes_job {
-  const int64_t* plan;
-  int n;
-  int64_t n_frames;
-  int64_t base;
-  const void* const* host_chunks;
-  int chunk_frames;
-  int64_t frame_elems;
-  const float* table;
-  void* out;
-} fvs_qwen_pixel_codes_job;
-int fvs_qwen_pixel_gather_codes_multi(const fvs_qwen_pixel_codes_job* jobs, int n_jobs, int dtype, fvs_stream_t stream);
 /* *dev_out = the device address of pinned host memory `host` (cudaHostGetDevicePointer); FVS_EINVAL if it is not pinned */
 int fvs_host_device_ptr(const void* host, void** dev_out);
 

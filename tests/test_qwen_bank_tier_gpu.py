@@ -1,7 +1,7 @@
-"""GPU tests of the two-tier feature bank of the Qwen2-VL streaming state (DESIGN.md §3.13): fvs_qwen_dam_gather against
-a torch gather, streams capped at every kind of frame count equal to the uncapped stream bit for bit, the reference
-goldens with every frame spilled, the real tower, checkpoints across caps, the HBM bound, reuse of the previous DAM,
-and the publication."""
+"""GPU tests of the two-tier feature bank of the Qwen2-VL streaming state (DESIGN.md §3.13): fvs_qwen_dam_gather_multi
+against a torch gather, streams capped at every kind of frame count equal to the uncapped stream bit for bit, the
+reference goldens with every frame spilled, the real tower, checkpoints across caps, the HBM bound, reuse of the
+previous DAM, and the publication."""
 import os
 import random
 import threading
@@ -58,7 +58,7 @@ def _host_tier(x, m, n_dev, F):
 
 @pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16])
 @pytest.mark.parametrize("grid, D, Dm", [((4, 4), 256, 512), ((24, 24), 1280, 3584)])
-def test_dam_gather_matches_torch(rt, dtype, grid, D, Dm):
+def test_dam_gather_table_matches_torch(rt, dtype, grid, D, Dm):
     from flash_vstream_b200.qwen import ops as Q
     g = torch.Generator().manual_seed(5)
     n, F = 11, 4
@@ -83,15 +83,16 @@ def test_dam_gather_matches_torch(rt, dtype, grid, D, Dm):
                 cnt = torch.zeros(1, dtype=torch.int64, device="cuda")
                 ox = torch.full((len(picks), hw, D), 7, dtype=dtype, device="cuda")
                 om = torch.full((len(picks), pm, Dm), 7, dtype=dtype, device="cuda")
-                Q.dam_gather(p, n, xd[:n_dev] if n_dev else None, md[:n_dev] if n_dev else None, n_dev,
-                             table if n_dev < n else None, F, hw * D, pm * Dm, prev=prev, spa_x_out=ox, merged_out=om,
-                             host_fetches=cnt)
+                bank = dict(picks=p, n_frames=n, dev_x=xd[:n_dev] if n_dev else None, n_dev=n_dev,
+                            chunks=table if n_dev < n else None, chunk_frames=F, x_frame_elems=hw * D,
+                            merged_frame_elems=pm * Dm)
+                Q.dam_gather_multi([dict(bank, dev_merged=md[:n_dev] if n_dev else None, prev=prev, spa_x_out=ox,
+                                         merged_out=om, host_fetches=cnt)])
                 assert same(ox, xd[p]) and same(om, md[p]), (n_dev, name, use_prev)
                 want = sum(1 for v in picks if v >= n_dev and not (use_prev and v in prev_picks))
                 assert int(cnt.item()) == want, (n_dev, name, use_prev)
                 ox2 = torch.empty_like(ox)              # one output alone (the restore rebuilds spa_x only)
-                Q.dam_gather(p, n, xd[:n_dev] if n_dev else None, None, n_dev, table if n_dev < n else None, F,
-                             hw * D, pm * Dm, spa_x_out=ox2)
+                Q.dam_gather_multi([dict(bank, dev_merged=None, spa_x_out=ox2)])
                 assert same(ox2, xd[p])
     torch.cuda.synchronize()
 

@@ -1,5 +1,6 @@
-"""Two-tier feature bank of the Qwen2-VL streaming state, host side: the exported gather, its refusals (returned before
-any CUDA call, nothing launched), where every frame lands, and the fvs_bank_device_frames knob."""
+"""Two-tier feature bank of the Qwen2-VL streaming state, host side: the exported gather (a one-job table), its
+refusals (returned before any CUDA call, nothing launched), where every frame lands, and the fvs_bank_device_frames
+knob."""
 import ctypes as C
 
 import pytest
@@ -12,18 +13,18 @@ from flash_vstream_b200.qwen import vstream_qwen2vl_realtime as rt
 A = 0x10000          # a 16-byte aligned stand-in address: the refusals happen before anything is dereferenced
 
 
-def test_symbols_exported():
+def test_gather_symbols_exported():
     lib = L.load()
-    for name in ("fvs_qwen_dam_gather", "fvs_host_device_ptr"):
+    for name in ("fvs_qwen_dam_gather_multi", "fvs_host_device_ptr"):
         assert hasattr(lib, name) and name in L.SIGNATURES
 
 
-def _gather(**kw):
+def _gather(dtype=L.BF16, **kw):
     a = dict(picks=A, n=4, n_frames=10, dev_x=A, dev_merged=A, n_dev=4, host_chunks=A, chunk_frames=3, prev_picks=A, m=2,
-             prev_x=A, prev_merged=A, x_frame_elems=64, merged_frame_elems=32, dtype=L.BF16, spa_x_out=A, merged_out=A,
-             host_fetches=A, stream=None)
+             prev_x=A, prev_merged=A, x_frame_elems=64, merged_frame_elems=32, spa_x_out=A, merged_out=A, host_fetches=A,
+             n_base=10)
     a.update(kw)
-    return L.load().fvs_qwen_dam_gather(*a.values())
+    return L.load().fvs_qwen_dam_gather_multi((L.QwenGatherJob * 1)(L.QwenGatherJob(**a)), 1, dtype, None)
 
 
 @pytest.mark.parametrize("kw, msg", [
@@ -48,7 +49,7 @@ def _gather(**kw):
     (dict(spa_x_out=A + 8), "aligned"),
     (dict(picks=A + 4), "8-byte"),
 ])
-def test_gather_refusals_launch_nothing(kw, msg):
+def test_gather_table_refusals_launch_nothing(kw, msg):
     lib = L.load()
     before = lib.fvs_launch_count()
     assert _gather(**kw) == L.FVS_EINVAL

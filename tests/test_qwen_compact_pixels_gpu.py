@@ -1,5 +1,5 @@
 """GPU tests of 8-bit pixel codes (DESIGN.md §3.20): FVS_PRE_QWEN_CODES then fvs_qwen_pixel_decode against the fp32
-pre-processing cast to the tower dtype, fvs_qwen_pixel_gather_codes_multi against a torch decode of the same frames,
+pre-processing cast to the tower dtype, fvs_qwen_pixel_gather_multi of codes against a torch decode of the same frames,
 and compact_pixels pools (lazy and bank-less) against their non-compact twins fed the same frames and draws: every
 13-item list, spa_x, video_embeds and the positions after every round, the pinned bytes, every legal checkpoint
 direction, and pool_memory_manager."""
@@ -58,7 +58,7 @@ def test_codes_then_decode_equals_the_cast_rows(rt, dtype):
 
 
 @pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16])
-def test_codes_gather_equals_torch_decode(rt, dtype):
+def test_pixel_gather_of_codes_equals_torch_decode(rt, dtype):
     from flash_vstream_b200.qwen import ops as Q
     from flash_vstream_b200.qwen.stream_state import PixelStore
     table = proc().device_table()
@@ -79,12 +79,12 @@ def test_codes_gather_equals_torch_decode(rt, dtype):
             if base <= f < n:
                 w[i] = decode_ref(codes[f - base].cuda()[None], table, dtype)[0].cpu()
         want.append((w, st))
-    Q.pixel_gather_codes_multi(jobs)
+    Q.pixel_gather_multi(jobs)
     for (w, _), job in zip(want, jobs):
         assert torch.equal(job[6].cpu().view(torch.int16), w.view(torch.int16))
     for (w, _), job in zip(want, jobs):                              # each job alone: the one-job table
         job[6].zero_()
-        Q.pixel_gather_codes_multi([job])
+        Q.pixel_gather_multi([job])
         assert torch.equal(job[6].cpu().view(torch.int16), w.view(torch.int16))
 
 

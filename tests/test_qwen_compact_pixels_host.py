@@ -205,9 +205,9 @@ def test_restore_refusals():
 
 
 # ---------------------------------------------------------------------------------------------------------- entry points
-def test_symbols_exported():
+def test_code_symbols_exported():
     lib = L.load()
-    for name in ("fvs_qwen_pixel_decode", "fvs_qwen_pixel_gather_codes_multi"):
+    for name in ("fvs_qwen_pixel_decode", "fvs_qwen_pixel_gather_multi"):
         assert hasattr(lib, name) and name in L.SIGNATURES
 
 
@@ -231,7 +231,7 @@ def test_decode_refusals_launch_nothing(args, msg):
 def _codes_job(**kw):
     a = dict(plan=A, n=3, n_frames=10, base=2, host_chunks=A, chunk_frames=4, frame_elems=4 * 1176, table=A, out=A)
     a.update(kw)
-    return L.QwenPixelCodesJob(**a)
+    return L.QwenPixelJob(**a)
 
 
 @pytest.mark.parametrize("kw, msg", [
@@ -247,16 +247,24 @@ def _codes_job(**kw):
     (dict(out=A + 8), "misaligned"),
     (dict(plan=A + 4), "misaligned"),
 ])
-def test_codes_gather_refusals_launch_nothing(kw, msg):
-    arr = (L.QwenPixelCodesJob * 3)(_codes_job(out=A << 8), _codes_job(**kw), _codes_job(out=A << 9))
-    _refused("fvs_qwen_pixel_gather_codes_multi", arr, 3, L.BF16, None, msg=msg)
-    assert "fvs_qwen_pixel_gather_codes_multi: job 1: " in L.load().fvs_last_error().decode()
+def test_pixel_gather_of_codes_refusals_launch_nothing(kw, msg):
+    arr = (L.QwenPixelJob * 3)(_codes_job(out=A << 8), _codes_job(**kw), _codes_job(out=A << 9))
+    _refused("fvs_qwen_pixel_gather_multi", arr, 3, L.BF16, None, msg=msg)
+    assert "fvs_qwen_pixel_gather_multi: job 1: " in L.load().fvs_last_error().decode()
 
 
-def test_codes_gather_refuses_dtype_and_shared_outputs():
-    arr = (L.QwenPixelCodesJob * 2)(_codes_job(), _codes_job(out=A + 2 * 1176))
-    _refused("fvs_qwen_pixel_gather_codes_multi", arr, 2, L.F32, None, msg="dtype must be f16 or bf16")
-    _refused("fvs_qwen_pixel_gather_codes_multi", arr, 2, L.BF16, None, msg="jobs 0 and 1 share an output")
+def test_pixel_gather_of_codes_refuses_dtype_and_shared_outputs():
+    arr = (L.QwenPixelJob * 2)(_codes_job(), _codes_job(out=A + 2 * 1176))
+    _refused("fvs_qwen_pixel_gather_multi", arr, 2, L.F32, None, msg="dtype must be f16 or bf16")
+    _refused("fvs_qwen_pixel_gather_multi", arr, 2, L.BF16, None, msg="jobs 0 and 1 share an output")
+
+
+def test_pixel_gather_refuses_a_mix_of_codes_and_rows():
+    """one call gathers tower-dtype rows (no table) or codes (a table in every job), never both"""
+    for first, second in ((dict(table=None, frame_elems=4 * 1176), dict()), (dict(), dict(table=None))):
+        arr = (L.QwenPixelJob * 2)(_codes_job(out=A << 8, **first), _codes_job(out=A << 9, **second))
+        _refused("fvs_qwen_pixel_gather_multi", arr, 2, L.BF16, None, msg="job 1: need a plan, a table, an output")
+        assert "code and row jobs do not mix" in L.load().fvs_last_error().decode()
 
 
 # ---------------------------------------------------------------------------------------------------------- SASS
@@ -290,7 +298,7 @@ def test_kernel_resources():
     assert find(r"resample_cols_kernelILi0E") == (40, 0, 0)                 # FVS_PRE_CLIP
     assert find(r"resample_cols_kernelILi1E") == (32, 0, 0)                 # FVS_PRE_QWEN
     assert find(r"resample_rows_kernel") == (30, 0, 0)
-    assert find(r"dam_gather_multi_kernelILi1E") == (38, 0, 0)              # also fvs_qwen_pixel_gather_multi's
+    assert find(r"dam_gather_multi_kernelILi1E") == (38, 0, 0)              # also the pixel gather's of tower-dtype rows
     assert find(r"dam_gather_multi_kernelILi16E") == (32, 0, 0)
     # the new kernels use no stack or local memory
     new = [r for k, r in res.items() if re.search(r"resample_cols_kernelILi2E|pixel_decode_kernel|pixel_codes_gather_kernel", k)]

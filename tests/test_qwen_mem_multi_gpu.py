@@ -203,7 +203,7 @@ def test_klarge_retrieve_multi_equals_single_calls(lib, metric, dtype):
         assert torch.equal(got[i][0], ri) and equal(got[i][1], rd), (metric, dtype, i)
 
 
-def test_dam_gather_multi_equals_single_calls(lib):
+def test_dam_gather_multi_equals_one_job_tables(lib):
     """per job: its own device tier, host chunks (some picks read there), previous DAM and host_fetches counter"""
     from flash_vstream_b200.qwen import ops as Q
     calls, refs = [], []
@@ -235,7 +235,7 @@ def test_dam_gather_multi_equals_single_calls(lib):
     strip = lambda a: {k: v for k, v in a.items() if k != "_keep"}
     Q.dam_gather_multi([strip(a) for a in calls])
     for a in refs:
-        Q.dam_gather(**strip(a))
+        Q.dam_gather_multi([strip(a)])
     torch.cuda.synchronize()
     fetched = 0
     for a, b in zip(calls, refs):

@@ -182,11 +182,11 @@ def test_retrieve_multi_refuses_host_tier_and_shared_outputs(lib):
     assert lib.fvs_launch_count() == n0
 
 
-def test_gather_multi_refuses_shared_counters(lib):
+def test_gather_table_refuses_shared_counters(lib):
     def gjob(base, **kw):
         a = FAKE + base * (1 << 50)
-        j = L.QwenGatherJob(picks=a, n=30, n_frames=100, dev_x=a + (1 << 44), dev_merged=a + 2 * (1 << 44), n_dev=100,
-                            x_frame_elems=576 * 1280, merged_frame_elems=144 * 512, spa_x_out=a + 3 * (1 << 44),
+        j = L.QwenGatherJob(picks=a, n=30, n_frames=100, n_base=100, dev_x=a + (1 << 44), dev_merged=a + 2 * (1 << 44),
+                            n_dev=100, x_frame_elems=576 * 1280, merged_frame_elems=144 * 512, spa_x_out=a + 3 * (1 << 44),
                             merged_out=a + 4 * (1 << 44), host_fetches=a + 5 * (1 << 44))
         for k, v in kw.items():
             setattr(j, k, v)

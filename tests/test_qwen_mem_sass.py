@@ -6,6 +6,7 @@ needed)."""
 import os
 import re
 import subprocess
+from pathlib import Path
 
 import pytest
 
@@ -59,3 +60,12 @@ def test_single_calls_are_one_job_tables():
     assert one[("mem_multi_kernel", (1, KUPDATE))][0] <= 80
     assert one[("klarge_multi_kernel", (1, 0, KL_SWEEP_EUCLIDEAN))][0] <= 100
     assert one[("klarge_multi_kernel", (1, 0, KL_SWEEP_COSINE))][0] <= 98
+
+
+def test_bank_kernels_are_one_per_operation():
+    """qwen_bank.cu has one kernel per operation: the DAM gather (every stream kind, and the pixel gather of tower-dtype
+    rows), the pick plan (with or without a bank), the bank scatter, the code decode and the code gather"""
+    src = (Path(__file__).resolve().parents[1] / "flash_vstream_b200" / "csrc" / "qwen_bank.cu").read_text()
+    kernels = re.findall(r"__global__\s+void\s+(?:__launch_bounds__\([^)]*\)\s+)?(\w+)", src)
+    assert sorted(kernels) == ["bank_scatter_kernel", "dam_gather_multi_kernel", "pick_plan_kernel",
+                               "pixel_codes_gather_kernel", "pixel_decode_kernel"], kernels

@@ -64,7 +64,7 @@ def holds_no_bank(st):
 
 
 # ---------------------------------------------------------------------------------------------------------- kernels
-def test_plan_prev_kernel_matches_numpy_and_single_calls(rt):
+def test_bankless_plan_matches_numpy_and_single_calls(rt):
     from flash_vstream_b200.qwen import ops as Q
     r = np.random.default_rng(4)
     cases, jobs = [], []
@@ -90,13 +90,13 @@ def test_plan_prev_kernel_matches_numpy_and_single_calls(rt):
                      count=torch.zeros(1, dtype=torch.int32, device="cuda"),
                      again=torch.zeros(1, dtype=torch.int64, device="cuda"))
             got.append(t)
-        js = [(t["picks"], t["frames"], len(fr), t["prev"], t["plan"], t["count"].data_ptr(), t["again"])
-              for t, (_, _, fr) in zip(got, cases)]
+        js = [(t["picks"], len(p), t["frames"], len(fr), t["plan"], t["count"].data_ptr(), 2, t["prev"], t["again"])
+              for t, (p, _, fr) in zip(got, cases)]               # no bank: byte 2 is stored
         if single:
             for jb in js:
-                Q.pick_plan_prev_multi([jb])
+                Q.pick_plan_multi([jb])
         else:
-            Q.pick_plan_prev_multi(js)
+            Q.pick_plan_multi(js)
         outs.append(got)
     for k, (picks, prev, fr) in enumerate(cases):
         want_fr = fr.copy()
@@ -110,7 +110,7 @@ def test_plan_prev_kernel_matches_numpy_and_single_calls(rt):
             assert len(want) == 0
 
 
-def test_fresh_gather_kernel_matches_torch_and_single_calls(rt):
+def test_bankless_dam_gather_matches_torch_and_single_calls(rt):
     from flash_vstream_b200.qwen import ops as Q
     g = torch.Generator().manual_seed(9)
     fx, fm, F = 16 * 32, 4 * 64, 5                               # 16 rows of 32 wide, 4 merged rows of 64; 5 per chunk
@@ -162,9 +162,9 @@ def test_fresh_gather_kernel_matches_torch_and_single_calls(rt):
                      host_fetches=torch.zeros(1, dtype=torch.int64, device="cuda")) for a, _, _ in jobs]
 
     multi, single = outs(), outs()
-    Q.dam_gather_fresh_multi(multi)
+    Q.dam_gather_multi(multi)
     for a in single:
-        Q.dam_gather_fresh_multi([a])
+        Q.dam_gather_multi([a])
     for (_, _, (wx, wm, fetches)), a, b in zip(jobs, multi, single):
         for o in (a, b):
             assert same(o["spa_x_out"], wx) and same(o["merged_out"], wm)

@@ -1,7 +1,7 @@
 """CPU tests of a Qwen2-VL stream without a full-resolution bank (DESIGN.md §3.19): the pick plan against the previous
-DAM restated in NumPy (what the GPU tests hold fvs_qwen_pick_plan_prev_multi and a bank-less stream's encode counts
-to), the count the host knows while the DAM is the whole bank, the knob's refusals, the checkpoint's tensor set, and
-the new entry points' refusals (returned before any CUDA call, nothing launched)."""
+DAM restated in NumPy (what the GPU tests hold fvs_qwen_pick_plan_multi and a bank-less stream's encode counts to),
+the count the host knows while the DAM is the whole bank, the knob's refusals, the checkpoint's tensor set, and the
+refusals of the plan and gather jobs a bank-less stream sends (returned before any CUDA call, nothing launched)."""
 import numpy as np
 import pytest
 import torch
@@ -149,9 +149,9 @@ def test_checkpoint_tensor_set_and_refusals():
         QwenStreamState.restore(bad, flash, None, "cpu", lazy_full_res=True)
 
 
-def test_symbols_exported():
+def test_bankless_symbols_exported():
     lib = L.load()
-    for name in ("fvs_qwen_pick_plan_prev_multi", "fvs_qwen_dam_gather_fresh_multi"):
+    for name in ("fvs_qwen_pick_plan_multi", "fvs_qwen_dam_gather_multi"):
         assert hasattr(lib, name) and name in L.SIGNATURES
 
 
@@ -166,23 +166,23 @@ def _refused(fn, arr, *args, msg):
 @pytest.mark.parametrize("kw, msg", [
     (dict(n=-1), "bad sizes"),
     (dict(m=70000), "bad sizes"),
-    (dict(picks=None), "null picks"),
+    (dict(picks=None, n=11), "null picks"),              # null picks stand for frames 0..n-1
     (dict(prev_picks=None), "null picks or previous"),
     (dict(frames=None), "null frame bytes"),
     (dict(count=None), "null frame bytes"),
     (dict(plan=A + 4), "misaligned"),
     (dict(re_encodes=A + 4), "misaligned"),
 ])
-def test_plan_prev_refusals_launch_nothing(kw, msg):
-    a = dict(picks=A, n=4, n_frames=10, frames=A, prev_picks=A, m=2, plan=A, count=A, re_encodes=A)
+def test_bankless_plan_refusals_launch_nothing(kw, msg):
+    a = dict(picks=A, n=4, n_frames=10, frames=A, prev_picks=A, m=2, plan=A, count=A, re_encodes=A, stored=2)
     a.update(kw)
-    _refused("fvs_qwen_pick_plan_prev_multi", (L.QwenPickPlanPrevJob * 1)(L.QwenPickPlanPrevJob(**a)), 1, None, msg=msg)
+    _refused("fvs_qwen_pick_plan_multi", (L.QwenPickPlanJob * 1)(L.QwenPickPlanJob(**a)), 1, None, msg=msg)
 
 
-def test_plan_prev_refuses_shared_outputs():
-    a = dict(picks=A, n=4, n_frames=10, frames=A, prev_picks=A, m=2, plan=A, count=A, re_encodes=A)
-    jobs = (L.QwenPickPlanPrevJob * 2)(L.QwenPickPlanPrevJob(**a), L.QwenPickPlanPrevJob(**dict(a, frames=2 * A)))
-    _refused("fvs_qwen_pick_plan_prev_multi", jobs, 2, None, msg="share an output")
+def test_bankless_plan_refuses_shared_outputs():
+    a = dict(picks=A, n=4, n_frames=10, frames=A, prev_picks=A, m=2, plan=A, count=A, re_encodes=A, stored=2)
+    jobs = (L.QwenPickPlanJob * 2)(L.QwenPickPlanJob(**a), L.QwenPickPlanJob(**dict(a, frames=2 * A)))
+    _refused("fvs_qwen_pick_plan_multi", jobs, 2, None, msg="share an output")
 
 
 def _fresh(**kw):
@@ -190,7 +190,7 @@ def _fresh(**kw):
              fresh_merged=A, n_base=5, dev_x=A, dev_merged=A, n_dev=3, host_chunks=A, chunk_frames=2, x_frame_elems=64,
              merged_frame_elems=32, spa_x_out=A, merged_out=A, host_fetches=A)
     a.update(kw)
-    return L.QwenFreshGatherJob(**a)
+    return L.QwenGatherJob(**a)
 
 
 @pytest.mark.parametrize("kw, msg", [
@@ -210,11 +210,11 @@ def _fresh(**kw):
     (dict(fresh_x=A + 8), "aligned"),
     (dict(fresh_frames=A + 4), "8-byte"),
 ])
-def test_fresh_gather_refusals_launch_nothing(kw, msg):
-    _refused("fvs_qwen_dam_gather_fresh_multi", (L.QwenFreshGatherJob * 1)(_fresh(**kw)), 1, L.BF16, None, msg=msg)
+def test_bankless_gather_refusals_launch_nothing(kw, msg):
+    _refused("fvs_qwen_dam_gather_multi", (L.QwenGatherJob * 1)(_fresh(**kw)), 1, L.BF16, None, msg=msg)
 
 
-def test_fresh_gather_refuses_dtype_and_shared_outputs():
-    _refused("fvs_qwen_dam_gather_fresh_multi", (L.QwenFreshGatherJob * 1)(_fresh()), 1, L.F32, None, msg="dtype")
-    jobs = (L.QwenFreshGatherJob * 2)(_fresh(), _fresh(merged_out=1 << 30, host_fetches=1 << 29))
-    _refused("fvs_qwen_dam_gather_fresh_multi", jobs, 2, L.BF16, None, msg="share an output")
+def test_bankless_gather_refuses_dtype_and_shared_outputs():
+    _refused("fvs_qwen_dam_gather_multi", (L.QwenGatherJob * 1)(_fresh()), 1, L.F32, None, msg="dtype")
+    jobs = (L.QwenGatherJob * 2)(_fresh(), _fresh(merged_out=1 << 30, host_fetches=1 << 29))
+    _refused("fvs_qwen_dam_gather_multi", jobs, 2, L.BF16, None, msg="share an output")
