@@ -381,7 +381,7 @@ class StreamBank:
         self.bank = L.Bank(self.prefix_buf.data_ptr(), self.long_work.data_ptr(), self.tur_work.data_ptr(),
                            self.frames.data_ptr(), self.header.data_ptr(), self.frames.shape[0], self.chunk_cap, 0, 0, 0, 0, 0,
                            self.device_frames or 0)
-        self.host_chunks: list = []      # pinned [per_chunk, a*a, D] chunks of frames >= device_frames
+        self.tier = HT.HostChunks()      # frames >= device_frames, laid out when the first one spills
 
     # ---- state as the reference sees it (views of the bank) ---------------------------------------------------------
     @property
@@ -408,6 +408,11 @@ class StreamBank:
         cur = self.prefix_buf[o2:o2 + b.n_cur * self.pa].view(b.n_cur, self.pa, self.D)
         return cur, lng, tur, self.frames[:0] if self.n_host() else self.frames[:b.n_frames]
 
+    @property
+    def host_chunks(self) -> list:
+        """the pinned chunks of the host tier (frames >= device_frames)"""
+        return self.tier.chunks
+
     def n_host(self) -> int:
         """frames of the stream kept in the host chunks (those at or past device_frames)"""
         return 0 if self.device_frames is None else max(0, self.bank.n_frames - self.device_frames)
@@ -416,46 +421,33 @@ class StreamBank:
         """the whole frame buffer [n_frames, a*a, D] (img_feature_buffer): the device view frames[:n_frames] while every
         frame is in HBM, else built in pinned host memory — device rows D2H, host chunks H2H (synchronises the current
         stream, so the spills of the last steps have landed)"""
-        n, nh = self.bank.n_frames, self.n_host()
-        if nh == 0:
-            return self.frames[:n]
-        N, F = self.device_frames, self._per_chunk()
-        out = torch.empty(n, self.pa, self.D, dtype=self.frames.dtype, pin_memory=True)
+        if self.n_host() == 0:
+            return self.frames[:self.bank.n_frames]
         with torch.cuda.device(self.device):
-            out[:N].copy_(self.frames[:N], non_blocking=True)
-            torch.cuda.current_stream().synchronize()
-        for c in range((nh + F - 1) // F):
-            cnt = min(F, nh - c * F)
-            out[N + c * F:N + c * F + cnt].copy_(self.host_chunks[c][:cnt])
-        return out
+            return self.tier.to_host(self.frames[:self.device_frames])
 
     def reset(self):
         L.check(self.lib.fvs_bank_reset(C.byref(self.bank), L.cur_stream()), "fvs_bank_reset")
-        self.host_chunks = []
+        self.tier = HT.HostChunks()
 
     # ---- host tier (device_frames) -------------------------------------------------------------------------------------
-    def _per_chunk(self) -> int:
-        return HT.chunk_frames(self.pa * self.D * self.frames.element_size(), self.CHUNK_BYTES)
-
-    def _chunk(self, c: int) -> torch.Tensor:
-        """pinned host chunk c [per_chunk, a*a, D], allocated on first use"""
-        while len(self.host_chunks) <= c:
-            self.host_chunks.append(torch.empty(self._per_chunk(), self.pa, self.D, dtype=self.frames.dtype, pin_memory=True))
-        return self.host_chunks[c]
+    def _host_tier(self) -> HT.HostChunks:
+        """the host tier, laid out by CHUNK_BYTES as it is when the first frame spills"""
+        if self.tier.dtype is None:
+            self.tier.lay_out(self.frames.dtype, [(self.pa, self.D)], self.CHUNK_BYTES)
+        return self.tier
 
     def _spill(self, n0: int, t: int) -> int:
         """after the step of frames [n0, n0 + t): copy those at or past device_frames from the slot to the host chunks,
         asynchronously on the current stream (ahead of the next step, which overwrites the slot).  The clip's frames are
         contiguous in `frames` from row min(n0, device_frames) (frame_row, csrc/stream_kernels.cu).  Returns the bytes."""
-        if self.device_frames is None:
+        N = self.device_frames
+        k = t if N is None else max(0, min(t, N - n0))      # the clip's frames below N, which stay in HBM
+        if k == t:
             return 0
-        row0, nbytes = min(n0, self.device_frames), 0
-        for c, dst, s, cnt in HT.placement(n0, t, self.device_frames, self._per_chunk()):
-            if c >= 0:
-                src = self.frames[row0 + s:row0 + s + cnt]
-                self._chunk(c)[dst:dst + cnt].copy_(src, non_blocking=True)
-                nbytes += src.numel() * src.element_size()
-        return nbytes
+        src = self.frames[min(n0, N) + k:min(n0, N) + t]
+        self._host_tier().write(n0 + k - N, [src])
+        return src.numel() * src.element_size()
 
     def _reserve_frames(self, t: int):
         if self.device_frames is not None:    # fixed at creation: frames [0, N) and one clip's slot
@@ -502,11 +494,10 @@ class StreamBank:
             L.check(self.lib.fvs_bank_restore(C.byref(self.cfg), C.byref(self.bank), n["n_tur"], n["n_long"], n["n_cur"],
                                               n["n_frames"], n["step"], *[t.data_ptr() if t.numel() else None for t in srcs],
                                               L.cur_stream()), "fvs_bank_restore")
-            self.host_chunks = []
-            frames, N = srcs[3], self.device_frames
-            for c, dst, s, cnt in HT.placement(0, n["n_frames"], N, self._per_chunk()):   # frames >= N: to the host tier
-                if c >= 0:
-                    self._chunk(c)[dst:dst + cnt].copy_(frames[s:s + cnt], non_blocking=True)
+            self.tier = HT.HostChunks()
+            N = self.device_frames
+            if N is not None and n["n_frames"] > N:           # frames >= N: to the host tier
+                self._host_tier().write(0, [srcs[3][N:n["n_frames"]]])
             self.ws.zero_()       # the step's arrival counters start at zero (a fresh bank's workspace is uninitialised)
             torch.cuda.current_stream().synchronize()    # the sources may be freed as soon as this returns
         self._last_T = 0

@@ -140,7 +140,7 @@ def encode_picked(states, readbacks: torch.Tensor, max_rows: int = TOWER_ROWS):
                                 inp[off: off + n * st.grid[0] * st.grid[1]], px.frame_elems, px.values))
             Q.pixel_gather_multi(gathers)
             feats = tower(inp, grids)
-            merged = merger(feats) if todo[0][0]._layout[2] is not None else None
+            merged = merger(feats) if len(todo[0][0].bank_tier.shapes) > 1 else None
             scatters = []
             for i, (off,) in places:
                 st, n = todo[i]

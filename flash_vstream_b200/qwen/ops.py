@@ -7,7 +7,7 @@ from typing import NamedTuple, Optional
 import torch
 
 from .. import _lib as L
-from ..host_tier import placement
+from ..host_tier import host_device_ptr, placement  # noqa: F401
 from ..ops import _c, _chk_cuda
 
 _ws_cache: dict = {}
@@ -367,14 +367,6 @@ def klarge_retrieve(tem_x: torch.Tensor, klarge_idx: torch.Tensor, bank, want_di
                                                 L.dtype_code(bank.dtype), code, L.ptr(idx), L.ptr(dist), L.ptr(ws),
                                                 ws.numel(), L.cur_stream()), "fvs_qwen_klarge_retrieve_tiered")
     return (idx, dist) if want_dist else idx
-
-
-def host_device_ptr(t: torch.Tensor) -> int:
-    """the mapped device address of a pinned host tensor (what a kernel dereferences for a zero-copy read)"""
-    assert not t.is_cuda
-    out = C.c_void_p()
-    L.check(L.load().fvs_host_device_ptr(t.data_ptr(), C.byref(out)), "fvs_host_device_ptr")
-    return out.value
 
 
 def am_rope(spa_positions: torch.Tensor, spa_grid, tem_positions: torch.Tensor, tem_grid, visual_start_id: int,

@@ -35,7 +35,7 @@ from . import compress_functions as CF
 from . import ops as Q
 from .. import ops as O
 from ..draws import GLOBAL, to_device
-from ..host_tier import CHUNK_BYTES, check_device_frames, chunk_frames, placement  # noqa: F401
+from ..host_tier import CHUNK_BYTES, HostChunks, check_device_frames, chunk_frames, placement  # noqa: F401
 
 _KMEANS_METHODS = ("kmeans_ordered", "fast_kmeans_ordered")
 PATCH_DIM = 3 * 2 * 14 * 14           # elements of one full-resolution pixel row (what the tower reads)
@@ -99,16 +99,10 @@ class QwenStreamState:
 
     def reset(self):
         self.bank_x, self.bank_small, self.bank_merged = RowBank(), RowBank(), RowBank()
-        self.host_chunks = []                 # pinned chunks of frames >= device_frames: [F x rows | F merged rows]
-        self._chunk_table = None              # device int64: the chunks' mapped device pointers
-        self.n_host = 0                       # frames in the host chunks
-        self._layout = None                   # (dtype, x row shape, merged row shape or None) of a bank frame
+        self.bank_tier = HostChunks()         # frames >= device_frames: x rows and (a part of their own) merged rows
+        self.small_tier = HostChunks()        # half-resolution frames >= small_device_frames
         self._prev_dam = None                 # (spa_positions, spa_x, DAM rows of video_embeds) before the current step
         self.host_fetches = None              # device int64 [1]: retrieved frames read from the host chunks so far
-        self.small_chunks = []                # pinned chunks of half-resolution frames >= small_device_frames: [F, hs*ws, D]
-        self._small_ptrs = []                 # their mapped device pointers
-        self.n_small_host = 0                 # half-resolution frames in those chunks
-        self._small_layout = None             # (dtype, row shape [hs*ws, D]) of a half-resolution frame
         self.n_frames = 0
         self.grid = None                      # (h, w) of a full-resolution frame; the half-resolution grid is (hs, ws)
         self.small_grid = None
@@ -302,7 +296,7 @@ class QwenStreamState:
         tem_pos = torch.round(tem_ts.float()).to(torch.int64)
         klarge = flash.spatial_method in ("klarge_retrieve", "klarge_retrieve_cos")
         if (klarge and n > flash.spatial_length and self.n_small_host == 0 and n_spa <= 64
-                and (d or {}).get("weight_order") is None and self._small_layout[0] in (torch.float16, torch.bfloat16)):
+                and (d or {}).get("weight_order") is None and self.small_tier.dtype in (torch.float16, torch.bfloat16)):
             heaviest = O.argsort_desc(tem_w)[:n_spa]                   # spatial_picks' ranking
             ctx["retrieve"] = (tem_x.reshape(n_tem, -1), heaviest, self.bank_small.rows().view(n, -1),
                                "cosine" if flash.spatial_method == "klarge_retrieve_cos" else "euclidean")
@@ -317,7 +311,7 @@ class QwenStreamState:
         h, w = self.grid
         tem_x, picks, n_spa = ctx["tem_x"], ctx["picks"], ctx["n_spa"]
         D = tem_x.shape[-1]
-        dt, dev = self._small_layout[0], tem_x.device
+        dt, dev = self.small_tier.dtype, tem_x.device
         # memory still filling: the DAM is the whole bank, a view of it (a state without a bank gathers it)
         whole = n_spa == self.n_frames and self.n_host == 0 and self.full_res_bank
         spa_x = self.bank_x.rows() if whole else torch.empty(n_spa, h * w, D, dtype=dt, device=dev)
@@ -347,53 +341,51 @@ class QwenStreamState:
         ve = self.video_embeds
         return self.spa_positions, self.spa_x, None if ve is None else ve[: m * self.spa_x.shape[1] // 4]
 
-    def _per_chunk(self) -> int:
-        dt, xs, ms = self._layout
-        return chunk_frames((xs.numel() + (0 if ms is None else ms.numel())) * dt.itemsize, self.CHUNK_BYTES)
+    @property
+    def n_host(self) -> int:
+        """frames of the full-resolution (and merged) bank in its host tier"""
+        return self.bank_tier.n
 
-    def _chunk(self, c: int, dev):
-        """views (x rows [F, ...], merged rows [F, ...] or None) of host chunk c, allocated (with its table entry) on first
-        use"""
-        dt, xs, ms = self._layout
-        F, fx, fm = self._per_chunk(), xs.numel(), 0 if ms is None else ms.numel()
-        self._chunk_table = grow_pinned(self.host_chunks, self._chunk_table, c, (F * (fx + fm),), dt, dev)
-        buf = self.host_chunks[c]
-        return buf[: F * fx].view(F, *xs), None if ms is None else buf[F * fx:].view(F, *ms)
+    @property
+    def n_small_host(self) -> int:
+        """frames of the half-resolution bank in its host tier"""
+        return self.small_tier.n
+
+    @property
+    def host_chunks(self) -> list:
+        """the pinned chunks of the full-resolution (and merged) bank's host tier"""
+        return self.bank_tier.chunks
+
+    @property
+    def small_chunks(self) -> list:
+        """the pinned chunks of the half-resolution bank's host tier"""
+        return self.small_tier.chunks
+
+    def _banks(self):
+        """the device tier of the full-resolution bank: one RowBank per part of bank_tier (x rows, merged rows)"""
+        return [self.bank_x, self.bank_merged][:len(self.bank_tier.shapes)]
 
     def _append_frames(self, x3, m3, dev):
         """frames x3 [t, h*w, D] (merged rows m3 [t, h*w/4, merger_dim] or None), on the device or the host, appended to
-        the two-tier bank; copies to the host chunks are asynchronous on the current stream, ordered before any later
-        gather that may read them"""
-        if self._layout is None:
-            self._layout = (x3.dtype, torch.Size(x3.shape[1:]), None if m3 is None else torch.Size(m3.shape[1:]))
-        n0 = self.bank_x.n + self.n_host
-        for c, dst, s, cnt in placement(n0, x3.shape[0], self.device_frames, self._per_chunk()):
-            if c < 0:
-                self.bank_x.append(x3[s: s + cnt].to(dev, non_blocking=True))
-                if m3 is not None:
-                    self.bank_merged.append(m3[s: s + cnt].to(dev, non_blocking=True))
-                continue
-            cx, cm = self._chunk(c, dev)
-            cx[dst: dst + cnt].copy_(x3[s: s + cnt], non_blocking=True)
-            if m3 is not None:
-                cm[dst: dst + cnt].copy_(m3[s: s + cnt], non_blocking=True)
-            self.n_host += cnt
+        the two-tier bank, which keeps merged rows when its first frames came with them"""
+        parts = [x3] if m3 is None else [x3, m3]
+        if self.bank_tier.dtype is None:
+            self.bank_tier.lay_out(x3.dtype, [r.shape[1:] for r in parts], self.CHUNK_BYTES)
+        _append_tiered(self._banks(), self.bank_tier, self.device_frames, x3.shape[0], parts, dev)
 
     def _append_lazy(self, pix3, dt, D, dev):
         """lazy_full_res: the clip's pixel rows pix3 [t, h*w, 1176] appended to the pixel store (asynchronous copies to its
         pinned chunks), and t bank slots (zero rows in HBM, chunk rows on the host; none without full_res_bank) with clear
         mask bytes"""
         t, hw = pix3.shape[0], pix3.shape[1]
-        if self._layout is None:
-            ms = None
-            if self.flash.spatial_length > 0 and self.merger is not None:
-                ms = torch.Size([hw // 4, int(self.merger.dim)])
-            self._layout = (dt, torch.Size([hw, D]), ms)
+        if self.bank_tier.dtype is None:
+            merged = self.flash.spatial_length > 0 and self.merger is not None
+            self.bank_tier.lay_out(dt, [(hw, D)] + ([(hw // 4, int(self.merger.dim))] if merged else []), self.CHUNK_BYTES)
         if self.pixels is None:
             self.pixels = self._pixel_store(hw, self.n_frames, pix3.dtype)
         self.pixels.append(pix3.reshape(t, -1), dev)
         if self.full_res_bank:
-            self._append_slots(t, dev)
+            _append_tiered(self._banks(), self.bank_tier, self.device_frames, t, None, dev)
         self.encoded.append(torch.zeros(t, dtype=torch.uint8, device=dev))
 
     def _pixel_store(self, hw: int, base: int, dtype) -> "PixelStore":
@@ -401,74 +393,46 @@ class QwenStreamState:
         (compact_pixels), or rows of `dtype`"""
         if self.compact_pixels:
             return PixelStore(torch.uint8, hw * PATCH_DIM, base, self.CHUNK_BYTES, values=self.pixel_table,
-                              out_dtype=self._layout[0])
+                              out_dtype=self.bank_tier.dtype)
         return PixelStore(dtype, hw * PATCH_DIM, base, self.CHUNK_BYTES)
 
-    def _append_slots(self, t: int, dev):
-        """t zero bank slots (rows in HBM, chunk rows on the host) at the end of the two-tier bank"""
-        dt, xs, ms = self._layout
-        for c, _, _, cnt in placement(self.bank_x.n + self.n_host, t, self.device_frames, self._per_chunk()):
-            if c < 0:
-                self.bank_x.append(torch.zeros((cnt,) + tuple(xs), dtype=dt, device=dev))
-                if ms is not None:
-                    self.bank_merged.append(torch.zeros((cnt,) + tuple(ms), dtype=dt, device=dev))
-                continue
-            self._chunk(c, dev)
-            self.n_host += cnt
-
-    def _bank_args(self) -> dict:
-        """this state's two-tier bank as the gather and scatter jobs read it; n_base: its frames (without
+    def _bank_args(self, dev) -> dict:
+        """this state's two-tier bank as the gather and scatter jobs on `dev` read it; n_base: its frames (without
         full_res_bank, those of the base bank, which may be fewer than the stream's)"""
-        dt, xs, ms = self._layout
-        return dict(n_base=self.bank_x.n + self.n_host, dev_x=self.bank_x.buf if self.bank_x.n else None,
+        tier = self.bank_tier
+        return dict(n_base=self.bank_x.n + tier.n, dev_x=self.bank_x.buf if self.bank_x.n else None,
                     dev_merged=self.bank_merged.buf if self.bank_merged.n else None, n_dev=self.bank_x.n,
-                    chunks=self._chunk_table, chunk_frames=self._per_chunk(), x_frame_elems=xs.numel(),
-                    merged_frame_elems=0 if ms is None else ms.numel())
+                    chunks=tier.table(dev), chunk_frames=tier.per_chunk, x_frame_elems=tier.shapes[0].numel(),
+                    merged_frame_elems=tier.shapes[1].numel() if len(tier.shapes) > 1 else 0)
 
     def _scatter_args(self, n: int, x_rows, merged_rows) -> dict:
         """the job of Q.bank_scatter_multi that writes the n frames of this state's last pick plan into its banks"""
-        bank = self._bank_args()
+        bank = self._bank_args(self._plan.device)
         return dict(bank, plan=self._plan, n=n, n_frames=bank["n_base"], x_rows=x_rows,
                     merged_rows=merged_rows if bank["merged_frame_elems"] else None)
 
-    def _small_per_chunk(self) -> int:
-        dt, ps = self._small_layout
-        return chunk_frames(ps.numel() * dt.itemsize, self.CHUNK_BYTES)
-
     def _append_small(self, s3, dev):
         """half-resolution frames s3 [t, hs*ws, D], on the device or the host, appended to the two-tier half-resolution
-        bank; copies to its host chunks are asynchronous on the current stream, ordered before the retrieval that sweeps
-        them"""
-        if self._small_layout is None:
-            self._small_layout = (s3.dtype, torch.Size(s3.shape[1:]))
-        dt, ps = self._small_layout
-        F = self._small_per_chunk()
-        for c, dst, s, cnt in placement(self.bank_small.n + self.n_small_host, s3.shape[0], self.small_device_frames, F):
-            if c < 0:
-                self.bank_small.append(s3[s: s + cnt].to(dev, non_blocking=True))
-                continue
-            while len(self.small_chunks) <= c:
-                buf = torch.empty((F,) + tuple(ps), dtype=dt, pin_memory=True)
-                self.small_chunks.append(buf)
-                self._small_ptrs.append(Q.host_device_ptr(buf))
-            self.small_chunks[c][dst: dst + cnt].copy_(s3[s: s + cnt], non_blocking=True)
-            self.n_small_host += cnt
+        bank"""
+        if self.small_tier.dtype is None:
+            self.small_tier.lay_out(s3.dtype, [s3.shape[1:]], self.CHUNK_BYTES)
+        _append_tiered([self.bank_small], self.small_tier, self.small_device_frames, s3.shape[0], [s3], dev)
 
     def _small_bank(self, D, dev):
         """the half-resolution bank as the retrieval reads it: the HBM rows [n * hs*ws, D] while every frame is there, a
         qwen.ops.TieredBank once frames have spilled"""
-        rb = self.bank_small
-        if self.n_small_host == 0:
+        rb, tier = self.bank_small, self.small_tier
+        if tier.n == 0:
             return rb.rows().view(-1, D)
-        return Q.TieredBank(rb.rows().view(rb.n, -1) if rb.n else None, rb.n, tuple(self._small_ptrs),
-                            self._small_per_chunk(), rb.n + self.n_small_host, self._small_layout[0], dev)
+        return Q.TieredBank(rb.rows().view(rb.n, -1) if rb.n else None, rb.n, tier.ptrs(), tier.per_chunk, rb.n + tier.n,
+                            tier.dtype, dev)
 
     def _gather_args(self, picks, spa_x, merged, prev) -> dict:
         """the Q.dam_gather_multi job that writes spa_x / merged for `picks` from the previous DAM `prev`, this step's
         fresh rows (without full_res_bank) and this state's bank"""
         if self.host_fetches is None:
             self.host_fetches = torch.zeros(1, dtype=torch.int64, device=picks.device)
-        return dict(self._bank_args(), picks=picks, n_frames=self.n_frames, prev=prev, fresh=self._fresh,
+        return dict(self._bank_args(picks.device), picks=picks, n_frames=self.n_frames, prev=prev, fresh=self._fresh,
                     spa_x_out=spa_x, merged_out=merged, host_fetches=self.host_fetches)
 
     def host_fetch_count(self) -> int:
@@ -480,22 +444,9 @@ class QwenStreamState:
         started here (a clip redone by complete() counts its encodes again; synchronises; tests and timing)"""
         return 0 if self.re_encodes is None else int(self.re_encodes.item())
 
-    def _bank_on_host(self, merged: bool) -> torch.Tensor:
-        """the whole full-resolution (or merged) bank as one pinned host tensor: device rows D2H, chunk rows H2H"""
-        dt, xs, ms = self._layout
-        rb = self.bank_merged if merged else self.bank_x
-        chunks = [self._chunk(c, None)[int(merged)] for c in range(len(self.host_chunks))]
-        return _on_host(rb, chunks, self.bank_x.n + self.n_host, ms if merged else xs, dt)
-
     def pinned_bytes(self) -> int:
         """bytes of pinned host memory the state holds: bank chunks, half-resolution chunks and pixel chunks"""
-        bufs = self.host_chunks + self.small_chunks + ([] if self.pixels is None else self.pixels.chunks)
-        return sum(b.numel() * b.element_size() for b in bufs)
-
-    def _small_on_host(self) -> torch.Tensor:
-        """the whole half-resolution bank as one pinned host tensor: device rows D2H, chunk rows H2H"""
-        dt, ps = self._small_layout
-        return _on_host(self.bank_small, self.small_chunks, self.n_frames, ps, dt)
+        return self.bank_tier.nbytes() + self.small_tier.nbytes() + (0 if self.pixels is None else self.pixels.tier.nbytes())
 
     def _compress_sync(self, cand, cand_w, T, d, start_idx, t):
         """every other branch of temporal_compress (:149-183): pass-through while the memory is filling, temporal_length 0,
@@ -528,7 +479,7 @@ class QwenStreamState:
         counters = {"n_frames": n, "steps": self.steps, "n_tem": self.n_tem,
                     "n_spa": 0 if self.spa_positions is None else int(self.spa_positions.numel()),
                     "fast_steps": self.fast_steps, "redone_steps": self.redone_steps,
-                    "merged": int(n > 0 and self._layout[2] is not None),
+                    "merged": int(n > 0 and len(self.bank_tier.shapes) > 1),
                     "tem_weights_dtype": None if self.tem_weights is None else CK.dtype_name(self.tem_weights.dtype),
                     "tem_timestamp_dtype": "float32" if n == 0 else CK.dtype_name(self.tem_timestamp.dtype)}
         if self.lazy_full_res and n:          # eager checkpoints carry neither the counter nor the tensors below
@@ -539,7 +490,6 @@ class QwenStreamState:
                 counters["bank_frames"] = self.bank_x.n + self.n_host
         if n == 0:
             return CK.qwen(self._config(0, "float16"), counters, {})
-        dt, ps = self._small_layout
         tensors = {"tem_x": self.tem_x, "tem_timestamp": self.tem_timestamp, "spa_positions": self.spa_positions}
         if self.tem_weights is not None:          # temporal_method 'sample' keeps no weights
             tensors["tem_weights"] = self.tem_weights
@@ -553,25 +503,25 @@ class QwenStreamState:
                     owned["pix_codes"] = self.pixels.rows_of(todo)
                     tensors["pixel_table"] = self.pixels.values
                 else:
-                    owned["pixels"] = self.pixels.rows_of(todo).view(len(todo), self._layout[1][0], PATCH_DIM)
+                    owned["pixels"] = self.pixels.rows_of(todo).view(len(todo), self.bank_tier.shapes[0][0], PATCH_DIM)
             if not self.full_res_bank:
                 tensors["spa_x"] = self.spa_x
             if self.n_small_host:
-                owned["bank_small"] = self._small_on_host()
+                owned["bank_small"] = self.small_tier.to_host(self.bank_small.rows() if self.bank_small.n else None)
             else:
                 tensors["bank_small"] = self.bank_small.rows()
-            for name, merged in (("bank_x", False), ("bank_merged", True)):
-                if merged and not counters["merged"]:
+            tier = self.bank_tier
+            for part, (name, rb) in enumerate((("bank_x", self.bank_x), ("bank_merged", self.bank_merged))):
+                if part and not counters["merged"]:
                     continue
-                rb = self.bank_merged if merged else self.bank_x
-                if self.n_host:
-                    owned[name] = self._bank_on_host(merged)
+                if tier.n:
+                    owned[name] = tier.to_host(rb.rows() if rb.n else None, part)
                 elif rb.n:
                     tensors[name] = rb.rows()
                 else:                             # no full_res_bank and no base bank: zero frames
-                    dt_, xs, ms = self._layout
-                    tensors[name] = torch.empty((0,) + tuple(ms if merged else xs), dtype=dt_)
-            ck = CK.qwen(self._config(int(ps[-1]), CK.dtype_name(dt)), counters, tensors, owned=owned)
+                    tensors[name] = torch.empty((0,) + tuple(tier.shapes[part]), dtype=tier.dtype)
+            small = self.small_tier
+            ck = CK.qwen(self._config(int(small.shapes[0][-1]), CK.dtype_name(small.dtype)), counters, tensors, owned=owned)
             torch.cuda.current_stream().synchronize()
         return ck
 
@@ -651,17 +601,17 @@ class QwenStreamState:
                 hw = int(c["grid"][0]) * int(c["grid"][1])
                 # the pixel store starts at the first frame with pixel rows only; frames without a stored row get them
                 base = todo[0] if todo else N
-                st.pixels = st._pixel_store(hw, base, st._layout[0])
+                st.pixels = st._pixel_store(hw, base, st.bank_tier.dtype)
                 if todo:
                     st.pixels.append(None, dev, t=N - base)
                     if compact_ck and not compact_pixels:     # decoded here into the rows the tower reads
-                        rows = Q.pixel_decode(get("pix_codes").view(-1, PATCH_DIM), get("pixel_table"), st._layout[0])
+                        rows = Q.pixel_decode(get("pix_codes").view(-1, PATCH_DIM), get("pixel_table"), st.bank_tier.dtype)
                         st.pixels.put(todo, rows.view(len(todo), -1).cpu())
                     else:
                         st.pixels.put(todo, ckpt.tensor("pix_codes" if compact_ck else "pixels").view(len(todo), -1))
                 st.n_encoded = N - len(todo)
                 if full_res_bank:                 # frames past the checkpoint's bank get zero slots, "not yet encoded"
-                    st._append_slots(N - (st.bank_x.n + st.n_host), dev)
+                    _append_tiered(st._banks(), st.bank_tier, st.device_frames, N - (st.bank_x.n + st.n_host), None, dev)
                     st.encoded.append(stored.to(torch.uint8).to(dev))
                 elif bankless_ck:                 # the base bank and the "encoded before" bytes carry over as they are
                     st.encoded.append(get("encoded"))
@@ -678,7 +628,7 @@ class QwenStreamState:
             if "spa_x" in ckpt.tensors:           # a stream without a bank: the DAM's rows as they were
                 st.spa_x = get("spa_x")
             else:
-                st.spa_x = torch.empty(n["n_spa"], h * w, int(c["dim"]), dtype=st._layout[0], device=dev)
+                st.spa_x = torch.empty(n["n_spa"], h * w, int(c["dim"]), dtype=st.bank_tier.dtype, device=dev)
                 if n["n_spa"]:
                     Q.dam_gather_multi([st._gather_args(st.spa_positions, st.spa_x, None, None)])
             st.video_embeds = get("video_embeds") if "video_embeds" in ckpt.tensors else None
@@ -809,33 +759,33 @@ def check_full_res_bank(v, lazy: bool, who: str = "full_res_bank", lazy_who: str
 
 class PixelStore:
     """lazy_full_res: the full-resolution pixel rows of frames [base, n) of a stream in pinned host chunks of
-    chunk_frames frames each (host_tier's chunk arithmetic with no device tier), with a device table of the chunks'
-    mapped pointers that fvs_qwen_pixel_gather_multi reads them through.  Frames below `base` (encoded before the stream
-    came here from a checkpoint) have no pixel rows; a restored stream's encoded frames above it have unwritten slots.
-    dtype: the rows' element type, the tower dtype or uint8 codes (compact_pixels); a store of codes holds `values`,
-    the float32 [3, 256] device table the gather decodes them through into `out_dtype`."""
+    chunk_frames frames each (`tier`, a HostChunks with no device tier: frame f is its frame f - base), with a device
+    table of the chunks' mapped pointers that fvs_qwen_pixel_gather_multi reads them through.  Frames below `base`
+    (encoded before the stream came here from a checkpoint) have no pixel rows; a restored stream's encoded frames above
+    it have unwritten slots.  dtype: the rows' element type, the tower dtype or uint8 codes (compact_pixels); a store of
+    codes holds `values`, the float32 [3, 256] device table the gather decodes them through into `out_dtype`."""
 
     def __init__(self, dtype, frame_elems: int, base: int, chunk_bytes: int = CHUNK_BYTES, values=None, out_dtype=None):
-        self.dtype, self.frame_elems, self.base, self.n = dtype, int(frame_elems), int(base), int(base)
+        self.dtype, self.frame_elems, self.base = dtype, int(frame_elems), int(base)
         if (dtype == torch.uint8) != (values is not None and out_dtype is not None):
             raise ValueError("PixelStore: uint8 codes go with their value table and the dtype they decode to")
         self.values, self.out_dtype = values, dtype if out_dtype is None else out_dtype
-        self.chunk_frames = chunk_frames(self.frame_elems * dtype.itemsize, chunk_bytes)
-        self.chunks, self.table = [], None
+        self.tier = HostChunks().lay_out(dtype, [(self.frame_elems,)], chunk_bytes)
+        self.table = None
+
+    chunk_frames = property(lambda self: self.tier.per_chunk)
+    chunks = property(lambda self: self.tier.chunks)
+    n = property(lambda self: self.base + self.tier.n)
 
     def append(self, rows: Optional[torch.Tensor], dev, t: Optional[int] = None):
         """rows [t, frame_elems] (device or host): asynchronous copies on the current stream; rows None: t slots left
         unwritten (frames whose rows are put() later or never read)"""
-        t = rows.shape[0] if rows is not None else int(t)
-        for c, dst, s, cnt in placement(self.n - self.base, t, 0, self.chunk_frames):
-            self.table = grow_pinned(self.chunks, self.table, c, (self.chunk_frames, self.frame_elems), self.dtype, dev)
-            if rows is not None:
-                self.chunks[c][dst: dst + cnt].copy_(rows[s: s + cnt], non_blocking=True)
-        self.n += t
+        self.tier.write(self.tier.n, None if rows is None else [rows], t)
+        self.table = self.tier.table(dev)
 
     def _row(self, f: int) -> torch.Tensor:
         c, r = divmod(f - self.base, self.chunk_frames)
-        return self.chunks[c][r]
+        return self.tier.view(c)[r]
 
     def rows_of(self, frames) -> torch.Tensor:
         """the rows of `frames` (each in [base, n)) as one pinned tensor [len(frames), frame_elems], once the pending
@@ -854,33 +804,16 @@ class PixelStore:
             self._row(int(f)).copy_(rows[i])
 
 
-def grow_pinned(chunks: list, table: Optional[torch.Tensor], c: int, shape, dtype, dev) -> torch.Tensor:
-    """pinned host chunks of `shape` appended to `chunks` until chunk c exists, each one's mapped device pointer stored
-    to its slot of `table` (device int64, grown by doubling; None: none yet), which kernels read the chunks through in
-    place -> the table"""
-    while len(chunks) <= c:
-        k = len(chunks)
-        buf = torch.empty(shape, dtype=dtype, pin_memory=True)
-        if table is None or table.numel() <= k:
-            tab = torch.zeros(max(16, 2 * k), dtype=torch.int64, device=dev)
-            if k:
-                tab[:k].copy_(table[:k])
-            table = tab
-        table[k].fill_(Q.host_device_ptr(buf))                  # stream-ordered: no host wait
-        chunks.append(buf)
-    return table
-
-
-def _on_host(rb: RowBank, chunks, n: int, row_shape, dt) -> torch.Tensor:
-    """frames [0, n) of a two-tier bank as one pinned host tensor: the device rows of `rb` D2H, then the filled rows of
-    the host chunks (views [F, *row_shape], in order) H2H"""
-    out = torch.empty((n,) + tuple(row_shape), dtype=dt, pin_memory=True)
-    if rb.n:
-        out[: rb.n].copy_(rb.rows(), non_blocking=True)
-    torch.cuda.current_stream().synchronize()                    # the spills of the last steps have landed
-    s = rb.n
-    for c in chunks:
-        cnt = min(c.shape[0], n - s)
-        out[s: s + cnt].copy_(c[:cnt])
-        s += cnt
-    return out
+def _append_tiered(banks, tier: HostChunks, cap: Optional[int], t: int, parts, dev):
+    """t frames appended to a two-tier bank: to `banks` (its device tier, one RowBank per part of `tier`) while fewer
+    than `cap` frames (None: no cap) are there, then to `tier`.  parts: the frames' rows per part [t, ...], on the device
+    or the host, or None for t zero slots (zero rows in HBM, unwritten host rows).  Copies are asynchronous on the
+    current stream, ordered before any later kernel that reads them."""
+    n0 = banks[0].n + tier.n
+    k = t if cap is None else max(0, min(t, cap - n0))
+    if k:
+        for p, rb in enumerate(banks):
+            rb.append(torch.zeros((k,) + tier.shapes[p], dtype=tier.dtype, device=dev) if parts is None
+                      else parts[p][:k].to(dev, non_blocking=True))
+    if k < t:
+        tier.write(tier.n, None if parts is None else [r[k:] for r in parts], t - k)
