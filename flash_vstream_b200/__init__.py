@@ -6,7 +6,7 @@ ViT-L/14 frame encoding + Flash-Memory consolidation, behind the reference's own
     flash_vstream_b200.clip_encoder         <->  flash_vstream.model.multimodal_encoder.clip_encoder
     flash_vstream_b200.ops                  tensor-level wrappers over the C ABI (include/fvs_b200.h)
     flash_vstream_b200.StreamPool           many streams on one GPU, stepped together (multistream.py)
-    flash_vstream_b200.CLIPFramePreprocessor, .Qwen2VLFramePreprocessor
+    flash_vstream_b200.CLIPFramePreprocessor, .Qwen2VLFramePreprocessor, .Qwen2VLVideoFetcher
                                             decoded uint8 frames -> tower pixels on the GPU (preprocess.py)
     flash_vstream_b200.StreamCheckpoint     a live stream's state on the host / on disk: suspend, resume, move (checkpoint.py)
     flash_vstream_b200.install()            rebinds the reference's modules to these implementations
@@ -32,7 +32,7 @@ def __getattr__(name):      # StreamPool imports torch: loaded on first use, so 
     if name == "StreamPool":
         from .multistream import StreamPool
         return StreamPool
-    if name in ("CLIPFramePreprocessor", "Qwen2VLFramePreprocessor"):
+    if name in ("CLIPFramePreprocessor", "Qwen2VLFramePreprocessor", "Qwen2VLVideoFetcher"):
         from . import preprocess
         return getattr(preprocess, name)
     if name == "StreamCheckpoint":

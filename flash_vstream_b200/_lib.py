@@ -67,7 +67,7 @@ class ResampleAxis(C.Structure):  # fvs_resample_axis
 
 class PreprocessJob(C.Structure):  # fvs_preprocess_job
     _fields_ = [("frames", C.c_void_p)] + [(n, C.c_int) for n in ("T", "H", "W", "C")] + \
-               [("x", ResampleAxis), ("y", ResampleAxis)]
+               [("x", ResampleAxis), ("y", ResampleAxis), ("x2", ResampleAxis), ("y2", ResampleAxis)]
 
 
 class QwenMemJob(C.Structure):  # fvs_qwen_mem_job
@@ -114,7 +114,7 @@ class QwenScatterJob(C.Structure):  # fvs_qwen_scatter_job
 
 
 QWEN_MEM_JOBS_PER_LAUNCH = 16
-PRE_CLIP, PRE_QWEN, PRE_QWEN_CODES = 0, 1, 2
+PRE_CLIP, PRE_QWEN, PRE_QWEN_CODES, PRE_RGB8 = 0, 1, 2, 3
 KLARGE_EUCLIDEAN, KLARGE_COSINE = 0, 1
 INPUT_PIXELS, INPUT_FEATURES = 0, 1
 

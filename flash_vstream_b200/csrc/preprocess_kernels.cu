@@ -10,7 +10,10 @@
 //
 // A call is a table of jobs (clips of any size; fvs_preprocess is the one-job case) and two launches per 32 jobs:
 // resample_rows_kernel (horizontal pass into a planar uint8 workspace [T, 3, rows, cols] per job) and resample_cols_kernel
-// (vertical pass, table lookup, and the layout write).  Both grids are flat: a block finds its job in the block-offset
+// (vertical pass, table lookup, and the layout write).  A two-stage job (Qwen2-VL's fetch_video resize, then its image
+// processor's) runs its first stage as an FVS_PRE_RGB8 job into its own workspace, in a launch pair of its own ahead of
+// the final one: that 8-bit image is exactly the PIL image the first resize returns, and the second stage reads it as
+// a single-stage job reads decoded frames.  Both grids are flat: a block finds its job in the block-offset
 // table, so the per-element code is the same whatever the jobs next to it.  Only the window of the resized image the
 // caller asks for is computed (the CLIP center crop): the outputs of the window are the same integers the full resize
 // computes there, because every output depends only on its own taps.
@@ -186,7 +189,8 @@ __device__ __forceinline__ void resample_row(const Job& a, int r, int t, uint8_t
 //   FVS_PRE_CLIP  f16 [T, 3, out_rows, cols];
 //   FVS_PRE_QWEN  fp32 [T/2 * gh * gw, 1176], row ((ti*gh/2 + bh)*gw/2 + bw)*4 + mh*2 + mw, column ((c*2 + tp)*14 + py)*14
 //                 + px; a one-frame clip fills both temporal slots;
-//   FVS_PRE_QWEN_CODES  the same rows and columns as uint8: the resampled byte itself, before the table lookup.
+//   FVS_PRE_QWEN_CODES  the same rows and columns as uint8: the resampled byte itself, before the table lookup;
+//   FVS_PRE_RGB8  uint8 [T, out_rows, cols, 3]: the resized 8-bit image itself.
 template <int kLayout>
 __device__ __forceinline__ void resample_col(const Job& a, int y, int t, const float* lut) {
   const int2 b = a.yb[y];
@@ -196,6 +200,10 @@ __device__ __forceinline__ void resample_col(const Job& a, int y, int t, const f
     const uint8_t* p = a.tmp + ((size_t(t) * 3 + c) * a.rows + (b.x - a.row0)) * a.cols + x;
     int acc = 1 << (kBits - 1);
     for (int j = 0; j < b.y; ++j) acc += int(p[size_t(j) * a.cols]) * k[j];
+    if (kLayout == FVS_PRE_RGB8) {
+      static_cast<uint8_t*>(a.out)[((size_t(t) * a.out_rows + y) * a.cols + x) * 3 + c] = uint8_t(clip8(acc));
+      continue;
+    }
     const float v = lut[c * 256 + clip8(acc)];
     if (kLayout == FVS_PRE_CLIP) {
       static_cast<__half*>(a.out)[((size_t(t) * 3 + c) * a.out_rows + y) * a.cols + x] = __float2half_rn(v);
@@ -226,7 +234,7 @@ __global__ void __launch_bounds__(kThreads) resample_rows_kernel(const __grid_co
 template <int kLayout>
 __global__ void __launch_bounds__(kThreads) resample_cols_kernel(const __grid_constant__ MultiArgs m) {
   __shared__ float lut[3 * 256];
-  if (kLayout != FVS_PRE_QWEN_CODES) {     // codes are the bytes before the lookup
+  if (kLayout == FVS_PRE_CLIP || kLayout == FVS_PRE_QWEN) {     // codes and images are the bytes before the lookup
     for (int i = threadIdx.x; i < 3 * 256; i += blockDim.x) lut[i] = m.table[i];
     __syncthreads();
   }
@@ -242,6 +250,18 @@ struct JobPlan {
   int64_t out_off, ws_off;        // output elements / workspace bytes before the job
 };
 
+bool two_stage(const fvs_preprocess_job& jb) { return jb.x2.out_size != 0 || jb.y2.out_size != 0; }
+
+// the axes of the job's last stage, the ones its layout is written from
+const fvs_resample_axis& final_x(const fvs_preprocess_job& jb) { return two_stage(jb) ? jb.x2 : jb.x; }
+const fvs_resample_axis& final_y(const fvs_preprocess_job& jb) { return two_stage(jb) ? jb.y2 : jb.y; }
+
+int check_row_span(const fvs_resample_axis& x, const char* api) {
+  FVS_REQUIRE(size_t(x.span_count) * 3 <= kRowSmemMax, "%s: a window reading %d source columns is wider than the %zu "
+              "supported", api, x.span_count, kRowSmemMax / 3);
+  return FVS_OK;
+}
+
 // every check fvs_preprocess makes of one clip; `api` names the job
 int check_job(const fvs_preprocess_job& jb, int layout, int pool, const char* api) {
   FVS_REQUIRE(jb.frames, "%s: null frames", api);
@@ -250,34 +270,52 @@ int check_job(const fvs_preprocess_job& jb, int layout, int pool, const char* ap
   FVS_REQUIRE(jb.T <= 65535, "%s: %d frames in one call (at most 65535)", api, jb.T);
   int r;
   if ((r = check_axis(&jb.x, jb.W, "x", api)) || (r = check_axis(&jb.y, jb.H, "y", api))) return r;
-  FVS_REQUIRE(size_t(jb.x.span_count) * 3 <= kRowSmemMax, "%s: a window reading %d source columns is wider than the %zu "
-              "supported", api, jb.x.span_count, kRowSmemMax / 3);
-  FVS_REQUIRE(layout == FVS_PRE_CLIP || layout == FVS_PRE_QWEN || layout == FVS_PRE_QWEN_CODES, "%s: unknown layout %d",
-              api, layout);
-  if (layout != FVS_PRE_CLIP) {
+  if ((r = check_row_span(jb.x, api))) return r;
+  if (two_stage(jb)) {       // the second stage resizes the first stage's window
+    if ((r = check_axis(&jb.x2, jb.x.count, "second-stage x", api)) ||
+        (r = check_axis(&jb.y2, jb.y.count, "second-stage y", api)) || (r = check_row_span(jb.x2, api)))
+      return r;
+  }
+  FVS_REQUIRE(layout == FVS_PRE_CLIP || layout == FVS_PRE_QWEN || layout == FVS_PRE_QWEN_CODES || layout == FVS_PRE_RGB8,
+              "%s: unknown layout %d", api, layout);
+  if (layout == FVS_PRE_QWEN || layout == FVS_PRE_QWEN_CODES) {
+    const fvs_resample_axis &x = final_x(jb), &y = final_y(jb);
     FVS_REQUIRE(jb.T == 1 || jb.T % kTemporal == 0, "%s: Qwen2-VL clips hold 1 or an even number of frames, not %d", api,
                 jb.T);
     FVS_REQUIRE(pool >= 1, "%s: pool %d < 1", api, pool);
     const int f = kPatch * kMerge * pool;
-    FVS_REQUIRE(jb.x.first == 0 && jb.x.count == jb.x.out_size && jb.y.first == 0 && jb.y.count == jb.y.out_size,
+    FVS_REQUIRE(x.first == 0 && x.count == x.out_size && y.first == 0 && y.count == y.out_size,
                 "%s: the Qwen2-VL layout takes the whole resized frame (no crop)", api);
-    FVS_REQUIRE(jb.y.count % f == 0 && jb.x.count % f == 0, "%s: resized %dx%d is not a multiple of %d (patch %d x merge "
-                "%d x pool %d)", api, jb.y.count, jb.x.count, f, kPatch, kMerge, pool);
+    FVS_REQUIRE(y.count % f == 0 && x.count % f == 0, "%s: resized %dx%d is not a multiple of %d (patch %d x merge "
+                "%d x pool %d)", api, y.count, x.count, f, kPatch, kMerge, pool);
   }
   return FVS_OK;
 }
 
 int64_t out_elements(const fvs_preprocess_job& jb, int layout) {
-  if (layout == FVS_PRE_CLIP) return int64_t(jb.T) * 3 * jb.y.count * jb.x.count;
-  return int64_t(jb.T > 1 ? jb.T / kTemporal : 1) * (jb.y.count / kPatch) * (jb.x.count / kPatch) * kQwenCols;
+  const fvs_resample_axis &x = final_x(jb), &y = final_y(jb);
+  if (layout == FVS_PRE_CLIP) return int64_t(jb.T) * 3 * y.count * x.count;
+  if (layout == FVS_PRE_RGB8) return int64_t(jb.T) * y.count * x.count * 3;
+  return int64_t(jb.T > 1 ? jb.T / kTemporal : 1) * (y.count / kPatch) * (x.count / kPatch) * kQwenCols;
 }
 
-// Validates every job (the error names the first bad one) and lays them out; returns the number of launch pairs.
+// A job's workspace: the planar scratch of its passes, then (two stages) the first stage's 8-bit image, which the
+// second stage reads while its own passes reuse the scratch.
+int64_t job_scratch_bytes(const fvs_preprocess_job& jb) {
+  const int64_t one = int64_t(workspace_bytes(jb.x, jb.y, jb.T));
+  return two_stage(jb) ? std::max(one, int64_t(workspace_bytes(jb.x2, jb.y2, jb.T))) : one;
+}
+int64_t job_workspace_bytes(const fvs_preprocess_job& jb) {
+  return job_scratch_bytes(jb) + (two_stage(jb) ? int64_t(jb.T) * jb.y.count * jb.x.count * 3 : 0);
+}
+
+// Validates every job (the error names the first bad one) and lays them out; returns the number of launch groups (of
+// up to 32 jobs each: one launch pair, two when a job of the group has two stages).
 // `one` keeps fvs_preprocess's own messages for its single clip.
 int plan_jobs(const fvs_preprocess_job* jobs, int n, int layout, int pool, JobPlan* plan, int64_t* out_total,
               int64_t* ws_total, const char* api, bool one) {
   FVS_REQUIRE(jobs && n > 0, "%s: no jobs", api);
-  int64_t out = 0, ws = 0, rows = 0, cols = 0;
+  int64_t out = 0, ws = 0, rows = 0, cols = 0, rows1 = 0, cols1 = 0;
   char name[96];
   for (int i = 0; i < n; ++i) {
     const fvs_preprocess_job& jb = jobs[i];
@@ -288,17 +326,73 @@ int plan_jobs(const fvs_preprocess_job* jobs, int n, int layout, int pool, JobPl
     }
     int r = check_job(jb, layout, pool, name);
     if (r) return r;
-    if (i % kMaxJobs == 0) rows = cols = 0;
+    if (i % kMaxJobs == 0) rows = cols = rows1 = cols1 = 0;
     plan[i] = {rows, cols, out, ws};
-    rows += int64_t(jb.y.span_count) * jb.T;
-    cols += int64_t(jb.y.count) * jb.T;
-    FVS_REQUIRE(rows <= INT32_MAX && cols <= INT32_MAX, "%s: more than %d blocks in one launch", name, INT32_MAX);
+    rows += int64_t(final_y(jb).span_count) * jb.T;
+    cols += int64_t(final_y(jb).count) * jb.T;
+    if (two_stage(jb)) {
+      rows1 += int64_t(jb.y.span_count) * jb.T;
+      cols1 += int64_t(jb.y.count) * jb.T;
+    }
+    FVS_REQUIRE(rows <= INT32_MAX && cols <= INT32_MAX && rows1 <= INT32_MAX && cols1 <= INT32_MAX,
+                "%s: more than %d blocks in one launch", name, INT32_MAX);
     out += out_elements(jb, layout);
-    ws += int64_t(workspace_bytes(jb.x, jb.y, jb.T));
+    ws += job_workspace_bytes(jb);
   }
   *out_total = out;
   *ws_total = ws;
   return (n + kMaxJobs - 1) / kMaxJobs;
+}
+
+Job make_job(const uint8_t* src, int T, int H, int W, const fvs_resample_axis& x, const fvs_resample_axis& y,
+             uint8_t* tmp, void* out) {
+  Job a;
+  a.src = src;
+  a.tmp = tmp;
+  a.out = out;
+  a.xb = reinterpret_cast<const int2*>(x.bounds);
+  a.xk = x.coeffs;
+  a.yb = reinterpret_cast<const int2*>(y.bounds);
+  a.yk = y.coeffs;
+  a.H = H;
+  a.W = W;
+  a.T = T;
+  a.xtaps = x.taps;
+  a.ytaps = y.taps;
+  a.cols = x.count;
+  a.rows = y.span_count;
+  a.row0 = y.span_first;
+  a.span0 = x.span_first;
+  a.span = x.span_count;
+  a.out_rows = y.count;
+  return a;
+}
+
+// one launch pair over up to kMaxJobs jobs
+int launch_pair(const Job* jobs, int n, const float* table, int layout, cudaStream_t st) {
+  MultiArgs m = {};
+  m.table = table;
+  m.n = n;
+  size_t row_smem = 0;
+  for (int k = 0; k < n; ++k) {
+    m.job[k] = jobs[k];
+    m.row_block0[k + 1] = m.row_block0[k] + jobs[k].rows * jobs[k].T;
+    m.col_block0[k + 1] = m.col_block0[k] + jobs[k].out_rows * jobs[k].T;
+    row_smem = std::max(row_smem, size_t(jobs[k].span) * 3);
+  }
+  resample_rows_kernel<<<m.row_block0[n], kThreads, row_smem, st>>>(m);
+  FVS_CHECK_LAUNCH("resample_rows_kernel");
+  if (layout == FVS_PRE_CLIP) {
+    resample_cols_kernel<FVS_PRE_CLIP><<<m.col_block0[n], kThreads, 0, st>>>(m);
+  } else if (layout == FVS_PRE_QWEN) {
+    resample_cols_kernel<FVS_PRE_QWEN><<<m.col_block0[n], kThreads, 0, st>>>(m);
+  } else if (layout == FVS_PRE_QWEN_CODES) {
+    resample_cols_kernel<FVS_PRE_QWEN_CODES><<<m.col_block0[n], kThreads, 0, st>>>(m);
+  } else {
+    resample_cols_kernel<FVS_PRE_RGB8><<<m.col_block0[n], kThreads, 0, st>>>(m);
+  }
+  FVS_CHECK_LAUNCH("resample_cols_kernel");
+  return FVS_OK;
 }
 
 int preprocess_jobs(const fvs_preprocess_job* jobs, int n, const float* table, int layout, int pool, void* out,
@@ -307,54 +401,31 @@ int preprocess_jobs(const fvs_preprocess_job* jobs, int n, const float* table, i
   FVS_REQUIRE(n > 0 && n <= (1 << 20), "%s: %d jobs", api, n);
   std::vector<JobPlan> plan(n);
   int64_t out_total = 0, ws_total = 0;
-  const int launches = plan_jobs(jobs, n, layout, pool, plan.data(), &out_total, &ws_total, api, one);
-  if (launches < 0) return launches;
+  const int groups = plan_jobs(jobs, n, layout, pool, plan.data(), &out_total, &ws_total, api, one);
+  if (groups < 0) return groups;
   FVS_REQUIRE(workspace_bytes_ >= size_t(ws_total), "%s: workspace of %zu bytes < %zu", api, workspace_bytes_,
               size_t(ws_total));
   const size_t esize = layout == FVS_PRE_CLIP ? sizeof(__half) : layout == FVS_PRE_QWEN ? sizeof(float) : 1;
-  for (int g = 0; g < launches; ++g) {
-    MultiArgs m = {};
-    m.table = table;
-    m.n = std::min(kMaxJobs, n - g * kMaxJobs);
-    size_t row_smem = 0;
-    for (int k = 0; k < m.n; ++k) {
+  for (int g = 0; g < groups; ++g) {
+    const int m = std::min(kMaxJobs, n - g * kMaxJobs);
+    Job first[kMaxJobs], last[kMaxJobs];
+    int n_first = 0;
+    for (int k = 0; k < m; ++k) {
       const fvs_preprocess_job& jb = jobs[g * kMaxJobs + k];
       const JobPlan& p = plan[g * kMaxJobs + k];
-      Job& a = m.job[k];
-      a.src = jb.frames;
-      a.tmp = static_cast<uint8_t*>(workspace) + p.ws_off;
-      a.out = static_cast<char*>(out) + p.out_off * esize;
-      a.xb = reinterpret_cast<const int2*>(jb.x.bounds);
-      a.xk = jb.x.coeffs;
-      a.yb = reinterpret_cast<const int2*>(jb.y.bounds);
-      a.yk = jb.y.coeffs;
-      a.H = jb.H;
-      a.W = jb.W;
-      a.T = jb.T;
-      a.xtaps = jb.x.taps;
-      a.ytaps = jb.y.taps;
-      a.cols = jb.x.count;
-      a.rows = jb.y.span_count;
-      a.row0 = jb.y.span_first;
-      a.span0 = jb.x.span_first;
-      a.span = jb.x.span_count;
-      a.out_rows = jb.y.count;
-      m.row_block0[k] = int(p.row_block);
-      m.col_block0[k] = int(p.col_block);
-      m.row_block0[k + 1] = int(p.row_block + int64_t(a.rows) * a.T);
-      m.col_block0[k + 1] = int(p.col_block + int64_t(a.out_rows) * a.T);
-      row_smem = std::max(row_smem, size_t(a.span) * 3);
+      uint8_t* tmp = static_cast<uint8_t*>(workspace) + p.ws_off;
+      void* o = static_cast<char*>(out) + p.out_off * esize;
+      if (two_stage(jb)) {
+        uint8_t* img = tmp + job_scratch_bytes(jb);
+        first[n_first++] = make_job(jb.frames, jb.T, jb.H, jb.W, jb.x, jb.y, tmp, img);
+        last[k] = make_job(img, jb.T, jb.y.count, jb.x.count, jb.x2, jb.y2, tmp, o);
+      } else {
+        last[k] = make_job(jb.frames, jb.T, jb.H, jb.W, jb.x, jb.y, tmp, o);
+      }
     }
-    resample_rows_kernel<<<m.row_block0[m.n], kThreads, row_smem, st>>>(m);
-    FVS_CHECK_LAUNCH("resample_rows_kernel");
-    if (layout == FVS_PRE_CLIP) {
-      resample_cols_kernel<FVS_PRE_CLIP><<<m.col_block0[m.n], kThreads, 0, st>>>(m);
-    } else if (layout == FVS_PRE_QWEN) {
-      resample_cols_kernel<FVS_PRE_QWEN><<<m.col_block0[m.n], kThreads, 0, st>>>(m);
-    } else {
-      resample_cols_kernel<FVS_PRE_QWEN_CODES><<<m.col_block0[m.n], kThreads, 0, st>>>(m);
-    }
-    FVS_CHECK_LAUNCH("resample_cols_kernel");
+    int r;
+    if (n_first && (r = launch_pair(first, n_first, table, FVS_PRE_RGB8, st))) return r;
+    if ((r = launch_pair(last, m, table, layout, st))) return r;
   }
   return FVS_OK;
 }

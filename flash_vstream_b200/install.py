@@ -64,3 +64,42 @@ def install_qwen():
         ref.weighted_kmeans_ordered_feature = my_qwen.weighted_kmeans_ordered_feature   # imported by name there
         patched.append(mod + ".FlashMemory")
     return patched
+
+
+def install_qwen_fetch(processor=None, device=None, vision_utils=None):
+    """GPU pre-processing for the unmodified Qwen2-VL evaluation drivers (inference_mcq_vqa.py:322-330, INTEGRATION.md
+    §7a).  Rebinds process_vision_info on qwen_vl_utils and qwen_vl_utils.vision_process (or on `vision_utils`, a module
+    with the same names) so that a video given as a list of frames comes back as the device uint8 [n, h, w, 3] tensor
+    of Qwen2VLVideoFetcher.fetch, the bytes of fetch_video's PIL images; images and path videos stay fetch_image's and
+    fetch_video's own.  With `processor` (a FlashVStreamQwen2VLProcessor), its image_processor becomes a
+    Qwen2VLVideoImageProcessor, so processor(text=..., videos=...) pre-processes those tensors on the GPU while the token
+    expansion and visual_position_ids stay the processor's own code.  Install it before the driver imports
+    process_vision_info by name (`from qwen_vl_utils import process_vision_info`)."""
+    from . import preprocess as P
+
+    patched = []
+    mods = [vision_utils] if vision_utils is not None else [importlib.import_module("qwen_vl_utils.vision_process"),
+                                                              importlib.import_module("qwen_vl_utils")]
+    vp = mods[0]
+    extract_vision_info, fetch_image, fetch_video = vp.extract_vision_info, vp.fetch_image, vp.fetch_video
+    fetcher = P.Qwen2VLVideoFetcher(P.Qwen2VLFramePreprocessor(device=device))
+
+    def process_vision_info(conversations):
+        """qwen_vl_utils.process_vision_info (vision_process.py:243-261), a list-of-frames video fetched on the GPU"""
+        image_inputs, video_inputs = [], []
+        for info in extract_vision_info(conversations):
+            if "image" in info or "image_url" in info:
+                image_inputs.append(fetch_image(info))
+            elif "video" in info:
+                video_inputs.append(fetcher.fetch(info) if isinstance(info["video"], (list, tuple)) else fetch_video(info))
+            else:
+                raise ValueError("image, image_url or video should in content.")
+        return image_inputs or None, video_inputs or None
+
+    for mod in mods:
+        mod.process_vision_info = process_vision_info
+        patched.append(f"{mod.__name__}.process_vision_info")
+    if processor is not None:
+        processor.image_processor = P.Qwen2VLVideoImageProcessor(processor.image_processor, device)
+        patched.append(f"{type(processor).__name__}.image_processor")
+    return patched

@@ -5,6 +5,9 @@ reference's CPU image processors (fvs_preprocess, csrc/preprocess_kernels.cu).
                                                         (Flash-VStream-LLaVA/flash_vstream/serve/cli_video_stream.py:186)
     Qwen2VLFramePreprocessor(...)(frames)            == the {'pixel_values_videos', 'video_grid_thw'} of
                                                         FlashVStreamQwen2VLImageProcessor (cli_server_2gpu.py:214-219)
+    Qwen2VLVideoFetcher(...).fetch(ele)              == np.stack(qwen_vl_utils.fetch_video(ele)), a list of frames
+    Qwen2VLVideoFetcher(...)(ele)                    == FlashVStreamQwen2VLImageProcessor(videos=[fetch_video(ele)])
+                                                        (inference_mcq_vqa.py:290-334)
 
 Frames are [T, H, W, 3] uint8 (what decord and np.asarray(PIL image) give): a CUDA tensor, or a host tensor / array
 that is copied to the device (non_blocking, so a pinned one does not block the host).  The resize is Pillow's BICUBIC
@@ -15,6 +18,8 @@ from __future__ import annotations
 
 import ctypes as C
 import math
+import os
+from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 
@@ -114,21 +119,27 @@ class _FramePreprocessor:
         device = torch.device(self.device if self.device is not None else "cuda")
         return device if device.index is not None else torch.device(device.type, torch.cuda.current_device())
 
-    def _plan(self, device, height, width):
+    def _axes(self, device, height, width, rows, cols):
+        """(x, y, device tables) of height x width -> rows = (out_h, first_y, count_y), cols = (out_w, first_x,
+        count_x) on `device`, planned once"""
         import torch
-        key = (device, height, width)
+        key = (device, height, width, rows, cols)
         plan = self._plans.get(key)
         if plan is None:
-            (oh, fy, cy), (ow, fx, cx), pool = self._windows(height, width)
             keep, axes = [], []
-            for size_in, size_out, first, count in ((width, ow, fx, cx), (height, oh, fy, cy)):
+            for size_in, (size_out, first, count) in ((width, cols), (height, rows)):
                 ax, bounds, coeffs = resample_plan(size_in, size_out, first, count)
                 b, k = torch.from_numpy(bounds).to(device), torch.from_numpy(coeffs).to(device)
                 ax.bounds, ax.coeffs = b.data_ptr(), k.data_ptr()
                 keep += [b, k]
                 axes.append(ax)
-            plan = self._plans[key] = (axes[0], axes[1], pool, keep)
+            plan = self._plans[key] = (axes[0], axes[1], keep)
         return plan
+
+    def _plan(self, device, height, width):
+        rows, cols, pool = self._windows(height, width)
+        x, y, keep = self._axes(device, height, width, rows, cols)
+        return x, y, pool, keep
 
     def _table(self, device):
         import torch
@@ -170,7 +181,8 @@ class _FramePreprocessor:
     @staticmethod
     def _out_dtype(layout):
         import torch
-        return {_lib.PRE_CLIP: torch.float16, _lib.PRE_QWEN: torch.float32, _lib.PRE_QWEN_CODES: torch.uint8}[layout]
+        return {_lib.PRE_CLIP: torch.float16, _lib.PRE_QWEN: torch.float32, _lib.PRE_QWEN_CODES: torch.uint8,
+                _lib.PRE_RGB8: torch.uint8}[layout]
 
     def _run(self, frames, out=None, workspace=None, layout=None):
         import torch
@@ -349,3 +361,227 @@ class Qwen2VLFramePreprocessor(_FramePreprocessor):
         out, views = self._many(clips, out, workspace, _lib.PRE_QWEN_CODES if codes else None)
         grids = [torch.tensor([self.grid_thw(*(int(v) for v in f.shape[:3]))], dtype=torch.int64) for f in clips]
         return out, views, grids
+
+
+# ---- qwen_vl_utils.fetch_video, list-of-frames branch (Flash-VStream-Qwen/qwen_vl_utils/vision_process.py) ----------
+FETCH_IMAGE_FACTOR, FETCH_MIN_PIXELS, FETCH_MAX_PIXELS, FETCH_MAX_RATIO = 28, 4 * 28 * 28, 16384 * 28 * 28, 200  # :15-18
+VIDEO_MIN_PIXELS, VIDEO_MAX_PIXELS, VIDEO_TOTAL_PIXELS = 128 * 28 * 28, 768 * 28 * 28, 24576 * 28 * 28        # :20-22
+FRAME_FACTOR, FPS_MAX_FRAMES = 2, 768                                                                         # :23, :26
+
+
+def fetch_smart_resize(height: int, width: int, factor: int = FETCH_IMAGE_FACTOR, min_pixels=FETCH_MIN_PIXELS,
+                       max_pixels=FETCH_MAX_PIXELS) -> tuple[int, int]:
+    """qwen_vl_utils' smart_resize (vision_process.py:44-70), the one fetch_image calls: unlike transformers' it keeps
+    each rounded side at least `factor`, and max_pixels may be a float"""
+    if max(height, width) / min(height, width) > FETCH_MAX_RATIO:
+        raise ValueError(f"absolute aspect ratio must be smaller than {FETCH_MAX_RATIO}, got "
+                         f"{max(height, width) / min(height, width)}")
+    h_bar = max(factor, round(height / factor) * factor)
+    w_bar = max(factor, round(width / factor) * factor)
+    if h_bar * w_bar > max_pixels:
+        beta = math.sqrt((height * width) / max_pixels)
+        h_bar = math.floor(height / beta / factor) * factor
+        w_bar = math.floor(width / beta / factor) * factor
+    elif h_bar * w_bar < min_pixels:
+        beta = math.sqrt(min_pixels / (height * width))
+        h_bar = math.ceil(height * beta / factor) * factor
+        w_bar = math.ceil(width * beta / factor) * factor
+    return h_bar, w_bar
+
+
+def _fetch_budget(n_frames: int, ele: dict):
+    """(nframes, min_pixels, max_pixels) of fetch_video's list branch (vision_process.py:197-211): max_pixels comes from
+    the frame count before the even-count padding"""
+    nframes = n_frames
+    if nframes > ele.get("max_frames", FPS_MAX_FRAMES):
+        nframes = math.floor(ele.get("max_frames", FPS_MAX_FRAMES) / FRAME_FACTOR) * FRAME_FACTOR
+    if nframes < 1:    # the reference divides by it next
+        raise ValueError(f"no frame to fetch: {n_frames} frames, max_frames {ele.get('max_frames', FPS_MAX_FRAMES)}")
+    min_pixels = ele.get("min_pixels", VIDEO_MIN_PIXELS)
+    total_pixels = ele.get("total_pixels", VIDEO_TOTAL_PIXELS)
+    max_pixels = max(min(VIDEO_MAX_PIXELS, total_pixels / nframes * FRAME_FACTOR), min_pixels * 1.05)
+    return nframes, min_pixels, ele.get("max_pixels", max_pixels)
+
+
+def fetch_video_picks(n_frames: int, ele: dict) -> list[int]:
+    """the indices into ele['video'] of the frames fetch_video returns, in order (vision_process.py:217-221): the
+    torch.linspace(...).round() pick, the `i in idx` selection, then the last pick repeated up to an even count"""
+    import torch
+    nframes, _, _ = _fetch_budget(n_frames, ele)
+    idx = set(torch.linspace(0, n_frames - 1, nframes).round().long().tolist())
+    picks = [i for i in range(n_frames) if i in idx]
+    return picks + picks[-1:] * (math.ceil(len(picks) / FRAME_FACTOR) * FRAME_FACTOR - len(picks))
+
+
+def fetch_video_size(height: int, width: int, n_frames: int, ele: dict) -> tuple[int, int]:
+    """(resized_height, resized_width) fetch_image gives a height x width frame of a list of n_frames
+    (vision_process.py:207-215, :96-113): resized_height / resized_width, when both are given, go through smart_resize
+    with fetch_image's default pixel bounds; otherwise the frame's own size does, with the video's bounds"""
+    if "resized_height" in ele and "resized_width" in ele:
+        h, w = fetch_smart_resize(ele["resized_height"], ele["resized_width"])
+    else:
+        _, min_pixels, max_pixels = _fetch_budget(n_frames, ele)
+        h, w = fetch_smart_resize(height, width, min_pixels=min_pixels, max_pixels=max_pixels)
+    if h <= 0 or w <= 0:
+        raise ValueError(f"a {height}x{width} frame resizes to {h}x{w}")
+    return h, w
+
+
+def _decoded(frame) -> np.ndarray:
+    """one frame of a fetch_video list as uint8 [H, W, 3]: a path or PIL image the way fetch_image reads it (PIL,
+    .convert('RGB')), an array as it is"""
+    from PIL import Image
+    if isinstance(frame, (str, os.PathLike)):
+        path = os.fspath(frame)
+        with Image.open(path[7:] if path.startswith("file://") else path) as im:
+            return np.asarray(im.convert("RGB"))
+    if isinstance(frame, Image.Image):
+        return np.asarray(frame.convert("RGB"))
+    a = np.asarray(frame)
+    if a.dtype != np.uint8 or a.ndim != 3 or a.shape[2] != 3:
+        raise ValueError(f"a frame must be a path, a PIL image or uint8 [H, W, 3], got {a.dtype} {a.shape}")
+    return a
+
+
+class Qwen2VLVideoFetcher:
+    """The two pre-processing steps of Qwen2-VL's evaluation drivers (inference_mcq_vqa.py:290-334) on the GPU,
+    bit-identical: qwen_vl_utils.fetch_video on a list of frames (vision_process.py:192-222: the frame pick, fetch_image's
+    Pillow BICUBIC resize to a multiple of 28, the even-count padding), then FlashVStreamQwen2VLImageProcessor on its
+    result (the second resize to a multiple of 28 * additional_pool_size, rescale, normalize, patchify), the second
+    step configured by `preprocessor` (default: Qwen2VLImageProcessor's settings).
+
+    An element is fetch_video's {'video': [frame, ...], 'max_frames', 'min_pixels', 'max_pixels', 'total_pixels',
+    'resized_height', 'resized_width'}, all keys but 'video' optional.  A frame is a decoded uint8 [H, W, 3] array, a
+    PIL image, or a path, which is decoded and converted to RGB with PIL on the host, in a thread pool.  Only the picked
+    frames are decoded and copied to the device, and every size is worked out before the copy, so a refused element
+    copies nothing.  The frames of one video must decode to one size (fetch_image would resize each on its own)."""
+
+    def __init__(self, preprocessor: Qwen2VLFramePreprocessor | None = None, decode_threads: int | None = None):
+        self.pre = preprocessor if preprocessor is not None else Qwen2VLFramePreprocessor()
+        self.decode_threads = int(decode_threads or min(32, os.cpu_count() or 1))
+
+    def _load(self, ele):
+        """-> (host uint8 [n, H, W, 3] frames of the fetched video, padding included, as a list of arrays, (h1, w1))"""
+        video = ele.get("video") if isinstance(ele, dict) else None
+        if not isinstance(video, (list, tuple)):
+            raise TypeError("a fetch_video element with a list of frames ({'video': [frame, ...], ...}) is expected")
+        picks = fetch_video_picks(len(video), ele)
+        unique = sorted(set(picks))
+        if any(isinstance(video[i], (str, os.PathLike)) for i in unique) and len(unique) > 1:
+            with ThreadPoolExecutor(min(self.decode_threads, len(unique))) as pool:
+                decoded = dict(zip(unique, pool.map(lambda i: _decoded(video[i]), unique)))
+        else:
+            decoded = {i: _decoded(video[i]) for i in unique}
+        sizes = {decoded[i].shape[:2] for i in unique}
+        if len(sizes) != 1:
+            raise ValueError(f"the frames of one video decode to more than one size: {sorted(sizes)}")
+        (H, W), = sizes
+        return [decoded[i] for i in picks], fetch_video_size(H, W, len(video), ele)
+
+    def _submit(self, eles, codes=None):
+        """every element through one fvs_preprocess_multi call -> (flat out, [(element offset, T, (h1, w1))])
+        codes=None: the fetched images themselves (FVS_PRE_RGB8); else the processor's rows (two-stage jobs)"""
+        import torch
+        if not isinstance(eles, (list, tuple)) or not eles:
+            raise ValueError("a non-empty list of fetch_video elements is expected")
+        loaded = [self._load(e) for e in eles]          # every refusal of the host arithmetic happens here
+        pre, device = self.pre, self.pre._device()
+        layout = _lib.PRE_RGB8 if codes is None else _lib.PRE_QWEN_CODES if codes else _lib.PRE_QWEN
+        n = len(loaded)
+        jobs = (_lib.PreprocessJob * n)()
+        hosts = []
+        for i, (frames, (h1, w1)) in enumerate(loaded):
+            T, (H, W) = len(frames), frames[0].shape[:2]
+            x, y, _ = pre._axes(device, H, W, (h1, 0, h1), (w1, 0, w1))
+            host = torch.empty((T, H, W, 3), dtype=torch.uint8, pin_memory=True)
+            np.stack(frames, out=host.numpy())
+            hosts.append(host)
+            jobs[i] = _lib.PreprocessJob(host.data_ptr(), T, H, W, 3, x, y)
+            if codes is not None:
+                h2, w2 = pre.resized(h1, w1)
+                jobs[i].x2, jobs[i].y2, _ = pre._axes(device, h1, w1, (h2, 0, h2), (w2, 0, w2))
+        lib = _lib.load()
+        plan, totals = (C.c_int64 * (4 * n))(), (C.c_int64 * 2)()
+        r = lib.fvs_preprocess_plan(jobs, n, layout, pre.pool, plan, totals)
+        if r < 0:
+            _lib.check(r, "fvs_preprocess_plan")
+        frames = [h.to(device, non_blocking=True) for h in hosts]
+        for i, f in enumerate(frames):
+            jobs[i].frames = f.data_ptr()
+        out = torch.empty(int(totals[0]), dtype=pre._out_dtype(layout), device=device)
+        workspace = torch.empty(int(totals[1]), dtype=torch.uint8, device=device)
+        with torch.cuda.device(device):
+            _lib.check(lib.fvs_preprocess_multi(jobs, n, pre._table(device).data_ptr(), layout, pre.pool,
+                                                out.data_ptr(), workspace.data_ptr(), workspace.numel(),
+                                                _lib.cur_stream()), "fvs_preprocess_multi")
+        return out, [(int(plan[4 * i + 2]), len(f), s) for i, (f, s) in enumerate(loaded)]
+
+    def fetch(self, ele):
+        """-> uint8 [n, h1, w1, 3] on the device: np.stack([np.asarray(im) for im in fetch_video(ele)])"""
+        out, [(_, T, (h1, w1))] = self._submit([ele])
+        return out.view(T, h1, w1, 3)
+
+    def many(self, eles, codes: bool = False):
+        """-> {'pixel_values_videos': fp32 [sum t*gh*gw, 1176] on the device (uint8 codes with codes=True, as
+        Qwen2VLFramePreprocessor gives), 'video_grid_thw': int64 [len(eles), 3] on the host}: what the image processor
+        returns for videos=[fetch_video(e) for e in eles], every video in one launch group per 32 videos"""
+        import torch
+        out, parts = self._submit(eles, codes=bool(codes))
+        grids = [self.pre.grid_thw(T, h1, w1) for _, T, (h1, w1) in parts]
+        return {"pixel_values_videos": out.view(-1, 3 * QWEN_TEMPORAL * QWEN_PATCH * QWEN_PATCH),
+                "video_grid_thw": torch.tensor(grids, dtype=torch.int64)}
+
+    def __call__(self, ele, codes: bool = False):
+        return self.many([ele], codes)
+
+
+def qwen_preprocessor_of(image_processor, additional_pool_size: int = 1, device=None) -> Qwen2VLFramePreprocessor:
+    """the Qwen2VLFramePreprocessor that computes what `image_processor` (a FlashVStreamQwen2VLImageProcessor, or
+    transformers' Qwen2VLImageProcessor) does to a video with additional_pool_size; raises NotImplementedError for a
+    configuration the kernels do not reproduce"""
+    p = image_processor
+    resample = getattr(p, "resample", None)
+    if resample is None or int(resample) != BICUBIC:
+        raise NotImplementedError(f"resample={resample!r}: only bicubic ({BICUBIC}) is implemented")
+    if not getattr(p, "do_resize", True):
+        raise NotImplementedError("do_resize=False is not implemented")
+    if (getattr(p, "patch_size", QWEN_PATCH), getattr(p, "merge_size", QWEN_MERGE),
+            getattr(p, "temporal_patch_size", QWEN_TEMPORAL)) != (QWEN_PATCH, QWEN_MERGE, QWEN_TEMPORAL):
+        raise NotImplementedError("only patch_size 14, merge_size 2 and temporal_patch_size 2 are implemented")
+    size = getattr(p, "size", None)
+    min_pixels = getattr(p, "min_pixels", None) or _field(size, "shortest_edge")
+    max_pixels = getattr(p, "max_pixels", None) or _field(size, "longest_edge")
+    norm = getattr(p, "do_normalize", True)
+    return Qwen2VLFramePreprocessor(min_pixels, max_pixels, additional_pool_size,
+                                    p.image_mean if norm else None, p.image_std if norm else None,
+                                    p.rescale_factor if getattr(p, "do_rescale", True) else None, device)
+
+
+class Qwen2VLVideoImageProcessor:
+    """A stand-in for a Qwen2-VL processor's `image_processor` (install.install_qwen_fetch): a videos= call whose videos
+    are all device uint8 [n, h, w, 3] tensors (what Qwen2VLVideoFetcher.fetch returns) is pre-processed on the GPU, one
+    launch pair per 32 videos, into the BatchFeature the wrapped processor returns for the same frames: the fp32 rows
+    'pixel_values_videos' on the device and the int64 'video_grid_thw' on the host.  Any other call, and every other
+    attribute, is the wrapped processor's own."""
+
+    def __init__(self, image_processor, device=None):
+        self.__dict__["image_processor"] = image_processor
+        self.__dict__["device"] = device
+        self.__dict__["_pre"] = {}
+
+    def __getattr__(self, name):
+        return getattr(self.__dict__["image_processor"], name)
+
+    def __call__(self, images=None, videos=None, return_tensors=None, additional_pool_size: int = 1, **kwargs):
+        import torch
+        if (images is not None or kwargs or not isinstance(videos, (list, tuple)) or not videos or
+                not all(isinstance(v, torch.Tensor) and v.is_cuda and v.dtype == torch.uint8 for v in videos)):
+            return self.image_processor(images=images, videos=videos, return_tensors=return_tensors,
+                                        additional_pool_size=additional_pool_size, **kwargs)
+        pre = self._pre.get(additional_pool_size)
+        if pre is None:
+            pre = self._pre[additional_pool_size] = qwen_preprocessor_of(self.image_processor, additional_pool_size,
+                                                                         self.device)
+        out, _, grids = pre.many(list(videos))
+        from transformers.feature_extraction_utils import BatchFeature
+        return BatchFeature(data={"pixel_values_videos": out, "video_grid_thw": torch.cat(grids)})

@@ -711,7 +711,7 @@ typedef struct fvs_resample_axis {
   const int32_t* bounds;        /* device int32 [count, 2] = {first source index, taps used}, 8-byte aligned */
   const int32_t* coeffs;        /* device int32 [count, taps], 22 fractional bits */
 } fvs_resample_axis;
-enum { FVS_PRE_CLIP = 0, FVS_PRE_QWEN = 1, FVS_PRE_QWEN_CODES = 2 };
+enum { FVS_PRE_CLIP = 0, FVS_PRE_QWEN = 1, FVS_PRE_QWEN_CODES = 2, FVS_PRE_RGB8 = 3 };
 
 /* Host: PIL's per-axis plan (precompute_coeffs + normalize_coeffs_8bpc, in double, in PIL's order, no FMA contraction)
  * for the window [first, first + count) of in_size -> out_size.  Fills every field of *axis_h but bounds / coeffs, which
@@ -729,6 +729,8 @@ size_t fvs_preprocess_workspace_bytes(const fvs_resample_axis* x_h, const fvs_re
  *                 temporal slots (:136-137).  The windows must be whole, T 1 or even, and both sizes multiples of 28 * pool.
  *   FVS_PRE_QWEN_CODES: out uint8 [max(T, 2) / 2 * gh * gw, 1176], FVS_PRE_QWEN's rows and columns holding the resampled
  *                 byte u itself instead of table[c][u], c = column / 392 (DESIGN.md §3.20); the same rules, the same plan.
+ *   FVS_PRE_RGB8: out uint8 [T, y.count, x.count, 3], the resized 8-bit image itself (np.asarray of the PIL image that
+ *                 Image.resize returns); the table is not read.
  * FVS_EINVAL, with nothing launched, on null pointers, C != 3, an empty input, a plan that does not match the frames or
  * fvs_resample_plan, a window outside the resized image, a workspace below fvs_preprocess_workspace_bytes, or a Qwen2-VL
  * call breaking the rules above. */
@@ -741,16 +743,25 @@ int fvs_preprocess(const uint8_t* frames, int T, int H, int W, int C, const fvs_
  * Qwen2-VL: fp32 rows [sum t * gh * gw, 1176]), and each takes its own slice of one workspace.  Every job's bits equal
  * fvs_preprocess on that clip alone (it is the one-job case of the same code).  One launch pair per 32 jobs: a flat grid
  * whose blocks find their job in a block-offset table passed as a kernel parameter.  Every job is checked as
- * fvs_preprocess checks its clip before anything is launched; FVS_EINVAL names the first bad job. */
+ * fvs_preprocess checks its clip before anything is launched; FVS_EINVAL names the first bad job.
+ * A job whose x2 / y2 are set (out_size != 0) has two stages, the chain of Qwen2-VL's evaluation drivers
+ * (qwen_vl_utils fetch_image's Pillow resize, then the image processor's, DESIGN.md §3.11): x / y resize the frames to
+ * an 8-bit RGB image [T, y.count, x.count, 3] kept in the job's workspace, exactly the bytes FVS_PRE_RGB8 writes, and
+ * x2 / y2 (planned for x.count -> x2.out_size, y.count -> y2.out_size) resize that image into `layout`.  A group of 32
+ * jobs holding a two-stage job takes a second launch pair, ahead of its own, for the first stages.  With x2 / y2 zeroed
+ * a job is the single-stage job it always was. */
 typedef struct fvs_preprocess_job {
   const uint8_t* frames;        /* device uint8 [T, H, W, C = 3] */
   int T, H, W, C;
   fvs_resample_axis x, y;
+  fvs_resample_axis x2, y2;     /* second stage, or all zero */
 } fvs_preprocess_job;
 /* Host plan of a job table (pure host arithmetic, validates like fvs_preprocess_multi, no CUDA call): plan_h [n_jobs, 4] =
  * {first block of the job in its rows launch, in its cols launch, output elements before it, workspace bytes before it};
- * an element is 2 bytes (CLIP), 4 (Qwen2-VL) or 1 (Qwen2-VL codes), and the codes layout plans as FVS_PRE_QWEN does;
- * totals_h [2] = {output elements, workspace bytes}.  Returns the number of launch pairs (>= 1) or a negative error. */
+ * an element is 2 bytes (CLIP), 4 (Qwen2-VL) or 1 (Qwen2-VL codes, RGB8), and the codes layout plans as FVS_PRE_QWEN
+ * does; the block offsets are those of the job's last stage.  totals_h [2] = {output elements, workspace bytes}; a
+ * two-stage job's workspace holds its first-stage image after the scratch of its passes.  Returns the number of groups
+ * of up to 32 jobs (>= 1) or a negative error. */
 int fvs_preprocess_plan(const fvs_preprocess_job* jobs_h, int n_jobs, int layout, int pool, int64_t* plan_h,
                         int64_t* totals_h);
 /* workspace: at least totals_h[1] bytes of fvs_preprocess_plan; out: totals_h[0] elements. */
